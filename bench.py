@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — allocation decisions/sec of the best-fit path on B200.
+"""bench.py — allocation decisions/sec of the best-fit path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl native|reference]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic requests: score R
 requests against the node's capacity table, write R device indices, the per-device
@@ -33,6 +34,12 @@ Timed legs (one JSON line on rank 0):
             loop and no Go toolchain exists here) on the host cores, bounded sample.
 
 --impl reference times that CPU port alone, all host threads, on the same config.
+
+--dump-outputs DIR writes, after the timed region, what its last (K-th) step returned to its caller:
+idx.npy (device index per request row, float32), demand.npy (per-device core and memory demand sums,
+float64) and table_out.npy (table', float32).  A batch of more than DUMP_ROWS rows is dumped as a fixed,
+seeded sample of rows, listed in rows.npy.  Inputs depend on the arguments only, so two builds run with
+the same arguments can be compared array for array.  With N > 1 every rank writes its own shard (_rank<r>).
 """
 from __future__ import annotations
 
@@ -58,7 +65,9 @@ REPLAYS = int(os.environ.get("EGPU_BENCH_REPLAYS", "101"))
 # stuck in the gate's own launch - and would sit there until its 2 s timeout: EGPU_BENCH_NO_GATE=1 leaves it out
 USE_GATE = [not os.environ.get("EGPU_BENCH_NO_GATE")]
 GATE_NOTE = [None]
-RING = 32  # batches in the rotation: 32 x 12 MB (1M rows) = 384 MB > 126 MB L2
+RING = 32  # batches in the rotation: 32 x 12 MB (1M rows) = 384 MB > 50 MB L2
+L2_BYTES = 50 << 20  # H100
+DUMP_ROWS = 1 << 22  # --dump-outputs: rows of idx (+ rows) kept per batch, 48 MB
 
 
 def peaks():
@@ -68,17 +77,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(workload):
-    """dram__bytes_read.sum + dram__bytes_write.sum per BATCH of the scan kernel, from the committed
-    `ncu --set full` capture of this workload (profiles/r2_traffic.json), else None."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    try:
-        return float(json.load(open(p))[workload]["traffic_per_batch"])
-    except Exception:
-        return None
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not measured)"
 
 
 class ClockSampler:
@@ -93,6 +92,7 @@ class ClockSampler:
         self.th = None
         self.proc = None
         self.how = None
+        self.power_limit_w = None
 
     def start(self):
         try:
@@ -111,6 +111,7 @@ class ClockSampler:
                     (pynvml.nvmlClocksEventReasonSwThermalSlowdown, "sw_thermal_slowdown"),
                     (pynvml.nvmlClocksEventReasonSwPowerCap, "sw_power_cap")]
             mx = float(pynvml.nvmlDeviceGetMaxClockInfo(h, pynvml.NVML_CLOCK_SM))
+            self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
 
             def pump():
                 while not self.stop_flag.is_set():
@@ -167,7 +168,7 @@ class ClockSampler:
         if not self.sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["clock sampling unavailable"]}
         return {"sm_mhz": float(np.median(self.sm)), "sm_max_mhz": max(self.mx), "reasons": sorted(self.reasons),
-                "samples": len(self.sm), "how": self.how}
+                "samples": len(self.sm), "how": self.how, "power_limit_w": self.power_limit_w}
 
 
 def make_host_batches(e, w, rank, nb, R):
@@ -208,7 +209,7 @@ def l2_label(R):
     """config.l2, identical in both arms (it describes the GPU arm's inputs; the CPU arm streams from host memory)"""
     nb = ring_batches(R)
     mb = nb * 12 * R / 1e6
-    return (f"GPU arm: inputs rotate through a ring of {nb} batches = {mb:.0f} MB (> 126 MB L2)" if nb * 12 * R > (126 << 20)
+    return (f"GPU arm: inputs rotate through a ring of {nb} batches = {mb:.0f} MB (> 50 MB L2)" if nb * 12 * R > L2_BYTES
             else f"GPU arm: ring of {nb} batches = {mb:.1f} MB (<= L2: small table)")
 
 
@@ -378,6 +379,22 @@ def summarise(ms_list, K):
                     "stream, max over ranks; CUDA event resolution on this part is ~2 us per region"}
 
 
+def dump_outputs(out_dir, leg, K, rank, world):
+    """What the K-th timed step returned: its ring entry's indices, demand sums and table' (see --dump-outputs)."""
+    os.makedirs(out_dir, exist_ok=True)
+    _, _, idx, delta, table_out = leg.ring[(K - 1) % leg.nb]
+    out = {"idx": idx[:leg.R].cpu().numpy()}
+    if leg.R > DUMP_ROWS:
+        rows = np.unique(np.random.default_rng(0).integers(0, leg.R, DUMP_ROWS))
+        out = {"idx": out["idx"][rows], "rows": rows.astype(np.float64)}
+    out["idx"] = out["idx"].astype(np.float32)  # indices are -1..63: exact in float32
+    out["demand"] = delta.cpu().numpy().astype(np.float64)
+    out["table_out"] = table_out.cpu().numpy().astype(np.float32)
+    sfx = f"_rank{rank}" if world > 1 else ""
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, f"{name}{sfx}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -392,7 +409,10 @@ def main():
                          "(peer-fused, EGPU_F_APPLY); or NCCL all-gather + apply_deltas")
     ap.add_argument("--force-peer", action="store_true", help="experiment: the sharded step structure even at N = 1 (exchange with self)")
     ap.add_argument("--cpu-budget", type=float, default=3.0, help="seconds per CPU-baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
 
     # stdout carries exactly one JSON line: whatever libraries print there (NCCL prints its
@@ -507,6 +527,8 @@ def main():
         return timed_replays(torch, dist, alloc, stream, g, world, dev, REPLAYS), counts[0]
 
     ms_list, launches = measure(leg)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, leg, K, rank, world)
     timing = summarise(ms_list, K)
     ms = timing["ms_per_step_median"] * K
     value = world * R * K / (ms * 1e-3)
@@ -803,7 +825,7 @@ def main():
                 del g
             best = row.get("k200", row.get("k20"))
             row.update({"us_per_launch_step": best["us_per_step"], "frac": best["frac"],
-                        "l2": "ring > L2" if lg.nb * 12 * lg.R > (126 << 20) else "ring <= L2 (small table)"})
+                        "l2": "ring > L2" if lg.nb * 12 * lg.R > L2_BYTES else "ring <= L2 (small table)"})
             sweep.append(row)
             del lg
             torch.cuda.empty_cache()
@@ -855,10 +877,10 @@ def main():
             "e2e_packed": e2e_packed,
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": ncu_traffic(args.workload), "kernel": kernel,
+                         "kernel": kernel,
                          "algorithmic_bytes_per_launch": alg_bytes_launch, "algorithmic_bytes_per_batch": 12 * R + 32 * D,
-                         "avg_launch_us": per_step_s * 1e6 * K / n_scan, "batches_per_launch": K / n_scan, "peak_source": peak_src,
-                         "note": "traffic = ncu dram bytes per BATCH of the committed capture (a launch carries batches_per_launch of them)"},
+                         "avg_launch_us": per_step_s * 1e6 * K / n_scan, "batches_per_launch": K / n_scan, "peak_source": peak_src},
+            "gpu": torch.cuda.get_device_name(dev),
             "per_call": per_call,
             "cpu_baseline": cpu,
             "clocks": clocks,

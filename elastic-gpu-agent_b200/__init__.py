@@ -1,6 +1,6 @@
-"""elastic-gpu-agent_b200 — B200-native best-fit allocation path for elastic-gpu-agent.
+"""elastic-gpu-agent_b200 — H100-native best-fit allocation path for elastic-gpu-agent.
 
-Only what the hot path needs: csrc/ (sm_100a kernels + the C ABI of
+Only what the hot path needs: csrc/ (sm_90a kernels + the C ABI of
 include/egpu_alloc.h), the ctypes binding, a thin host wrapper and the
 synthetic-workload generator.  Import as `elastic_gpu_agent_b200` (the
 directory name carries a hyphen; the sibling shim package maps it).

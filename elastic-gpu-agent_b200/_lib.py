@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI declared in include/egpu_alloc.h.
 
-The library is built in-tree by __graft_entry__.build() (nvcc, sm_100a) as
+The library is built in-tree by __graft_entry__.build() (nvcc, sm_90a) as
 elastic-gpu-agent_b200/lib/libegpu_alloc.so.  Importing this module without it
 raises: there is no Python or CPU fallback for the allocation path.
 """
@@ -69,7 +69,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU fallback.")
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     vp = C.c_void_p
     sigs = {

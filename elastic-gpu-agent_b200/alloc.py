@@ -37,7 +37,7 @@ def _stream(stream):
 
 
 class BestFitAllocator:
-    """Best-fit device choice over a node-local capacity table on one B200."""
+    """Best-fit device choice over a node-local capacity table on one H100."""
 
     def __init__(self, cuda_device: int = 0):
         self._lib = L.load()

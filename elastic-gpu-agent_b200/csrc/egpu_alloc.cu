@@ -1,4 +1,4 @@
-// egpu_alloc.cu — best-fit fractional-GPU allocation on B200 (sm_100a) + its C ABI.
+// egpu_alloc.cu — best-fit fractional-GPU allocation on H100 (sm_90a) + its C ABI.
 //
 // Product path.  There is no CPU fallback in this file and nothing here
 // includes or links oracle/: when no CUDA device is usable every entry point
@@ -197,7 +197,7 @@ int launch_snapshot(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int
     }
     // Early trigger (griddepcontrol.launch_dependents before the work is done) only helps when
     // the next launch is another scan of a pipelined stream, so only those launches do it.
-    // (Checked on B200, scripts/probes/pdl_event_probe.cu and scripts/eager_probe.py: events
+    // (What scripts/probes/pdl_event_probe.cu and scripts/eager_probe.py check: events
     // and ordinary kernels enqueued after a PDL launch still wait for its completion.)
     if (user_flags & EGPU_F_INPUTS_READY) flags |= kFlagEarlyTrigger;
     const unsigned long long slot = (finalize ? (ctx->seq % kEpiSlots) : static_cast<unsigned long long>(kEpiSlots)) |
@@ -206,12 +206,12 @@ int launch_snapshot(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int
     // Grid: one resident wave at most.  A lone launch wants every SM pulling at once
     // (8 rows per thread, one trip); launches of a pipelined stream overlap each
     // other, so a smaller grid with more rows per thread (48) costs fewer CTA
-    // launches, fewer atomics and leaves room for the neighbours — measured best on
-    // B200 at R = 1M.  The zero-copy path passes its own hint (see egpu_bestfit_batch).
+    // launches, fewer atomics and leaves room for the neighbours (scripts/tune_sweep.sh
+    // re-measures the choice at R = 1M).  The zero-copy path passes its own hint (see egpu_bestfit_batch).
     const int64_t nvec = R >> 2;
     int rpt = 8;
     // (measured and dropped: giving the launches of a pipelined stream that could not themselves be
-    // pipelined - the first of a graph - the lone-launch grid: 2.80 against 2.68 us per step)
+    // pipelined - the first of a graph - the lone-launch grid: slower per step)
     if (user_flags & EGPU_F_INPUTS_READY) rpt = (lut_variant || ctx->D <= 16) ? 48 : 8;  // measured, scripts/tune_*.sh
     else if (lut_variant) rpt = 32;  // the lookup scan has a 13 KB per-CTA table tile to amortise
     if (rpt_hint > 0) rpt = rpt_hint;
@@ -353,7 +353,7 @@ int launch_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cud
     if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
     // CTAs resident at once, x waves.  One wave is best for 1 M-row batches (every extra CTA is an extra
     // epilogue); for a few huge batches two waves of half-size CTAs let the hardware's CTA scheduler even
-    // out the SMs (64 Mi rows: 129 -> 124 us per batch, same-box A/B with EGPU_MULTI_WAVES)
+    // out the SMs (64 Mi rows; EGPU_MULTI_WAVES overrides the choice for an A/B)
     const int waves = ctx->multi_waves > 0 ? ctx->multi_waves : (max_r >= (16ll << 20) ? 2 : 1);
     const int64_t cap = static_cast<int64_t>(ctx->sm_count) * per_sm * waves;
     int64_t extra = 0;

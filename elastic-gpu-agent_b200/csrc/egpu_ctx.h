@@ -58,7 +58,7 @@ struct egpu_ctx {
     bool attached = false;
     bool lut_dirty = true;            // table changed since the lookup tables were built
     int dev = -1;
-    int sm_count = 148;
+    int sm_count = 132;  // H100 SXM; egpu_ctx_create reads the device's own count
     cudaStream_t stream = nullptr;
     DevState* d_state = nullptr;
     bool has_table = false;

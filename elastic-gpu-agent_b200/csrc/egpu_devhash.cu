@@ -88,8 +88,7 @@ __global__ void pack_ids_kernel(const char* __restrict__ flat, long long flat_by
 // range in key order.  When the largest set fits shared memory (<= 16 384 keys = 128 KB; a node-scale
 // container has 4 K .. 16 K IDs) one CTA per set runs a bitonic network over its range, padded to a
 // power of two with all-ones keys (no packed ID has a 0xF nibble): 105 barrier-separated steps at
-// 16 K, ~20 us for the whole batch, against ten global radix passes of three kernels (~0.55 ms for
-// 934 k IDs).  Equal keys are equal IDs, so the network's instability is invisible.
+// 16 K, against ten global radix passes of three kernels over the whole batch.  Equal keys are equal IDs, so the network's instability is invisible.
 constexpr int kSortSmemMaxKeys = 16384;
 __global__ void __launch_bounds__(1024)
 sort_sets_smem_kernel(unsigned long long* __restrict__ key, const long long* __restrict__ set_off) {

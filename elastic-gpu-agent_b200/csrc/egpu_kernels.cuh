@@ -1,4 +1,4 @@
-// egpu_kernels.cuh — sm_100a kernels of the best-fit allocation path.
+// egpu_kernels.cuh — sm_90a kernels of the best-fit allocation path.
 //
 // Everything here is integer compare / subtract / min over int32 arrays that
 // stream through HBM once: 12 algorithmic bytes per decision (two int32 in,

@@ -1,4 +1,4 @@
-// egpu_scan.cuh — snapshot-mode kernels of the best-fit path (sm_100a): the register scan
+// egpu_scan.cuh — snapshot-mode kernels of the best-fit path (sm_90a): the register scan
 // (bestfit_sorted_kernel and its multi-batch form), its packed-format twin, the literal grid
 // scan, the lookup-table scan for large D (single- and multi-batch) with its table builder, the
 // shared epilogue (demand sums with the arrival count inside them, publication by each word's finisher, fused peer push / apply),
@@ -779,7 +779,7 @@ lut_build_kernel(const DevState* __restrict__ st, DevLut* __restrict__ lut) {
     }
 }
 
-// Demand sums of the lookup scan.  64-bit shared-memory adds compile to CAS loops on sm_100a
+// Demand sums of the lookup scan.  64-bit shared-memory adds compile to CAS loops on sm_90a
 // (ATOMS.CAST.SPIN.64) and lane-private 64-bit sums cost 16.6 KB per warp; what is used instead is
 // native 32-bit ATOMS.ADD: two UNCONDITIONAL adds per request - word 0 = core | (mem >> 16) << 20,
 // word 1 = mem & 0xffff - into one of 8 copies of a small table per warp (copy = lane / 4; the
@@ -790,7 +790,7 @@ lut_build_kernel(const DevState* __restrict__ st, DevLut* __restrict__ lut) {
 // (Measured and dropped, DESIGN.md 7.2: round 1's three conditional adds into one table per warp;
 // 64-bit sums in columns owned by lane pairs with the half-warps taking turns - fewer shared-memory
 // wavefronts, 7.95 M against 10.3 M per 20 M decisions, but 8.3 KB per warp halves the occupancy.)
-// (4 copies of 8 lanes would fit four CTAs per SM instead of three: measured slower, 2.97 against 2.77 us per
+// (4 copies of 8 lanes would fit four CTAs per SM instead of three: measured slower per
 // batch - the extra bank conflicts of the adds cost more than the occupancy brings)
 constexpr int kLutCopies = 8;
 constexpr int kLutLanesPerCopy = 32 / kLutCopies;

@@ -1,5 +1,5 @@
 /*
- * egpu_alloc.h — C ABI of the B200-native best-fit allocation path.
+ * egpu_alloc.h — C ABI of the H100-native best-fit allocation path.
  *
  * This is the drop-in boundary: a Go DaemonSet (elastic-gpu-agent) binds these
  * symbols through cgo; nothing in the signatures is a CUDA, torch or C++ type.
@@ -70,7 +70,7 @@ extern "C" {
 
 #define EGPU_MAX_DEVICES   64
 #define EGPU_CORE_MAX      100              /* pkg/common/const.go:4 */
-#define EGPU_MEM_MAX       ((1 << 18) - 1)  /* MiB; B200 reports 183359 */
+#define EGPU_MEM_MAX       ((1 << 18) - 1)  /* MiB; an H100 80GB reports 81559 */
 #define EGPU_MAX_ROWS      2147483647       /* requests per batch (R): the scans index with 32 bits */
 #define EGPU_IDX_INFEASIBLE (-1)
 #define EGPU_IDX_DEFERRED   (-2)            /* prefix-commit mode only */
@@ -133,7 +133,7 @@ const char* egpu_strerror(int code);
  * record a parse error was found in.  The pointer stays valid for the life of the context;
  * the text is overwritten by the next failing call. */
 const char* egpu_last_error(egpu_ctx* ctx);
-/* 1 = CUDA sm_100a path.  (0 is reserved; this library never returns it.) */
+/* 1 = CUDA sm_90a path.  (0 is reserved; this library never returns it.) */
 int  egpu_backend(egpu_ctx* ctx);
 /* number of kernels this context has launched since creation */
 int64_t egpu_launch_count(egpu_ctx* ctx);
@@ -205,9 +205,8 @@ void egpu_host_free(egpu_ctx* ctx, void* p);
 
 /* Pins caller-owned memory in place (cudaHostRegister, mapped) so that buffers the caller already
  * has - a Go slice it keeps for the life of the plugin, say - take the zero-staging path of
- * egpu_bestfit_batch / _packed instead of being copied through HBM: on a PCIe Gen5 B200 that is
- * ~0.2 ms instead of ~1 ms per 1 M requests.  Registration costs about a millisecond per 10 MB, so
- * it pays only for buffers that are reused.  The range must stay allocated until
+ * egpu_bestfit_batch / _packed instead of being copied through HBM.  Registration is slow next to
+ * one call, so it pays only for buffers that are reused.  The range must stay allocated until
  * egpu_host_unregister (a cgo caller must not hand over memory the Go runtime may release:
  * allocate it with C.malloc or keep it pinned with runtime.Pinner).  The context does not track
  * registrations. */

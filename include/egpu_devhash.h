@@ -7,7 +7,7 @@
  *   Device.Equals    pkg/types/device.go:27-29   Hash == && List == (&& ResourceName ==)
  * used by Allocate (pkg/plugins/gpushare.go:44,179), PreStartContainer (:92,217) and — once
  * per candidate container on the node — by KubeletDeviceLocator.Locate
- * (pkg/kube/locator.go:62-90), the reference's real CPU hot loop: at B200 scale the
+ * (pkg/kube/locator.go:62-90), the reference's real CPU hot loop: at node scale the
  * gpu-memory plugin hands out one ID per MiB, so a 16 GiB container is 16384 strings to
  * sort and hash, for every candidate, on every container start.
  *

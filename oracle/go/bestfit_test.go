@@ -3,7 +3,7 @@ package bestfit
 
 import "testing"
 
-const capMem = 183359 // MiB a B200 reports
+const capMem = 183359 // MiB per card of the synthetic node (elastic-gpu-agent_b200/synth.py)
 
 func fullTable() ([]int32, []int32) {
 	fc, fm := make([]int32, 8), make([]int32, 8)

@@ -78,7 +78,7 @@ def test_cuda_device_hash_message_length_sweep(alloc, egpu):
 @pytest.mark.gpu
 def test_cuda_long_messages_block_count_sweep(alloc, egpu):
     """The one-CTA-per-message SHA-256 (few long sets): list lengths whose padded messages span one to
-    sixty-odd groups of 32 blocks (its schedule ring), group counts odd and even, and the B200
+    sixty-odd groups of 32 blocks (its schedule ring), group counts odd and even, and
     node-scale sizes; full 256-bit digests against hashlib."""
     import random
     from elastic_gpu_agent_b200 import devhash

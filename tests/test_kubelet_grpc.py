@@ -126,16 +126,20 @@ def serve_and_talk(tmp_path, handle, lib, oracle_c, resource=CORE):
     import grpc
     from elastic_gpu_agent_b200 import kubelet_plugin as kp
     T = kp.messages()
-    sock = f"unix://{tmp_path}/elastic-gpushare-core.sock"      # pkg/plugins/base.go:226
-    server = grpc.server(futures.ThreadPoolExecutor(max_workers=4))
-    kp.add_to_server(kp.BestFitDevicePlugin(handle, resource, lib), server)
-    server.add_insecure_port(sock)
-    server.start()
-    try:
-        with grpc.insecure_channel(sock) as ch:
-            conversation(kp.KubeletStub(ch), T, oracle_c, resource)
-    finally:
-        server.stop(0)
+    # a unix socket path holds at most 107 bytes and tmp_path can be longer: bind a path relative to
+    # tmp_path instead (both ends resolve it against the working directory while the test runs)
+    sock = "unix:elastic-gpushare-core.sock"                    # pkg/plugins/base.go:226
+    with pytest.MonkeyPatch.context() as mp:
+        mp.chdir(tmp_path)
+        server = grpc.server(futures.ThreadPoolExecutor(max_workers=4))
+        kp.add_to_server(kp.BestFitDevicePlugin(handle, resource, lib), server)
+        server.add_insecure_port(sock)
+        server.start()
+        try:
+            with grpc.insecure_channel(sock) as ch:
+                conversation(kp.KubeletStub(ch), T, oracle_c, resource)
+        finally:
+            server.stop(0)
 
 
 def test_wire_format_matches_the_v1beta1_field_numbers():

@@ -61,9 +61,9 @@ def test_preferred_allocation_best_fit_and_must_include(alloc, egpu):
 
 
 @pytest.mark.gpu
-def test_preferred_allocation_memory_resource_at_b200_scale(alloc, egpu):
-    """gpu-memory advertises one ID per MiB (pkg/plugins/gpushare.go:159-168): a B200
-    contributes 183359 IDs.  Two GPUs, one half full."""
+def test_preferred_allocation_memory_resource_at_full_card_scale(alloc, egpu):
+    """gpu-memory advertises one ID per MiB (pkg/plugins/gpushare.go:159-168): a 180 GB card
+    contributes 183359 IDs (an H100 80GB 81559).  Two GPUs, one half full."""
     from elastic_gpu_agent_b200 import plugin
     available = ["%d-%02d" % (0, u) for u in range(100_000, 183_359)] + ["%d-%02d" % (1, u) for u in range(0, 183_359)]
     ids, gpu = plugin.preferred_allocation(alloc, available, [], 16_384, plugin.RESOURCE_MEM)

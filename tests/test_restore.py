@@ -140,7 +140,7 @@ def test_cuda_flat_form_random_vs_oracle(alloc):
 def test_cuda_restore_after_churn_equals_live_table(alloc, egpu, events, mem_cap):
     """cfg5-style churn through the sequential replay, then the persisted state of what is still
     placed is restored on a fresh table: it must equal the live table (the 'diff after churn' is
-    empty), at B200 scale (one gpu-memory ID per MiB)."""
+    empty), up to the scale of a 180 GB card (one gpu-memory ID per MiB)."""
     from elastic_gpu_agent_b200 import restore
     D = 8
     kind, a, b = egpu.synth.churn_events(5, events)
