@@ -120,6 +120,7 @@ def load() -> C.CDLL:
         "egpu_device_id_format": (C.c_int, [C.c_int32, C.c_int64, C.c_char_p, C.c_int64]),
         "egpu_device_id_parse": (C.c_int, [C.c_char_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
         "egpu_preferred_allocation": (C.c_int, [vp, vp, C.c_int64, vp, C.c_int64, C.c_int32, C.c_int, vp, C.POINTER(C.c_int32)]),
+        "egpu_preferred_allocation_batch": (C.c_int, [vp, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp, vp, vp, vp]),
         "egpu_table_restore_flat": (C.c_int, [vp, vp, vp, C.c_int64, vp, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int,
                                               vp, vp]),
         "egpu_table_restore": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64, vp, vp, C.c_int64, vp, vp, C.c_int32, C.c_int, vp, vp,

@@ -616,7 +616,9 @@ void* mapped_alias(const void* p) {
 
 extern "C" {
 
-int egpu_abi_version(void) { return 1004; }  // 1.4: + multi-batch launches, stateless query, start gate (additive)
+// 1.4: + multi-batch launches, stateless query, start gate (additive)
+// 1.5: + egpu_preferred_allocation_batch (additive)
+int egpu_abi_version(void) { return 1005; }
 
 const char* egpu_strerror(int code) {
     switch (code) {

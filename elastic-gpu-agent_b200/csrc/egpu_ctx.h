@@ -99,7 +99,7 @@ struct egpu_ctx {
     bool replay2_configured = false;
     bool sort_sets_configured = false;  // sort_sets_smem_kernel may use 128 KB of dynamic shared memory
     bool replay_general = false;      // EGPU_REPLAY_GENERAL=1: lane = device kernel even for D <= 8 (tests)
-    // grow-only device arena for multi-kernel host-buffer pipelines (egpu_devhash.cu)
+    // grow-only device arena for multi-kernel host-buffer pipelines (egpu_devhash.cu, egpu_prefalloc.cu)
     void* arena = nullptr;
     size_t arena_cap = 0;
     char last_err[256] = {0};
@@ -113,6 +113,19 @@ inline int cuda_fail(egpu_ctx* ctx, cudaError_t e, const char* what) {
 
 // egpu_alloc.cu: body of egpu_table_set for callers that already hold ctx->mu
 int egpu_table_set_locked(egpu_ctx* ctx, const int32_t* free_core, const int32_t* free_mem, int32_t D);
+
+namespace egpu {
+// egpu_devhash.cu: the identity pipeline's stable LSD radix sort and exclusive scan, for the other
+// pipelines.  Both return the number of kernels they launched on s.
+// words of the sort's histogram for n keys
+size_t radix_hist_words(long long n);
+// sorts (key, val) pairs of n < 2^31 elements by the low n_digits 4-bit digits of key, stably; the
+// sorted pairs end in key / val (the pointers are swapped with the scratch pair after every pass)
+int radix_sort_pairs(cudaStream_t s, unsigned long long*& key, uint32_t*& val, unsigned long long*& key_tmp,
+                     uint32_t*& val_tmp, long long n, int n_digits, uint32_t* hist);
+// out[0..n] = exclusive prefix sums of v[0..n); blk holds (n + 1023) / 1024 + 1 words
+int exclusive_scan_u32(cudaStream_t s, const uint32_t* v, long long n, unsigned long long* blk, unsigned long long* out);
+}  // namespace egpu
 
 #define EGPU_CUDA(ctx, call)                                   \
     do {                                                       \

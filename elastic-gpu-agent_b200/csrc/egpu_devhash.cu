@@ -560,6 +560,35 @@ __global__ void locate_init_kernel(int* __restrict__ equal, const long long* __r
     equal[s] = (s > 0 && (set_off[s + 1] - set_off[s]) == (set_off[1] - set_off[0])) ? 1 : 0;
 }
 
+// ---- the sort and the scan for other pipelines of the library (egpu_prefalloc.cu) -------
+size_t radix_hist_words(long long n) {
+    const long long tiles = (n + kSortTile - 1) / kSortTile;
+    return 16 * static_cast<size_t>(tiles > 0 ? tiles : 1);
+}
+
+int radix_sort_pairs(cudaStream_t s, unsigned long long*& key, uint32_t*& val, unsigned long long*& key_tmp,
+                     uint32_t*& val_tmp, long long n, int n_digits, uint32_t* hist) {
+    if (n <= 0) return 0;
+    const unsigned tiles = static_cast<unsigned>((n + kSortTile - 1) / kSortTile);
+    for (int j = 0; j < n_digits; ++j) {
+        radix_hist_kernel<<<tiles, kSortThreads, 0, s>>>(key, val, n, 4 * j, hist);
+        radix_scan_kernel<<<1, 1024, 0, s>>>(hist, static_cast<int>(16 * tiles));
+        radix_scatter_kernel<<<tiles, kSortThreads, 0, s>>>(key, val, n, 4 * j, hist, key_tmp, val_tmp);
+        std::swap(key, key_tmp);
+        std::swap(val, val_tmp);
+    }
+    return 3 * n_digits;
+}
+
+int exclusive_scan_u32(cudaStream_t s, const uint32_t* v, long long n, unsigned long long* blk, unsigned long long* out) {
+    if (n <= 0) return 0;
+    const unsigned nblk = static_cast<unsigned>((n + 1023) / 1024);
+    scan_block_sums_kernel<<<nblk, 1024, 0, s>>>(v, n, blk);
+    scan_blocks_kernel<<<1, 1024, 0, s>>>(blk, nblk);
+    scan_apply_kernel<<<nblk, 1024, 0, s>>>(v, n, blk, out);
+    return 3;
+}
+
 }  // namespace egpu
 
 using namespace egpu;

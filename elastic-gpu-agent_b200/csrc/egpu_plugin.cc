@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/egpu_plugin.h"
+#include "egpu_id_grammar.h"
 
 extern "C" {
 
@@ -23,31 +24,8 @@ int egpu_device_id_format(int32_t gpu, int64_t unit, char* out, int64_t cap) {
 
 int egpu_device_id_parse(const char* id, int32_t* gpu, int64_t* unit) {
     if (!id || !gpu || !unit) return EGPU_ERR_INVALID;
-    const char* p = id;
-    if (*p < '0' || *p > '9') return EGPU_ERR_PARSE;
-    int64_t g = 0;
-    int digits = 0;
-    while (*p >= '0' && *p <= '9') {
-        g = g * 10 + (*p - '0');
-        if (++digits > 9) return EGPU_ERR_PARSE;
-        ++p;
-    }
-    if (digits > 1 && id[0] == '0') return EGPU_ERR_PARSE;  // %d never pads the GPU index
-    if (*p != '-') return EGPU_ERR_PARSE;
-    ++p;
-    const char* u0 = p;
-    int64_t u = 0;
-    digits = 0;
-    while (*p >= '0' && *p <= '9') {
-        u = u * 10 + (*p - '0');
-        if (++digits > 15) return EGPU_ERR_PARSE;
-        ++p;
-    }
-    if (*p != '\0' || digits < 2) return EGPU_ERR_PARSE;       // %02d: at least two digits
-    if (digits > 2 && u0[0] == '0') return EGPU_ERR_PARSE;     // padding only up to two digits
-    *gpu = static_cast<int32_t>(g);
-    *unit = u;
-    return EGPU_OK;
+    // the grammar is shared with the device pipeline of egpu_preferred_allocation_batch
+    return egpu_id_grammar(id, -1, gpu, unit) == 0 ? EGPU_OK : EGPU_ERR_PARSE;
 }
 
 int egpu_preferred_allocation(egpu_ctx* ctx, const char* const* available_ids, int64_t n_available,

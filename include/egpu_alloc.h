@@ -140,8 +140,8 @@ int64_t egpu_launch_count(egpu_ctx* ctx);
 int  egpu_set_variant(egpu_ctx* ctx, int variant);
 /* ABI version: major*1000 + minor.  Minor revisions only add entry points (1.1 placement
  * restore, 1.2 prefix-commit over row shards, 1.3 rounds, 1.4 multi-batch launches, stateless query,
- * start gate, host registration); a caller built against 1.0 keeps
- * working. */
+ * start gate, host registration, 1.5 preferred allocation for many container requests from flat ID
+ * buffers); a caller built against 1.0 keeps working. */
 int  egpu_abi_version(void);
 
 /* ---- capacity table --------------------------------------------------- */

@@ -15,6 +15,10 @@
  * The choice itself is made by the CUDA best-fit scan (egpu_bestfit_query); this file
  * only turns ID strings into the capacity table and the answer back into IDs.  No CPU
  * fallback: without a context (no GPU) the call fails.
+ *
+ * egpu_preferred_allocation_batch answers every container request of a PreferredAllocationRequest
+ * in one call from flat ID buffers; parsing, counting, must-include matching, the best-fit choice
+ * and the ID selection all run on the GPU, with the answers of egpu_preferred_allocation.
  */
 #ifndef EGPU_PLUGIN_H
 #define EGPU_PLUGIN_H
@@ -61,6 +65,46 @@ int egpu_preferred_allocation(egpu_ctx* ctx, const char* const* available_ids, i
                               const char* const* must_include_ids, int64_t n_must,
                               int32_t allocation_size, int resource, int32_t* out_positions,
                               int32_t* out_gpu);
+
+#define EGPU_PREFALLOC_MAX_REQUESTS 65536  /* container requests per egpu_preferred_allocation_batch call */
+
+/* Every ContainerPreferredAllocationRequest of one PreferredAllocationRequest (or of several) in one
+ * call, with all ID work on the GPU.
+ * IDs: the layout of egpu_device_hash_batch - ids_flat, id_offsets[n_ids + 1] (int64 byte offsets,
+ * id_offsets[0] == 0, no separators, no NULs; the buffer is id_offsets[n_ids] bytes long) and
+ * set_offsets[2 * n_req + 1] (id indices).  Set 2q holds request q's available IDs, in the message's
+ * order; set 2q + 1 holds its must-include IDs.  allocation_size[n_req].
+ * Outputs:
+ *   out_positions  request q's answer starts at sum_{q' < q} max(allocation_size[q'], 0); entries are
+ *                  indices into request q's own available list (0-based), as egpu_preferred_allocation
+ *                  returns them; -1 in every slot of a request whose code is not EGPU_OK
+ *   out_gpu[n_req] first chosen GPU, -1 when the code is not EGPU_OK (may be NULL)
+ *   out_rc[n_req]  exactly what egpu_preferred_allocation returns for that request alone:
+ *                  EGPU_OK, EGPU_ERR_UNSAT, EGPU_ERR_PARSE or EGPU_ERR_INVALID
+ * Per request, the first rule that applies decides the code (the order egpu_preferred_allocation
+ * checks them in):
+ *   1. allocation_size < 0: INVALID
+ *   2. more must-include IDs than allocation_size: UNSAT, before any ID is parsed
+ *   3. the first bad available ID in list order: malformed (including offsets that decrease or leave
+ *      the buffer) PARSE, GPU index >= EGPU_MAX_DEVICES INVALID
+ *   4. no available IDs: OK when allocation_size is 0, else UNSAT
+ *   5. a whole-card size (gpu-core, > 100) that is not a multiple of 100: UNSAT
+ *   6. must-include IDs in order, the first failure: malformed PARSE; not among the available IDs
+ *      UNSAT; more pinned GPUs than the request takes UNSAT
+ *   7. no feasible GPU at some pick: UNSAT
+ *   8. fewer IDs to give than asked for: UNSAT
+ * Duplicate IDs count as often as they are listed (capped at a card's units); a must-include ID is
+ * the first position of its string and is given once however often it is listed.
+ * Return: EGPU_OK when out_rc is valid; EGPU_ERR_INVALID for call-level argument errors (NULL ctx, NULL
+ * pointers with non-zero counts, bad resource, n_ids >= 2^31, n_req > EGPU_PREFALLOC_MAX_REQUESTS,
+ * a negative buffer length, set offsets that do not start at 0, are not monotone or do not end at
+ * n_ids); EGPU_ERR_NOMEM / EGPU_ERR_CUDA as elsewhere.  The context's own table is neither read nor
+ * written.  The number of kernel launches does not depend on n_req. */
+int egpu_preferred_allocation_batch(egpu_ctx* ctx, int resource,
+                                    const char* ids_flat, const int64_t* id_offsets, int64_t n_ids,
+                                    const int64_t* set_offsets, int64_t n_req,
+                                    const int32_t* allocation_size,
+                                    int32_t* out_positions, int32_t* out_gpu, int32_t* out_rc);
 
 #ifdef __cplusplus
 }
