@@ -15,6 +15,7 @@
 #include <cstdlib>
 #include <algorithm>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <new>
 #include <vector>
@@ -35,26 +36,104 @@ namespace {
 
 constexpr int64_t kMaxRows = (1ll << 31) - 1;  // EGPU_MAX_ROWS
 
-template <int DT, int THREADS>
-SnapLaunch make_launch(bool grid_variant) {
-    SnapLaunch l;
-    l.fn = grid_variant ? bestfit_grid_kernel<DT, THREADS> : bestfit_sorted_kernel<DT, THREADS>;
-    l.threads = THREADS;
-    l.smem = sizeof(SnapSmem<DT, THREADS>);
-    l.ctas_per_sm = 0;
-    return l;
+int d_bucket(int D) { return D <= 8 ? 0 : D <= 16 ? 1 : D <= 32 ? 2 : 3; }
+
+// ---- kernel table: one kernel per scan family and D bucket ----
+template <class Fn>
+struct Kernel {
+    Fn fn;
+    int threads;
+    size_t smem;  // dynamic shared memory
+};
+template <class Fn>
+constexpr Kernel<Fn> kernel(Fn fn, int threads, size_t smem) { return {fn, threads, smem}; }
+
+// The register scans run 256 threads up to D = 32 and 128 at D = 64; the lookup scan is one
+// kernel for every D.
+template <int F, int B>
+constexpr auto family_kernel() {
+    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
+    constexpr size_t snap = sizeof(SnapSmem<DT, T>), lut = sizeof(LutSmem<256>);
+    if constexpr (F == kScanSorted) return kernel(bestfit_sorted_kernel<DT, T, false>, T, snap);
+    else if constexpr (F == kScanSortedContig) return kernel(bestfit_sorted_kernel<DT, T, true>, T, snap);
+    else if constexpr (F == kScanGrid) return kernel(bestfit_grid_kernel<DT, T>, T, snap);
+    else if constexpr (F == kScanLut) return kernel(bestfit_lut_kernel<256, false>, 256, lut);
+    else if constexpr (F == kScanLutContig) return kernel(bestfit_lut_kernel<256, true>, 256, lut);
+    else if constexpr (F == kScanSortedMulti) return kernel(bestfit_sorted_multi_kernel<DT, T>, T, snap);
+    else if constexpr (F == kScanLutMulti) return kernel(bestfit_lut_multi_kernel<256>, 256, lut);
+    else return kernel(bestfit_sorted_packed_kernel<DT, T>, T, snap);
+}
+template <int F>
+constexpr decltype(family_kernel<F, 0>()) kKernels[4] = {family_kernel<F, 0>(), family_kernel<F, 1>(), family_kernel<F, 2>(),
+                                                         family_kernel<F, 3>()};
+
+// Resident CTAs per SM of family F's kernel for D devices.  The first use on a context opts in to
+// the kernel's dynamic shared memory and asks the occupancy.
+template <int F>
+int resident_ctas(egpu_ctx* ctx, int D, int* per_sm) {
+    const auto& k = kKernels<F>[d_bucket(D)];
+    int& n = ctx->scan_ctas_per_sm[F][d_bucket(D)];
+    if (n == 0) {
+        EGPU_CUDA(ctx, cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(k.smem)));
+        int m = 0;
+        EGPU_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m, k.fn, k.threads, k.smem));
+        n = m < 1 ? 1 : m;
+    }
+    *per_sm = n;
+    return EGPU_OK;
 }
 
-SnapLaunch pick_launch(int D, bool grid_variant) {
-    if (D <= 8) return make_launch<8, 256>(grid_variant);
-    if (D <= 16) return make_launch<16, 256>(grid_variant);
-    if (D <= 32) return make_launch<32, 256>(grid_variant);
-    return make_launch<64, 128>(grid_variant);
+// Programmatic dependent launch: the kernel may be scheduled while its predecessor on the stream
+// still runs; each scan orders itself with griddepcontrol.wait (see order_scan).
+template <class Fn, class... A>
+int launch_pdl(egpu_ctx* ctx, const Kernel<Fn>& k, int64_t grid, cudaStream_t s, const A&... args) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.blockDim = dim3(static_cast<unsigned>(k.threads));
+    cfg.dynamicSmemBytes = k.smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, k.fn, args...));
+    return EGPU_OK;
 }
 
-// host copy of resort_table_cta: sorted view of a freshly set table
-void fill_sorted(DevState& h) {
-    const int D = h.D;
+// blocks of a grid-stride kernel over n items, per_block items a block: at most 8 per SM
+unsigned capped_blocks(const egpu_ctx* ctx, int64_t n, int64_t per_block) {
+    int64_t blocks = (n + per_block - 1) / per_block;
+    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * 8;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    return static_cast<unsigned>(blocks);
+}
+
+bool lut_variant(const egpu_ctx* ctx) {
+    return ctx->variant == EGPU_VARIANT_LUT || (ctx->variant == EGPU_VARIANT_AUTO && ctx->D > 16);
+}
+
+// the lookup scans read ctx->d_lut: rebuild it on the launching stream after the table changed
+int refresh_lut(egpu_ctx* ctx, cudaStream_t s) {
+    if (!ctx->lut_dirty) return EGPU_OK;
+    lut_build_kernel<<<1, 256, 0, s>>>(ctx->d_state, ctx->d_lut);
+    EGPU_CUDA(ctx, cudaGetLastError());
+    ctx->launches += 1;
+    ctx->lut_dirty = false;
+    ctx->prev_is_scan = false;
+    return EGPU_OK;
+}
+
+// Host image of a table: the part of DevState before `peer` (free capacity, D, candidate masks and
+// the sorted view that resort_table_cta keeps on the device)
+void table_image(DevState& h, const int32_t* free_core, const int32_t* free_mem, int D) {
+    std::memset(&h, 0, offsetof(DevState, peer));
+    std::memcpy(h.free_core, free_core, sizeof(int32_t) * D);
+    std::memcpy(h.free_mem, free_mem, sizeof(int32_t) * D);
+    h.D = D;
+    h.cand_xor = kGuards;
+    h.cand_mask = kCandMask;
     for (int j = 0; j < kMaxD; ++j) {
         h.sorted_k[j] = kPadWord;
         h.sorted_dev[j] = -1;
@@ -75,19 +154,28 @@ void fill_sorted(DevState& h) {
 }
 
 // ---- output ranges of the launches in flight (pipelined launches must not share outputs) ----
+using Range = egpu_ctx::Range;
+// the outputs of one batch: indices, demand sums, table'
+void batch_ranges(Range* r, const int32_t* idx, int64_t R, const void* delta, const int32_t* table_out, int D) {
+    const uintptr_t pi = reinterpret_cast<uintptr_t>(idx), pd = reinterpret_cast<uintptr_t>(delta),
+                    pt = reinterpret_cast<uintptr_t>(table_out);
+    r[0] = {pi, pi + static_cast<uintptr_t>(R) * sizeof(int32_t)};
+    r[1] = {pd, pd + (pd ? sizeof(long long) * 2 * D : 0)};
+    r[2] = {pt, pt + (pt ? sizeof(int32_t) * 3 * D : 0)};
+}
 // `r[0..n)`: drops empty ranges, sorts by address; returns the new count, or -1 when two of
 // them overlap each other.
-int prepare_ranges(egpu_ctx::Range* r, int n) {
+int prepare_ranges(Range* r, int n) {
     int m = 0;
     for (int i = 0; i < n; ++i)
         if (r[i].hi > r[i].lo) r[m++] = r[i];
-    std::sort(r, r + m, [](const egpu_ctx::Range& a, const egpu_ctx::Range& b) { return a.lo < b.lo; });
+    std::sort(r, r + m, [](const Range& a, const Range& b) { return a.lo < b.lo; });
     for (int i = 1; i < m; ++i)
         if (r[i].lo < r[i - 1].hi) return -1;
     return m;
 }
 // both sorted and internally disjoint: one sweep
-bool overlaps_inflight(const std::vector<egpu_ctx::Range>& f, const egpu_ctx::Range* r, int n) {
+bool overlaps_inflight(const std::vector<Range>& f, const Range* r, int n) {
     size_t i = 0;
     int k = 0;
     while (i < f.size() && k < n) {
@@ -97,95 +185,38 @@ bool overlaps_inflight(const std::vector<egpu_ctx::Range>& f, const egpu_ctx::Ra
     }
     return false;
 }
-void add_inflight(egpu_ctx* ctx, const egpu_ctx::Range* r, int n) {
-    ctx->range_tmp.resize(ctx->inflight.size() + static_cast<size_t>(n));
-    std::merge(ctx->inflight.begin(), ctx->inflight.end(), r, r + n, ctx->range_tmp.begin(),
-               [](const egpu_ctx::Range& a, const egpu_ctx::Range& b) { return a.lo < b.lo; });
-    ctx->inflight.swap(ctx->range_tmp);
-}
 void new_group(egpu_ctx* ctx) {
     ctx->group_len = 0;
     ctx->group_mbatches = 0;
     ctx->inflight.clear();
 }
 
-// first use of a kernel on this context: opt in to its shared-memory size, ask occupancy
-int configure_launch(egpu_ctx* ctx, SnapLaunch& l, int D, bool grid_variant, bool lut_variant, bool contig) {
-    if (l.ctas_per_sm != 0) return EGPU_OK;
-    const int bucket = D <= 8 ? 0 : D <= 16 ? 1 : D <= 32 ? 2 : 3;
-    int per_sm = 0;
-    if (lut_variant) {
-        l.threads = 256;
-        l.lut_fn = contig ? bestfit_lut_kernel<256, true> : bestfit_lut_kernel<256, false>;
-        l.smem = sizeof(LutSmem<256>);
-        EGPU_CUDA(ctx, cudaFuncSetAttribute(l.lut_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(l.smem)));
-        EGPU_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l.lut_fn, l.threads, l.smem));
-    } else {
-        l = pick_launch(D, grid_variant);
-        if (!grid_variant && !contig && bucket == 0 && ctx->threads8 != 256)  // experiment knob: CTA size of the D <= 8 scan
-            l = ctx->threads8 == 128 ? make_launch<8, 128>(false) : make_launch<8, 512>(false);
-        if (contig) {
-            l.fn = bucket == 0 ? bestfit_sorted_kernel<8, 256, true> : bucket == 1 ? bestfit_sorted_kernel<16, 256, true>
-                   : bucket == 2 ? bestfit_sorted_kernel<32, 256, true> : bestfit_sorted_kernel<64, 128, true>;
-        }
-        EGPU_CUDA(ctx, cudaFuncSetAttribute(l.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(l.smem)));
-        EGPU_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l.fn, l.threads, l.smem));
-    }
-    l.ctas_per_sm = per_sm < 1 ? 1 : per_sm;
-    return EGPU_OK;
-}
-
-// user_flags: EGPU_F_COMMIT | EGPU_F_INPUTS_READY.  finalize = 0 only for the
-// chunked host pipeline (accumulate demand sums across launches).
-int launch_snapshot(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx,
-                    long long* d_delta, int32_t* d_table_out, int user_flags, bool finalize, cudaStream_t s,
-                    int rpt_hint = 0, unsigned long long push_step_plus1 = 0, bool contig = false, int* n_tiles_out = nullptr,
-                    int lag = 0) {
-    if (R > kMaxRows) return EGPU_ERR_INVALID;  // the scans index 128-bit vectors with 32 bits
-    const bool grid_variant = ctx->variant == EGPU_VARIANT_GRID;
-    const bool lut_variant = ctx->variant == EGPU_VARIANT_LUT || (ctx->variant == EGPU_VARIANT_AUTO && ctx->D > 16);
-    const int bucket = ctx->D <= 8 ? 0 : ctx->D <= 16 ? 1 : ctx->D <= 32 ? 2 : 3;
-    if (contig && grid_variant) return EGPU_ERR_STATE;  // the literal variant has no prefix-commit mode
-    SnapLaunch& l = ctx->snap[contig ? (lut_variant ? 4 : 3) : grid_variant ? 1 : (lut_variant ? 2 : 0)][bucket];
-    {
-        const int rc = configure_launch(ctx, l, ctx->D, grid_variant, lut_variant, contig);
-        if (rc != EGPU_OK) return rc;
-    }
-    if (lut_variant && ctx->lut_dirty) {  // refresh the lookup tables on the launching stream
-        lut_build_kernel<<<1, 256, 0, s>>>(ctx->d_state, ctx->d_lut);
-        EGPU_CUDA(ctx, cudaGetLastError());
-        ctx->launches += 1;
-        ctx->lut_dirty = false;
-        ctx->prev_is_scan = false;
-    }
-    int flags = (finalize ? kFlagFinalize : 0) | ((user_flags & EGPU_F_COMMIT) ? kFlagCommit : 0);
-    // Programmatic dependent launch.  Every scan carries the PDL attribute, so the
-    // hardware may schedule it while its predecessor is still running.  A fully
-    // ordered launch waits (griddepcontrol.wait) before it touches anything.  A
-    // pipelined launch (kFlagLateWait) runs scan and epilogue at once — its epilogue
-    // state is its own slot — and waits only before exiting.  That is allowed when
-    //  - the caller vouches its inputs were complete before the previous launch on
-    //    this stream (EGPU_F_INPUTS_READY),
-    //  - the previous launch was a scan of this context on the same stream that
-    //    does not rewrite the table, and this one is a plain finalising scan,
-    //  - it does not commit (a committing launch rewrites the table the launches still in
-    //    flight read and compute their table' from: it is always fully ordered),
-    //  - its outputs (indices, demand sums, table') are disjoint from the outputs
-    //    of every launch since the last fully ordered one, and
-    //  - fewer than pipe_group launches have been issued since then, which bounds
-    //    the launches in flight to pipe_group + 1 < kEpiSlots.
-    egpu_ctx::Range mine[3] = {
-        {reinterpret_cast<uintptr_t>(d_idx), reinterpret_cast<uintptr_t>(d_idx) + static_cast<uintptr_t>(R) * sizeof(int32_t)},
-        {reinterpret_cast<uintptr_t>(d_delta), reinterpret_cast<uintptr_t>(d_delta) + (d_delta ? sizeof(long long) * 2 * ctx->D : 0)},
-        {reinterpret_cast<uintptr_t>(d_table_out), reinterpret_cast<uintptr_t>(d_table_out) + (d_table_out ? sizeof(int32_t) * 3 * ctx->D : 0)}};
-    const int n_mine = prepare_ranges(mine, 3);
-    if (n_mine < 0) return EGPU_ERR_INVALID;  // two of this launch's own outputs overlap
-    bool pipelined = !grid_variant && !contig && finalize && (user_flags & EGPU_F_INPUTS_READY) && !(user_flags & EGPU_F_COMMIT) &&
-                     ctx->prev_is_scan && !ctx->prev_changes_table && ctx->prev_stream == s && ctx->group_len > 0 &&
-                     !overlaps_inflight(ctx->inflight, mine, n_mine);
+// Ordering of a scan behind the launches before it (programmatic dependent launch); returns its
+// kFlagLateWait | kFlagBoundary | kFlagEarlyTrigger bits.  Every scan carries the PDL attribute,
+// so the hardware may schedule it while its predecessor is still running.  A fully ordered launch
+// waits (griddepcontrol.wait) before it touches anything.  A pipelined launch (kFlagLateWait) runs
+// scan and epilogue at once - its epilogue state is its own slot - and waits only before exiting.
+// That is allowed when
+//  - the caller vouches its inputs were complete before the previous launch on this stream
+//    (EGPU_F_INPUTS_READY), and `eligible` holds: the launch's own conditions (a single-batch
+//    launch must not commit - a committing launch rewrites the table the launches still in flight
+//    read and compute their table' from - and must be a plain scan, neither CONTIG nor the grid
+//    variant),
+//  - the previous launch was a scan of this context on the same stream that does not rewrite
+//    the table,
+//  - its outputs (indices, demand sums, table') are disjoint from the outputs of every launch
+//    since the last fully ordered one, and
+//  - fewer than pipe_group launches have been issued since then, which bounds the launches in
+//    flight to pipe_group + 1 < kEpiSlots, and the epi_multi slots of those launches and this
+//    one's `batches` (0 for a single-batch launch) stay within half of that ring.
+// Otherwise the launch is fully ordered and opens a new group.
+int order_scan(egpu_ctx* ctx, int user_flags, bool eligible, int batches, cudaStream_t s, const Range* mine, int n_mine) {
+    int flags = 0;
+    const bool pipelined = (user_flags & EGPU_F_INPUTS_READY) && eligible && ctx->prev_is_scan && !ctx->prev_changes_table &&
+                           ctx->prev_stream == s && ctx->group_len > 0 && !overlaps_inflight(ctx->inflight, mine, n_mine);
     if (pipelined) {
         flags |= kFlagLateWait;
-        if (ctx->group_len >= ctx->pipe_group) {
+        if (ctx->group_len >= ctx->pipe_group || ctx->group_mbatches + batches > kMultiSlots - kMultiMax) {
             // group boundary: this launch still scans alongside its predecessors, but it waits
             // for them before its epilogue and only then lets its successors start; it becomes
             // the first member of the next group
@@ -200,148 +231,154 @@ int launch_snapshot(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int
     // (What scripts/probes/pdl_event_probe.cu and scripts/eager_probe.py check: events
     // and ordinary kernels enqueued after a PDL launch still wait for its completion.)
     if (user_flags & EGPU_F_INPUTS_READY) flags |= kFlagEarlyTrigger;
-    const unsigned long long slot = (finalize ? (ctx->seq % kEpiSlots) : static_cast<unsigned long long>(kEpiSlots)) |
-                                    (push_step_plus1 << 8) | (static_cast<unsigned long long>(lag) << 56);
+    return flags;
+}
+
+// Bookkeeping of a scan launched under order_scan: `batches` = 0 for a single-batch launch (one
+// epilogue slot of the seq ring), K for a multi-batch one (K slots of the mseq ring).
+void record_scan(egpu_ctx* ctx, cudaStream_t s, const Range* mine, int n_mine, int batches, bool changes_table) {
+    ctx->launches += 1;
+    if (batches) ctx->mseq += static_cast<uint64_t>(batches);
+    else ctx->seq += 1;
+    ctx->range_tmp.resize(ctx->inflight.size() + static_cast<size_t>(n_mine));
+    std::merge(ctx->inflight.begin(), ctx->inflight.end(), mine, mine + n_mine, ctx->range_tmp.begin(),
+               [](const Range& a, const Range& b) { return a.lo < b.lo; });
+    ctx->inflight.swap(ctx->range_tmp);
+    ctx->group_len += 1;
+    ctx->group_mbatches += batches;
+    ctx->prev_is_scan = true;
+    ctx->prev_changes_table = changes_table;
+    ctx->prev_stream = s;
+}
+
+// ---- single-batch scans ----
+struct Snapshot {
+    const int32_t* rc;
+    const int32_t* rm;
+    int64_t R;
+    int32_t* idx;
+    long long* delta = nullptr;
+    int32_t* table_out = nullptr;
+    int user_flags = 0;                          // EGPU_F_COMMIT | EGPU_F_INPUTS_READY
+    int rpt_hint = 0;                            // rows per thread, 0 = the default rule below
+    unsigned long long push_step_plus1 = 0;      // exchange step + 1 the epilogue pushes the demand to, 0 = none
+    int lag = 0;                                 // lagged apply (egpu_bestfit_batch_shard_lag_dev)
+    bool contig = false;                         // prefix-commit: contiguous tiles, per-tile sums in ctx->d_tile_sums
+};
+
+template <int F>
+int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_tiles_out) {
+    constexpr bool lut = F == kScanLut || F == kScanLutContig, grid_variant = F == kScanGrid;
+    const auto& k = kKernels<F>[d_bucket(ctx->D)];
+    int per_sm = 0;
+    int rc = resident_ctas<F>(ctx, ctx->D, &per_sm);
+    if (rc != EGPU_OK) return rc;
+    if (lut) {
+        rc = refresh_lut(ctx, s);
+        if (rc != EGPU_OK) return rc;
+    }
+    Range mine[3];
+    batch_ranges(mine, a.idx, a.R, a.delta, a.table_out, ctx->D);
+    const int n_mine = prepare_ranges(mine, 3);
+    if (n_mine < 0) return EGPU_ERR_INVALID;  // two of this launch's own outputs overlap
+    const bool commit = (a.user_flags & EGPU_F_COMMIT) != 0;
+    const int flags = kFlagFinalize | (commit ? kFlagCommit : 0) |
+                      order_scan(ctx, a.user_flags, !grid_variant && !a.contig && !commit, 0, s, mine, n_mine);
+    const unsigned long long slot = (ctx->seq % kEpiSlots) | (a.push_step_plus1 << 8) | (static_cast<unsigned long long>(a.lag) << 56);
 
     // Grid: one resident wave at most.  A lone launch wants every SM pulling at once
     // (8 rows per thread, one trip); launches of a pipelined stream overlap each
     // other, so a smaller grid with more rows per thread (48) costs fewer CTA
     // launches, fewer atomics and leaves room for the neighbours (scripts/tune_sweep.sh
     // re-measures the choice at R = 1M).  The zero-copy path passes its own hint (see egpu_bestfit_batch).
-    const int64_t nvec = R >> 2;
+    const int64_t nvec = a.R >> 2;
     int rpt = 8;
     // (measured and dropped: giving the launches of a pipelined stream that could not themselves be
     // pipelined - the first of a graph - the lone-launch grid: slower per step)
-    if (user_flags & EGPU_F_INPUTS_READY) rpt = (lut_variant || ctx->D <= 16) ? 48 : 8;  // measured, scripts/tune_*.sh
-    else if (lut_variant) rpt = 32;  // the lookup scan has a 13 KB per-CTA table tile to amortise
-    if (rpt_hint > 0) rpt = rpt_hint;
+    if (a.user_flags & EGPU_F_INPUTS_READY) rpt = (lut || ctx->D <= 16) ? 48 : 8;  // measured, scripts/tune_*.sh
+    else if (lut) rpt = 32;  // the lookup scan has a 13 KB per-CTA table tile to amortise
+    if (a.rpt_hint > 0) rpt = a.rpt_hint;
     if (ctx->rows_per_thread > 0) rpt = ctx->rows_per_thread;
     if (grid_variant) rpt = 4;
-    const int64_t per_cta = static_cast<int64_t>(l.threads) * ((rpt + 3) / 4);
+    const int64_t per_cta = static_cast<int64_t>(k.threads) * ((rpt + 3) / 4);
     int64_t want = (nvec + per_cta - 1) / per_cta;
-    int per_sm = l.ctas_per_sm;
     if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
     // one resident wave; two for a huge batch (the CTA scheduler then evens out the SMs, see launch_multi)
-    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * per_sm * ((R >= (16ll << 20) && !contig) ? 2 : 1);
+    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * per_sm * ((a.R >= (16ll << 20) && !a.contig) ? 2 : 1);
     if (want > cap) want = cap;
     if (want < 1) want = 1;
     // lane-private sums hold 2^19 rows per lane (kAccShift): keep rows/thread below that
-    const int64_t rows_per_thread = R / (want * l.threads) + 8;
+    const int64_t rows_per_thread = a.R / (want * k.threads) + 8;
     if (rows_per_thread >= (1ll << 19)) return EGPU_ERR_INVALID;
 
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(want));
-    cfg.blockDim = dim3(static_cast<unsigned>(l.threads));
-    cfg.dynamicSmemBytes = l.smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     unsigned long long* tile_sums = nullptr;
-    if (contig) {  // one tile per CTA: make room for their sums
-        if (want > ctx->tile_cap) {
-            cudaFree(ctx->d_tile_sums);
-            ctx->d_tile_sums = nullptr;
-            ctx->tile_cap = 0;
-            EGPU_CUDA(ctx, cudaMalloc(&ctx->d_tile_sums, sizeof(unsigned long long) * 2 * kMaxD * static_cast<size_t>(want)));
-            ctx->tile_cap = want;
-        }
+    if (a.contig) {  // one tile per CTA: make room for their sums
+        const size_t bytes = sizeof(unsigned long long) * 2 * kMaxD * static_cast<size_t>(want);
+        EGPU_CUDA(ctx, grow(ctx->tile_bytes, bytes, bytes, &ctx->d_tile_sums));
         tile_sums = ctx->d_tile_sums;
-        if (n_tiles_out) *n_tiles_out = static_cast<int>(want);
+        *n_tiles_out = static_cast<int>(want);
     }
-    if (lut_variant)
-        EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, l.lut_fn, ctx->d_state, d_rc, d_rm, static_cast<long long>(R), d_idx,
-                                          d_delta, d_table_out, flags, slot, static_cast<const DevLut*>(ctx->d_lut), tile_sums));
+    if constexpr (lut)
+        rc = launch_pdl(ctx, k, want, s, ctx->d_state, a.rc, a.rm, static_cast<long long>(a.R), a.idx, a.delta, a.table_out, flags,
+                        slot, static_cast<const DevLut*>(ctx->d_lut), tile_sums);
     else
-        EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, l.fn, ctx->d_state, d_rc, d_rm, static_cast<long long>(R), d_idx,
-                                          d_delta, d_table_out, flags, slot, tile_sums));
-    if (flags & kFlagCommit) ctx->lut_dirty = true;
-    ctx->launches += 1;
-    ctx->seq += 1;
-    add_inflight(ctx, mine, n_mine);
-    ctx->group_len += 1;
-    ctx->prev_is_scan = finalize;
-    ctx->prev_changes_table = (flags & kFlagCommit) != 0;
-    ctx->prev_stream = s;
+        rc = launch_pdl(ctx, k, want, s, ctx->d_state, a.rc, a.rm, static_cast<long long>(a.R), a.idx, a.delta, a.table_out, flags,
+                        slot, tile_sums);
+    if (rc != EGPU_OK) return rc;
+    if (commit) ctx->lut_dirty = true;
+    record_scan(ctx, s, mine, n_mine, 0, commit);
     return EGPU_OK;
+}
+
+// One scan of one batch against the context's table, in the kernel the context's variant picks.
+// A CONTIG scan reports its tile count in *n_tiles_out.
+int launch_snapshot(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_tiles_out = nullptr) {
+    if (a.R > kMaxRows) return EGPU_ERR_INVALID;  // the scans index 128-bit vectors with 32 bits
+    const bool grid_variant = ctx->variant == EGPU_VARIANT_GRID;
+    if (a.contig && grid_variant) return EGPU_ERR_STATE;  // the literal variant has no prefix-commit mode
+    if (lut_variant(ctx))
+        return a.contig ? launch_snapshot_as<kScanLutContig>(ctx, a, s, n_tiles_out) : launch_snapshot_as<kScanLut>(ctx, a, s, n_tiles_out);
+    if (grid_variant) return launch_snapshot_as<kScanGrid>(ctx, a, s, n_tiles_out);
+    return a.contig ? launch_snapshot_as<kScanSortedContig>(ctx, a, s, n_tiles_out) : launch_snapshot_as<kScanSorted>(ctx, a, s, n_tiles_out);
 }
 
 // Multi-batch launch: K batches, all scored against the current table, one grid (CTA (b, t) =
 // tile t of batch b), one epilogue slot per batch.  Pipelines behind its predecessor under the
-// same conditions as launch_snapshot; a launch group never holds more than half of the
-// epi_multi ring, so the slots of everything that can be in flight are distinct.
+// conditions of order_scan; a launch group never holds more than half of the epi_multi ring,
+// so the slots of everything that can be in flight are distinct.
 // push_base = first exchange step + 1 when every batch also pushes its demand vector to the peers.
-int launch_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cudaStream_t s, unsigned long long push_base) {
-    if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // the literal variant has no multi-batch form
-    const bool lut_variant = ctx->variant == EGPU_VARIANT_LUT || (ctx->variant == EGPU_VARIANT_AUTO && ctx->D > 16);
-    const int bucket = ctx->D <= 8 ? 0 : ctx->D <= 16 ? 1 : ctx->D <= 32 ? 2 : 3;
-    MultiLaunch& l = ctx->multi[lut_variant ? 1 : 0][bucket];
-    if (l.ctas_per_sm == 0) {
-        int per_sm = 0;
-        if (lut_variant) {
-            l.lut_fn = bestfit_lut_multi_kernel<256>;
-            l.threads = 256;
-            l.smem = sizeof(LutSmem<256>);
-            EGPU_CUDA(ctx, cudaFuncSetAttribute(l.lut_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(l.smem)));
-            EGPU_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l.lut_fn, l.threads, l.smem));
-        } else {
-            static const SortedMultiKernel fns[4] = {bestfit_sorted_multi_kernel<8, 256>, bestfit_sorted_multi_kernel<16, 256>,
-                                                     bestfit_sorted_multi_kernel<32, 256>, bestfit_sorted_multi_kernel<64, 128>};
-            static const int threads[4] = {256, 256, 256, 128};
-            static const size_t smem[4] = {sizeof(SnapSmem<8, 256>), sizeof(SnapSmem<16, 256>), sizeof(SnapSmem<32, 256>),
-                                           sizeof(SnapSmem<64, 128>)};
-            l.fn = fns[bucket];
-            l.threads = threads[bucket];
-            l.smem = smem[bucket];
-            EGPU_CUDA(ctx, cudaFuncSetAttribute(l.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(l.smem)));
-            EGPU_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, l.fn, l.threads, l.smem));
-        }
-        l.ctas_per_sm = per_sm < 1 ? 1 : per_sm;
-    }
-    if (lut_variant && ctx->lut_dirty) {
-        lut_build_kernel<<<1, 256, 0, s>>>(ctx->d_state, ctx->d_lut);
-        EGPU_CUDA(ctx, cudaGetLastError());
-        ctx->launches += 1;
-        ctx->lut_dirty = false;
-        ctx->prev_is_scan = false;
+template <int F>
+int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cudaStream_t s, unsigned long long push_base) {
+    constexpr bool lut = F == kScanLutMulti;
+    const auto& k = kKernels<F>[d_bucket(ctx->D)];
+    int per_sm = 0;
+    int rc = resident_ctas<F>(ctx, ctx->D, &per_sm);
+    if (rc != EGPU_OK) return rc;
+    if (lut) {
+        rc = refresh_lut(ctx, s);
+        if (rc != EGPU_OK) return rc;
     }
     MultiArgs args;
     std::memset(&args, 0, sizeof args);
-    egpu_ctx::Range* mine = ctx->multi_ranges;
+    Range* mine = ctx->multi_ranges;
     int64_t max_r = 0;
-    for (int k = 0; k < K; ++k) {
-        const egpu_batch& b = bs[k];
-        args.b[k].rc = b.d_req_core;
-        args.b[k].rm = b.d_req_mem;
-        args.b[k].idx = b.d_out_idx;
-        args.b[k].delta = reinterpret_cast<long long*>(b.d_delta);
+    for (int b = 0; b < K; ++b) {
+        const egpu_batch& in = bs[b];
+        BatchDesc& d = args.b[b];
+        d.rc = in.d_req_core;
+        d.rm = in.d_req_mem;
+        d.idx = in.d_out_idx;
+        d.delta = reinterpret_cast<long long*>(in.d_delta);
         // sharded: table' comes from an apply call, or (EGPU_F_APPLY) from the batch's own last CTA
-        args.b[k].table_out = (push_base && !(user_flags & EGPU_F_APPLY)) ? nullptr : b.d_table_out;
-        args.b[k].R = b.R;
-        if (b.R > max_r) max_r = b.R;
-        const uintptr_t pi = reinterpret_cast<uintptr_t>(b.d_out_idx), pd = reinterpret_cast<uintptr_t>(b.d_delta),
-                        pt = reinterpret_cast<uintptr_t>(args.b[k].table_out);
-        mine[3 * k] = {pi, pi + static_cast<uintptr_t>(b.R) * sizeof(int32_t)};
-        mine[3 * k + 1] = {pd, pd + (pd ? sizeof(long long) * 2 * ctx->D : 0)};
-        mine[3 * k + 2] = {pt, pt + (pt ? sizeof(int32_t) * 3 * ctx->D : 0)};
+        d.table_out = (push_base && !(user_flags & EGPU_F_APPLY)) ? nullptr : in.d_table_out;
+        d.R = in.R;
+        if (in.R > max_r) max_r = in.R;
+        batch_ranges(mine + 3 * b, d.idx, d.R, d.delta, d.table_out, ctx->D);
     }
     const int n_mine = prepare_ranges(mine, 3 * K);
     if (n_mine < 0) return EGPU_ERR_INVALID;  // two batches of one launch share an output: their order would be undefined
-    int flags = kFlagFinalize | ((push_base && (user_flags & EGPU_F_APPLY)) ? kFlagApplyNow : 0);
-    bool pipelined = (user_flags & EGPU_F_INPUTS_READY) && ctx->prev_is_scan && !ctx->prev_changes_table && ctx->prev_stream == s &&
-                     ctx->group_len > 0 && !overlaps_inflight(ctx->inflight, mine, n_mine);
-    if (pipelined) {
-        flags |= kFlagLateWait;
-        if (ctx->group_len >= ctx->pipe_group || ctx->group_mbatches + K > kMultiSlots - kMultiMax) {
-            flags |= kFlagBoundary;
-            new_group(ctx);
-        }
-    } else {
-        new_group(ctx);
-    }
-    if (user_flags & EGPU_F_INPUTS_READY) flags |= kFlagEarlyTrigger;
+    const int flags = kFlagFinalize | ((push_base && (user_flags & EGPU_F_APPLY)) ? kFlagApplyNow : 0) |
+                      order_scan(ctx, user_flags, true, K, s, mine, n_mine);
 
     // Tiles per batch.  Batches below 512 Ki rows: enough CTAs that a thread has >= multi_rpt rows,
     // at most the resident capacity of the GPU (one wave: there, every extra CTA costs an epilogue
@@ -353,11 +390,10 @@ int launch_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cud
     // evenly, the first `extra` batches get one more.  Measured on an H100: DESIGN.md 4.1e.
     const int64_t nvec = max_r >> 2;
     const bool small = max_r < (512ll << 10);
-    const int64_t rpt = small ? ctx->multi_rpt : (lut_variant ? 28 : 20);
-    const int64_t per_cta = static_cast<int64_t>(l.threads) * ((rpt + 3) / 4);
+    const int64_t rpt = small ? ctx->multi_rpt : (lut ? 28 : 20);
+    const int64_t per_cta = static_cast<int64_t>(k.threads) * ((rpt + 3) / 4);
     int64_t tiles = (nvec + per_cta - 1) / per_cta;
     if (tiles < 1) tiles = 1;
-    int per_sm = l.ctas_per_sm;
     if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
     const int64_t wave = static_cast<int64_t>(ctx->sm_count) * per_sm;
     int64_t extra = 0;
@@ -371,53 +407,50 @@ int launch_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cud
         }
     }
     if (tiles > 0xffff) tiles = 0xffff;
-    if (max_r / (tiles * l.threads) + 8 >= (1ll << 19)) return EGPU_ERR_INVALID;  // lane-private sums hold 2^19 rows per lane
+    if (max_r / (tiles * k.threads) + 8 >= (1ll << 19)) return EGPU_ERR_INVALID;  // lane-private sums hold 2^19 rows per lane
     const int tiles_extra = static_cast<int>(tiles | (extra << 16));
     const int64_t n_ctas = tiles * K + extra;
 
     const unsigned int slot_base = static_cast<unsigned int>(ctx->mseq % kMultiSlots);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(n_ctas));
-    cfg.blockDim = dim3(static_cast<unsigned>(l.threads));
-    cfg.dynamicSmemBytes = l.smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (lut_variant)
-        EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, l.lut_fn, ctx->d_state, args, tiles_extra, flags, slot_base, push_base,
-                                          static_cast<const DevLut*>(ctx->d_lut)));
+    if constexpr (lut)
+        rc = launch_pdl(ctx, k, n_ctas, s, ctx->d_state, args, tiles_extra, flags, slot_base, push_base,
+                        static_cast<const DevLut*>(ctx->d_lut));
     else
-        EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, l.fn, ctx->d_state, args, tiles_extra, flags, slot_base, push_base));
-    ctx->launches += 1;
-    ctx->mseq += static_cast<uint64_t>(K);
-    add_inflight(ctx, mine, n_mine);
-    ctx->group_len += 1;
-    ctx->group_mbatches += K;
-    ctx->prev_is_scan = true;
-    ctx->prev_changes_table = false;
-    ctx->prev_stream = s;
+        rc = launch_pdl(ctx, k, n_ctas, s, ctx->d_state, args, tiles_extra, flags, slot_base, push_base);
+    if (rc != EGPU_OK) return rc;
+    record_scan(ctx, s, mine, n_mine, K, false);
     return EGPU_OK;
+}
+
+int launch_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cudaStream_t s, unsigned long long push_base) {
+    if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // the literal variant has no multi-batch form
+    return lut_variant(ctx) ? launch_multi_as<kScanLutMulti>(ctx, bs, K, user_flags, s, push_base)
+                            : launch_multi_as<kScanSortedMulti>(ctx, bs, K, user_flags, s, push_base);
+}
+
+// First half of a prefix-commit (spec 2.5): the CONTIG scan, which neither commits nor returns
+// delta / table' (its sums are the uncapped ones); push_step_plus1 as in Snapshot.  Returns the
+// PrefixOut the next kernels fill and the tile count of the scan.
+int prefix_scan(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx,
+                unsigned long long push_step_plus1, cudaStream_t s, PrefixOut** pf, int* n_tiles) {
+    if (!ctx->d_prefix_out) EGPU_CUDA(ctx, cudaMalloc(&ctx->d_prefix_out, sizeof(PrefixOut) + sizeof(long long) * 2 * kMaxD));
+    *pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
+    Snapshot a{d_rc, d_rm, R, d_idx};
+    a.push_step_plus1 = push_step_plus1;
+    a.contig = true;
+    return launch_snapshot(ctx, a, s, n_tiles);
 }
 
 // Prefix-commit pipeline on device buffers (spec 2.5): CONTIG scan -> per-device cut ->
 // rewrite of the deferred indices -> delta / table' of the committed rows only.
 int launch_prefix_commit(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx,
                          long long* d_delta, int32_t* d_table_out, int user_flags, cudaStream_t s) {
-    if (!ctx->d_prefix_out) EGPU_CUDA(ctx, cudaMalloc(&ctx->d_prefix_out, sizeof(PrefixOut) + sizeof(long long) * 2 * kMaxD));
+    PrefixOut* pf = nullptr;
     int n_tiles = 0;
-    // the scan itself must neither publish nor commit: its sums are the uncapped ones
-    int rc = launch_snapshot(ctx, d_rc, d_rm, R, d_idx, nullptr, nullptr, 0, true, s, 0, 0, true, &n_tiles);
+    const int rc = prefix_scan(ctx, d_rc, d_rm, R, d_idx, 0, s, &pf, &n_tiles);
     if (rc != EGPU_OK) return rc;
-    PrefixOut* pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
     prefix_cut_kernel<<<ctx->D, 256, 0, s>>>(ctx->d_state, d_idx, d_rc, d_rm, R, n_tiles, ctx->d_tile_sums, pf);
-    int64_t blocks = (R + 1023) / 1024;
-    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * 8;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    prefix_apply_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(pf, ctx->D, R, d_idx);
+    prefix_apply_kernel<<<capped_blocks(ctx, R, 1024), 256, 0, s>>>(pf, ctx->D, R, d_idx);
     prefix_finalize_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, pf, d_delta, d_table_out, (user_flags & EGPU_F_COMMIT) ? 1 : 0);
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 3;
@@ -451,13 +484,7 @@ int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t 
     const size_t per = (sizeof(int32_t) * static_cast<size_t>(R) + 255) & ~static_cast<size_t>(255);
     constexpr size_t kHead = 2048;  // RoundInfo
     const size_t need = kHead + tiles_bytes + 8 * per;
-    if (need > ctx->rounds_bytes) {
-        if (ctx->d_rounds) cudaFree(ctx->d_rounds);
-        ctx->d_rounds = nullptr;
-        ctx->rounds_bytes = 0;
-        EGPU_CUDA(ctx, cudaMalloc(&ctx->d_rounds, need));
-        ctx->rounds_bytes = need;
-    }
+    EGPU_CUDA(ctx, grow(ctx->rounds_bytes, need, need, &ctx->d_rounds));
     static_assert(sizeof(RoundInfo) <= kHead, "round info header");
     char* base = static_cast<char*>(ctx->d_rounds);
     RoundInfo* d_info = reinterpret_cast<RoundInfo*>(base);
@@ -477,9 +504,7 @@ int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t 
         int rc = launch_prefix_commit(ctx, cur_rc, cur_rm, n, cur_idx, d_info->delta, nullptr, EGPU_F_COMMIT, s);
         if (rc != EGPU_OK) return rc;
         if (cur_map) {
-            int64_t blocks = (n + 255) / 256;
-            if (blocks > static_cast<int64_t>(ctx->sm_count) * 8) blocks = static_cast<int64_t>(ctx->sm_count) * 8;
-            round_writeback_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(cur_idx, cur_map, n, d_idx);
+            round_writeback_kernel<<<capped_blocks(ctx, n, 256), 256, 0, s>>>(cur_idx, cur_map, n, d_idx);
             ctx->launches += 1;
         }
         const int64_t tiles = (n + kCompactTile - 1) / kCompactTile;
@@ -512,20 +537,14 @@ int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t 
 // `step + 1` the committed demand after the cut (pushed by prefix_push_kernel).
 int launch_prefix_commit_shard(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx,
                                long long* d_delta, int32_t* d_table_out, int user_flags, uint64_t step, cudaStream_t s) {
-    if (!ctx->d_prefix_out) EGPU_CUDA(ctx, cudaMalloc(&ctx->d_prefix_out, sizeof(PrefixOut) + sizeof(long long) * 2 * kMaxD));
-    PrefixOut* pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
-    long long* base = reinterpret_cast<long long*>(pf + 1);
+    PrefixOut* pf = nullptr;
     int n_tiles = 0;
-    // finalising scan without commit: its epilogue publishes (and pushes) the uncapped sums
-    int rc = launch_snapshot(ctx, d_rc, d_rm, R, d_idx, nullptr, nullptr, 0, true, s, 0, step + 1, true, &n_tiles);
+    const int rc = prefix_scan(ctx, d_rc, d_rm, R, d_idx, step + 1, s, &pf, &n_tiles);
     if (rc != EGPU_OK) return rc;
+    long long* base = reinterpret_cast<long long*>(pf + 1);
     prefix_base_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, step + 1, base);
     prefix_cut_kernel<<<ctx->D, 256, 0, s>>>(ctx->d_state, d_idx, d_rc, d_rm, R, n_tiles, ctx->d_tile_sums, pf, base);
-    int64_t blocks = (R + 1023) / 1024;
-    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * 8;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    prefix_apply_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(pf, ctx->D, R, d_idx);
+    prefix_apply_kernel<<<capped_blocks(ctx, R, 1024), 256, 0, s>>>(pf, ctx->D, R, d_idx);
     prefix_push_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, pf, step + 2, d_delta);
     ApplyOuts outs{};
     outs.table_out[0] = d_table_out;
@@ -537,45 +556,24 @@ int launch_prefix_commit_shard(egpu_ctx* ctx, const int32_t* d_rc, const int32_t
     return EGPU_OK;
 }
 
-using PackedKernel = void (*)(DevState*, const uint32_t*, long long, signed char*, long long*, int32_t*, int, unsigned long long);
-
 // Packed-format scan: always a fully ordered launch (it serves the synchronous host path).
 int launch_packed(egpu_ctx* ctx, const uint32_t* d_req, int64_t R, signed char* d_idx8, long long* d_delta,
                   int32_t* d_table_out, int user_flags, cudaStream_t s, int rows_per_thread) {
-    const int bucket = ctx->D <= 8 ? 0 : ctx->D <= 16 ? 1 : ctx->D <= 32 ? 2 : 3;
-    static const PackedKernel fns[4] = {bestfit_sorted_packed_kernel<8, 256>, bestfit_sorted_packed_kernel<16, 256>,
-                                        bestfit_sorted_packed_kernel<32, 256>, bestfit_sorted_packed_kernel<64, 128>};
-    static const int threads[4] = {256, 256, 256, 128};
-    static const size_t smem[4] = {sizeof(SnapSmem<8, 256>), sizeof(SnapSmem<16, 256>), sizeof(SnapSmem<32, 256>),
-                                   sizeof(SnapSmem<64, 128>)};
-    int& per_sm = ctx->packed_ctas_per_sm[bucket];
-    if (per_sm == 0) {
-        EGPU_CUDA(ctx, cudaFuncSetAttribute(fns[bucket], cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem[bucket])));
-        int n = 0;
-        EGPU_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fns[bucket], threads[bucket], smem[bucket]));
-        per_sm = n < 1 ? 1 : n;
-    }
+    const auto& k = kKernels<kScanPacked>[d_bucket(ctx->D)];
+    int per_sm = 0;
+    int rc = resident_ctas<kScanPacked>(ctx, ctx->D, &per_sm);
+    if (rc != EGPU_OK) return rc;
     const int64_t nchunk = R >> 9;  // 512 requests per warp trip
-    const int64_t per_cta = static_cast<int64_t>(threads[bucket] / 32) * ((rows_per_thread + 15) / 16);
+    const int64_t per_cta = static_cast<int64_t>(k.threads / 32) * ((rows_per_thread + 15) / 16);
     int64_t want = (nchunk + per_cta - 1) / per_cta;
     const int64_t cap = static_cast<int64_t>(ctx->sm_count) * per_sm;
     if (want > cap) want = cap;
     if (want < 1) want = 1;
-    if (R / (want * threads[bucket]) + 16 >= (1ll << 19)) return EGPU_ERR_INVALID;
+    if (R / (want * k.threads) + 16 >= (1ll << 19)) return EGPU_ERR_INVALID;
     const int flags = kFlagFinalize | ((user_flags & EGPU_F_COMMIT) ? kFlagCommit : 0);
     const unsigned long long slot = ctx->seq % kEpiSlots;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(want));
-    cfg.blockDim = dim3(static_cast<unsigned>(threads[bucket]));
-    cfg.dynamicSmemBytes = smem[bucket];
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, fns[bucket], ctx->d_state, d_req, static_cast<long long>(R), d_idx8, d_delta,
-                                      d_table_out, flags, slot));
+    rc = launch_pdl(ctx, k, want, s, ctx->d_state, d_req, static_cast<long long>(R), d_idx8, d_delta, d_table_out, flags, slot);
+    if (rc != EGPU_OK) return rc;
     ctx->launches += 1;
     ctx->seq += 1;
     new_group(ctx);
@@ -584,23 +582,37 @@ int launch_packed(egpu_ctx* ctx, const uint32_t* d_req, int64_t R, signed char* 
     return EGPU_OK;
 }
 
+// staging of the host-buffer entry points: three arrays of at least `rows` int32, doubling
 int ensure_staging(egpu_ctx* ctx, int64_t rows) {
-    if (rows <= ctx->d_cap_rows) return EGPU_OK;
-    int64_t cap = ctx->d_cap_rows ? ctx->d_cap_rows : 1024;
-    while (cap < rows) cap *= 2;
-    if (ctx->d_req_core) cudaFree(ctx->d_req_core);
-    if (ctx->d_req_mem) cudaFree(ctx->d_req_mem);
-    if (ctx->d_idx) cudaFree(ctx->d_idx);
-    ctx->d_req_core = ctx->d_req_mem = ctx->d_idx = nullptr;
-    ctx->d_cap_rows = 0;
-    EGPU_CUDA(ctx, cudaMalloc(&ctx->d_req_core, sizeof(int32_t) * cap));
-    EGPU_CUDA(ctx, cudaMalloc(&ctx->d_req_mem, sizeof(int32_t) * cap));
-    EGPU_CUDA(ctx, cudaMalloc(&ctx->d_idx, sizeof(int32_t) * cap));
-    ctx->d_cap_rows = cap;
+    const size_t need = sizeof(int32_t) * static_cast<size_t>(rows);
+    size_t bytes = ctx->staging_bytes ? ctx->staging_bytes : sizeof(int32_t) * 1024;
+    while (bytes < need) bytes *= 2;
+    EGPU_CUDA(ctx, grow(ctx->staging_bytes, need, bytes, &ctx->d_req_core, &ctx->d_req_mem, &ctx->d_idx));
     return EGPU_OK;
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// device row arrays of an entry point: present when there are rows, 16-byte aligned (the scans
+// move 128-bit vectors)
+bool rows_ok(int64_t R, std::initializer_list<const void*> arrays) {
+    for (const void* p : arrays)
+        if ((R > 0 && !p) || !aligned16(p)) return false;
+    return true;
+}
+
+// What an entry point needs of the context, each level including the ones before it.
+enum Needs { kNeedsDevice, kNeedsTable, kNeedsPeers };
+
+// The part of an entry point after it took ctx->mu: checks the state it needs, selects the
+// context's device and the stream to launch on (the caller's, or the context's for nullptr).
+int enter(egpu_ctx* ctx, Needs needs, void* stream, cudaStream_t* s) {
+    if (needs >= kNeedsTable && !ctx->has_table) return EGPU_ERR_NO_TABLE;
+    if (needs >= kNeedsPeers && !ctx->attached) return EGPU_ERR_STATE;
+    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
+    *s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    return EGPU_OK;
+}
 
 // device-visible alias of a pinned (mapped) host allocation, nullptr for anything else
 void* mapped_alias(const void* p) {
@@ -657,10 +669,6 @@ int egpu_ctx_create(int cuda_device, egpu_ctx** out) {
         if (const char* e = std::getenv("EGPU_ROWS_PER_THREAD")) ctx->rows_per_thread = std::atoi(e);
         if (const char* e = std::getenv("EGPU_REPLAY_GENERAL")) ctx->replay_general = std::atoi(e) != 0;
         if (const char* e = std::getenv("EGPU_REPLAY_VARIANT")) ctx->replay_variant = std::atoi(e);
-        if (const char* e = std::getenv("EGPU_THREADS8")) {
-            const int v = std::atoi(e);
-            ctx->threads8 = (v == 128 || v == 512) ? v : 256;
-        }
         if (const char* e = std::getenv("EGPU_MULTI_RPT")) ctx->multi_rpt = std::max(4, std::min(4096, std::atoi(e)));
         if (const char* e = std::getenv("EGPU_PIPE_GROUP")) {
             const int g = std::atoi(e);
@@ -762,13 +770,7 @@ void egpu_note_error(egpu_ctx* ctx, const char* msg) {
 int egpu_table_set_locked(egpu_ctx* ctx, const int32_t* free_core, const int32_t* free_mem, int32_t D) {
     EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
     DevState h;
-    std::memset(&h, 0, sizeof h);
-    std::memcpy(h.free_core, free_core, sizeof(int32_t) * D);
-    std::memcpy(h.free_mem, free_mem, sizeof(int32_t) * D);
-    h.D = D;
-    h.cand_xor = kGuards;
-    h.cand_mask = kCandMask;
-    fill_sorted(h);
+    table_image(h, free_core, free_mem, D);
     // pageable source: the copy is staged before the call returns
     // only the table part: the peer configuration (egpu_peer_attach) and the epilogue slots
     // that follow stay as they are
@@ -838,18 +840,16 @@ int egpu_host_unregister(egpu_ctx* ctx, void* p) {
 int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                            int32_t* d_out_idx, int64_t* d_delta, int32_t* d_table_out, int flags,
                            void* stream) {
-    if (!ctx || R < 0) return EGPU_ERR_INVALID;
-    if (R > 0 && (!d_req_core || !d_req_mem || !d_out_idx)) return EGPU_ERR_INVALID;
-    if (!aligned16(d_req_core) || !aligned16(d_req_mem) || !aligned16(d_out_idx)) return EGPU_ERR_INVALID;
+    if (!ctx || R < 0 || !rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsTable, stream, &s);
+    if (rc != EGPU_OK) return rc;
     if (flags & EGPU_F_PREFIX_COMMIT)
         return launch_prefix_commit(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out,
                                     flags, s);
-    return launch_snapshot(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta),
-                           d_table_out, flags, true, s);
+    Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags};
+    return launch_snapshot(ctx, a, s);
 }
 
 static int check_batches(const egpu_batch* batches, int32_t K) {
@@ -857,41 +857,40 @@ static int check_batches(const egpu_batch* batches, int32_t K) {
     for (int k = 0; k < K; ++k) {
         const egpu_batch& b = batches[k];
         if (b.R < 0 || b.R > kMaxRows) return EGPU_ERR_INVALID;
-        if (b.R > 0 && (!b.d_req_core || !b.d_req_mem || !b.d_out_idx)) return EGPU_ERR_INVALID;
-        if (!aligned16(b.d_req_core) || !aligned16(b.d_req_mem) || !aligned16(b.d_out_idx)) return EGPU_ERR_INVALID;
+        if (!rows_ok(b.R, {b.d_req_core, b.d_req_mem, b.d_out_idx})) return EGPU_ERR_INVALID;
     }
     return EGPU_OK;
 }
 
 int egpu_bestfit_batches_dev(egpu_ctx* ctx, const egpu_batch* batches, int32_t K, int flags, void* stream) {
     if (!ctx || (flags & ~EGPU_F_INPUTS_READY)) return EGPU_ERR_INVALID;
-    const int rc = check_batches(batches, K);
+    int rc = check_batches(batches, K);
     if (rc != EGPU_OK) return rc;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    rc = enter(ctx, kNeedsTable, stream, &s);
+    if (rc != EGPU_OK) return rc;
     return launch_multi(ctx, batches, K, flags, s, 0);
 }
 
 int egpu_bestfit_batches_shard_dev(egpu_ctx* ctx, const egpu_batch* batches, int32_t K, int flags, uint64_t first_step,
                                    void* stream) {
     if (!ctx || (flags & ~(EGPU_F_INPUTS_READY | EGPU_F_APPLY)) || first_step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    const int rc = check_batches(batches, K);
+    int rc = check_batches(batches, K);
     if (rc != EGPU_OK) return rc;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    if (!ctx->attached) return EGPU_ERR_STATE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    rc = enter(ctx, kNeedsPeers, stream, &s);
+    if (rc != EGPU_OK) return rc;
     return launch_multi(ctx, batches, K, flags, s, first_step + 1);
 }
 
 int egpu_peer_gate_dev(egpu_ctx* ctx, void* stream) {
     if (!ctx) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsDevice, stream, &s);
+    if (rc != EGPU_OK) return rc;
     gate_kernel<<<1, 32, 0, s>>>(ctx->d_state, ctx->h_gate_dev);
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
@@ -929,40 +928,35 @@ int egpu_bestfit_query(egpu_ctx* ctx, const int32_t* free_core, const int32_t* f
     }
     if (R == 0) return EGPU_OK;
     std::lock_guard<std::mutex> g(ctx->mu);
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = ctx->stream;
+    cudaStream_t s;
+    int rc = enter(ctx, kNeedsDevice, nullptr, &s);
+    if (rc != EGPU_OK) return rc;
     if (!ctx->d_qstate) {
         EGPU_CUDA(ctx, cudaMalloc(&ctx->d_qstate, sizeof(DevState)));
         EGPU_CUDA(ctx, cudaMemsetAsync(ctx->d_qstate, 0, sizeof(DevState), s));
     }
     // the scratch table: same layout and sorted view as the context's own, in its own DevState
     DevState* h = reinterpret_cast<DevState*>(ctx->h_qtable);
-    std::memset(h, 0, offsetof(DevState, peer));
-    std::memcpy(h->free_core, free_core, sizeof(int32_t) * D);
-    std::memcpy(h->free_mem, free_mem, sizeof(int32_t) * D);
-    h->D = D;
-    h->cand_xor = kGuards;
-    h->cand_mask = kCandMask;
-    fill_sorted(*h);
+    table_image(*h, free_core, free_mem, D);
     EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_qstate, h, offsetof(DevState, peer), cudaMemcpyHostToDevice, s));
-    int rc = ensure_staging(ctx, R);
+    rc = ensure_staging(ctx, R);
     if (rc != EGPU_OK) return rc;
     EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
     EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
     // the register scan whatever the context's variant: one table, used once - lookup tables would not pay
-    const int bucket = D <= 8 ? 0 : D <= 16 ? 1 : D <= 32 ? 2 : 3;
-    SnapLaunch& l = ctx->snap[0][bucket];
-    rc = configure_launch(ctx, l, D, false, false, false);
+    const auto& k = kKernels<kScanSorted>[d_bucket(D)];
+    int per_sm = 0;
+    rc = resident_ctas<kScanSorted>(ctx, D, &per_sm);
     if (rc != EGPU_OK) return rc;
     const int64_t nvec = R >> 2;
-    const int64_t per_cta = static_cast<int64_t>(l.threads) * 2;
+    const int64_t per_cta = static_cast<int64_t>(k.threads) * 2;
     int64_t want = (nvec + per_cta - 1) / per_cta;
-    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * l.ctas_per_sm;
+    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * per_sm;
     if (want > cap) want = cap;
     if (want < 1) want = 1;
-    if (R / (want * l.threads) + 8 >= (1ll << 19)) return EGPU_ERR_INVALID;
+    if (R / (want * k.threads) + 8 >= (1ll << 19)) return EGPU_ERR_INVALID;
     // fully ordered launch (no PDL flags), epilogue slot 0 of the scratch state, nothing published
-    l.fn<<<static_cast<unsigned>(want), l.threads, l.smem, s>>>(ctx->d_qstate, ctx->d_req_core, ctx->d_req_mem,
+    k.fn<<<static_cast<unsigned>(want), k.threads, k.smem, s>>>(ctx->d_qstate, ctx->d_req_core, ctx->d_req_mem,
                                                                 static_cast<long long>(R), ctx->d_idx, nullptr, nullptr,
                                                                 kFlagFinalize, 0ull, nullptr);
     EGPU_CUDA(ctx, cudaGetLastError());
@@ -978,11 +972,11 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     if (!ctx || R < 0) return EGPU_ERR_INVALID;
     if (R > 0 && (!req_core || !req_mem || !out_idx)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = ctx->stream;
+    cudaStream_t s;
+    int rc = enter(ctx, kNeedsTable, nullptr, &s);
+    if (rc != EGPU_OK) return rc;
     const int D = ctx->D;
-    int rc;
+    const int user_flags = (commit & EGPU_F_COMMIT) ? EGPU_F_COMMIT : 0;
     // Zero-copy: when all three caller arrays are pinned (egpu_host_alloc or
     // cudaHostRegister) and 16-byte aligned, the scan reads the requests and writes
     // the indices straight across PCIe — one launch, no staging in HBM, reads and
@@ -994,7 +988,9 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     if (!prefix && zc && zm && zi && aligned16(zc) && aligned16(zm) && aligned16(zi) && !ctx->no_zero_copy) {
         // 64 rows per thread: few CTAs, many trips, so reads of later rows and writes of
         // earlier ones are on the link at the same time (PCIe is full duplex)
-        rc = launch_snapshot(ctx, zc, zm, R, zi, ctx->h_delta_dev, nullptr, (commit & EGPU_F_COMMIT) ? EGPU_F_COMMIT : 0, true, s, 64);
+        Snapshot a{zc, zm, R, zi, ctx->h_delta_dev, nullptr, user_flags};
+        a.rpt_hint = 64;
+        rc = launch_snapshot(ctx, a, s);
         if (rc != EGPU_OK) return rc;
         EGPU_CUDA(ctx, cudaStreamSynchronize(s));
     } else {
@@ -1004,10 +1000,8 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
             EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
             EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
         }
-        rc = prefix ? launch_prefix_commit(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr,
-                                           (commit & EGPU_F_COMMIT) ? EGPU_F_COMMIT : 0, s)
-                    : launch_snapshot(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr,
-                                      (commit & EGPU_F_COMMIT) ? EGPU_F_COMMIT : 0, true, s);
+        rc = prefix ? launch_prefix_commit(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, user_flags, s)
+                    : launch_snapshot(ctx, Snapshot{ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, user_flags}, s);
         if (rc != EGPU_OK) return rc;
         if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, sizeof(int32_t) * R, cudaMemcpyDeviceToHost, s));
         EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
@@ -1024,10 +1018,10 @@ int egpu_bestfit_batch_rounds(egpu_ctx* ctx, const int32_t* req_core, const int3
     if (!ctx || R < 0 || R >= (1ll << 31) || max_rounds < 1) return EGPU_ERR_INVALID;
     if (R > 0 && (!req_core || !req_mem || !out_idx)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = ctx->stream;
-    int rc = ensure_staging(ctx, R > 0 ? R : 1);
+    cudaStream_t s;
+    int rc = enter(ctx, kNeedsTable, nullptr, &s);
+    if (rc != EGPU_OK) return rc;
+    rc = ensure_staging(ctx, R > 0 ? R : 1);
     if (rc != EGPU_OK) return rc;
     if (R > 0) {
         EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
@@ -1051,17 +1045,16 @@ int egpu_bestfit_batch_rounds(egpu_ctx* ctx, const int32_t* req_core, const int3
 int egpu_bestfit_batch_rounds_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                                   int32_t* d_out_idx, int64_t* out_delta /* host [2*D] */, int32_t max_rounds,
                                   int32_t* out_rounds, int64_t* out_deferred, void* stream) {
-    if (!ctx || R < 0 || R >= (1ll << 31) || max_rounds < 1) return EGPU_ERR_INVALID;
-    if (R > 0 && (!d_req_core || !d_req_mem || !d_out_idx)) return EGPU_ERR_INVALID;
-    if (!aligned16(d_req_core) || !aligned16(d_req_mem) || !aligned16(d_out_idx)) return EGPU_ERR_INVALID;
+    if (!ctx || R < 0 || R >= (1ll << 31) || max_rounds < 1 || !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
+        return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    int rc = enter(ctx, kNeedsTable, stream, &s);
+    if (rc != EGPU_OK) return rc;
     long long total[2 * kMaxD];
     int32_t rounds = 0;
     int64_t left = 0;
-    const int rc = run_rounds(ctx, d_req_core, d_req_mem, R, d_out_idx, max_rounds, total, &rounds, &left, s);
+    rc = run_rounds(ctx, d_req_core, d_req_mem, R, d_out_idx, max_rounds, total, &rounds, &left, s);
     if (rc != EGPU_OK) return rc;
     EGPU_CUDA(ctx, cudaStreamSynchronize(s));
     if (out_delta) std::memcpy(out_delta, total, sizeof(int64_t) * 2 * ctx->D);
@@ -1132,28 +1125,25 @@ int egpu_bestfit_batch_shard_dev(egpu_ctx* ctx, const int32_t* d_req_core, const
     // the commit happens in apply_peers; prefix-commit over shards has its own entry point;
     // step + 1 travels in 48 bits of the launch word
     if (!ctx || R < 0 || (flags & ~EGPU_F_INPUTS_READY) || step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    if (R > 0 && (!d_req_core || !d_req_mem || !d_out_idx)) return EGPU_ERR_INVALID;
-    if (!aligned16(d_req_core) || !aligned16(d_req_mem) || !aligned16(d_out_idx)) return EGPU_ERR_INVALID;
+    if (!rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    if (!ctx->attached) return EGPU_ERR_STATE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    return launch_snapshot(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), nullptr,
-                           flags, true, s, 0, step + 1);
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsPeers, stream, &s);
+    if (rc != EGPU_OK) return rc;
+    Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), nullptr, flags};
+    a.push_step_plus1 = step + 1;
+    return launch_snapshot(ctx, a, s);
 }
 
 int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                                         int32_t* d_out_idx, int64_t* d_delta, int32_t* d_table_out, int flags,
                                         uint64_t step, void* stream) {
     if (!ctx || R < 0 || step >= (1ull << 47) || (flags & ~(EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT))) return EGPU_ERR_INVALID;
-    if (R > 0 && (!d_req_core || !d_req_mem || !d_out_idx)) return EGPU_ERR_INVALID;
-    if (!aligned16(d_req_core) || !aligned16(d_req_mem) || !aligned16(d_out_idx)) return EGPU_ERR_INVALID;
+    if (!rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    if (!ctx->attached) return EGPU_ERR_STATE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsPeers, stream, &s);
+    if (rc != EGPU_OK) return rc;
     return launch_prefix_commit_shard(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta),
                                       d_table_out, flags, step, s);
 }
@@ -1162,25 +1152,24 @@ int egpu_bestfit_batch_shard_lag_dev(egpu_ctx* ctx, const int32_t* d_req_core, c
                                      int32_t* d_out_idx, int64_t* d_delta, int flags, uint64_t step, int lag,
                                      int32_t* d_table_out_lagged, void* stream) {
     if (!ctx || R < 0 || (flags & EGPU_F_COMMIT) || lag < 1 || lag > 16 || step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    if (R > 0 && (!d_req_core || !d_req_mem || !d_out_idx)) return EGPU_ERR_INVALID;
-    if (!aligned16(d_req_core) || !aligned16(d_req_mem) || !aligned16(d_out_idx)) return EGPU_ERR_INVALID;
+    if (!rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    if (!ctx->attached) return EGPU_ERR_STATE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    return launch_snapshot(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out_lagged,
-                           flags, true, s, 0, step + 1, false, nullptr, lag);
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsPeers, stream, &s);
+    if (rc != EGPU_OK) return rc;
+    Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out_lagged, flags};
+    a.push_step_plus1 = step + 1;
+    a.lag = lag;
+    return launch_snapshot(ctx, a, s);
 }
 
 int egpu_table_apply_peers_multi_dev(egpu_ctx* ctx, uint64_t first_step, int nsteps, int32_t* const* d_table_outs,
                                      int commit, void* stream) {
     if (!ctx || nsteps < 1 || nsteps > kApplyMax) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    if (!ctx->attached) return EGPU_ERR_STATE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsPeers, stream, &s);
+    if (rc != EGPU_OK) return rc;
     if (commit) {
         ctx->lut_dirty = true;
         ctx->prev_is_scan = false;  // the next scan must see the new table
@@ -1213,13 +1202,11 @@ int64_t egpu_peer_last_timeout(egpu_ctx* ctx) {
 
 int egpu_bestfit_batch_packed_dev(egpu_ctx* ctx, const uint32_t* d_req_packed, int64_t R, int8_t* d_out_idx8,
                                   int64_t* d_delta, int32_t* d_table_out, int flags, void* stream) {
-    if (!ctx || R < 0) return EGPU_ERR_INVALID;
-    if (R > 0 && (!d_req_packed || !d_out_idx8)) return EGPU_ERR_INVALID;
-    if (!aligned16(d_req_packed) || !aligned16(d_out_idx8)) return EGPU_ERR_INVALID;
+    if (!ctx || R < 0 || !rows_ok(R, {d_req_packed, d_out_idx8})) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsTable, stream, &s);
+    if (rc != EGPU_OK) return rc;
     return launch_packed(ctx, d_req_packed, R, reinterpret_cast<signed char*>(d_out_idx8), reinterpret_cast<long long*>(d_delta),
                          d_table_out, flags, s, 16);
 }
@@ -1229,11 +1216,10 @@ int egpu_bestfit_batch_packed(egpu_ctx* ctx, const uint32_t* req_packed, int64_t
     if (!ctx || R < 0) return EGPU_ERR_INVALID;
     if (R > 0 && (!req_packed || !out_idx8)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = ctx->stream;
+    cudaStream_t s;
+    int rc = enter(ctx, kNeedsTable, nullptr, &s);
+    if (rc != EGPU_OK) return rc;
     const int D = ctx->D;
-    int rc;
     const uint32_t* zr = R > 0 ? static_cast<const uint32_t*>(mapped_alias(req_packed)) : nullptr;
     signed char* zi = R > 0 ? static_cast<signed char*>(mapped_alias(out_idx8)) : nullptr;
     if (zr && zi && aligned16(zr) && aligned16(zi) && !ctx->no_zero_copy) {  // zero-copy across PCIe, see egpu_bestfit_batch
@@ -1260,9 +1246,9 @@ int egpu_table_apply_deltas_dev(egpu_ctx* ctx, const int64_t* d_deltas, int G, i
                                 int commit, void* stream) {
     if (!ctx || !d_deltas || G < 1) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->has_table) return EGPU_ERR_NO_TABLE;
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsTable, stream, &s);
+    if (rc != EGPU_OK) return rc;
     ctx->prev_is_scan = false;
     if (commit) ctx->lut_dirty = true;
     apply_deltas_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, reinterpret_cast<const long long*>(d_deltas), G,
@@ -1278,13 +1264,11 @@ int egpu_synth_requests_dev(egpu_ctx* ctx, int dist, uint64_t seed, int64_t firs
     if (R == 0) return EGPU_OK;
     if (!d_req_core || !d_req_mem) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
-    EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-    int64_t blocks = (R + 255) / 256;
-    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * 8;
-    if (blocks > cap) blocks = cap;
+    cudaStream_t s;
+    const int rc = enter(ctx, kNeedsDevice, stream, &s);
+    if (rc != EGPU_OK) return rc;
     ctx->prev_is_scan = false;
-    synth_requests_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(dist, seed, first_row, R, d_req_core, d_req_mem);
+    synth_requests_kernel<<<capped_blocks(ctx, R, 256), 256, 0, s>>>(dist, seed, first_row, R, d_req_core, d_req_mem);
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
     return EGPU_OK;
@@ -1301,22 +1285,15 @@ int egpu_replay(egpu_ctx* ctx, const int32_t* kind, const int32_t* a, const int3
     // staging comes from the context's grow-only arena (three inputs, one output, the `live`
     // map when it does not fit in shared memory): no cudaMalloc/cudaFree on the call path
     cudaStream_t s = ctx->stream;
-    const size_t ebytes = (sizeof(int32_t) * static_cast<size_t>(E) + 255) & ~static_cast<size_t>(255);
-    const size_t lbytes = E > kReplaySmemEvents ? ((static_cast<size_t>(E) + 255) & ~static_cast<size_t>(255)) : 0;
-    const size_t need = 4 * ebytes + lbytes;
-    if (need > ctx->arena_cap) {
-        if (ctx->arena) cudaFree(ctx->arena);
-        ctx->arena = nullptr;
-        ctx->arena_cap = 0;
-        EGPU_CUDA(ctx, cudaMalloc(&ctx->arena, need + need / 4));
-        ctx->arena_cap = need + need / 4;
-    }
-    char* base = static_cast<char*>(ctx->arena);
-    int32_t* d_kind = reinterpret_cast<int32_t*>(base);
-    int32_t* d_a = reinterpret_cast<int32_t*>(base + ebytes);
-    int32_t* d_b = reinterpret_cast<int32_t*>(base + 2 * ebytes);
-    int32_t* d_out = reinterpret_cast<int32_t*>(base + 3 * ebytes);
-    signed char* d_live = lbytes ? reinterpret_cast<signed char*>(base + 4 * ebytes) : nullptr;
+    const size_t ebytes = sizeof(int32_t) * static_cast<size_t>(E);
+    void *kind_p, *a_p, *b_p, *out_p, *live_p = nullptr;
+    const ArenaWant wants[] = {{&kind_p, ebytes}, {&a_p, ebytes}, {&b_p, ebytes}, {&out_p, ebytes}, {&live_p, static_cast<size_t>(E)}};
+    EGPU_CUDA(ctx, arena_carve(ctx, wants, E > kReplaySmemEvents ? 5 : 4));
+    int32_t* d_kind = static_cast<int32_t*>(kind_p);
+    int32_t* d_a = static_cast<int32_t*>(a_p);
+    int32_t* d_b = static_cast<int32_t*>(b_p);
+    int32_t* d_out = static_cast<int32_t*>(out_p);
+    signed char* d_live = static_cast<signed char*>(live_p);
     size_t smem = 0;
     if (E <= kReplaySmemEvents) {
         smem = static_cast<size_t>((E + 15) & ~15ll);

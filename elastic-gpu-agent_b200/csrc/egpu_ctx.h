@@ -13,41 +13,21 @@
 
 using namespace egpu;  // internal header: the context is made of the kernels' types
 
-using SnapKernel = void (*)(egpu::DevState*, const int32_t*, const int32_t*, long long, int32_t*, long long*, int32_t*, int,
-                            unsigned long long, unsigned long long*);
-
-using LutKernel = void (*)(egpu::DevState*, const int32_t*, const int32_t*, long long, int32_t*, long long*, int32_t*, int,
-                           unsigned long long, const egpu::DevLut*, unsigned long long*);
-
-struct SnapLaunch {
-    SnapKernel fn = nullptr;
-    LutKernel lut_fn = nullptr;  // set instead of fn for the lookup-table scan
-    int threads = 0;
-    size_t smem = 0;
-    int ctas_per_sm = 0;  // 0 = not configured yet on this context
-};
-
-using SortedMultiKernel = void (*)(egpu::DevState*, const egpu::MultiArgs, int, int, unsigned int, unsigned long long);
-using LutMultiKernel = void (*)(egpu::DevState*, const egpu::MultiArgs, int, int, unsigned int, unsigned long long,
-                                const egpu::DevLut*);
-struct MultiLaunch {
-    SortedMultiKernel fn = nullptr;
-    LutMultiKernel lut_fn = nullptr;
-    int threads = 0;
-    size_t smem = 0;
-    int ctas_per_sm = 0;
+// The scan kernels the launchers of egpu_alloc.cu choose from, one per D bucket (D <= 8, 16, 32, 64)
+enum ScanFamily {
+    kScanSorted, kScanSortedContig, kScanGrid, kScanLut, kScanLutContig, kScanSortedMulti, kScanLutMulti, kScanPacked,
+    kScanFamilies
 };
 
 struct egpu_ctx {
     std::mutex mu;
-    SnapLaunch snap[5][4];            // [sorted, grid, lut, sorted CONTIG, lut CONTIG][D bucket]
-    MultiLaunch multi[2][4];          // multi-batch launches: [sorted, lut][D bucket]
+    int scan_ctas_per_sm[kScanFamilies][4] = {};  // resident CTAs per SM of each scan kernel, 0 = not asked yet
     void* h_qtable = nullptr;         // pinned host image of that table (the part of DevState before `peer`)
     DevState* d_qstate = nullptr;     // scratch table of egpu_bestfit_query (the context's own table is not touched)
     unsigned long long* h_gate = nullptr;      // pinned: start gates the host has opened (egpu_peer_gate_open)
     unsigned long long* h_gate_dev = nullptr;  // its device-visible alias
     unsigned long long* d_tile_sums = nullptr;  // prefix-commit: per-tile per-device sums [tiles][2*64]
-    int64_t tile_cap = 0;
+    size_t tile_bytes = 0;
     void* d_prefix_out = nullptr;     // PrefixOut
     void* d_rounds = nullptr;         // scratch of egpu_bestfit_batch_rounds (grow-only)
     size_t rounds_bytes = 0;
@@ -69,7 +49,7 @@ struct egpu_ctx {
     int32_t* d_req_core = nullptr;
     int32_t* d_req_mem = nullptr;
     int32_t* d_idx = nullptr;
-    int64_t d_cap_rows = 0;
+    size_t staging_bytes = 0;         // bytes of each of the three
     long long* d_delta = nullptr;     // int64[2*64]
     int32_t* d_table_out = nullptr;   // int32[3*64]
     long long* h_delta = nullptr;     // pinned
@@ -77,7 +57,7 @@ struct egpu_ctx {
     bool no_zero_copy = false;        // EGPU_NO_ZERO_COPY=1: always stage through HBM
     int32_t* h_table = nullptr;       // pinned int32[3*64]
     bool replay_configured = false;   // shared-memory opt-in of the replay kernels done
-    // bookkeeping for programmatic dependent launch (see launch_snapshot)
+    // bookkeeping for programmatic dependent launch (see order_scan in egpu_alloc.cu)
     bool prev_is_scan = false;        // the last kernel this context launched was a snapshot scan ...
     bool prev_changes_table = false;  // ... and it may rewrite the table (commit)
     cudaStream_t prev_stream = nullptr;
@@ -93,13 +73,11 @@ struct egpu_ctx {
     int pipe_group = 24;              // launches per group (EGPU_PIPE_GROUP, <= kPipeGroupMax)
     int ctas_per_sm_cap = 0;          // 0 = occupancy limit (EGPU_CTAS_PER_SM overrides)
     int rows_per_thread = 0;          // grid sizing target (EGPU_ROWS_PER_THREAD), 0 = default
-    int packed_ctas_per_sm[4] = {0, 0, 0, 0};  // occupancy of the packed-format scan per D bucket, 0 = not asked yet
-    int threads8 = 256;               // CTA size of the D <= 8 register scan (EGPU_THREADS8 = 128 | 256 | 512)
     int replay_variant = 2;           // 2 = two-warp kernel where it applies (EGPU_REPLAY_VARIANT=1: round 1's one-warp kernels)
     bool replay2_configured = false;
     bool sort_sets_configured = false;  // sort_sets_smem_kernel may use 128 KB of dynamic shared memory
     bool replay_general = false;      // EGPU_REPLAY_GENERAL=1: lane = device kernel even for D <= 8 (tests)
-    // grow-only device arena for multi-kernel host-buffer pipelines (egpu_devhash.cu, egpu_prefalloc.cu)
+    // grow-only device arena for multi-kernel host-buffer pipelines (arena_carve)
     void* arena = nullptr;
     size_t arena_cap = 0;
     char last_err[256] = {0};
@@ -109,6 +87,40 @@ inline int cuda_fail(egpu_ctx* ctx, cudaError_t e, const char* what) {
     if (ctx) std::snprintf(ctx->last_err, sizeof ctx->last_err, "%s: %s", what, cudaGetErrorString(e));
     (void)cudaGetLastError();
     return e == cudaErrorMemoryAllocation ? EGPU_ERR_NOMEM : EGPU_ERR_CUDA;
+}
+
+// Grow-only device scratch: when `need` bytes do not fit in `cap`, frees every buffer in `bufs` and
+// gives each `alloc` (>= need) fresh bytes; contents are not kept.  `cap` is 0 until all are allocated.
+template <class... T>
+cudaError_t grow(size_t& cap, size_t need, size_t alloc, T**... bufs) {
+    if (need <= cap) return cudaSuccess;
+    cap = 0;
+    ((cudaFree(*bufs), *bufs = nullptr), ...);
+    cudaError_t e = cudaSuccess;
+    ((e = e == cudaSuccess ? cudaMalloc(bufs, alloc) : e), ...);
+    if (e == cudaSuccess) cap = alloc;
+    return e;
+}
+
+// Scratch of one call, carved from the context's arena in 256-byte aligned pieces (an empty want
+// still gets one).  Every piece is sized before anything is enqueued, so a failed allocation leaves
+// no work half done; the arena grows with 25 % slack and is only touched under ctx->mu.
+struct ArenaWant {
+    void** p;
+    size_t bytes;
+};
+inline cudaError_t arena_carve(egpu_ctx* ctx, const ArenaWant* wants, int n) {
+    auto piece = [](size_t bytes) { return ((bytes ? bytes : 16) + 255) & ~static_cast<size_t>(255); };
+    size_t total = 0;
+    for (int i = 0; i < n; ++i) total += piece(wants[i].bytes);
+    const cudaError_t e = grow(ctx->arena_cap, total, total + total / 4, &ctx->arena);
+    if (e != cudaSuccess) return e;
+    size_t used = 0;
+    for (int i = 0; i < n; ++i) {
+        *wants[i].p = static_cast<char*>(ctx->arena) + used;
+        used += piece(wants[i].bytes);
+    }
+    return cudaSuccess;
 }
 
 // egpu_alloc.cu: body of egpu_table_set for callers that already hold ctx->mu

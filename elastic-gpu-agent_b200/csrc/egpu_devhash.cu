@@ -595,29 +595,6 @@ using namespace egpu;
 
 namespace {
 
-// Buffers are carved from the context's grow-only arena: cudaMalloc/cudaFree per call
-// would cost more than the kernels.  plan() sizes it, alloc() hands out 256-byte aligned
-// pieces; the arena is only touched under the context mutex.
-struct Arena {
-    egpu_ctx* ctx;
-    size_t used = 0;
-    explicit Arena(egpu_ctx* c) : ctx(c) {}
-    cudaError_t reserve(size_t bytes) {
-        if (bytes <= ctx->arena_cap) return cudaSuccess;
-        if (ctx->arena) cudaFree(ctx->arena);
-        ctx->arena = nullptr;
-        ctx->arena_cap = 0;
-        size_t cap = bytes + bytes / 4;
-        cudaError_t e = cudaMalloc(&ctx->arena, cap);
-        if (e == cudaSuccess) ctx->arena_cap = cap;
-        return e;
-    }
-    void* take(size_t bytes) {
-        void* p = static_cast<char*>(ctx->arena) + used;
-        used += (bytes + 255) & ~static_cast<size_t>(255);
-        return p;
-    }
-};
 struct DevBuf {
     void* p = nullptr;
     template <class T>
@@ -652,18 +629,15 @@ int run_hash(egpu_ctx* ctx, HashRun& r, const char* ids_flat, const int64_t* id_
     const size_t n = static_cast<size_t>(n_ids);
     const int64_t tiles = (n_ids + kSortTile - 1) / kSortTile;
     const size_t msg_cap = static_cast<size_t>(flat_bytes) + n + static_cast<size_t>(n_sets) * 128 + 64;
-    struct Want { DevBuf* b; size_t bytes; } wants[] = {
-        {&r.flat, static_cast<size_t>(flat_bytes)}, {&r.id_off, sizeof(long long) * (n + 1)},
-        {&r.set_off, sizeof(long long) * (n_sets + 1)}, {&r.key_a, 8 * n}, {&r.key_b, 8 * n}, {&r.set_a, 4 * n},
-        {&r.set_b, 4 * n}, {&r.len1, 4 * n}, {&r.pref, 8 * (n + 1)}, {&r.blk, 8 * ((n + 1023) / 1024 + 1)},
-        {&r.hist, 4 * 16 * static_cast<size_t>(tiles > 0 ? tiles : 1)}, {&r.msg_base, 8 * static_cast<size_t>(n_sets + 1)},
-        {&r.msg_len, 8 * static_cast<size_t>(n_sets)}, {&r.digest, 32 * static_cast<size_t>(n_sets)}, {&r.err, sizeof(HashErr)},
-        {&r.equal, sizeof(int) * static_cast<size_t>(n_sets)}, {&r.msg, need_digest ? msg_cap : 16}};
-    size_t total = 0;
-    for (const Want& w : wants) total += ((w.bytes ? w.bytes : 16) + 255) & ~static_cast<size_t>(255);
-    Arena arena(ctx);
-    EGPU_CUDA(ctx, arena.reserve(total));
-    for (const Want& w : wants) w.b->p = arena.take(w.bytes ? w.bytes : 16);
+    // scratch: the context's grow-only arena (cudaMalloc/cudaFree per call would cost more than the kernels)
+    const ArenaWant wants[] = {
+        {&r.flat.p, static_cast<size_t>(flat_bytes)}, {&r.id_off.p, sizeof(long long) * (n + 1)},
+        {&r.set_off.p, sizeof(long long) * (n_sets + 1)}, {&r.key_a.p, 8 * n}, {&r.key_b.p, 8 * n}, {&r.set_a.p, 4 * n},
+        {&r.set_b.p, 4 * n}, {&r.len1.p, 4 * n}, {&r.pref.p, 8 * (n + 1)}, {&r.blk.p, 8 * ((n + 1023) / 1024 + 1)},
+        {&r.hist.p, 4 * 16 * static_cast<size_t>(tiles > 0 ? tiles : 1)}, {&r.msg_base.p, 8 * static_cast<size_t>(n_sets + 1)},
+        {&r.msg_len.p, 8 * static_cast<size_t>(n_sets)}, {&r.digest.p, 32 * static_cast<size_t>(n_sets)}, {&r.err.p, sizeof(HashErr)},
+        {&r.equal.p, sizeof(int) * static_cast<size_t>(n_sets)}, {&r.msg.p, need_digest ? msg_cap : 16}};
+    EGPU_CUDA(ctx, arena_carve(ctx, wants, sizeof wants / sizeof wants[0]));
     EGPU_CUDA(ctx, cudaMemsetAsync(r.err.p, 0, sizeof(HashErr), s));
     if (flat_bytes) EGPU_CUDA(ctx, cudaMemcpyAsync(r.flat.p, ids_flat, flat_bytes, cudaMemcpyHostToDevice, s));
     EGPU_CUDA(ctx, cudaMemcpyAsync(r.id_off.p, id_offsets, sizeof(long long) * (n + 1), cudaMemcpyHostToDevice, s));

@@ -116,7 +116,7 @@ struct DevState {
     unsigned long long gate_epoch;        // start gates passed so far (egpu_peer_gate_dev)
     unsigned long long gate_timeouts;     // ... of which gave up waiting (~2 s) for the host or a peer
 };
-constexpr int kEpiSlots = 32;      // ring used by pipelined launches; slot 32 = accumulate-only launches
+constexpr int kEpiSlots = 32;      // ring used by pipelined launches; slot 32 is spare
 constexpr int kPipeGroupMax = 24;  // at most this many launches between two fully ordered ones
 constexpr int kMultiSlots = 128;   // DevState::epi_multi
 constexpr int kMultiMax = 64;      // batches per multi-batch launch (descriptors travel as kernel parameters)

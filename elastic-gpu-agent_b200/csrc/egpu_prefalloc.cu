@@ -407,30 +407,14 @@ extern "C" int egpu_preferred_allocation_batch(egpu_ctx* ctx, int resource, cons
          *rank = nullptr, *blk = nullptr, *hist = nullptr, *first_bad = nullptr, *must_bad = nullptr, *pin_first = nullptr,
          *cnt = nullptr, *mcnt = nullptr, *rc = nullptr, *gpu = nullptr, *e_cnt = nullptr, *e_base = nullptr,
          *run_start = nullptr, *skey = nullptr, *sval = nullptr, *smk = nullptr, *out = nullptr;
-    struct Want { void** p; size_t bytes; } wants[] = {
+    const ArenaWant wants[] = {
         {&flat, static_cast<size_t>(flat_bytes)}, {&id_off, 8 * (n + 1)}, {&set_off, 8 * (static_cast<size_t>(n_sets) + 1)},
         {&d_req, sizeof(PaReq) * nr}, {&gu, 8 * n}, {&set_of, 4 * n}, {&slot_of, 4 * n}, {&key_a, 8 * n}, {&key_b, 8 * n},
         {&val_a, 4 * n}, {&val_b, 4 * n}, {&flag, 4 * n}, {&rank, 8 * (n + 1)}, {&blk, 8 * ((n + 1023) / 1024 + 1)},
         {&hist, 4 * radix_hist_words(n_ids)}, {&first_bad, 8 * nr}, {&must_bad, 8 * nr}, {&pin_first, 4 * cells},
         {&cnt, 4 * cells}, {&mcnt, 4 * cells}, {&rc, 4 * nr}, {&gpu, 4 * nr}, {&e_cnt, 4 * cells}, {&e_base, 4 * cells},
         {&run_start, 4 * cells}, {&skey, 8 * H}, {&sval, 4 * H}, {&smk, 4 * H}, {&out, 4 * static_cast<size_t>(dev_out)}};
-    size_t total = 0;
-    for (const Want& w : wants) total += ((w.bytes ? w.bytes : 16) + 255) & ~static_cast<size_t>(255);
-    if (total > ctx->arena_cap) {
-        if (ctx->arena) cudaFree(ctx->arena);
-        ctx->arena = nullptr;
-        ctx->arena_cap = 0;
-        const size_t cap = total + total / 4;
-        EGPU_CUDA(ctx, cudaMalloc(&ctx->arena, cap));
-        ctx->arena_cap = cap;
-    }
-    {
-        size_t used = 0;
-        for (const Want& w : wants) {
-            *w.p = static_cast<char*>(ctx->arena) + used;
-            used += ((w.bytes ? w.bytes : 16) + 255) & ~static_cast<size_t>(255);
-        }
-    }
+    EGPU_CUDA(ctx, arena_carve(ctx, wants, sizeof wants / sizeof wants[0]));
     // the per-request state and the must-include table start empty: 0xff.. = "none" for the minima and keys
     EGPU_CUDA(ctx, cudaMemsetAsync(first_bad, 0xff, 8 * nr, s));
     EGPU_CUDA(ctx, cudaMemsetAsync(must_bad, 0xff, 8 * nr, s));
