@@ -126,11 +126,13 @@ int refresh_lut(egpu_ctx* ctx, cudaStream_t s) {
 }
 
 // Host image of a table: the part of DevState before `peer` (free capacity, D, candidate masks and
-// the sorted view that resort_table_cta keeps on the device)
-void table_image(DevState& h, const int32_t* free_core, const int32_t* free_mem, int D) {
+// the sorted view that resort_table_cta keeps on the device); oversub may be nullptr (no flags)
+void table_image(DevState& h, const int32_t* free_core, const int32_t* free_mem, const int32_t* oversub, int D) {
     std::memset(&h, 0, offsetof(DevState, peer));
     std::memcpy(h.free_core, free_core, sizeof(int32_t) * D);
     std::memcpy(h.free_mem, free_mem, sizeof(int32_t) * D);
+    if (oversub)
+        for (int d = 0; d < D; ++d) h.oversub[d] = oversub[d] ? 1 : 0;
     h.D = D;
     h.cand_xor = kGuards;
     h.cand_mask = kCandMask;
@@ -753,7 +755,7 @@ int egpu_table_set(egpu_ctx* ctx, const int32_t* free_core, const int32_t* free_
         if (free_mem[d] < 0 || free_mem[d] > EGPU_MEM_MAX) return EGPU_ERR_INVALID;
     }
     std::lock_guard<std::mutex> g(ctx->mu);
-    return egpu_table_set_locked(ctx, free_core, free_mem, D);
+    return egpu_table_set_locked(ctx, free_core, free_mem, nullptr, D);
 }
 
 }  // extern "C"
@@ -766,11 +768,11 @@ void egpu_note_error(egpu_ctx* ctx, const char* msg) {
 }
 
 // body of egpu_table_set; the caller holds ctx->mu and has validated the arguments
-// (also used by egpu_table_restore_flat, egpu_devhash.cu)
-int egpu_table_set_locked(egpu_ctx* ctx, const int32_t* free_core, const int32_t* free_mem, int32_t D) {
+// (also used by egpu_table_restore_flat, egpu_devhash.cu, which installs its flags too)
+int egpu_table_set_locked(egpu_ctx* ctx, const int32_t* free_core, const int32_t* free_mem, const int32_t* oversub, int32_t D) {
     EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
     DevState h;
-    table_image(h, free_core, free_mem, D);
+    table_image(h, free_core, free_mem, oversub, D);
     // pageable source: the copy is staged before the call returns
     // only the table part: the peer configuration (egpu_peer_attach) and the epilogue slots
     // that follow stay as they are
@@ -937,7 +939,7 @@ int egpu_bestfit_query(egpu_ctx* ctx, const int32_t* free_core, const int32_t* f
     }
     // the scratch table: same layout and sorted view as the context's own, in its own DevState
     DevState* h = reinterpret_cast<DevState*>(ctx->h_qtable);
-    table_image(*h, free_core, free_mem, D);
+    table_image(*h, free_core, free_mem, nullptr, D);
     EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_qstate, h, offsetof(DevState, peer), cudaMemcpyHostToDevice, s));
     rc = ensure_staging(ctx, R);
     if (rc != EGPU_OK) return rc;

@@ -123,8 +123,9 @@ inline cudaError_t arena_carve(egpu_ctx* ctx, const ArenaWant* wants, int n) {
     return cudaSuccess;
 }
 
-// egpu_alloc.cu: body of egpu_table_set for callers that already hold ctx->mu
-int egpu_table_set_locked(egpu_ctx* ctx, const int32_t* free_core, const int32_t* free_mem, int32_t D);
+// egpu_alloc.cu: body of egpu_table_set for callers that already hold ctx->mu.  oversub[D] are the
+// table's oversubscription flags (nullptr: none, as egpu_table_set installs it).
+int egpu_table_set_locked(egpu_ctx* ctx, const int32_t* free_core, const int32_t* free_mem, const int32_t* oversub, int32_t D);
 
 namespace egpu {
 // egpu_devhash.cu: the identity pipeline's stable LSD radix sort and exclusive scan, for the other

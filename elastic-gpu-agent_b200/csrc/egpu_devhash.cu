@@ -952,6 +952,7 @@ extern "C" int egpu_table_restore_flat(egpu_ctx* ctx, const char* ids_flat, cons
     }
     std::memcpy(out_table, table.data(), sizeof(int32_t) * 3 * static_cast<size_t>(D));
     if (out_status && n_sets) std::memcpy(out_status, status.data(), sizeof(int32_t) * static_cast<size_t>(n_sets));
-    if (flags & EGPU_RESTORE_INSTALL) return egpu_table_set_locked(ctx, table.data(), table.data() + D, D);
+    // the installed table keeps the oversubscription flags, as a committing batch's table does (DESIGN.md §2.4)
+    if (flags & EGPU_RESTORE_INSTALL) return egpu_table_set_locked(ctx, table.data(), table.data() + D, table.data() + 2 * D, D);
     return EGPU_OK;
 }

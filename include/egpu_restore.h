@@ -57,7 +57,9 @@ extern "C" {
 
 /* flags */
 #define EGPU_RESTORE_VERIFY  1 /* recompute every entry's identity and drop mismatches */
-#define EGPU_RESTORE_INSTALL 2 /* make the restored table the context's table (egpu_table_set) */
+#define EGPU_RESTORE_INSTALL 2 /* make the restored table the context's table, as egpu_table_set does, but
+                                  with out_table's oversubscription flags: they stay set until the next
+                                  egpu_table_set, as after a committing batch */
 
 /* Already-parsed form.  Entries = device-ID sets in the layout of egpu_device_hash_batch:
  *   ids_flat / id_offsets[n_ids + 1] / set_offsets[n_sets + 1]
