@@ -235,6 +235,24 @@ class BestFitAllocator:
         rc = self._lib.egpu_bestfit_batches_dev(self._h, arr, len(arr), L.F_INPUTS_READY if inputs_ready else 0, _stream(stream))
         self._check(rc, "egpu_bestfit_batches_dev")
 
+    @staticmethod
+    def make_packed_batches(batches):
+        """(d_req_packed, R, d_idx8, d_delta, d_table_out) tuples -> the egpu_batch array of a packed
+        multi-batch launch (d_req_mem stays NULL; pass it to bestfit_batches_packed_dev)."""
+        arr = (L.Batch * len(batches))()
+        for k, (p, R, i, dl, to) in enumerate(batches):
+            arr[k] = L.Batch(p or None, None, int(R), i or None, dl or None, to or None)
+        return arr
+
+    def bestfit_batches_packed_dev(self, batches, stream: int | None = None, inputs_ready: bool = False):
+        """egpu_bestfit_batches_dev with EGPU_F_PACKED: up to 64 batches of packed words (uint32 in, int8
+        indices out) scored against the current table in one launch.  `batches`: tuples as
+        make_packed_batches takes, or the array it returns."""
+        arr = batches if isinstance(batches, C.Array) else self.make_packed_batches(batches)
+        flags = L.F_PACKED | (L.F_INPUTS_READY if inputs_ready else 0)
+        rc = self._lib.egpu_bestfit_batches_dev(self._h, arr, len(arr), flags, _stream(stream))
+        self._check(rc, "egpu_bestfit_batches_dev")
+
     def bestfit_batches_shard_dev(self, batches, first_step: int, stream: int | None = None, inputs_ready: bool = False,
                                   apply: bool = False):
         """K sharded steps in one launch: batch k = exchange step first_step + k.  apply: the CTAs that complete a

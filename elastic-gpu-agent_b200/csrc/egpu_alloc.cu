@@ -67,20 +67,35 @@ template <int F>
 constexpr decltype(family_kernel<F, 0>()) kKernels[4] = {family_kernel<F, 0>(), family_kernel<F, 1>(), family_kernel<F, 2>(),
                                                          family_kernel<F, 3>()};
 
-// Resident CTAs per SM of family F's kernel for D devices.  The first use on a context opts in to
-// the kernel's dynamic shared memory and asks the occupancy.
-template <int F>
-int resident_ctas(egpu_ctx* ctx, int D, int* per_sm) {
-    const auto& k = kKernels<F>[d_bucket(D)];
-    int& n = ctx->scan_ctas_per_sm[F][d_bucket(D)];
-    if (n == 0) {
+// The packed multi-batch kernels: the same CTA sizes and shared memory as the int32 multi-batch
+// kernels of their bucket, and the same kernel types, so a launcher takes either table.
+template <int P, int B>
+constexpr auto packed_kernel() {
+    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
+    if constexpr (P == kPackedSortedMulti) return kernel(bestfit_sorted_packed_multi_kernel<DT, T>, T, sizeof(SnapSmem<DT, T>));
+    else return kernel(bestfit_lut_packed_multi_kernel<256>, 256, sizeof(LutSmem<256>));
+}
+template <int P>
+constexpr decltype(packed_kernel<P, 0>()) kPackedKernels[4] = {packed_kernel<P, 0>(), packed_kernel<P, 1>(), packed_kernel<P, 2>(),
+                                                               packed_kernel<P, 3>()};
+
+// Resident CTAs per SM of kernel k; `cached` is its entry in the context's occupancy cache.  The
+// first use on a context opts in to the kernel's dynamic shared memory and asks the occupancy.
+template <class Fn>
+int resident_ctas(egpu_ctx* ctx, const Kernel<Fn>& k, int& cached, int* per_sm) {
+    if (cached == 0) {
         EGPU_CUDA(ctx, cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(k.smem)));
         int m = 0;
         EGPU_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m, k.fn, k.threads, k.smem));
-        n = m < 1 ? 1 : m;
+        cached = m < 1 ? 1 : m;
     }
-    *per_sm = n;
+    *per_sm = cached;
     return EGPU_OK;
+}
+// ... of family F's kernel for D devices
+template <int F>
+int resident_ctas(egpu_ctx* ctx, int D, int* per_sm) {
+    return resident_ctas(ctx, kKernels<F>[d_bucket(D)], ctx->scan_ctas_per_sm[F][d_bucket(D)], per_sm);
 }
 
 // Programmatic dependent launch: the kernel may be scheduled while its predecessor on the stream
@@ -157,11 +172,11 @@ void table_image(DevState& h, const int32_t* free_core, const int32_t* free_mem,
 
 // ---- output ranges of the launches in flight (pipelined launches must not share outputs) ----
 using Range = egpu_ctx::Range;
-// the outputs of one batch: indices, demand sums, table'
-void batch_ranges(Range* r, const int32_t* idx, int64_t R, const void* delta, const int32_t* table_out, int D) {
+// the outputs of one batch: indices (idx_bytes each: int32, or int8 in the packed format), demand sums, table'
+void batch_ranges(Range* r, const void* idx, int64_t R, size_t idx_bytes, const void* delta, const int32_t* table_out, int D) {
     const uintptr_t pi = reinterpret_cast<uintptr_t>(idx), pd = reinterpret_cast<uintptr_t>(delta),
                     pt = reinterpret_cast<uintptr_t>(table_out);
-    r[0] = {pi, pi + static_cast<uintptr_t>(R) * sizeof(int32_t)};
+    r[0] = {pi, pi + static_cast<uintptr_t>(R) * idx_bytes};
     r[1] = {pd, pd + (pd ? sizeof(long long) * 2 * D : 0)};
     r[2] = {pt, pt + (pt ? sizeof(int32_t) * 3 * D : 0)};
 }
@@ -280,7 +295,7 @@ int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_
         if (rc != EGPU_OK) return rc;
     }
     Range mine[3];
-    batch_ranges(mine, a.idx, a.R, a.delta, a.table_out, ctx->D);
+    batch_ranges(mine, a.idx, a.R, sizeof(int32_t), a.delta, a.table_out, ctx->D);
     const int n_mine = prepare_ranges(mine, 3);
     if (n_mine < 0) return EGPU_ERR_INVALID;  // two of this launch's own outputs overlap
     const bool commit = (a.user_flags & EGPU_F_COMMIT) != 0;
@@ -349,12 +364,17 @@ int launch_snapshot(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_til
 // conditions of order_scan; a launch group never holds more than half of the epi_multi ring,
 // so the slots of everything that can be in flight are distinct.
 // push_base = first exchange step + 1 when every batch also pushes its demand vector to the peers.
+// EGPU_F_PACKED: the batches are in the packed format (d_req_core = words, d_out_idx = int8 indices)
+// and run in the packed twin of family F's kernel; everything else is the same launch.
 template <int F>
 int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cudaStream_t s, unsigned long long push_base) {
     constexpr bool lut = F == kScanLutMulti;
-    const auto& k = kKernels<F>[d_bucket(ctx->D)];
+    constexpr int P = lut ? kPackedLutMulti : kPackedSortedMulti;
+    const bool packed = (user_flags & EGPU_F_PACKED) != 0;
+    const int bucket = d_bucket(ctx->D);
+    const auto& k = packed ? kPackedKernels<P>[bucket] : kKernels<F>[bucket];
     int per_sm = 0;
-    int rc = resident_ctas<F>(ctx, ctx->D, &per_sm);
+    int rc = resident_ctas(ctx, k, packed ? ctx->packed_ctas_per_sm[P][bucket] : ctx->scan_ctas_per_sm[F][bucket], &per_sm);
     if (rc != EGPU_OK) return rc;
     if (lut) {
         rc = refresh_lut(ctx, s);
@@ -375,7 +395,7 @@ int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, 
         d.table_out = (push_base && !(user_flags & EGPU_F_APPLY)) ? nullptr : in.d_table_out;
         d.R = in.R;
         if (in.R > max_r) max_r = in.R;
-        batch_ranges(mine + 3 * b, d.idx, d.R, d.delta, d.table_out, ctx->D);
+        batch_ranges(mine + 3 * b, d.idx, d.R, packed ? sizeof(int8_t) : sizeof(int32_t), d.delta, d.table_out, ctx->D);
     }
     const int n_mine = prepare_ranges(mine, 3 * K);
     if (n_mine < 0) return EGPU_ERR_INVALID;  // two batches of one launch share an output: their order would be undefined
@@ -389,10 +409,12 @@ int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, 
     // many that takes.  The SMs do not stream at the same rate (in one wave the CTAs' exit times
     // spread over a third of the launch); with several waves of small CTAs the hardware scheduler
     // hands the next CTA to whichever SM frees a slot first.  Either way the CTAs are shared out
-    // evenly, the first `extra` batches get one more.  Measured on an H100: DESIGN.md 4.1e.
+    // evenly, the first `extra` batches get one more.  Packed rows are 5 bytes instead of 12, and
+    // their large batches want longer CTAs: 48 rows per thread (56 in the lookup scan) measured
+    // fastest of 20 / 28, 32 / 40 and 48 / 56.  Measured on an H100: DESIGN.md 4.1e.
     const int64_t nvec = max_r >> 2;
     const bool small = max_r < (512ll << 10);
-    const int64_t rpt = small ? ctx->multi_rpt : (lut ? 28 : 20);
+    const int64_t rpt = small ? ctx->multi_rpt : packed ? (lut ? 56 : 48) : (lut ? 28 : 20);
     const int64_t per_cta = static_cast<int64_t>(k.threads) * ((rpt + 3) / 4);
     int64_t tiles = (nvec + per_cta - 1) / per_cta;
     if (tiles < 1) tiles = 1;
@@ -632,7 +654,8 @@ extern "C" {
 
 // 1.4: + multi-batch launches, stateless query, start gate (additive)
 // 1.5: + egpu_preferred_allocation_batch (additive)
-int egpu_abi_version(void) { return 1005; }
+// 1.6: + EGPU_F_PACKED multi-batch launches (additive)
+int egpu_abi_version(void) { return 1006; }
 
 const char* egpu_strerror(int code) {
     switch (code) {
@@ -854,19 +877,23 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32
     return launch_snapshot(ctx, a, s);
 }
 
-static int check_batches(const egpu_batch* batches, int32_t K) {
+// packed: d_req_core holds the words and d_req_mem must be NULL, so that a packed batch handed over
+// without EGPU_F_PACKED (d_req_mem NULL, R > 0) is refused rather than read as int32 arrays
+static int check_batches(const egpu_batch* batches, int32_t K, bool packed = false) {
     if (!batches || K < 1 || K > EGPU_MAX_BATCHES) return EGPU_ERR_INVALID;
     for (int k = 0; k < K; ++k) {
         const egpu_batch& b = batches[k];
         if (b.R < 0 || b.R > kMaxRows) return EGPU_ERR_INVALID;
-        if (!rows_ok(b.R, {b.d_req_core, b.d_req_mem, b.d_out_idx})) return EGPU_ERR_INVALID;
+        if (packed ? (b.d_req_mem || !rows_ok(b.R, {b.d_req_core, b.d_out_idx}))
+                   : !rows_ok(b.R, {b.d_req_core, b.d_req_mem, b.d_out_idx}))
+            return EGPU_ERR_INVALID;
     }
     return EGPU_OK;
 }
 
 int egpu_bestfit_batches_dev(egpu_ctx* ctx, const egpu_batch* batches, int32_t K, int flags, void* stream) {
-    if (!ctx || (flags & ~EGPU_F_INPUTS_READY)) return EGPU_ERR_INVALID;
-    int rc = check_batches(batches, K);
+    if (!ctx || (flags & ~(EGPU_F_INPUTS_READY | EGPU_F_PACKED))) return EGPU_ERR_INVALID;
+    int rc = check_batches(batches, K, (flags & EGPU_F_PACKED) != 0);
     if (rc != EGPU_OK) return rc;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;

@@ -192,6 +192,10 @@ __device__ __forceinline__ void st_stream_v4(int32_t* p, const int4& v) {
                  "r"(v.y), "r"(v.z), "r"(v.w)
                  : "memory");
 }
+// four int8 indices of the packed format in one 32-bit store
+__device__ __forceinline__ void st_stream_u32(uint32_t* p, uint32_t v) {
+    asm volatile("st.global.L1::no_allocate.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
 
 // programmatic dependent launch (PDL): the next launch in the stream may start
 // once every CTA of this one has executed the trigger; `wait` blocks until the

@@ -372,23 +372,40 @@ __device__ __forceinline__ void snapshot_epilogue(SnapSmem<DT, THREADS>& s, DevS
                                    table_out, flags, ec, tile_sums);
 }
 
+// Packed wire format (include/egpu_alloc.h: EGPU_PACK_REQUEST): word core << 18 | mem -> the scans'
+// request word core << 24 | mem << 5.  A word >= 2^25 is not a request and becomes core 127, which
+// no table row holds (free_core <= 100): infeasible everywhere, as core 101..127 of a well-formed
+// word is.  Every packed scan decodes through here.
+__device__ __forceinline__ uint32_t packed_request_word(uint32_t pw) {
+    return (pw >> 25) ? (127u << 24) : (((pw & ~0x3FFFFu) << 6) | ((pw & 0x3FFFFu) << 5));
+}
+
+// Row format of a scan's input policy.  kRowsInt32: req_core / req_mem int32 arrays, out_idx int32.
+// kRowsPacked: req_core holds the packed uint32 words, req_mem is not read, out_idx holds int8
+// indices.  Both move one 128-bit request vector per 4 rows (packed: one load instead of two, and
+// one 32-bit store of four indices instead of a 128-bit one); the vector mapping, the ragged tail
+// and the demand sums are the same code.
+enum RowFormat { kRowsInt32, kRowsPacked };
+
 // The scan of one batch by one CTA: tile `tile` of `n_tiles` (in a single-batch launch the grid's
 // CTAs are the tiles; in a multi-batch launch every batch has its own run of tiles).
 // CONTIG = false: vectors are dealt round-robin over the batch's tiles (the product mapping).
 // CONTIG = true (prefix-commit mode): tile b scans the contiguous rows of "tile" b and the
 // epilogue leaves its per-device sums in tile_sums[b][*]; everything else is the same code.
 // Returns D.  Leaves the demand sums in s.hist; the caller runs snapshot_epilogue.
-template <int DT, int THREADS, bool CONTIG>
+template <int DT, int THREADS, bool CONTIG, RowFormat FMT = kRowsInt32>
 __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevState* __restrict__ st,
                                                 const int32_t* __restrict__ req_core, const int32_t* __restrict__ req_mem,
                                                 long long R, int32_t* __restrict__ out_idx, int tile_i, int n_tiles) {
+    constexpr bool packed = FMT == kRowsPacked;
     const int tid = threadIdx.x;
     const int lane = tid & 31;
     const int warp = tid >> 5;
     // 32-bit vector indices (the entry points keep R below 2^31): one IMAD.WIDE per address, 32-bit compares
-    const int4* __restrict__ vc = reinterpret_cast<const int4*>(req_core);
+    const int4* __restrict__ vc = reinterpret_cast<const int4*>(req_core);  // packed: 4 words per vector
     const int4* __restrict__ vm = reinterpret_cast<const int4*>(req_mem);
     int4* __restrict__ vo = reinterpret_cast<int4*>(out_idx);
+    uint32_t* __restrict__ vo8 = reinterpret_cast<uint32_t*>(out_idx);  // packed: 4 int8 indices per vector
     int nvec = static_cast<int>(R >> 2);  // CONTIG: end of this CTA's tile
     int stride = n_tiles * THREADS;
     int v = tile_i * THREADS + tid;
@@ -406,11 +423,11 @@ __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevSta
     bool has0 = v < nvec, has1 = (v + stride) < nvec;
     if (has0) {
         c0 = ld_stream_v4(vc + v);
-        m0 = ld_stream_v4(vm + v);
+        if constexpr (!packed) m0 = ld_stream_v4(vm + v);
     }
     if (has1) {
         c1 = ld_stream_v4(vc + (v + stride));
-        m1 = ld_stream_v4(vm + (v + stride));
+        if constexpr (!packed) m1 = ld_stream_v4(vm + (v + stride));
     }
 
     // sorted table rows: uniform loads straight into registers, no barrier
@@ -443,6 +460,17 @@ __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevSta
         r.w = decide(c.w, m.w);
         return r;
     };
+    // packed: the decode of bestfit_sorted_packed_kernel, four indices to one word
+    auto decide_word = [&](uint32_t pw) -> int32_t {
+        const uint32_t best = first_feasible<DT>(K, packed_request_word(pw), gx, gm);
+        const int32_t idx = tile[best];
+        hist_add<DT, THREADS>(s, warp, lane, idx, static_cast<int32_t>((pw >> 18) & 127u), static_cast<int32_t>(pw & 0x3FFFFu));
+        return idx;
+    };
+    auto decide4_words = [&](const int4& w) -> uint32_t {
+        return (static_cast<uint32_t>(decide_word(w.x)) & 0xffu) | ((static_cast<uint32_t>(decide_word(w.y)) & 0xffu) << 8) |
+               ((static_cast<uint32_t>(decide_word(w.z)) & 0xffu) << 16) | (static_cast<uint32_t>(decide_word(w.w)) << 24);
+    };
 
     while (has0) {
         const int vn = v + 2 * stride;
@@ -450,14 +478,19 @@ __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevSta
         int4 nc0 = make_int4(0, 0, 0, 0), nm0 = nc0, nc1 = nc0, nm1 = nc0;
         if (nhas0) {
             nc0 = ld_stream_v4(vc + vn);
-            nm0 = ld_stream_v4(vm + vn);
+            if constexpr (!packed) nm0 = ld_stream_v4(vm + vn);
         }
         if (nhas1) {
             nc1 = ld_stream_v4(vc + (vn + stride));
-            nm1 = ld_stream_v4(vm + (vn + stride));
+            if constexpr (!packed) nm1 = ld_stream_v4(vm + (vn + stride));
         }
-        st_stream_v4(vo + v, decide4(c0, m0));
-        if (has1) st_stream_v4(vo + (v + stride), decide4(c1, m1));
+        if constexpr (packed) {
+            st_stream_u32(vo8 + v, decide4_words(c0));
+            if (has1) st_stream_u32(vo8 + (v + stride), decide4_words(c1));
+        } else {
+            st_stream_v4(vo + v, decide4(c0, m0));
+            if (has1) st_stream_v4(vo + (v + stride), decide4(c1, m1));
+        }
         v = vn;
         has0 = nhas0;
         has1 = nhas1;
@@ -466,7 +499,10 @@ __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevSta
     // ragged tail: R % 4 rows, scalar (they are the LAST rows: in CONTIG mode they belong to the last tile)
     if (tile_i == (CONTIG ? n_tiles - 1 : 0) && tid < static_cast<int>(R & 3)) {
         const long long r = ((R >> 2) << 2) + tid;
-        out_idx[r] = decide(req_core[r], req_mem[r]);
+        if constexpr (packed)
+            reinterpret_cast<signed char*>(out_idx)[r] = static_cast<signed char>(decide_word(reinterpret_cast<const uint32_t*>(req_core)[r]));
+        else
+            out_idx[r] = decide(req_core[r], req_mem[r]);
     }
     return D;
 }
@@ -519,10 +555,10 @@ __device__ __forceinline__ void multi_cta_to_tile(int tiles_extra, int& batch, i
 // own CTAs as soon as that batch is done.  One launch latency, one ramp and one tail for K batches
 // instead of K: what the per-launch fixed cost (first DRAM touch, the epilogue's atomics) was
 // eating at R = 1 M, and the launch floor at R = 1 k .. 100 k.
-template <int DT, int THREADS>
-__global__ void __launch_bounds__(THREADS)
-bestfit_sorted_multi_kernel(DevState* __restrict__ st, const __grid_constant__ MultiArgs args, int tiles_extra, int flags,
-                            unsigned int slot_base, unsigned long long push_base) {
+// Body of the register-scan multi-batch kernels, in either row format.
+template <int DT, int THREADS, RowFormat FMT>
+__device__ __forceinline__ void sorted_multi_cta(DevState* __restrict__ st, const MultiArgs& args, int tiles_extra, int flags,
+                                                 unsigned int slot_base, unsigned long long push_base) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     auto& s = *reinterpret_cast<SnapSmem<DT, THREADS>*>(smem_raw);
     const bool late = (flags & kFlagLateWait) != 0;
@@ -532,7 +568,7 @@ bestfit_sorted_multi_kernel(DevState* __restrict__ st, const __grid_constant__ M
     int batch, tile_i, tiles;
     multi_cta_to_tile(tiles_extra, batch, tile_i, tiles);
     const BatchDesc b = args.b[batch];  // one read of the parameter space, then registers
-    const int D = sorted_scan_rows<DT, THREADS, false>(s, st, b.rc, b.rm, b.R, b.idx, tile_i, tiles);
+    const int D = sorted_scan_rows<DT, THREADS, false, FMT>(s, st, b.rc, b.rm, b.R, b.idx, tile_i, tiles);
     if (boundary) {
         pdl_wait();
         pdl_trigger();
@@ -546,6 +582,22 @@ bestfit_sorted_multi_kernel(DevState* __restrict__ st, const __grid_constant__ M
     ec.apply_now = (flags & kFlagApplyNow) != 0;
     snapshot_epilogue<DT, THREADS>(s, st, D, b.delta, b.table_out, flags, ec);
     if (late && !boundary) pdl_wait();
+}
+
+template <int DT, int THREADS>
+__global__ void __launch_bounds__(THREADS)
+bestfit_sorted_multi_kernel(DevState* __restrict__ st, const __grid_constant__ MultiArgs args, int tiles_extra, int flags,
+                            unsigned int slot_base, unsigned long long push_base) {
+    sorted_multi_cta<DT, THREADS, kRowsInt32>(st, args, tiles_extra, flags, slot_base, push_base);
+}
+
+// Packed multi-batch launch (egpu_bestfit_batches_dev with EGPU_F_PACKED): the same grid, tiles and
+// epilogue slots; every batch's rc holds R packed words and its idx R int8 indices (rm is NULL).
+template <int DT, int THREADS>
+__global__ void __launch_bounds__(THREADS)
+bestfit_sorted_packed_multi_kernel(DevState* __restrict__ st, const __grid_constant__ MultiArgs args, int tiles_extra, int flags,
+                                   unsigned int slot_base, unsigned long long push_base) {
+    sorted_multi_cta<DT, THREADS, kRowsPacked>(st, args, tiles_extra, flags, slot_base, push_base);
 }
 
 // Packed wire format (include/egpu_alloc.h: egpu_bestfit_batch_packed): one uint32 per request
@@ -596,9 +648,7 @@ bestfit_sorted_packed_kernel(DevState* __restrict__ st, const uint32_t* __restri
     __syncwarp();
 
     auto decide = [&](uint32_t pw) -> uint32_t {
-        // core << 18 | mem  ->  core << 24 | mem << 5; out-of-format words fail every guard
-        const uint32_t q = (pw >> 25) ? (127u << 24) : (((pw & ~0x3FFFFu) << 6) | ((pw & 0x3FFFFu) << 5));
-        const uint32_t best = first_feasible<DT>(K, q, gx, gm);
+        const uint32_t best = first_feasible<DT>(K, packed_request_word(pw), gx, gm);
         const int32_t idx = tile[best];
         hist_add<DT, THREADS>(s, warp, lane, idx, static_cast<int32_t>((pw >> 18) & 127u), static_cast<int32_t>(pw & 0x3FFFFu));
         return static_cast<uint32_t>(idx) & 0xffu;
@@ -806,19 +856,36 @@ struct LutSmem {
     alignas(16) uint32_t hist32[THREADS / 32][kLutCopies * kLutCopyStride];
 };
 
+// packed word -> the (core, mem) of the int32 form (a word >= 2^25: core 127, infeasible everywhere)
+__device__ __forceinline__ void unpack_request(uint32_t pw, int32_t& core, int32_t& mem) {
+    const uint32_t q = packed_request_word(pw);
+    core = static_cast<int32_t>(q >> 24);
+    mem = static_cast<int32_t>((q >> 5) & 0x3FFFFu);
+}
+
 // The lookup scan of one batch by one CTA (tile `tile_i` of `n_tiles`, as sorted_scan_rows).
 // Leaves the warp sums in sm.sWarpAcc; the caller synchronises and runs epilogue_publish.
-template <int THREADS, bool CONTIG>
+// Packed rows (FMT = kRowsPacked) are decoded into the int32 form as they are loaded; the trip is the
+// same two 4-row vectors per lane, so kLutFlushTrips holds for both formats.
+template <int THREADS, bool CONTIG, RowFormat FMT = kRowsInt32>
 __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __restrict__ st,
                                              const int32_t* __restrict__ req_core, const int32_t* __restrict__ req_mem,
                                              long long R, int32_t* __restrict__ out_idx, const DevLut* __restrict__ glut,
                                              int tile_i, int n_tiles) {
+    constexpr bool packed = FMT == kRowsPacked;
     const int tid = threadIdx.x;
     const int lane = tid & 31;
     const int warp = tid >> 5;
-    const int4* __restrict__ vc = reinterpret_cast<const int4*>(req_core);
+    const int4* __restrict__ vc = reinterpret_cast<const int4*>(req_core);  // packed: 4 words per vector
     const int4* __restrict__ vm = reinterpret_cast<const int4*>(req_mem);
     int4* __restrict__ vo = reinterpret_cast<int4*>(out_idx);
+    uint32_t* __restrict__ vo8 = reinterpret_cast<uint32_t*>(out_idx);  // packed: 4 int8 indices per vector
+    auto unpack4 = [](const int4& w, int4& c, int4& m) {
+        unpack_request(static_cast<uint32_t>(w.x), c.x, m.x);
+        unpack_request(static_cast<uint32_t>(w.y), c.y, m.y);
+        unpack_request(static_cast<uint32_t>(w.z), c.z, m.z);
+        unpack_request(static_cast<uint32_t>(w.w), c.w, m.w);
+    };
     int nvec = static_cast<int>(R >> 2);
     int stride = n_tiles * THREADS;
     int v = tile_i * THREADS + tid;
@@ -833,12 +900,20 @@ __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __r
     int4 c0 = make_int4(-1, -1, -1, -1), m0 = c0, c1 = c0, m1 = c0;
     bool has0 = v < nvec, has1 = (v + stride) < nvec;
     if (has0) {
-        c0 = ld_stream_v4(vc + v);
-        m0 = ld_stream_v4(vm + v);
+        if constexpr (packed) {
+            unpack4(ld_stream_v4(vc + v), c0, m0);
+        } else {
+            c0 = ld_stream_v4(vc + v);
+            m0 = ld_stream_v4(vm + v);
+        }
     }
     if (has1) {
-        c1 = ld_stream_v4(vc + (v + stride));
-        m1 = ld_stream_v4(vm + (v + stride));
+        if constexpr (packed) {
+            unpack4(ld_stream_v4(vc + (v + stride)), c1, m1);
+        } else {
+            c1 = ld_stream_v4(vc + (v + stride));
+            m1 = ld_stream_v4(vm + (v + stride));
+        }
     }
     // shared-memory tile of the lookup tables (15 KB, L2-resident source)
     {
@@ -930,19 +1005,32 @@ __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __r
         const bool nhas0 = vn < nvec, nhas1 = (vn + stride) < nvec;
         int4 nc0 = make_int4(-1, -1, -1, -1), nm0 = nc0, nc1 = nc0, nm1 = nc0;
         if (nhas0) {
-            nc0 = ld_stream_v4(vc + vn);
-            nm0 = ld_stream_v4(vm + vn);
+            if constexpr (packed) {
+                unpack4(ld_stream_v4(vc + vn), nc0, nm0);
+            } else {
+                nc0 = ld_stream_v4(vc + vn);
+                nm0 = ld_stream_v4(vm + vn);
+            }
         }
         if (nhas1) {
-            nc1 = ld_stream_v4(vc + (vn + stride));
-            nm1 = ld_stream_v4(vm + (vn + stride));
+            if constexpr (packed) {
+                unpack4(ld_stream_v4(vc + (vn + stride)), nc1, nm1);
+            } else {
+                nc1 = ld_stream_v4(vc + (vn + stride));
+                nm1 = ld_stream_v4(vm + (vn + stride));
+            }
         }
         // no branch around the lookups (lanes past the end carry infeasible requests): the eight
         // requests of a trip overlap their dependent reads
         const uint4 d0 = lookup4(c0, m0);
         const uint4 d1 = lookup4(c1, m1);
-        if (has0) st_stream_v4(vo + v, as_idx4(d0));
-        if (has1) st_stream_v4(vo + (v + stride), as_idx4(d1));
+        if constexpr (packed) {  // devices 0..63 or 0xFF: already the int8 bytes
+            if (has0) st_stream_u32(vo8 + v, d0.x | (d0.y << 8) | (d0.z << 16) | (d0.w << 24));
+            if (has1) st_stream_u32(vo8 + (v + stride), d1.x | (d1.y << 8) | (d1.z << 16) | (d1.w << 24));
+        } else {
+            if (has0) st_stream_v4(vo + v, as_idx4(d0));
+            if (has1) st_stream_v4(vo + (v + stride), as_idx4(d1));
+        }
         add4(d0, c0, m0);
         add4(d1, c1, m1);
         v = vn;
@@ -953,10 +1041,18 @@ __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __r
     if (tile_i == (CONTIG ? n_tiles - 1 : 0) && warp == 0) {  // ragged tail: R % 4 rows (the last ones), lanes 0..2 of warp 0
         const bool mine = lane < static_cast<int>(R & 3);
         const long long r = ((R >> 2) << 2) + lane;
-        const int32_t c = mine ? req_core[r] : -1, m = mine ? req_mem[r] : -1;
-        const uint32_t dev = lookup(c, m);
-        if (mine) out_idx[r] = static_cast<int32_t>(static_cast<int8_t>(dev));
-        add1(dev, c, m);
+        if constexpr (packed) {
+            int32_t c = -1, m = -1;
+            if (mine) unpack_request(reinterpret_cast<const uint32_t*>(req_core)[r], c, m);
+            const uint32_t dev = lookup(c, m);
+            if (mine) reinterpret_cast<signed char*>(out_idx)[r] = static_cast<signed char>(dev);
+            add1(dev, c, m);
+        } else {
+            const int32_t c = mine ? req_core[r] : -1, m = mine ? req_mem[r] : -1;
+            const uint32_t dev = lookup(c, m);
+            if (mine) out_idx[r] = static_cast<int32_t>(static_cast<int8_t>(dev));
+            add1(dev, c, m);
+        }
     }
     flush32();
 #pragma unroll
@@ -991,11 +1087,10 @@ bestfit_lut_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_co
     if (late && !boundary) pdl_wait();
 }
 
-// Multi-batch form of the lookup scan (see bestfit_sorted_multi_kernel).
-template <int THREADS>
-__global__ void __launch_bounds__(THREADS)
-bestfit_lut_multi_kernel(DevState* __restrict__ st, const __grid_constant__ MultiArgs args, int tiles_extra, int flags,
-                         unsigned int slot_base, unsigned long long push_base, const DevLut* __restrict__ glut) {
+// Multi-batch form of the lookup scan (see bestfit_sorted_multi_kernel), in either row format.
+template <int THREADS, RowFormat FMT>
+__device__ __forceinline__ void lut_multi_cta(DevState* __restrict__ st, const MultiArgs& args, int tiles_extra, int flags,
+                                              unsigned int slot_base, unsigned long long push_base, const DevLut* __restrict__ glut) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     auto& sm = *reinterpret_cast<LutSmem<THREADS>*>(smem_raw);
     const bool late = (flags & kFlagLateWait) != 0;
@@ -1005,7 +1100,7 @@ bestfit_lut_multi_kernel(DevState* __restrict__ st, const __grid_constant__ Mult
     int batch, tile_i, tiles;
     multi_cta_to_tile(tiles_extra, batch, tile_i, tiles);
     const BatchDesc b = args.b[batch];
-    const int D = lut_scan_rows<THREADS, false>(sm, st, b.rc, b.rm, b.R, b.idx, glut, tile_i, tiles);
+    const int D = lut_scan_rows<THREADS, false, FMT>(sm, st, b.rc, b.rm, b.R, b.idx, glut, tile_i, tiles);
     if (boundary) {
         pdl_wait();
         pdl_trigger();
@@ -1021,6 +1116,21 @@ bestfit_lut_multi_kernel(DevState* __restrict__ st, const __grid_constant__ Mult
     epilogue_publish<THREADS / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, sm.sFc, sm.sFm, sm.sPosDev, &sm.sLast, st, D,
                                    b.delta, b.table_out, flags, ec);
     if (late && !boundary) pdl_wait();
+}
+
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS)
+bestfit_lut_multi_kernel(DevState* __restrict__ st, const __grid_constant__ MultiArgs args, int tiles_extra, int flags,
+                         unsigned int slot_base, unsigned long long push_base, const DevLut* __restrict__ glut) {
+    lut_multi_cta<THREADS, kRowsInt32>(st, args, tiles_extra, flags, slot_base, push_base, glut);
+}
+
+// Packed multi-batch launch of the lookup scan (see bestfit_sorted_packed_multi_kernel).
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS)
+bestfit_lut_packed_multi_kernel(DevState* __restrict__ st, const __grid_constant__ MultiArgs args, int tiles_extra, int flags,
+                                unsigned int slot_base, unsigned long long push_base, const DevLut* __restrict__ glut) {
+    lut_multi_cta<THREADS, kRowsPacked>(st, args, tiles_extra, flags, slot_base, push_base, glut);
 }
 
 // Multi-GPU step 2: table' = table - sum over ranks of their demand vectors.

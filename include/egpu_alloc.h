@@ -111,6 +111,9 @@ extern "C" {
                                     no second stream.  Never commits.  Every rank must issue the same launch; start the
                                     ranks together (egpu_peer_gate_dev) or the wait is as long as their skew. */
 
+#define EGPU_F_PACKED       16   /* egpu_bestfit_batches_dev only: every batch is in the packed format of
+                                    egpu_bestfit_batch_packed (5 bytes per decision instead of 12); see there. */
+
 /* kernel variants for the snapshot scan (egpu_set_variant) */
 #define EGPU_VARIANT_AUTO    0   /* SORTED for D <= 16, LUT above */
 #define EGPU_VARIANT_GRID    1   /* direct (device x request) score grid, min over packed keys */
@@ -141,7 +144,7 @@ int  egpu_set_variant(egpu_ctx* ctx, int variant);
 /* ABI version: major*1000 + minor.  Minor revisions only add entry points (1.1 placement
  * restore, 1.2 prefix-commit over row shards, 1.3 rounds, 1.4 multi-batch launches, stateless query,
  * start gate, host registration, 1.5 preferred allocation for many container requests from flat ID
- * buffers); a caller built against 1.0 keeps working. */
+ * buffers, 1.6 EGPU_F_PACKED multi-batch launches); a caller built against 1.0 keeps working. */
 int  egpu_abi_version(void);
 
 /* ---- capacity table --------------------------------------------------- */
@@ -234,13 +237,27 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core,
  * launch; at R <= 100 k it is nearly all of it).  Asynchronous on `stream`.  flags:
  * EGPU_F_INPUTS_READY only (a multi-batch launch never commits: install a table' with
  * egpu_table_set or a committing single-batch call).  Outputs of different batches must not
- * overlap (EGPU_ERR_INVALID).  Batches may have different R (R = 0 allowed). */
+ * overlap (EGPU_ERR_INVALID).  Batches may have different R (R = 0 allowed).
+ *
+ * Packed batches (flags EGPU_F_PACKED, alone or with EGPU_F_INPUTS_READY): every batch of the call
+ * is in the wire format of egpu_bestfit_batch_packed, and the fields are read as
+ *   d_req_core   R packed words (const uint32_t* cast to the field's type), 16-byte aligned;
+ *   d_req_mem    must be NULL (EGPU_ERR_INVALID otherwise);
+ *   d_out_idx    R int8 indices (int8_t* cast to the field's type), 16-byte aligned;
+ *   d_delta, d_table_out  as above.
+ * Words >= 2^25 and core 101..127 are infeasible requests (-1).  Everything else is as for int32
+ * batches - K <= 64, ragged and empty batches, never commits, EGPU_F_INPUTS_READY pipelining (packed
+ * and int32 launches may follow each other in one pipelined stream), EGPU_ERR_STATE under
+ * EGPU_VARIANT_GRID - and outputs of different batches must not overlap: an index array covers R
+ * bytes.  Without the flag a batch with R > 0 and a NULL d_req_mem is refused, so packed batches
+ * handed over without it are never read as int32 arrays.  egpu_bestfit_batches_shard_dev refuses
+ * the flag. */
 #define EGPU_MAX_BATCHES 64
 typedef struct egpu_batch {
-    const int32_t* d_req_core;
-    const int32_t* d_req_mem;
+    const int32_t* d_req_core;   /* EGPU_F_PACKED: the packed words */
+    const int32_t* d_req_mem;    /* EGPU_F_PACKED: NULL */
     int64_t        R;
-    int32_t*       d_out_idx;
+    int32_t*       d_out_idx;    /* EGPU_F_PACKED: int8 indices */
     int64_t*       d_delta;      /* int64[2*D] or NULL */
     int32_t*       d_table_out;  /* int32[3*D] or NULL */
 } egpu_batch;
