@@ -79,6 +79,18 @@ template <int P>
 constexpr decltype(packed_kernel<P, 0>()) kPackedKernels[4] = {packed_kernel<P, 0>(), packed_kernel<P, 1>(), packed_kernel<P, 2>(),
                                                                packed_kernel<P, 3>()};
 
+// The packed prefix-commit scans: twins of the CONTIG kernels of their bucket, same CTA sizes,
+// shared memory and kernel types.
+template <int P, int B>
+constexpr auto packed_contig_kernel() {
+    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
+    if constexpr (P == kPackedSortedContig) return kernel(bestfit_sorted_packed_contig_kernel<DT, T>, T, sizeof(SnapSmem<DT, T>));
+    else return kernel(bestfit_lut_packed_contig_kernel<256>, 256, sizeof(LutSmem<256>));
+}
+template <int P>
+constexpr decltype(packed_contig_kernel<P, 0>()) kPackedContigKernels[4] = {packed_contig_kernel<P, 0>(), packed_contig_kernel<P, 1>(),
+                                                                            packed_contig_kernel<P, 2>(), packed_contig_kernel<P, 3>()};
+
 // Resident CTAs per SM of kernel k; `cached` is its entry in the context's occupancy cache.  The
 // first use on a context opts in to the kernel's dynamic shared memory and asks the occupancy.
 template <class Fn>
@@ -281,21 +293,24 @@ struct Snapshot {
     unsigned long long push_step_plus1 = 0;      // exchange step + 1 the epilogue pushes the demand to, 0 = none
     int lag = 0;                                 // lagged apply (egpu_bestfit_batch_shard_lag_dev)
     bool contig = false;                         // prefix-commit: contiguous tiles, per-tile sums in ctx->d_tile_sums
+    bool packed = false;                         // contig only: rc = packed words, rm unused, idx = int8 indices
 };
 
 template <int F>
 int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_tiles_out) {
     constexpr bool lut = F == kScanLut || F == kScanLutContig, grid_variant = F == kScanGrid;
-    const auto& k = kKernels<F>[d_bucket(ctx->D)];
+    constexpr int P = lut ? kPackedLutContig : kPackedSortedContig;
+    const int bucket = d_bucket(ctx->D);
+    const auto& k = a.packed ? kPackedContigKernels<P>[bucket] : kKernels<F>[bucket];
     int per_sm = 0;
-    int rc = resident_ctas<F>(ctx, ctx->D, &per_sm);
+    int rc = resident_ctas(ctx, k, a.packed ? ctx->packed_contig_ctas_per_sm[P][bucket] : ctx->scan_ctas_per_sm[F][bucket], &per_sm);
     if (rc != EGPU_OK) return rc;
     if (lut) {
         rc = refresh_lut(ctx, s);
         if (rc != EGPU_OK) return rc;
     }
     Range mine[3];
-    batch_ranges(mine, a.idx, a.R, sizeof(int32_t), a.delta, a.table_out, ctx->D);
+    batch_ranges(mine, a.idx, a.R, a.packed ? sizeof(int8_t) : sizeof(int32_t), a.delta, a.table_out, ctx->D);
     const int n_mine = prepare_ranges(mine, 3);
     if (n_mine < 0) return EGPU_ERR_INVALID;  // two of this launch's own outputs overlap
     const bool commit = (a.user_flags & EGPU_F_COMMIT) != 0;
@@ -454,27 +469,37 @@ int launch_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cud
 
 // First half of a prefix-commit (spec 2.5): the CONTIG scan, which neither commits nor returns
 // delta / table' (its sums are the uncapped ones); push_step_plus1 as in Snapshot.  Returns the
-// PrefixOut the next kernels fill and the tile count of the scan.
-int prefix_scan(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx,
+// PrefixOut the next kernels fill and the tile count of the scan.  kRowsPacked: d_rc holds the
+// packed words (d_rm unused) and d_idx receives int8 indices.
+int prefix_scan(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx, RowFormat fmt,
                 unsigned long long push_step_plus1, cudaStream_t s, PrefixOut** pf, int* n_tiles) {
     if (!ctx->d_prefix_out) EGPU_CUDA(ctx, cudaMalloc(&ctx->d_prefix_out, sizeof(PrefixOut) + sizeof(long long) * 2 * kMaxD));
     *pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
     Snapshot a{d_rc, d_rm, R, d_idx};
     a.push_step_plus1 = push_step_plus1;
     a.contig = true;
+    a.packed = fmt == kRowsPacked;
     return launch_snapshot(ctx, a, s, n_tiles);
 }
 
 // Prefix-commit pipeline on device buffers (spec 2.5): CONTIG scan -> per-device cut ->
-// rewrite of the deferred indices -> delta / table' of the committed rows only.
+// rewrite of the deferred indices -> delta / table' of the committed rows only.  Rows in
+// either format (see prefix_scan); the cut and the rewrite read the scan's format.
 int launch_prefix_commit(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx,
-                         long long* d_delta, int32_t* d_table_out, int user_flags, cudaStream_t s) {
+                         long long* d_delta, int32_t* d_table_out, int user_flags, cudaStream_t s, RowFormat fmt = kRowsInt32) {
     PrefixOut* pf = nullptr;
     int n_tiles = 0;
-    const int rc = prefix_scan(ctx, d_rc, d_rm, R, d_idx, 0, s, &pf, &n_tiles);
+    const int rc = prefix_scan(ctx, d_rc, d_rm, R, d_idx, fmt, 0, s, &pf, &n_tiles);
     if (rc != EGPU_OK) return rc;
-    prefix_cut_kernel<<<ctx->D, 256, 0, s>>>(ctx->d_state, d_idx, d_rc, d_rm, R, n_tiles, ctx->d_tile_sums, pf);
-    prefix_apply_kernel<<<capped_blocks(ctx, R, 1024), 256, 0, s>>>(pf, ctx->D, R, d_idx);
+    if (fmt == kRowsPacked) {
+        signed char* idx8 = reinterpret_cast<signed char*>(d_idx);
+        prefix_cut_packed_kernel<<<ctx->D, 256, 0, s>>>(ctx->d_state, idx8, reinterpret_cast<const uint32_t*>(d_rc), R, n_tiles,
+                                                        ctx->d_tile_sums, pf);
+        prefix_apply_packed_kernel<<<capped_blocks(ctx, R, 1024), 256, 0, s>>>(pf, ctx->D, R, idx8);
+    } else {
+        prefix_cut_kernel<<<ctx->D, 256, 0, s>>>(ctx->d_state, d_idx, d_rc, d_rm, R, n_tiles, ctx->d_tile_sums, pf);
+        prefix_apply_kernel<<<capped_blocks(ctx, R, 1024), 256, 0, s>>>(pf, ctx->D, R, d_idx);
+    }
     prefix_finalize_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, pf, d_delta, d_table_out, (user_flags & EGPU_F_COMMIT) ? 1 : 0);
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 3;
@@ -563,7 +588,7 @@ int launch_prefix_commit_shard(egpu_ctx* ctx, const int32_t* d_rc, const int32_t
                                long long* d_delta, int32_t* d_table_out, int user_flags, uint64_t step, cudaStream_t s) {
     PrefixOut* pf = nullptr;
     int n_tiles = 0;
-    const int rc = prefix_scan(ctx, d_rc, d_rm, R, d_idx, step + 1, s, &pf, &n_tiles);
+    const int rc = prefix_scan(ctx, d_rc, d_rm, R, d_idx, kRowsInt32, step + 1, s, &pf, &n_tiles);
     if (rc != EGPU_OK) return rc;
     long long* base = reinterpret_cast<long long*>(pf + 1);
     prefix_base_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, step + 1, base);
@@ -655,7 +680,8 @@ extern "C" {
 // 1.4: + multi-batch launches, stateless query, start gate (additive)
 // 1.5: + egpu_preferred_allocation_batch (additive)
 // 1.6: + EGPU_F_PACKED multi-batch launches (additive)
-int egpu_abi_version(void) { return 1006; }
+// 1.7: + EGPU_F_PACKED prefix-commit on egpu_bestfit_batch / egpu_bestfit_batch_dev (additive)
+int egpu_abi_version(void) { return 1007; }
 
 const char* egpu_strerror(int code) {
     switch (code) {
@@ -865,14 +891,20 @@ int egpu_host_unregister(egpu_ctx* ctx, void* p) {
 int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                            int32_t* d_out_idx, int64_t* d_delta, int32_t* d_table_out, int flags,
                            void* stream) {
-    if (!ctx || R < 0 || !rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
+    // EGPU_F_PACKED: prefix-commit only, d_req_core = words, d_req_mem NULL, d_out_idx = int8 indices.
+    // Without it a NULL d_req_mem (R > 0) stays refused, so words are never read as int32 arrays.
+    const bool packed = (flags & EGPU_F_PACKED) != 0;
+    if (!ctx || R < 0) return EGPU_ERR_INVALID;
+    if (packed ? (!(flags & EGPU_F_PREFIX_COMMIT) || d_req_mem || !rows_ok(R, {d_req_core, d_out_idx}))
+               : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
+        return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
     if (flags & EGPU_F_PREFIX_COMMIT)
         return launch_prefix_commit(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out,
-                                    flags, s);
+                                    flags, s, packed ? kRowsPacked : kRowsInt32);
     Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags};
     return launch_snapshot(ctx, a, s);
 }
@@ -998,8 +1030,13 @@ int egpu_bestfit_query(egpu_ctx* ctx, const int32_t* free_core, const int32_t* f
 
 int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* req_mem, int64_t R,
                        int32_t* out_idx, int64_t* out_delta_core, int64_t* out_delta_mem, int commit) {
+    // `commit` carries EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT, and EGPU_F_PACKED with the latter:
+    // req_core = words, req_mem NULL, out_idx = int8 indices (as in egpu_bestfit_batch_dev)
+    const bool prefix = (commit & EGPU_F_PREFIX_COMMIT) != 0;
+    const bool packed = (commit & EGPU_F_PACKED) != 0;
     if (!ctx || R < 0) return EGPU_ERR_INVALID;
-    if (R > 0 && (!req_core || !req_mem || !out_idx)) return EGPU_ERR_INVALID;
+    if (packed ? (!prefix || req_mem || (R > 0 && (!req_core || !out_idx))) : (R > 0 && (!req_core || !req_mem || !out_idx)))
+        return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, nullptr, &s);
@@ -1010,10 +1047,9 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     // cudaHostRegister) and 16-byte aligned, the scan reads the requests and writes
     // the indices straight across PCIe — one launch, no staging in HBM, reads and
     // writes overlap on the full-duplex link.  Demand sums land in pinned memory too.
-    const int32_t* zc = R > 0 ? static_cast<const int32_t*>(mapped_alias(req_core)) : nullptr;
-    const int32_t* zm = R > 0 ? static_cast<const int32_t*>(mapped_alias(req_mem)) : nullptr;
-    int32_t* zi = R > 0 ? static_cast<int32_t*>(mapped_alias(out_idx)) : nullptr;
-    const bool prefix = (commit & EGPU_F_PREFIX_COMMIT) != 0;  // `commit` carries EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT
+    const int32_t* zc = R > 0 && !prefix ? static_cast<const int32_t*>(mapped_alias(req_core)) : nullptr;
+    const int32_t* zm = R > 0 && !prefix ? static_cast<const int32_t*>(mapped_alias(req_mem)) : nullptr;
+    int32_t* zi = R > 0 && !prefix ? static_cast<int32_t*>(mapped_alias(out_idx)) : nullptr;
     if (!prefix && zc && zm && zi && aligned16(zc) && aligned16(zm) && aligned16(zi) && !ctx->no_zero_copy) {
         // 64 rows per thread: few CTAs, many trips, so reads of later rows and writes of
         // earlier ones are on the link at the same time (PCIe is full duplex)
@@ -1025,14 +1061,16 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     } else {
         rc = ensure_staging(ctx, R > 0 ? R : 1);
         if (rc != EGPU_OK) return rc;
-        if (R > 0) {
+        if (R > 0) {  // packed: 4 bytes per row in (the words, in d_req_core), 1 out
             EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-            EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
+            if (!packed) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
         }
-        rc = prefix ? launch_prefix_commit(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, user_flags, s)
+        rc = prefix ? launch_prefix_commit(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, user_flags, s,
+                                           packed ? kRowsPacked : kRowsInt32)
                     : launch_snapshot(ctx, Snapshot{ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, user_flags}, s);
         if (rc != EGPU_OK) return rc;
-        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, sizeof(int32_t) * R, cudaMemcpyDeviceToHost, s));
+        const size_t idx_bytes = packed ? sizeof(int8_t) : sizeof(int32_t);
+        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, idx_bytes * R, cudaMemcpyDeviceToHost, s));
         EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
         EGPU_CUDA(ctx, cudaStreamSynchronize(s));
     }

@@ -507,6 +507,28 @@ __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevSta
     return D;
 }
 
+// Body of the single-batch register-scan kernels, in either row format.
+template <int DT, int THREADS, bool CONTIG, RowFormat FMT>
+__device__ __forceinline__ void sorted_snapshot_cta(DevState* __restrict__ st, const int32_t* __restrict__ req_core,
+                                                    const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
+                                                    long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags,
+                                                    unsigned long long slot_step, unsigned long long* __restrict__ tile_sums) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& s = *reinterpret_cast<SnapSmem<DT, THREADS>*>(smem_raw);
+    const bool late = (flags & kFlagLateWait) != 0;
+    const bool boundary = (flags & kFlagBoundary) != 0;
+    if (!late) pdl_wait();  // predecessor may have produced our inputs or changed the table
+    if ((flags & kFlagEarlyTrigger) && !boundary) pdl_trigger();
+    const int D = sorted_scan_rows<DT, THREADS, CONTIG, FMT>(s, st, req_core, req_mem, R, out_idx, static_cast<int>(blockIdx.x),
+                                                             static_cast<int>(gridDim.x));
+    if (boundary) {  // everything older must be complete before the next group may start
+        pdl_wait();
+        pdl_trigger();
+    }
+    snapshot_epilogue<DT, THREADS>(s, st, D, delta_out, table_out, flags, epi_from_word(st, slot_step), CONTIG ? tile_sums : nullptr);
+    if (late && !boundary) pdl_wait();  // do not complete before the predecessor has: keeps stream order transitive
+}
+
 template <int DT, int THREADS, bool CONTIG = false>
 __global__ void __launch_bounds__(THREADS)  // (forcing 5 CTAs/SM = 48 registers was measured slower: ptxas then puts
                                             //  more of the adds on the ALU pipe; same-box A/B, DESIGN.md 7.2)
@@ -514,20 +536,21 @@ bestfit_sorted_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req
                       const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
                       long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags, unsigned long long slot_step,
                       unsigned long long* __restrict__ tile_sums) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    auto& s = *reinterpret_cast<SnapSmem<DT, THREADS>*>(smem_raw);
-    const bool late = (flags & kFlagLateWait) != 0;
-    const bool boundary = (flags & kFlagBoundary) != 0;
-    if (!late) pdl_wait();  // predecessor may have produced our inputs or changed the table
-    if ((flags & kFlagEarlyTrigger) && !boundary) pdl_trigger();
-    const int D = sorted_scan_rows<DT, THREADS, CONTIG>(s, st, req_core, req_mem, R, out_idx, static_cast<int>(blockIdx.x),
-                                                        static_cast<int>(gridDim.x));
-    if (boundary) {  // everything older must be complete before the next group may start
-        pdl_wait();
-        pdl_trigger();
-    }
-    snapshot_epilogue<DT, THREADS>(s, st, D, delta_out, table_out, flags, epi_from_word(st, slot_step), CONTIG ? tile_sums : nullptr);
-    if (late && !boundary) pdl_wait();  // do not complete before the predecessor has: keeps stream order transitive
+    sorted_snapshot_cta<DT, THREADS, CONTIG, kRowsInt32>(st, req_core, req_mem, R, out_idx, delta_out, table_out, flags, slot_step,
+                                                         tile_sums);
+}
+
+// Packed prefix-commit scan (egpu_bestfit_batch[_dev] with EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT): the
+// CONTIG tiles and per-tile sums of bestfit_sorted_kernel<DT, THREADS, true>; req_core holds R packed
+// words, req_mem is not read and out_idx receives R int8 indices.
+template <int DT, int THREADS>
+__global__ void __launch_bounds__(THREADS)
+bestfit_sorted_packed_contig_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_core,
+                                    const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
+                                    long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags,
+                                    unsigned long long slot_step, unsigned long long* __restrict__ tile_sums) {
+    sorted_snapshot_cta<DT, THREADS, true, kRowsPacked>(st, req_core, req_mem, R, out_idx, delta_out, table_out, flags, slot_step,
+                                                        tile_sums);
 }
 
 // Grid of a multi-batch launch: the first `extra` batches have base + 1 tiles (CTAs), the others
@@ -1063,19 +1086,20 @@ __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __r
     return D;
 }
 
-template <int THREADS, bool CONTIG = false>
-__global__ void __launch_bounds__(THREADS)
-bestfit_lut_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_core,
-                   const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
-                   long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags, unsigned long long slot_step,
-                   const DevLut* __restrict__ glut, unsigned long long* __restrict__ tile_sums) {
+// Body of the single-batch lookup-scan kernels, in either row format.
+template <int THREADS, bool CONTIG, RowFormat FMT>
+__device__ __forceinline__ void lut_snapshot_cta(DevState* __restrict__ st, const int32_t* __restrict__ req_core,
+                                                 const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
+                                                 long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags,
+                                                 unsigned long long slot_step, const DevLut* __restrict__ glut,
+                                                 unsigned long long* __restrict__ tile_sums) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     auto& sm = *reinterpret_cast<LutSmem<THREADS>*>(smem_raw);
     const bool late = (flags & kFlagLateWait) != 0;
     const bool boundary = (flags & kFlagBoundary) != 0;
     if (!late) pdl_wait();
     if ((flags & kFlagEarlyTrigger) && !boundary) pdl_trigger();
-    const int D = lut_scan_rows<THREADS, CONTIG>(sm, st, req_core, req_mem, R, out_idx, glut, static_cast<int>(blockIdx.x),
+    const int D = lut_scan_rows<THREADS, CONTIG, FMT>(sm, st, req_core, req_mem, R, out_idx, glut, static_cast<int>(blockIdx.x),
                                                       static_cast<int>(gridDim.x));
     if (boundary) {
         pdl_wait();
@@ -1085,6 +1109,28 @@ bestfit_lut_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_co
     epilogue_publish<THREADS / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, sm.sFc, sm.sFm, sm.sPosDev, &sm.sLast, st, D,
                                    delta_out, table_out, flags, epi_from_word(st, slot_step), CONTIG ? tile_sums : nullptr);
     if (late && !boundary) pdl_wait();
+}
+
+template <int THREADS, bool CONTIG = false>
+__global__ void __launch_bounds__(THREADS)
+bestfit_lut_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_core,
+                   const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
+                   long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags, unsigned long long slot_step,
+                   const DevLut* __restrict__ glut, unsigned long long* __restrict__ tile_sums) {
+    lut_snapshot_cta<THREADS, CONTIG, kRowsInt32>(st, req_core, req_mem, R, out_idx, delta_out, table_out, flags, slot_step, glut,
+                                                  tile_sums);
+}
+
+// Packed prefix-commit scan in the lookup scan (see bestfit_sorted_packed_contig_kernel).
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS)
+bestfit_lut_packed_contig_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_core,
+                                 const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
+                                 long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags,
+                                 unsigned long long slot_step, const DevLut* __restrict__ glut,
+                                 unsigned long long* __restrict__ tile_sums) {
+    lut_snapshot_cta<THREADS, true, kRowsPacked>(st, req_core, req_mem, R, out_idx, delta_out, table_out, flags, slot_step, glut,
+                                                 tile_sums);
 }
 
 // Multi-batch form of the lookup scan (see bestfit_sorted_multi_kernel), in either row format.
@@ -1317,11 +1363,24 @@ __device__ __forceinline__ void block_scan2(unsigned long long& a, unsigned long
     b = ib - b + wb;
 }
 
-__global__ void __launch_bounds__(256)
-prefix_cut_kernel(const DevState* __restrict__ st, const int32_t* __restrict__ idx, const int32_t* __restrict__ req_core,
-                  const int32_t* __restrict__ req_mem, long long R, int n_tiles,
-                  const unsigned long long* __restrict__ tile_sums, PrefixOut* __restrict__ out,
-                  const long long* __restrict__ base = nullptr /* [2][kMaxD]: demand of the lower ranks' rows */) {
+// The cut of device blockIdx.x, in either row format of the scan before it (kRowsPacked: idx holds
+// int8 indices, req_core the packed words, req_mem is not read; a row that chose a device is
+// feasible, hence a well-formed word).
+template <RowFormat FMT>
+__device__ __forceinline__ void prefix_cut_cta(const DevState* __restrict__ st, const int32_t* __restrict__ idx,
+                                               const int32_t* __restrict__ req_core, const int32_t* __restrict__ req_mem,
+                                               long long R, int n_tiles, const unsigned long long* __restrict__ tile_sums,
+                                               PrefixOut* __restrict__ out, const long long* __restrict__ base) {
+    constexpr bool packed = FMT == kRowsPacked;
+    const signed char* __restrict__ idx8 = reinterpret_cast<const signed char*>(idx);
+    const uint32_t* __restrict__ words = reinterpret_cast<const uint32_t*>(req_core);
+    auto chose = [&](long long r) -> int { return packed ? static_cast<int>(idx8[r]) : static_cast<int>(idx[r]); };
+    auto core_of = [&](long long r) -> unsigned long long {
+        return packed ? static_cast<unsigned long long>((words[r] >> 18) & 127u) : static_cast<unsigned long long>(req_core[r]);
+    };
+    auto mem_of = [&](long long r) -> unsigned long long {
+        return packed ? static_cast<unsigned long long>(words[r] & 0x3FFFFu) : static_cast<unsigned long long>(req_mem[r]);
+    };
     constexpr int T = 256;
     __shared__ unsigned long long sh[2 * (T / 32)];
     __shared__ long long sCutTile, sCutRow;
@@ -1399,9 +1458,9 @@ prefix_cut_kernel(const DevState* __restrict__ st, const int32_t* __restrict__ i
         unsigned long long c = 0, m = 0;
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-            const bool mine = (r + k) < row_hi && idx[r + k] == d;
-            c4[k] = mine ? static_cast<unsigned long long>(req_core[r + k]) : 0ull;
-            m4[k] = mine ? static_cast<unsigned long long>(req_mem[r + k]) : 0ull;
+            const bool mine = (r + k) < row_hi && chose(r + k) == d;
+            c4[k] = mine ? core_of(r + k) : 0ull;
+            m4[k] = mine ? mem_of(r + k) : 0ull;
             c += c4[k];
             m += m4[k];
         }
@@ -1410,7 +1469,7 @@ prefix_cut_kernel(const DevState* __restrict__ st, const int32_t* __restrict__ i
         unsigned long long pc = base_c + c, pm = base_m + m;  // demand before this thread's first row
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-            if ((r + k) < row_hi && idx[r + k] == d) {
+            if ((r + k) < row_hi && chose(r + k) == d) {
                 // monotone demand: exactly one row fits before it and not with it - the cut
                 if ((pc + c4[k] > cap_c || pm + m4[k] > cap_m) && pc <= cap_c && pm <= cap_m) {
                     sCutRow = r + k;
@@ -1435,6 +1494,22 @@ prefix_cut_kernel(const DevState* __restrict__ st, const int32_t* __restrict__ i
 }
 
 __global__ void __launch_bounds__(256)
+prefix_cut_kernel(const DevState* __restrict__ st, const int32_t* __restrict__ idx, const int32_t* __restrict__ req_core,
+                  const int32_t* __restrict__ req_mem, long long R, int n_tiles,
+                  const unsigned long long* __restrict__ tile_sums, PrefixOut* __restrict__ out,
+                  const long long* __restrict__ base = nullptr /* [2][kMaxD]: demand of the lower ranks' rows */) {
+    prefix_cut_cta<kRowsInt32>(st, idx, req_core, req_mem, R, n_tiles, tile_sums, out, base);
+}
+
+// The cut after a packed CONTIG scan: idx holds R int8 indices, words R packed words (single GPU).
+__global__ void __launch_bounds__(256)
+prefix_cut_packed_kernel(const DevState* __restrict__ st, const signed char* __restrict__ idx, const uint32_t* __restrict__ words,
+                         long long R, int n_tiles, const unsigned long long* __restrict__ tile_sums, PrefixOut* __restrict__ out) {
+    prefix_cut_cta<kRowsPacked>(st, reinterpret_cast<const int32_t*>(idx), reinterpret_cast<const int32_t*>(words), nullptr, R,
+                                n_tiles, tile_sums, out, nullptr);
+}
+
+__global__ void __launch_bounds__(256)
 prefix_apply_kernel(const PrefixOut* __restrict__ pf, int D, long long R, int32_t* __restrict__ idx) {
     __shared__ long long sCut[kMaxD];
     if (threadIdx.x < kMaxD) sCut[threadIdx.x] = threadIdx.x < D ? pf->cut[threadIdx.x] : 0;
@@ -1442,6 +1517,33 @@ prefix_apply_kernel(const PrefixOut* __restrict__ pf, int D, long long R, int32_
     const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
     for (long long r = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; r < R; r += stride) {
         const int32_t i = idx[r];
+        if (i >= 0 && r >= sCut[i]) idx[r] = -2;
+    }
+}
+
+// prefix_apply_kernel on int8 indices (16-byte aligned): four of them per 32-bit word and thread,
+// rewritten only when one of them is deferred; the R % 4 tail rows by the first threads of block 0.
+__global__ void __launch_bounds__(256)
+prefix_apply_packed_kernel(const PrefixOut* __restrict__ pf, int D, long long R, signed char* __restrict__ idx) {
+    __shared__ long long sCut[kMaxD];
+    if (threadIdx.x < kMaxD) sCut[threadIdx.x] = threadIdx.x < D ? pf->cut[threadIdx.x] : 0;
+    __syncthreads();
+    uint32_t* __restrict__ w4 = reinterpret_cast<uint32_t*>(idx);
+    const long long nw = R >> 2;
+    const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+    for (long long q = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; q < nw; q += stride) {
+        const uint32_t w = w4[q];
+        uint32_t o = w;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int i = static_cast<signed char>(w >> (8 * k));
+            if (i >= 0 && 4 * q + k >= sCut[i]) o = (o & ~(0xffu << (8 * k))) | (0xfeu << (8 * k));  // -2
+        }
+        if (o != w) w4[q] = o;
+    }
+    if (blockIdx.x == 0 && threadIdx.x < static_cast<unsigned>(R & 3)) {
+        const long long r = 4 * nw + threadIdx.x;
+        const int i = idx[r];
         if (i >= 0 && r >= sCut[i]) idx[r] = -2;
     }
 }

@@ -111,8 +111,10 @@ extern "C" {
                                     no second stream.  Never commits.  Every rank must issue the same launch; start the
                                     ranks together (egpu_peer_gate_dev) or the wait is as long as their skew. */
 
-#define EGPU_F_PACKED       16   /* egpu_bestfit_batches_dev only: every batch is in the packed format of
-                                    egpu_bestfit_batch_packed (5 bytes per decision instead of 12); see there. */
+#define EGPU_F_PACKED       16   /* the packed format of egpu_bestfit_batch_packed (5 bytes per decision
+                                    instead of 12) on egpu_bestfit_batches_dev (see there) and, together with
+                                    EGPU_F_PREFIX_COMMIT only, on egpu_bestfit_batch / egpu_bestfit_batch_dev:
+                                    see egpu_bestfit_batch_dev.  egpu_bestfit_batches_shard_dev refuses it. */
 
 /* kernel variants for the snapshot scan (egpu_set_variant) */
 #define EGPU_VARIANT_AUTO    0   /* SORTED for D <= 16, LUT above */
@@ -144,7 +146,8 @@ int  egpu_set_variant(egpu_ctx* ctx, int variant);
 /* ABI version: major*1000 + minor.  Minor revisions only add entry points (1.1 placement
  * restore, 1.2 prefix-commit over row shards, 1.3 rounds, 1.4 multi-batch launches, stateless query,
  * start gate, host registration, 1.5 preferred allocation for many container requests from flat ID
- * buffers, 1.6 EGPU_F_PACKED multi-batch launches); a caller built against 1.0 keeps working. */
+ * buffers, 1.6 EGPU_F_PACKED multi-batch launches, 1.7 EGPU_F_PACKED prefix-commit on egpu_bestfit_batch and
+ * egpu_bestfit_batch_dev); a caller built against 1.0 keeps working. */
 int  egpu_abi_version(void);
 
 /* ---- capacity table --------------------------------------------------- */
@@ -161,7 +164,9 @@ int egpu_table_size(egpu_ctx* ctx);
 /* Scores R requests against the current table.  Copies inputs H2D from the
  * caller's arrays (pinned or pageable), runs the scan, copies idx and deltas
  * back; returns when the outputs are valid.  out_delta_* have D entries and
- * may be NULL.  commit != 0 installs table' as the current table. */
+ * may be NULL.  commit != 0 installs table' as the current table.  `commit` also takes
+ * EGPU_F_PREFIX_COMMIT, and with it EGPU_F_PACKED (packed prefix-commit: see egpu_bestfit_batch_dev;
+ * the words are staged through HBM, 4 bytes per row in and 1 out). */
 int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core,
                        const int32_t* req_mem, int64_t R, int32_t* out_idx,
                        int64_t* out_delta_core, int64_t* out_delta_mem,
@@ -193,7 +198,9 @@ int egpu_bestfit_batch_rounds_dev(egpu_ctx* ctx, const int32_t* d_req_core,
 /* Packed wire format, for callers bound by PCIe rather than by the scan: 5 bytes per decision
  * instead of 12.  req_packed[r] = EGPU_PACK_REQUEST(core, mem) (core in 0..127, mem in
  * 0..2^18-1; any word >= 2^25, e.g. EGPU_PACKED_INVALID, is an infeasible request);
- * out_idx8[r] = device index 0..63 or -1.  Everything else as egpu_bestfit_batch. */
+ * out_idx8[r] = device index 0..63 or -1.  Everything else as egpu_bestfit_batch.  Snapshot mode only:
+ * EGPU_F_PREFIX_COMMIT is not implemented here (packed prefix-commit is egpu_bestfit_batch[_dev] with
+ * EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT). */
 #define EGPU_PACK_REQUEST(core, mem) (((uint32_t)(core) << 18) | (uint32_t)(mem))
 #define EGPU_PACKED_INVALID 0xFFFFFFFFu
 int egpu_bestfit_batch_packed(egpu_ctx* ctx, const uint32_t* req_packed, int64_t R, int8_t* out_idx8,
@@ -223,7 +230,19 @@ int  egpu_host_unregister(egpu_ctx* ctx, void* p);
  * cudaStreamLegacy, not 0).  d_delta is int64[2*D]: core sums then mem sums; it
  * is overwritten, not accumulated.  d_table_out (may be NULL) receives
  * int32[3*D]: free_core', free_mem', oversub.  flags: EGPU_F_*.  The three
- * request/index arrays must be 16-byte aligned (128-bit accesses). */
+ * request/index arrays must be 16-byte aligned (128-bit accesses).
+ *
+ * Packed prefix-commit (flags EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT [| EGPU_F_COMMIT]
+ * [| EGPU_F_INPUTS_READY]):
+ *   d_req_core   R packed words (EGPU_PACK_REQUEST; const uint32_t* cast to the argument's type);
+ *   d_req_mem    must be NULL;
+ *   d_out_idx    R int8 indices (int8_t* cast to the argument's type): device, -1 or EGPU_IDX_DEFERRED.
+ * Semantics are the int32 prefix-commit's on the requests the words stand for; words >= 2^25 and
+ * core 101..127 are infeasible.  EGPU_ERR_STATE under EGPU_VARIANT_GRID.  EGPU_ERR_INVALID, before
+ * anything is launched or written: EGPU_F_PACKED without EGPU_F_PREFIX_COMMIT (packed snapshots are
+ * egpu_bestfit_batch_packed[_dev]), a non-NULL d_req_mem, NULL or (_dev) misaligned words or indices
+ * with R > 0.  Without EGPU_F_PACKED a NULL d_req_mem with R > 0 is refused, so packed words are never
+ * read as int32 arrays. */
 int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core,
                            const int32_t* d_req_mem, int64_t R,
                            int32_t* d_out_idx, int64_t* d_delta,
