@@ -36,6 +36,7 @@ F_INPUTS_READY = 2
 F_PREFIX_COMMIT = 4
 F_APPLY = 8
 F_PACKED = 16
+F_ROUNDS = 32
 IDX_DEFERRED = -2
 
 EV_ALLOC = 0

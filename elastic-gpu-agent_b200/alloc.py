@@ -181,9 +181,11 @@ class BestFitAllocator:
         self._check(rc, "egpu_bestfit_batch_packed")
         return idx, dc, dm
 
-    def bestfit_packed_prefix(self, words, commit: bool = False):
+    def bestfit_packed_prefix(self, words, commit: bool = False, rounds: bool = False):
         """Prefix-commit (spec 2.5) on packed words: egpu_bestfit_batch with EGPU_F_PACKED |
-        EGPU_F_PREFIX_COMMIT.  Returns (idx int8[R] with -2 = DEFERRED, delta_core int64[D], delta_mem int64[D])."""
+        EGPU_F_PREFIX_COMMIT.  Returns (idx int8[R] with -2 = DEFERRED, delta_core int64[D], delta_mem int64[D]).
+        rounds=True adds EGPU_F_ROUNDS (and commits): rounds to the fixed point, no -2 left, and the sums
+        are the demand committed over all rounds."""
         p = np.ascontiguousarray(words, dtype=np.uint32)
         D = self._lib.egpu_table_size(self._h)
         if D < 0:
@@ -192,7 +194,8 @@ class BestFitAllocator:
         dc = np.zeros(D, dtype=np.int64)
         dm = np.zeros(D, dtype=np.int64)
         rc = self._lib.egpu_bestfit_batch(self._h, _ptr(p), None, p.size, _ptr(idx), _ptr(dc), _ptr(dm),
-                                          L.F_PACKED | L.F_PREFIX_COMMIT | (L.F_COMMIT if commit else 0))
+                                          L.F_PACKED | L.F_PREFIX_COMMIT | (L.F_COMMIT if commit or rounds else 0) |
+                                          (L.F_ROUNDS if rounds else 0))
         self._check(rc, "egpu_bestfit_batch")
         return idx, dc, dm
 
@@ -236,10 +239,11 @@ class BestFitAllocator:
         self._check(rc, "egpu_bestfit_batch_dev")
 
     def bestfit_packed_prefix_dev(self, d_words: int, R: int, d_idx8: int, d_delta: int = 0, d_table_out: int = 0,
-                                  commit: bool = False, stream: int | None = None):
+                                  commit: bool = False, stream: int | None = None, rounds: bool = False):
         """egpu_bestfit_batch_dev with EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT: R packed words in, R int8
-        indices out (-2 = DEFERRED), both 16-byte aligned."""
-        flags = L.F_PACKED | L.F_PREFIX_COMMIT | (L.F_COMMIT if commit else 0)
+        indices out (-2 = DEFERRED), both 16-byte aligned.  rounds=True adds EGPU_F_ROUNDS (and commits):
+        rounds to the fixed point; the call then synchronises `stream`."""
+        flags = L.F_PACKED | L.F_PREFIX_COMMIT | (L.F_COMMIT if commit or rounds else 0) | (L.F_ROUNDS if rounds else 0)
         rc = self._lib.egpu_bestfit_batch_dev(self._h, C.c_void_p(d_words), None, int(R), C.c_void_p(d_idx8),
                                               C.c_void_p(d_delta or None), C.c_void_p(d_table_out or None), flags,
                                               _stream(stream))

@@ -512,15 +512,18 @@ int launch_prefix_commit(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm
 // runs on the caller's device arrays; the rows it defers are gathered, in order, into dense
 // scratch arrays and re-submitted against the table round 1 committed, and so on.  Every round
 // needs two numbers on the host (rows still deferred, the round's committed demand), so this
-// is a synchronous host loop around asynchronous launches.
+// is a synchronous host loop around asynchronous launches.  Rows in either format (see
+// prefix_scan); d_table_out (may be NULL) receives every round's table', so the last one stays.
 struct RoundInfo {
     unsigned long long deferred;
     long long delta[2 * kMaxD];
 };
 
 int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx, int max_rounds,
-               long long* total_delta /* host [2*D] */, int32_t* rounds_out, int64_t* left_out, cudaStream_t s) {
+               long long* total_delta /* host [2*D] */, int32_t* rounds_out, int64_t* left_out, cudaStream_t s,
+               RowFormat fmt = kRowsInt32, int32_t* d_table_out = nullptr) {
     const int D = ctx->D;
+    const bool packed = fmt == kRowsPacked;
     for (int j = 0; j < 2 * D; ++j) total_delta[j] = 0;
     *rounds_out = 0;
     *left_out = 0;
@@ -528,11 +531,14 @@ int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t 
     // Scratch owned by the context, grow-only, sized by R BEFORE anything is committed (a failed
     // allocation must not leave a half-committed batch): round info, tile counts, and two sets
     // of (core, mem, caller's row, index) arrays - the deferred rows of any round are at most R.
+    // Packed: two sets of (words, caller's row, int8 index), 9 bytes per row each.
+    auto align = [](size_t b) { return (b + 255) & ~static_cast<size_t>(255); };
     const int64_t tiles_cap = (R + kCompactTile - 1) / kCompactTile;
-    const size_t tiles_bytes = (sizeof(unsigned int) * static_cast<size_t>(tiles_cap) + 255) & ~static_cast<size_t>(255);
-    const size_t per = (sizeof(int32_t) * static_cast<size_t>(R) + 255) & ~static_cast<size_t>(255);
+    const size_t tiles_bytes = align(sizeof(unsigned int) * static_cast<size_t>(tiles_cap));
+    const size_t per = align(sizeof(int32_t) * static_cast<size_t>(R));
+    const size_t sub[4] = {per, packed ? 0 : per, per, packed ? align(static_cast<size_t>(R)) : per};  // rc, rm, map, idx
     constexpr size_t kHead = 2048;  // RoundInfo
-    const size_t need = kHead + tiles_bytes + 8 * per;
+    const size_t need = kHead + tiles_bytes + 2 * (sub[0] + sub[1] + sub[2] + sub[3]);
     EGPU_CUDA(ctx, grow(ctx->rounds_bytes, need, need, &ctx->d_rounds));
     static_assert(sizeof(RoundInfo) <= kHead, "round info header");
     char* base = static_cast<char*>(ctx->d_rounds);
@@ -544,20 +550,31 @@ int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t 
     const int32_t* cur_map = nullptr;
     int32_t* cur_idx = d_idx;
     int64_t n = R;
-    int32_t* set[2][4];  // rc, rm, map, idx
+    int32_t* set[2][4];  // rc, rm (packed: none), map, idx
+    size_t off = kHead + tiles_bytes;
     for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 4; ++b) set[a][b] = reinterpret_cast<int32_t*>(base + kHead + tiles_bytes + per * (a * 4 + b));
+        for (int b = 0; b < 4; ++b) {
+            set[a][b] = sub[b] ? reinterpret_cast<int32_t*>(base + off) : nullptr;
+            off += sub[b];
+        }
     int which = 0;
     RoundInfo h{};
+    auto idx8 = [](const int32_t* p) { return reinterpret_cast<signed char*>(const_cast<int32_t*>(p)); };
     for (int round = 1;; ++round) {
-        int rc = launch_prefix_commit(ctx, cur_rc, cur_rm, n, cur_idx, d_info->delta, nullptr, EGPU_F_COMMIT, s);
+        int rc = launch_prefix_commit(ctx, cur_rc, cur_rm, n, cur_idx, d_info->delta, d_table_out, EGPU_F_COMMIT, s, fmt);
         if (rc != EGPU_OK) return rc;
         if (cur_map) {
-            round_writeback_kernel<<<capped_blocks(ctx, n, 256), 256, 0, s>>>(cur_idx, cur_map, n, d_idx);
+            if (packed)
+                round_writeback_packed_kernel<<<capped_blocks(ctx, n, 256), 256, 0, s>>>(idx8(cur_idx), cur_map, n, idx8(d_idx));
+            else
+                round_writeback_kernel<<<capped_blocks(ctx, n, 256), 256, 0, s>>>(cur_idx, cur_map, n, d_idx);
             ctx->launches += 1;
         }
         const int64_t tiles = (n + kCompactTile - 1) / kCompactTile;
-        deferred_count_kernel<<<static_cast<unsigned>(tiles), 256, 0, s>>>(cur_idx, n, d_tiles);
+        if (packed)
+            deferred_count_packed_kernel<<<static_cast<unsigned>(tiles), 256, 0, s>>>(idx8(cur_idx), n, d_tiles);
+        else
+            deferred_count_kernel<<<static_cast<unsigned>(tiles), 256, 0, s>>>(cur_idx, n, d_tiles);
         deferred_scan_kernel<<<1, 1024, 0, s>>>(d_tiles, tiles, &d_info->deferred);
         ctx->launches += 2;
         EGPU_CUDA(ctx, cudaGetLastError());
@@ -568,8 +585,12 @@ int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t 
         *left_out = static_cast<int64_t>(h.deferred);
         if (h.deferred == 0 || round >= max_rounds) return EGPU_OK;
         int32_t** nxt = set[which];
-        deferred_scatter_kernel<<<static_cast<unsigned>(tiles), 256, 0, s>>>(cur_idx, cur_rc, cur_rm, cur_map, n, d_tiles, nxt[0], nxt[1],
-                                                                               nxt[2]);
+        if (packed)
+            deferred_scatter_packed_kernel<<<static_cast<unsigned>(tiles), 256, 0, s>>>(
+                idx8(cur_idx), reinterpret_cast<const uint32_t*>(cur_rc), cur_map, n, d_tiles, reinterpret_cast<uint32_t*>(nxt[0]), nxt[2]);
+        else
+            deferred_scatter_kernel<<<static_cast<unsigned>(tiles), 256, 0, s>>>(cur_idx, cur_rc, cur_rm, cur_map, n, d_tiles, nxt[0],
+                                                                                   nxt[1], nxt[2]);
         ctx->launches += 1;
         EGPU_CUDA(ctx, cudaGetLastError());
         cur_rc = nxt[0];
@@ -579,6 +600,31 @@ int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t 
         n = static_cast<int64_t>(h.deferred);
         which ^= 1;
     }
+}
+
+// EGPU_F_ROUNDS: packed prefix-commit rounds until nothing is deferred, on device words and int8
+// indices.  Leaves the demand committed over all rounds in host total[2*D] and, when d_delta is
+// given, in d_delta; d_table_out receives the last round's table'.  R = 0 is the packed
+// prefix-commit with R = 0.  The caller synchronises `s`.
+int launch_packed_rounds(egpu_ctx* ctx, const int32_t* d_words, int64_t R, int32_t* d_idx8, long long* d_delta,
+                         int32_t* d_table_out, long long* total /* host [2*D] */, cudaStream_t s) {
+    if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // no prefix-commit mode
+    if (R == 0) {
+        for (int j = 0; j < 2 * ctx->D; ++j) total[j] = 0;
+        return launch_prefix_commit(ctx, d_words, nullptr, 0, d_idx8, d_delta, d_table_out, EGPU_F_COMMIT, s, kRowsPacked);
+    }
+    int32_t rounds = 0;
+    int64_t left = 0;
+    const int rc = run_rounds(ctx, d_words, nullptr, R, d_idx8, INT32_MAX, total, &rounds, &left, s, kRowsPacked, d_table_out);
+    if (rc != EGPU_OK) return rc;
+    if (d_delta) EGPU_CUDA(ctx, cudaMemcpyAsync(d_delta, total, sizeof(long long) * 2 * ctx->D, cudaMemcpyHostToDevice, s));
+    return EGPU_OK;
+}
+
+// The flags EGPU_F_ROUNDS is valid with: all of kRoundsNeeds, optionally EGPU_F_INPUTS_READY
+constexpr int kRoundsNeeds = EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS;
+bool rounds_flags_ok(int flags, int64_t R) {
+    return (flags & ~(kRoundsNeeds | EGPU_F_INPUTS_READY)) == 0 && (flags & kRoundsNeeds) == kRoundsNeeds && R < (1ll << 31);
 }
 
 // Prefix-commit over row shards (one rank per GPU, rank-major row order).  Two exchange
@@ -681,7 +727,8 @@ extern "C" {
 // 1.5: + egpu_preferred_allocation_batch (additive)
 // 1.6: + EGPU_F_PACKED multi-batch launches (additive)
 // 1.7: + EGPU_F_PACKED prefix-commit on egpu_bestfit_batch / egpu_bestfit_batch_dev (additive)
-int egpu_abi_version(void) { return 1007; }
+// 1.8: + EGPU_F_ROUNDS, packed prefix-commit rounds on the same two entry points (additive)
+int egpu_abi_version(void) { return 1008; }
 
 const char* egpu_strerror(int code) {
     switch (code) {
@@ -893,15 +940,24 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32
                            void* stream) {
     // EGPU_F_PACKED: prefix-commit only, d_req_core = words, d_req_mem NULL, d_out_idx = int8 indices.
     // Without it a NULL d_req_mem (R > 0) stays refused, so words are never read as int32 arrays.
+    // EGPU_F_ROUNDS: that, committing, to the fixed point; synchronises the stream.
     const bool packed = (flags & EGPU_F_PACKED) != 0;
-    if (!ctx || R < 0) return EGPU_ERR_INVALID;
+    const bool rounds = (flags & EGPU_F_ROUNDS) != 0;
+    if (!ctx || R < 0 || (rounds && !rounds_flags_ok(flags, R))) return EGPU_ERR_INVALID;
     if (packed ? (!(flags & EGPU_F_PREFIX_COMMIT) || d_req_mem || !rows_ok(R, {d_req_core, d_out_idx}))
                : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
         return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
-    const int rc = enter(ctx, kNeedsTable, stream, &s);
+    int rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
+    if (rounds) {
+        long long total[2 * kMaxD];
+        rc = launch_packed_rounds(ctx, d_req_core, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, total, s);
+        if (rc != EGPU_OK) return rc;
+        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
+        return EGPU_OK;
+    }
     if (flags & EGPU_F_PREFIX_COMMIT)
         return launch_prefix_commit(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out,
                                     flags, s, packed ? kRowsPacked : kRowsInt32);
@@ -1034,7 +1090,8 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     // req_core = words, req_mem NULL, out_idx = int8 indices (as in egpu_bestfit_batch_dev)
     const bool prefix = (commit & EGPU_F_PREFIX_COMMIT) != 0;
     const bool packed = (commit & EGPU_F_PACKED) != 0;
-    if (!ctx || R < 0) return EGPU_ERR_INVALID;
+    const bool rounds = (commit & EGPU_F_ROUNDS) != 0;
+    if (!ctx || R < 0 || (rounds && !rounds_flags_ok(commit, R))) return EGPU_ERR_INVALID;
     if (packed ? (!prefix || req_mem || (R > 0 && (!req_core || !out_idx))) : (R > 0 && (!req_core || !req_mem || !out_idx)))
         return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
@@ -1042,6 +1099,19 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     int rc = enter(ctx, kNeedsTable, nullptr, &s);
     if (rc != EGPU_OK) return rc;
     const int D = ctx->D;
+    if (rounds) {  // packed rounds to the fixed point, staged through HBM: 4 bytes per row in, 1 out
+        long long total[2 * kMaxD];
+        rc = ensure_staging(ctx, R > 0 ? R : 1);
+        if (rc != EGPU_OK) return rc;
+        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
+        rc = launch_packed_rounds(ctx, ctx->d_req_core, R, ctx->d_idx, nullptr, nullptr, total, s);
+        if (rc != EGPU_OK) return rc;
+        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, sizeof(int8_t) * R, cudaMemcpyDeviceToHost, s));
+        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
+        if (out_delta_core) std::memcpy(out_delta_core, total, sizeof(int64_t) * D);
+        if (out_delta_mem) std::memcpy(out_delta_mem, total + D, sizeof(int64_t) * D);
+        return EGPU_OK;
+    }
     const int user_flags = (commit & EGPU_F_COMMIT) ? EGPU_F_COMMIT : 0;
     // Zero-copy: when all three caller arrays are pinned (egpu_host_alloc or
     // cudaHostRegister) and 16-byte aligned, the scan reads the requests and writes

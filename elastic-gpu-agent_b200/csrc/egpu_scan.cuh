@@ -1630,16 +1630,36 @@ prefix_push_kernel(DevState* __restrict__ st, const PrefixOut* __restrict__ pf, 
 // original order, against the table that round committed.  These kernels gather them into
 // dense arrays (with the index of the caller's row each one came from) and write a later
 // round's results back.  Tiles of 1024 rows, 4 consecutive rows per thread, so positions
-// inside a tile follow the row order.
+// inside a tile follow the row order.  Both row formats (RowFormat): kRowsPacked gathers the
+// words (in the rc arrays; rm is not used) and reads and writes int8 indices.
 constexpr int kCompactTile = 1024;
 
-__global__ void __launch_bounds__(256)
-deferred_count_kernel(const int32_t* __restrict__ idx, long long n, unsigned int* __restrict__ tile_count) {
+// Bit k set: int8 index r0 + k (r0 a multiple of 4) is -2.  One 32-bit load where all four rows
+// exist; byte loads at the tail, since round 1's indices are the caller's array of exactly n bytes.
+__device__ __forceinline__ unsigned int deferred_mask_packed(const signed char* __restrict__ idx8, long long r0, long long n) {
+    unsigned int f = 0;
+    if (r0 + 4 <= n) {
+        const uint32_t w = *reinterpret_cast<const uint32_t*>(idx8 + r0);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) f |= ((w >> (8 * k)) & 0xffu) == 0xfeu ? 1u << k : 0u;
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) f |= (r0 + k < n && idx8[r0 + k] == -2) ? 1u << k : 0u;
+    }
+    return f;
+}
+
+template <RowFormat FMT>
+__device__ __forceinline__ void deferred_count_cta(const int32_t* __restrict__ idx, long long n, unsigned int* __restrict__ tile_count) {
     __shared__ unsigned int sWarp[8];
     const long long r0 = static_cast<long long>(blockIdx.x) * kCompactTile + 4ll * threadIdx.x;
     unsigned int c = 0;
+    if constexpr (FMT == kRowsPacked) {
+        c = __popc(deferred_mask_packed(reinterpret_cast<const signed char*>(idx), r0, n));
+    } else {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) c += (r0 + k < n && idx[r0 + k] == -2) ? 1u : 0u;
+        for (int k = 0; k < 4; ++k) c += (r0 + k < n && idx[r0 + k] == -2) ? 1u : 0u;
+    }
     c = __reduce_add_sync(0xffffffffu, c);
     if ((threadIdx.x & 31) == 0) sWarp[threadIdx.x >> 5] = c;
     __syncthreads();
@@ -1648,6 +1668,16 @@ deferred_count_kernel(const int32_t* __restrict__ idx, long long n, unsigned int
         for (int w = 0; w < 8; ++w) t += sWarp[w];
         tile_count[blockIdx.x] = t;
     }
+}
+
+__global__ void __launch_bounds__(256)
+deferred_count_kernel(const int32_t* __restrict__ idx, long long n, unsigned int* __restrict__ tile_count) {
+    deferred_count_cta<kRowsInt32>(idx, n, tile_count);
+}
+
+__global__ void __launch_bounds__(256)
+deferred_count_packed_kernel(const signed char* __restrict__ idx, long long n, unsigned int* __restrict__ tile_count) {
+    deferred_count_cta<kRowsPacked>(reinterpret_cast<const int32_t*>(idx), n, tile_count);
 }
 
 // exclusive scan of the tile counts in place; one CTA walks them 1024 at a time
@@ -1688,20 +1718,28 @@ deferred_scan_kernel(unsigned int* __restrict__ tile_count, long long n_tiles, u
     if (threadIdx.x == 0) *total = sCarry;
 }
 
-__global__ void __launch_bounds__(256)
-deferred_scatter_kernel(const int32_t* __restrict__ idx, const int32_t* __restrict__ rc, const int32_t* __restrict__ rm,
-                        const int32_t* __restrict__ map /* nullptr: the rows are the caller's own */, long long n,
-                        const unsigned int* __restrict__ tile_off, int32_t* __restrict__ out_rc, int32_t* __restrict__ out_rm,
-                        int32_t* __restrict__ out_map) {
+template <RowFormat FMT>
+__device__ __forceinline__ void deferred_scatter_cta(const int32_t* __restrict__ idx, const int32_t* __restrict__ rc,
+                                                     const int32_t* __restrict__ rm, const int32_t* __restrict__ map, long long n,
+                                                     const unsigned int* __restrict__ tile_off, int32_t* __restrict__ out_rc,
+                                                     int32_t* __restrict__ out_rm, int32_t* __restrict__ out_map) {
+    constexpr bool packed = FMT == kRowsPacked;
     __shared__ unsigned int sWarp[8];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long r0 = static_cast<long long>(blockIdx.x) * kCompactTile + 4ll * threadIdx.x;
     bool f[4];
     unsigned int c = 0;
+    if constexpr (packed) {
+        const unsigned int m = deferred_mask_packed(reinterpret_cast<const signed char*>(idx), r0, n);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        f[k] = r0 + k < n && idx[r0 + k] == -2;
-        c += f[k] ? 1u : 0u;
+        for (int k = 0; k < 4; ++k) f[k] = (m >> k) & 1u;
+        c = __popc(m);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            f[k] = r0 + k < n && idx[r0 + k] == -2;
+            c += f[k] ? 1u : 0u;
+        }
     }
     unsigned int x = c;
 #pragma unroll
@@ -1717,19 +1755,58 @@ deferred_scatter_kernel(const int32_t* __restrict__ idx, const int32_t* __restri
     for (int k = 0; k < 4; ++k) {
         if (f[k]) {
             out_rc[pos] = rc[r0 + k];
-            out_rm[pos] = rm[r0 + k];
+            if constexpr (!packed) out_rm[pos] = rm[r0 + k];
             out_map[pos] = map ? map[r0 + k] : static_cast<int32_t>(r0 + k);
             ++pos;
         }
     }
 }
 
+__global__ void __launch_bounds__(256)
+deferred_scatter_kernel(const int32_t* __restrict__ idx, const int32_t* __restrict__ rc, const int32_t* __restrict__ rm,
+                        const int32_t* __restrict__ map /* nullptr: the rows are the caller's own */, long long n,
+                        const unsigned int* __restrict__ tile_off, int32_t* __restrict__ out_rc, int32_t* __restrict__ out_rm,
+                        int32_t* __restrict__ out_map) {
+    deferred_scatter_cta<kRowsInt32>(idx, rc, rm, map, n, tile_off, out_rc, out_rm, out_map);
+}
+
+// the deferred rows' words (and caller's rows) of int8 indices idx into dense out_words / out_map
+__global__ void __launch_bounds__(256)
+deferred_scatter_packed_kernel(const signed char* __restrict__ idx, const uint32_t* __restrict__ words,
+                               const int32_t* __restrict__ map /* nullptr: the rows are the caller's own */, long long n,
+                               const unsigned int* __restrict__ tile_off, uint32_t* __restrict__ out_words,
+                               int32_t* __restrict__ out_map) {
+    deferred_scatter_cta<kRowsPacked>(reinterpret_cast<const int32_t*>(idx), reinterpret_cast<const int32_t*>(words), nullptr, map, n,
+                                      tile_off, reinterpret_cast<int32_t*>(out_words), nullptr, out_map);
+}
+
 // a later round's answers (device, -1 or still -2) back to the caller's rows
+template <RowFormat FMT>
+__device__ __forceinline__ void round_writeback_rows(const int32_t* __restrict__ idx_k, const int32_t* __restrict__ map, long long n,
+                                                     int32_t* __restrict__ out_idx) {
+    const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+    if constexpr (FMT == kRowsPacked) {
+        // Single-byte stores: the caller's rows are scattered, so neighbouring bytes of one word may be
+        // written by different threads at once.  The GPU writes a byte store with a byte mask, not as
+        // a read-modify-write of the containing word, so these stores do not clobber each other.
+        const signed char* __restrict__ src = reinterpret_cast<const signed char*>(idx_k);
+        signed char* __restrict__ dst = reinterpret_cast<signed char*>(out_idx);
+        for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) dst[map[i]] = src[i];
+    } else {
+        for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) out_idx[map[i]] = idx_k[i];
+    }
+}
+
 __global__ void __launch_bounds__(256)
 round_writeback_kernel(const int32_t* __restrict__ idx_k, const int32_t* __restrict__ map, long long n,
                        int32_t* __restrict__ out_idx) {
-    const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) out_idx[map[i]] = idx_k[i];
+    round_writeback_rows<kRowsInt32>(idx_k, map, n, out_idx);
+}
+
+__global__ void __launch_bounds__(256)
+round_writeback_packed_kernel(const signed char* __restrict__ idx_k, const int32_t* __restrict__ map, long long n,
+                              signed char* __restrict__ out_idx) {
+    round_writeback_rows<kRowsPacked>(reinterpret_cast<const int32_t*>(idx_k), map, n, reinterpret_cast<int32_t*>(out_idx));
 }
 
 }  // namespace egpu

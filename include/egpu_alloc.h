@@ -116,6 +116,12 @@ extern "C" {
                                     EGPU_F_PREFIX_COMMIT only, on egpu_bestfit_batch / egpu_bestfit_batch_dev:
                                     see egpu_bestfit_batch_dev.  egpu_bestfit_batches_shard_dev refuses it. */
 
+#define EGPU_F_ROUNDS       32   /* egpu_bestfit_batch / egpu_bestfit_batch_dev only, and only as
+                                    EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS
+                                    [| EGPU_F_INPUTS_READY]: packed prefix-commit rounds to the fixed point
+                                    (egpu_bestfit_batch_rounds on packed words, no round limit); see
+                                    egpu_bestfit_batch_dev.  egpu_bestfit_batches_dev refuses it. */
+
 /* kernel variants for the snapshot scan (egpu_set_variant) */
 #define EGPU_VARIANT_AUTO    0   /* SORTED for D <= 16, LUT above */
 #define EGPU_VARIANT_GRID    1   /* direct (device x request) score grid, min over packed keys */
@@ -147,7 +153,8 @@ int  egpu_set_variant(egpu_ctx* ctx, int variant);
  * restore, 1.2 prefix-commit over row shards, 1.3 rounds, 1.4 multi-batch launches, stateless query,
  * start gate, host registration, 1.5 preferred allocation for many container requests from flat ID
  * buffers, 1.6 EGPU_F_PACKED multi-batch launches, 1.7 EGPU_F_PACKED prefix-commit on egpu_bestfit_batch and
- * egpu_bestfit_batch_dev); a caller built against 1.0 keeps working. */
+ * egpu_bestfit_batch_dev, 1.8 EGPU_F_ROUNDS packed rounds on the same two); a caller built against 1.0 keeps
+ * working. */
 int  egpu_abi_version(void);
 
 /* ---- capacity table --------------------------------------------------- */
@@ -166,7 +173,9 @@ int egpu_table_size(egpu_ctx* ctx);
  * back; returns when the outputs are valid.  out_delta_* have D entries and
  * may be NULL.  commit != 0 installs table' as the current table.  `commit` also takes
  * EGPU_F_PREFIX_COMMIT, and with it EGPU_F_PACKED (packed prefix-commit: see egpu_bestfit_batch_dev;
- * the words are staged through HBM, 4 bytes per row in and 1 out). */
+ * the words are staged through HBM, 4 bytes per row in and 1 out), and with those and EGPU_F_COMMIT,
+ * EGPU_F_ROUNDS (packed rounds to the fixed point, staged the same way; out_delta_* receive the demand
+ * committed over all rounds). */
 int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core,
                        const int32_t* req_mem, int64_t R, int32_t* out_idx,
                        int64_t* out_delta_core, int64_t* out_delta_mem,
@@ -242,7 +251,20 @@ int  egpu_host_unregister(egpu_ctx* ctx, void* p);
  * anything is launched or written: EGPU_F_PACKED without EGPU_F_PREFIX_COMMIT (packed snapshots are
  * egpu_bestfit_batch_packed[_dev]), a non-NULL d_req_mem, NULL or (_dev) misaligned words or indices
  * with R > 0.  Without EGPU_F_PACKED a NULL d_req_mem with R > 0 is refused, so packed words are never
- * read as int32 arrays. */
+ * read as int32 arrays.
+ *
+ * Packed rounds (flags EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS
+ * [| EGPU_F_INPUTS_READY]): the arguments of packed prefix-commit, and the semantics of
+ * egpu_bestfit_batch_rounds with no round limit: committing rounds run until one defers nothing, so
+ * every index ends as a device or -1, never EGPU_IDX_DEFERRED, and the table is never oversubscribed
+ * (sticky oversubscription flags are kept, as there).  d_delta (may be NULL) receives the demand
+ * committed over all rounds, int64[2*D]; d_table_out (may be NULL) the last round's table', oversub
+ * words 0.  THIS CALL SYNCHRONISES `stream` before it returns: every round needs its deferred count on
+ * the host.  Scratch (18 bytes per request, kept by the context) is allocated before round 1: an
+ * allocation failure returns EGPU_ERR_NOMEM with nothing committed.  R = 0 is the packed prefix-commit
+ * with R = 0.  EGPU_ERR_STATE under EGPU_VARIANT_GRID.  EGPU_ERR_INVALID, before anything is launched
+ * or written: EGPU_F_ROUNDS with any other combination of flags, R >= 2^31, and everything packed
+ * prefix-commit refuses. */
 int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core,
                            const int32_t* d_req_mem, int64_t R,
                            int32_t* d_out_idx, int64_t* d_delta,
