@@ -366,6 +366,35 @@ class BestFitAllocator:
                                                         C.c_void_p(d_table_out_lagged or None), _stream(stream))
         self._check(rc, "egpu_bestfit_batch_shard_lag_dev")
 
+    # packed sharded calls: R packed words in, R int8 indices out (both 16-byte aligned); d_req_mem is always NULL
+    def bestfit_shard_packed_dev(self, d_words: int, R: int, d_idx8: int, d_delta: int, step: int, stream: int | None = None,
+                                 inputs_ready: bool = False):
+        """egpu_bestfit_batch_shard_dev with EGPU_F_PACKED."""
+        rc = self._lib.egpu_bestfit_batch_shard_dev(self._h, C.c_void_p(d_words), None, int(R), C.c_void_p(d_idx8),
+                                                    C.c_void_p(d_delta or None),
+                                                    L.F_PACKED | (L.F_INPUTS_READY if inputs_ready else 0), int(step),
+                                                    _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_shard_dev")
+
+    def bestfit_shard_lag_packed_dev(self, d_words: int, R: int, d_idx8: int, d_delta: int, step: int, lag: int,
+                                     d_table_out_lagged: int = 0, stream: int | None = None, inputs_ready: bool = False):
+        """egpu_bestfit_batch_shard_lag_dev with EGPU_F_PACKED (and d_req_mem NULL, which packed mode needs)."""
+        rc = self._lib.egpu_bestfit_batch_shard_lag_dev(self._h, C.c_void_p(d_words), None, int(R), C.c_void_p(d_idx8),
+                                                        C.c_void_p(d_delta or None),
+                                                        L.F_PACKED | (L.F_INPUTS_READY if inputs_ready else 0), int(step), int(lag),
+                                                        C.c_void_p(d_table_out_lagged or None), _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_shard_lag_dev")
+
+    def bestfit_shard_prefix_packed_dev(self, d_words: int, R: int, d_idx8: int, d_delta: int, d_table_out: int, step: int,
+                                        commit: bool = False, stream: int | None = None):
+        """egpu_bestfit_batch_shard_prefix_dev with EGPU_F_PACKED: rank-major prefix-commit on words (-2 = DEFERRED);
+        consumes exchange steps `step` and `step + 1`."""
+        rc = self._lib.egpu_bestfit_batch_shard_prefix_dev(self._h, C.c_void_p(d_words), None, int(R), C.c_void_p(d_idx8),
+                                                           C.c_void_p(d_delta or None), C.c_void_p(d_table_out or None),
+                                                           L.F_PACKED | L.F_PREFIX_COMMIT | (L.F_COMMIT if commit else 0), int(step),
+                                                           _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_shard_prefix_dev")
+
     def apply_peers_dev(self, step: int, d_table_out: int = 0, commit: bool = False, stream: int | None = None):
         rc = self._lib.egpu_table_apply_peers_dev(self._h, int(step), C.c_void_p(d_table_out or None),
                                                   1 if commit else 0, _stream(stream))

@@ -91,6 +91,18 @@ template <int P>
 constexpr decltype(packed_contig_kernel<P, 0>()) kPackedContigKernels[4] = {packed_contig_kernel<P, 0>(), packed_contig_kernel<P, 1>(),
                                                                             packed_contig_kernel<P, 2>(), packed_contig_kernel<P, 3>()};
 
+// The packed sharded scans: twins of the round-robin single-batch kernels of their bucket, same CTA
+// sizes, shared memory and kernel types.
+template <int P, int B>
+constexpr auto packed_snap_kernel() {
+    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
+    if constexpr (P == kPackedSortedSnap) return kernel(bestfit_sorted_packed_snap_kernel<DT, T>, T, sizeof(SnapSmem<DT, T>));
+    else return kernel(bestfit_lut_packed_snap_kernel<256>, 256, sizeof(LutSmem<256>));
+}
+template <int P>
+constexpr decltype(packed_snap_kernel<P, 0>()) kPackedSnapKernels[4] = {packed_snap_kernel<P, 0>(), packed_snap_kernel<P, 1>(),
+                                                                        packed_snap_kernel<P, 2>(), packed_snap_kernel<P, 3>()};
+
 // Resident CTAs per SM of kernel k; `cached` is its entry in the context's occupancy cache.  The
 // first use on a context opts in to the kernel's dynamic shared memory and asks the occupancy.
 template <class Fn>
@@ -293,17 +305,20 @@ struct Snapshot {
     unsigned long long push_step_plus1 = 0;      // exchange step + 1 the epilogue pushes the demand to, 0 = none
     int lag = 0;                                 // lagged apply (egpu_bestfit_batch_shard_lag_dev)
     bool contig = false;                         // prefix-commit: contiguous tiles, per-tile sums in ctx->d_tile_sums
-    bool packed = false;                         // contig only: rc = packed words, rm unused, idx = int8 indices
+    bool packed = false;                         // rc = packed words, rm unused, idx = int8 indices (CONTIG: prefix-commit,
+                                                 // otherwise a sharded scan); not in the grid variant
 };
 
 template <int F>
 int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_tiles_out) {
     constexpr bool lut = F == kScanLut || F == kScanLutContig, grid_variant = F == kScanGrid;
-    constexpr int P = lut ? kPackedLutContig : kPackedSortedContig;
+    constexpr int P = lut ? kPackedLutContig : kPackedSortedContig, Q = lut ? kPackedLutSnap : kPackedSortedSnap;
     const int bucket = d_bucket(ctx->D);
-    const auto& k = a.packed ? kPackedContigKernels<P>[bucket] : kKernels<F>[bucket];
+    const auto& k = !a.packed ? kKernels<F>[bucket] : a.contig ? kPackedContigKernels<P>[bucket] : kPackedSnapKernels<Q>[bucket];
+    int& cached = !a.packed ? ctx->scan_ctas_per_sm[F][bucket]
+                            : a.contig ? ctx->packed_contig_ctas_per_sm[P][bucket] : ctx->packed_snap_ctas_per_sm[Q][bucket];
     int per_sm = 0;
-    int rc = resident_ctas(ctx, k, a.packed ? ctx->packed_contig_ctas_per_sm[P][bucket] : ctx->scan_ctas_per_sm[F][bucket], &per_sm);
+    int rc = resident_ctas(ctx, k, cached, &per_sm);
     if (rc != EGPU_OK) return rc;
     if (lut) {
         rc = refresh_lut(ctx, s);
@@ -329,6 +344,9 @@ int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_
     // pipelined - the first of a graph - the lone-launch grid: slower per step)
     if (a.user_flags & EGPU_F_INPUTS_READY) rpt = (lut || ctx->D <= 16) ? 48 : 8;  // measured, scripts/tune_*.sh
     else if (lut) rpt = 32;  // the lookup scan has a 13 KB per-CTA table tile to amortise
+    // a lone packed sharded register scan: 5-byte rows want longer CTAs (16 measured faster than 8 at D = 8; twice
+    // the other rules measured slower or level, DESIGN.md 4.1c)
+    else if (a.packed && !a.contig) rpt = 16;
     if (a.rpt_hint > 0) rpt = a.rpt_hint;
     if (ctx->rows_per_thread > 0) rpt = ctx->rows_per_thread;
     if (grid_variant) rpt = 4;
@@ -367,7 +385,7 @@ int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_
 int launch_snapshot(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_tiles_out = nullptr) {
     if (a.R > kMaxRows) return EGPU_ERR_INVALID;  // the scans index 128-bit vectors with 32 bits
     const bool grid_variant = ctx->variant == EGPU_VARIANT_GRID;
-    if (a.contig && grid_variant) return EGPU_ERR_STATE;  // the literal variant has no prefix-commit mode
+    if ((a.contig || a.packed) && grid_variant) return EGPU_ERR_STATE;  // the literal variant has no prefix-commit mode, no packed form
     if (lut_variant(ctx))
         return a.contig ? launch_snapshot_as<kScanLutContig>(ctx, a, s, n_tiles_out) : launch_snapshot_as<kScanLut>(ctx, a, s, n_tiles_out);
     if (grid_variant) return launch_snapshot_as<kScanGrid>(ctx, a, s, n_tiles_out);
@@ -629,17 +647,26 @@ bool rounds_flags_ok(int flags, int64_t R) {
 
 // Prefix-commit over row shards (one rank per GPU, rank-major row order).  Two exchange
 // steps: `step` carries the uncapped demand of every shard (pushed by the scan itself),
-// `step + 1` the committed demand after the cut (pushed by prefix_push_kernel).
+// `step + 1` the committed demand after the cut (pushed by prefix_push_kernel).  Rows in either
+// format (see prefix_scan); base, push and apply do not see them.
 int launch_prefix_commit_shard(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx,
-                               long long* d_delta, int32_t* d_table_out, int user_flags, uint64_t step, cudaStream_t s) {
+                               long long* d_delta, int32_t* d_table_out, int user_flags, uint64_t step, cudaStream_t s,
+                               RowFormat fmt) {
     PrefixOut* pf = nullptr;
     int n_tiles = 0;
-    const int rc = prefix_scan(ctx, d_rc, d_rm, R, d_idx, kRowsInt32, step + 1, s, &pf, &n_tiles);
+    const int rc = prefix_scan(ctx, d_rc, d_rm, R, d_idx, fmt, step + 1, s, &pf, &n_tiles);
     if (rc != EGPU_OK) return rc;
     long long* base = reinterpret_cast<long long*>(pf + 1);
     prefix_base_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, step + 1, base);
-    prefix_cut_kernel<<<ctx->D, 256, 0, s>>>(ctx->d_state, d_idx, d_rc, d_rm, R, n_tiles, ctx->d_tile_sums, pf, base);
-    prefix_apply_kernel<<<capped_blocks(ctx, R, 1024), 256, 0, s>>>(pf, ctx->D, R, d_idx);
+    if (fmt == kRowsPacked) {
+        signed char* idx8 = reinterpret_cast<signed char*>(d_idx);
+        prefix_cut_packed_shard_kernel<<<ctx->D, 256, 0, s>>>(ctx->d_state, idx8, reinterpret_cast<const uint32_t*>(d_rc), R, n_tiles,
+                                                              ctx->d_tile_sums, pf, base);
+        prefix_apply_packed_kernel<<<capped_blocks(ctx, R, 1024), 256, 0, s>>>(pf, ctx->D, R, idx8);
+    } else {
+        prefix_cut_kernel<<<ctx->D, 256, 0, s>>>(ctx->d_state, d_idx, d_rc, d_rm, R, n_tiles, ctx->d_tile_sums, pf, base);
+        prefix_apply_kernel<<<capped_blocks(ctx, R, 1024), 256, 0, s>>>(pf, ctx->D, R, d_idx);
+    }
     prefix_push_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, pf, step + 2, d_delta);
     ApplyOuts outs{};
     outs.table_out[0] = d_table_out;
@@ -728,7 +755,8 @@ extern "C" {
 // 1.6: + EGPU_F_PACKED multi-batch launches (additive)
 // 1.7: + EGPU_F_PACKED prefix-commit on egpu_bestfit_batch / egpu_bestfit_batch_dev (additive)
 // 1.8: + EGPU_F_ROUNDS, packed prefix-commit rounds on the same two entry points (additive)
-int egpu_abi_version(void) { return 1008; }
+// 1.9: + EGPU_F_PACKED on egpu_bestfit_batch_shard_dev, _shard_lag_dev and _shard_prefix_dev (additive)
+int egpu_abi_version(void) { return 1009; }
 
 const char* egpu_strerror(int code) {
     switch (code) {
@@ -1260,36 +1288,46 @@ int egpu_peer_detach(egpu_ctx* ctx) {
 int egpu_bestfit_batch_shard_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                                  int32_t* d_out_idx, int64_t* d_delta, int flags, uint64_t step, void* stream) {
     // the commit happens in apply_peers; prefix-commit over shards has its own entry point;
-    // step + 1 travels in 48 bits of the launch word
-    if (!ctx || R < 0 || (flags & ~EGPU_F_INPUTS_READY) || step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    if (!rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
+    // step + 1 travels in 48 bits of the launch word.  EGPU_F_PACKED: words in d_req_core, d_req_mem
+    // NULL, int8 indices (as in egpu_bestfit_batch_dev)
+    const bool packed = (flags & EGPU_F_PACKED) != 0;
+    if (!ctx || R < 0 || (flags & ~(EGPU_F_INPUTS_READY | EGPU_F_PACKED)) || step >= (1ull << 47)) return EGPU_ERR_INVALID;
+    if (packed ? (d_req_mem || !rows_ok(R, {d_req_core, d_out_idx})) : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
+        return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
     Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), nullptr, flags};
     a.push_step_plus1 = step + 1;
+    a.packed = packed;
     return launch_snapshot(ctx, a, s);
 }
 
 int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                                         int32_t* d_out_idx, int64_t* d_delta, int32_t* d_table_out, int flags,
                                         uint64_t step, void* stream) {
-    if (!ctx || R < 0 || step >= (1ull << 47) || (flags & ~(EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT))) return EGPU_ERR_INVALID;
-    if (!rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
+    const bool packed = (flags & EGPU_F_PACKED) != 0;
+    if (!ctx || R < 0 || step >= (1ull << 47) || (flags & ~(EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT | EGPU_F_PACKED)))
+        return EGPU_ERR_INVALID;
+    if (packed ? (d_req_mem || !rows_ok(R, {d_req_core, d_out_idx})) : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
+        return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
     return launch_prefix_commit_shard(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta),
-                                      d_table_out, flags, step, s);
+                                      d_table_out, flags, step, s, packed ? kRowsPacked : kRowsInt32);
 }
 
 int egpu_bestfit_batch_shard_lag_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                                      int32_t* d_out_idx, int64_t* d_delta, int flags, uint64_t step, int lag,
                                      int32_t* d_table_out_lagged, void* stream) {
+    // This entry point never checked flags other than EGPU_F_COMMIT, so a call with EGPU_F_PACKED and
+    // two int32 arrays has always run as int32 and still does: packed needs the flag AND a NULL d_req_mem.
+    const bool packed = (flags & EGPU_F_PACKED) && !d_req_mem;
     if (!ctx || R < 0 || (flags & EGPU_F_COMMIT) || lag < 1 || lag > 16 || step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    if (!rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
+    if (packed ? !rows_ok(R, {d_req_core, d_out_idx}) : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
@@ -1297,6 +1335,7 @@ int egpu_bestfit_batch_shard_lag_dev(egpu_ctx* ctx, const int32_t* d_req_core, c
     Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out_lagged, flags};
     a.push_step_plus1 = step + 1;
     a.lag = lag;
+    a.packed = packed;
     return launch_snapshot(ctx, a, s);
 }
 

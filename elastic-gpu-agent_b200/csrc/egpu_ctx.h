@@ -22,12 +22,15 @@ enum ScanFamily {
 enum PackedFamily { kPackedSortedMulti, kPackedLutMulti, kPackedFamilies };
 // The packed prefix-commit scans (CONTIG tiles; egpu_bestfit_batch[_dev] with EGPU_F_PACKED), per D bucket
 enum PackedContigFamily { kPackedSortedContig, kPackedLutContig, kPackedContigFamilies };
+// The packed sharded scans (round-robin tiles; egpu_bestfit_batch_shard[_lag]_dev with EGPU_F_PACKED), per D bucket
+enum PackedSnapFamily { kPackedSortedSnap, kPackedLutSnap, kPackedSnapFamilies };
 
 struct egpu_ctx {
     std::mutex mu;
     int scan_ctas_per_sm[kScanFamilies][4] = {};  // resident CTAs per SM of each scan kernel, 0 = not asked yet
     int packed_ctas_per_sm[kPackedFamilies][4] = {};  // ... and of each packed multi-batch kernel
     int packed_contig_ctas_per_sm[kPackedContigFamilies][4] = {};  // ... and of each packed prefix-commit scan
+    int packed_snap_ctas_per_sm[kPackedSnapFamilies][4] = {};  // ... and of each packed sharded scan
     void* h_qtable = nullptr;         // pinned host image of that table (the part of DevState before `peer`)
     DevState* d_qstate = nullptr;     // scratch table of egpu_bestfit_query (the context's own table is not touched)
     unsigned long long* h_gate = nullptr;      // pinned: start gates the host has opened (egpu_peer_gate_open)

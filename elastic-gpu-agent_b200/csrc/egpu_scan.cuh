@@ -553,6 +553,19 @@ bestfit_sorted_packed_contig_kernel(DevState* __restrict__ st, const int32_t* __
                                                         tile_sums);
 }
 
+// Packed sharded scan (egpu_bestfit_batch_shard_dev / _shard_lag_dev with EGPU_F_PACKED): the
+// round-robin tiles, push and lagged apply of bestfit_sorted_kernel<DT, THREADS, false> on R packed
+// words and R int8 indices (req_mem is not read, tile_sums unused).
+template <int DT, int THREADS>
+__global__ void __launch_bounds__(THREADS)
+bestfit_sorted_packed_snap_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_core,
+                                  const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
+                                  long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags,
+                                  unsigned long long slot_step, unsigned long long* __restrict__ tile_sums) {
+    sorted_snapshot_cta<DT, THREADS, false, kRowsPacked>(st, req_core, req_mem, R, out_idx, delta_out, table_out, flags, slot_step,
+                                                         tile_sums);
+}
+
 // Grid of a multi-batch launch: the first `extra` batches have base + 1 tiles (CTAs), the others
 // base, so that K * base + extra can be exactly the number of CTAs the GPU holds at once (every SM
 // equally loaded) whatever K is.  tiles_extra = base | extra << 16.
@@ -1133,6 +1146,18 @@ bestfit_lut_packed_contig_kernel(DevState* __restrict__ st, const int32_t* __res
                                                  tile_sums);
 }
 
+// Packed sharded scan in the lookup scan (see bestfit_sorted_packed_snap_kernel).
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS)
+bestfit_lut_packed_snap_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_core,
+                               const int32_t* __restrict__ req_mem, long long R, int32_t* __restrict__ out_idx,
+                               long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int flags,
+                               unsigned long long slot_step, const DevLut* __restrict__ glut,
+                               unsigned long long* __restrict__ tile_sums) {
+    lut_snapshot_cta<THREADS, false, kRowsPacked>(st, req_core, req_mem, R, out_idx, delta_out, table_out, flags, slot_step, glut,
+                                                  tile_sums);
+}
+
 // Multi-batch form of the lookup scan (see bestfit_sorted_multi_kernel), in either row format.
 template <int THREADS, RowFormat FMT>
 __device__ __forceinline__ void lut_multi_cta(DevState* __restrict__ st, const MultiArgs& args, int tiles_extra, int flags,
@@ -1507,6 +1532,18 @@ prefix_cut_packed_kernel(const DevState* __restrict__ st, const signed char* __r
                          long long R, int n_tiles, const unsigned long long* __restrict__ tile_sums, PrefixOut* __restrict__ out) {
     prefix_cut_cta<kRowsPacked>(st, reinterpret_cast<const int32_t*>(idx), reinterpret_cast<const int32_t*>(words), nullptr, R,
                                 n_tiles, tile_sums, out, nullptr);
+}
+
+// The same cut over row shards: base[2][kMaxD] = demand of the lower ranks' rows (prefix_base_kernel).
+// A twin rather than a defaulted `base` on prefix_cut_packed_kernel, which keeps the single-GPU cut
+// free of the base loads.
+__global__ void __launch_bounds__(256)
+prefix_cut_packed_shard_kernel(const DevState* __restrict__ st, const signed char* __restrict__ idx,
+                               const uint32_t* __restrict__ words, long long R, int n_tiles,
+                               const unsigned long long* __restrict__ tile_sums, PrefixOut* __restrict__ out,
+                               const long long* __restrict__ base) {
+    prefix_cut_cta<kRowsPacked>(st, reinterpret_cast<const int32_t*>(idx), reinterpret_cast<const int32_t*>(words), nullptr, R,
+                                n_tiles, tile_sums, out, base);
 }
 
 __global__ void __launch_bounds__(256)

@@ -114,7 +114,10 @@ extern "C" {
 #define EGPU_F_PACKED       16   /* the packed format of egpu_bestfit_batch_packed (5 bytes per decision
                                     instead of 12) on egpu_bestfit_batches_dev (see there) and, together with
                                     EGPU_F_PREFIX_COMMIT only, on egpu_bestfit_batch / egpu_bestfit_batch_dev:
-                                    see egpu_bestfit_batch_dev.  egpu_bestfit_batches_shard_dev refuses it. */
+                                    see egpu_bestfit_batch_dev; and on the sharded single-batch calls
+                                    egpu_bestfit_batch_shard_dev, egpu_bestfit_batch_shard_lag_dev and
+                                    egpu_bestfit_batch_shard_prefix_dev (see there).
+                                    egpu_bestfit_batches_shard_dev refuses it. */
 
 #define EGPU_F_ROUNDS       32   /* egpu_bestfit_batch / egpu_bestfit_batch_dev only, and only as
                                     EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS
@@ -153,8 +156,9 @@ int  egpu_set_variant(egpu_ctx* ctx, int variant);
  * restore, 1.2 prefix-commit over row shards, 1.3 rounds, 1.4 multi-batch launches, stateless query,
  * start gate, host registration, 1.5 preferred allocation for many container requests from flat ID
  * buffers, 1.6 EGPU_F_PACKED multi-batch launches, 1.7 EGPU_F_PACKED prefix-commit on egpu_bestfit_batch and
- * egpu_bestfit_batch_dev, 1.8 EGPU_F_ROUNDS packed rounds on the same two); a caller built against 1.0 keeps
- * working. */
+ * egpu_bestfit_batch_dev, 1.8 EGPU_F_ROUNDS packed rounds on the same two, 1.9 EGPU_F_PACKED on
+ * egpu_bestfit_batch_shard_dev, egpu_bestfit_batch_shard_lag_dev and egpu_bestfit_batch_shard_prefix_dev); a
+ * caller built against 1.0 keeps working. */
 int  egpu_abi_version(void);
 
 /* ---- capacity table --------------------------------------------------- */
@@ -336,7 +340,19 @@ int egpu_table_apply_deltas_dev(egpu_ctx* ctx, const int64_t* d_deltas, int G,
  *       have landed locally, applies their sum: table' (and commit) as in snapshot mode.
  * `step` must increase by one per sharded step on every rank; a rank's scans may run at
  * most 128 steps ahead of its own applies (256 exchange slots: then no peer can be more than
- * 255 steps ahead of what this rank has consumed).  The scan itself never commits. */
+ * 255 steps ahead of what this rank has consumed).  The scan itself never commits.
+ *
+ * Packed sharded scans (egpu_bestfit_batch_shard_dev flags EGPU_F_PACKED [| EGPU_F_INPUTS_READY]):
+ * the arguments of the packed prefix-commit of egpu_bestfit_batch_dev -
+ *   d_req_core   R packed words (EGPU_PACK_REQUEST; const uint32_t* cast to the argument's type), 16-byte aligned;
+ *   d_req_mem    must be NULL;
+ *   d_out_idx    R int8 indices (int8_t* cast to the argument's type), 16-byte aligned: device or -1.
+ * Words >= 2^25 and core 101..127 are infeasible.  The demand vector pushed for `step` is the one the
+ * int32 call pushes for the requests the words stand for, so the apply calls are the same and ranks
+ * may mix formats.  Packed and int32 sharded scans may follow each other in one EGPU_F_INPUTS_READY
+ * pipelined stream.  EGPU_ERR_STATE under EGPU_VARIANT_GRID.  EGPU_ERR_INVALID, before anything is
+ * launched or written: a non-NULL d_req_mem, NULL words or indices with R > 0, misaligned words or
+ * indices. */
 #define EGPU_IPC_HANDLE_BYTES 64
 #define EGPU_MAX_RANKS 8
 int egpu_peer_export(egpu_ctx* ctx, void* handle_out);
@@ -377,7 +393,11 @@ int64_t egpu_peer_gate_timeouts(egpu_ctx* ctx);
  * advances `step` by 2.  Outputs: d_out_idx with EGPU_IDX_DEFERRED for the rows beyond the
  * cut; d_delta[2*D] = THIS rank's committed demand (may be NULL); d_table_out[3*D] =
  * table - committed demand of all ranks, identical on every rank (may be NULL);
- * EGPU_F_COMMIT installs it.  Never oversubscribes. */
+ * EGPU_F_COMMIT installs it.  Never oversubscribes.
+ * flags EGPU_F_PACKED [| EGPU_F_PREFIX_COMMIT] [| EGPU_F_COMMIT]: the same on packed words, with the
+ * arguments and refusals of the packed sharded scan (egpu_bestfit_batch_shard_dev above); d_out_idx
+ * receives int8 indices: device, -1 or EGPU_IDX_DEFERRED.  The exchange steps carry the same vectors
+ * as in the int32 call.  EGPU_ERR_STATE under EGPU_VARIANT_GRID (in either format). */
 int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core,
                                         const int32_t* d_req_mem, int64_t R,
                                         int32_t* d_out_idx, int64_t* d_delta,
@@ -390,7 +410,11 @@ int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core
  * egpu_table_apply_peers_multi_dev(first_step = last - lag + 1, lag steps) for the tail.
  * The wait for step - lag is the back-pressure: no rank gets more than `lag` steps ahead
  * of the slowest.  A sequence restarted from step 0 (a replayed CUDA graph) must be
- * separated from the previous one by a barrier across the ranks.  Never commits. */
+ * separated from the previous one by a barrier across the ranks.  Never commits.
+ * Packed: EGPU_F_PACKED AND a NULL d_req_mem run the packed sharded scan (arguments as for
+ * egpu_bestfit_batch_shard_dev with EGPU_F_PACKED; the lagged table' is the same in both formats).
+ * COMPATIBILITY: this call has never checked flags other than EGPU_F_COMMIT, so EGPU_F_PACKED with a
+ * non-NULL d_req_mem still runs the int32 scan on two int32 arrays, as it did before 1.9. */
 int egpu_bestfit_batch_shard_lag_dev(egpu_ctx* ctx, const int32_t* d_req_core,
                                      const int32_t* d_req_mem, int64_t R,
                                      int32_t* d_out_idx, int64_t* d_delta, int flags,
