@@ -37,6 +37,7 @@ F_PREFIX_COMMIT = 4
 F_APPLY = 8
 F_PACKED = 16
 F_ROUNDS = 32
+F_DEVICE_ROUNDS = 128
 IDX_DEFERRED = -2
 
 EV_ALLOC = 0

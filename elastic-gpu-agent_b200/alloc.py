@@ -121,12 +121,16 @@ class BestFitAllocator:
         self._check(rc, "egpu_bestfit_batch")
         return idx, dc, dm
 
-    def bestfit_rounds(self, req_core, req_mem, max_rounds: int = 1 << 20):
+    def bestfit_rounds(self, req_core, req_mem, max_rounds: int = 1 << 20, device: bool = False):
         """egpu_bestfit_batch_rounds: committing prefix-commit rounds until nothing is deferred.
-        Returns (idx, delta_core, delta_mem, rounds, still_deferred)."""
+        Returns (idx, delta_core, delta_mem, rounds, still_deferred).  device=True: the same rounds with no
+        round limit in one launch (egpu_bestfit_batch with EGPU_F_DEVICE_ROUNDS); max_rounds must stay at its
+        default, and rounds comes back as None (the launch does not report it) with still_deferred 0."""
         rc_, rm_ = _i32(req_core), _i32(req_mem)
         if rc_.shape != rm_.shape or rc_.ndim != 1:
             raise L.EgpuError(L.ERR_INVALID, "bestfit_rounds")
+        if device and max_rounds != 1 << 20:
+            raise ValueError("bestfit_rounds(device=True) has no round limit")
         D = self._lib.egpu_table_size(self._h)
         if D < 0:
             raise L.EgpuError(D, "egpu_table_size")
@@ -134,6 +138,11 @@ class BestFitAllocator:
         idx = np.empty(R, dtype=np.int32)
         dc = np.zeros(D, dtype=np.int64)
         dm = np.zeros(D, dtype=np.int64)
+        if device:
+            rc = self._lib.egpu_bestfit_batch(self._h, _ptr(rc_), _ptr(rm_), R, _ptr(idx), _ptr(dc), _ptr(dm),
+                                              L.F_PREFIX_COMMIT | L.F_COMMIT | L.F_ROUNDS | L.F_DEVICE_ROUNDS)
+            self._check(rc, "egpu_bestfit_batch")
+            return idx, dc, dm, None, 0
         rounds, left = C.c_int32(0), C.c_int64(0)
         rc = self._lib.egpu_bestfit_batch_rounds(self._h, _ptr(rc_), _ptr(rm_), R, _ptr(idx), _ptr(dc), _ptr(dm),
                                                  int(max_rounds), C.byref(rounds), C.byref(left))
@@ -152,6 +161,27 @@ class BestFitAllocator:
                                                      _ptr(delta), int(max_rounds), C.byref(rounds), C.byref(left), _stream(stream))
         self._check(rc, "egpu_bestfit_batch_rounds_dev")
         return delta, int(rounds.value), int(left.value)
+
+    def bestfit_rounds_device_dev(self, d_core: int, d_mem: int, R: int, d_idx: int, d_delta: int = 0, d_table_out: int = 0,
+                                  stream: int | None = None):
+        """egpu_bestfit_batch_dev with EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS:
+        the rounds of bestfit_rounds_dev with no round limit, in one launch, asynchronous on `stream` (no
+        synchronisation).  d_delta (int64[2*D]) receives the demand committed over all rounds, d_table_out
+        (int32[3*D]) the last round's table'; both may be 0."""
+        flags = L.F_PREFIX_COMMIT | L.F_COMMIT | L.F_ROUNDS | L.F_DEVICE_ROUNDS
+        rc = self._lib.egpu_bestfit_batch_dev(self._h, C.c_void_p(d_core), C.c_void_p(d_mem), int(R), C.c_void_p(d_idx),
+                                              C.c_void_p(d_delta or None), C.c_void_p(d_table_out or None), flags,
+                                              _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_dev")
+
+    def bestfit_packed_rounds_device_dev(self, d_words: int, R: int, d_idx8: int, d_delta: int = 0, d_table_out: int = 0,
+                                         stream: int | None = None):
+        """bestfit_rounds_device_dev on packed words (EGPU_F_PACKED): R words in, R int8 indices out."""
+        flags = L.F_PACKED | L.F_PREFIX_COMMIT | L.F_COMMIT | L.F_ROUNDS | L.F_DEVICE_ROUNDS
+        rc = self._lib.egpu_bestfit_batch_dev(self._h, C.c_void_p(d_words), None, int(R), C.c_void_p(d_idx8),
+                                              C.c_void_p(d_delta or None), C.c_void_p(d_table_out or None), flags,
+                                              _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_dev")
 
     def bestfit_raw(self, p_core: int, p_mem: int, R: int, p_idx: int, p_dc: int, p_dm: int, commit: bool = False):
         """Same call on raw host addresses (e.g. pinned buffers from host_alloc)."""
@@ -181,11 +211,14 @@ class BestFitAllocator:
         self._check(rc, "egpu_bestfit_batch_packed")
         return idx, dc, dm
 
-    def bestfit_packed_prefix(self, words, commit: bool = False, rounds: bool = False):
+    def bestfit_packed_prefix(self, words, commit: bool = False, rounds: bool = False, device: bool = False):
         """Prefix-commit (spec 2.5) on packed words: egpu_bestfit_batch with EGPU_F_PACKED |
         EGPU_F_PREFIX_COMMIT.  Returns (idx int8[R] with -2 = DEFERRED, delta_core int64[D], delta_mem int64[D]).
         rounds=True adds EGPU_F_ROUNDS (and commits): rounds to the fixed point, no -2 left, and the sums
-        are the demand committed over all rounds."""
+        are the demand committed over all rounds.  device=True (with rounds) adds EGPU_F_DEVICE_ROUNDS: the
+        same rounds in one launch."""
+        if device and not rounds:
+            raise ValueError("device=True needs rounds=True")
         p = np.ascontiguousarray(words, dtype=np.uint32)
         D = self._lib.egpu_table_size(self._h)
         if D < 0:
@@ -195,7 +228,7 @@ class BestFitAllocator:
         dm = np.zeros(D, dtype=np.int64)
         rc = self._lib.egpu_bestfit_batch(self._h, _ptr(p), None, p.size, _ptr(idx), _ptr(dc), _ptr(dm),
                                           L.F_PACKED | L.F_PREFIX_COMMIT | (L.F_COMMIT if commit or rounds else 0) |
-                                          (L.F_ROUNDS if rounds else 0))
+                                          (L.F_ROUNDS if rounds else 0) | (L.F_DEVICE_ROUNDS if device else 0))
         self._check(rc, "egpu_bestfit_batch")
         return idx, dc, dm
 

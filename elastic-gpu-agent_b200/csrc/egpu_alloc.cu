@@ -103,6 +103,19 @@ template <int P>
 constexpr decltype(packed_snap_kernel<P, 0>()) kPackedSnapKernels[4] = {packed_snap_kernel<P, 0>(), packed_snap_kernel<P, 1>(),
                                                                         packed_snap_kernel<P, 2>(), packed_snap_kernel<P, 3>()};
 
+// The one-launch rounds kernels (EGPU_F_DEVICE_ROUNDS): kRoundsThreads per CTA in every bucket, the
+// register scan's SnapSmem or the lookup scan's LutSmem of that CTA size, one kernel type for all.
+template <int F, RowFormat FMT, int B>
+constexpr auto rounds_kernel() {
+    constexpr int DT = 8 << B;
+    if constexpr (F == kRoundsSorted)
+        return kernel(rounds_sorted_kernel<DT, FMT>, kRoundsThreads, sizeof(SnapSmem<DT, kRoundsThreads>));
+    else return kernel(rounds_lut_kernel<FMT>, kRoundsThreads, sizeof(LutSmem<kRoundsThreads>));
+}
+template <int F, RowFormat FMT>
+constexpr decltype(rounds_kernel<F, FMT, 0>()) kRoundsKernels[4] = {rounds_kernel<F, FMT, 0>(), rounds_kernel<F, FMT, 1>(),
+                                                                   rounds_kernel<F, FMT, 2>(), rounds_kernel<F, FMT, 3>()};
+
 // Resident CTAs per SM of kernel k; `cached` is its entry in the context's occupancy cache.  The
 // first use on a context opts in to the kernel's dynamic shared memory and asks the occupancy.
 template <class Fn>
@@ -537,6 +550,39 @@ struct RoundInfo {
     long long delta[2 * kMaxD];
 };
 
+// Scratch of the rounds (run_rounds and the one-launch rounds), owned by the context, grow-only,
+// sized by R BEFORE anything is committed (a failed allocation must not leave a half-committed
+// batch): a head (round info; the one-launch rounds keep their grid-barrier words at kRoundsCtlOff),
+// tile counts, and two sets of (core, mem, caller's row, index) arrays - the deferred rows of any
+// round are at most R.  Packed: two sets of (words, caller's row, int8 index), 9 bytes per row each.
+constexpr size_t kRoundsHead = 2048;
+constexpr size_t kRoundsCtlOff = 1536;
+static_assert(sizeof(RoundInfo) <= kRoundsCtlOff && kRoundsCtlOff + sizeof(RoundsCtl) <= kRoundsHead, "rounds scratch head");
+struct RoundsScratch {
+    RoundInfo* info;
+    unsigned int* tiles;
+    int32_t* set[2][4];  // rc, rm (packed: none), map, idx
+};
+int rounds_scratch(egpu_ctx* ctx, int64_t R, bool packed, RoundsScratch* out) {
+    auto align = [](size_t b) { return (b + 255) & ~static_cast<size_t>(255); };
+    const int64_t tiles_cap = (R + kCompactTile - 1) / kCompactTile;
+    const size_t tiles_bytes = align(sizeof(unsigned int) * static_cast<size_t>(tiles_cap));
+    const size_t per = align(sizeof(int32_t) * static_cast<size_t>(R));
+    const size_t sub[4] = {per, packed ? 0 : per, per, packed ? align(static_cast<size_t>(R)) : per};  // rc, rm, map, idx
+    const size_t need = kRoundsHead + tiles_bytes + 2 * (sub[0] + sub[1] + sub[2] + sub[3]);
+    EGPU_CUDA(ctx, grow(ctx->rounds_bytes, need, need, &ctx->d_rounds));
+    char* base = static_cast<char*>(ctx->d_rounds);
+    out->info = reinterpret_cast<RoundInfo*>(base);
+    out->tiles = reinterpret_cast<unsigned int*>(base + kRoundsHead);
+    size_t off = kRoundsHead + tiles_bytes;
+    for (int a = 0; a < 2; ++a)
+        for (int b = 0; b < 4; ++b) {
+            out->set[a][b] = sub[b] ? reinterpret_cast<int32_t*>(base + off) : nullptr;
+            off += sub[b];
+        }
+    return EGPU_OK;
+}
+
 int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx, int max_rounds,
                long long* total_delta /* host [2*D] */, int32_t* rounds_out, int64_t* left_out, cudaStream_t s,
                RowFormat fmt = kRowsInt32, int32_t* d_table_out = nullptr) {
@@ -546,35 +592,18 @@ int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t 
     *rounds_out = 0;
     *left_out = 0;
     if (R == 0 || max_rounds < 1) return EGPU_OK;
-    // Scratch owned by the context, grow-only, sized by R BEFORE anything is committed (a failed
-    // allocation must not leave a half-committed batch): round info, tile counts, and two sets
-    // of (core, mem, caller's row, index) arrays - the deferred rows of any round are at most R.
-    // Packed: two sets of (words, caller's row, int8 index), 9 bytes per row each.
-    auto align = [](size_t b) { return (b + 255) & ~static_cast<size_t>(255); };
-    const int64_t tiles_cap = (R + kCompactTile - 1) / kCompactTile;
-    const size_t tiles_bytes = align(sizeof(unsigned int) * static_cast<size_t>(tiles_cap));
-    const size_t per = align(sizeof(int32_t) * static_cast<size_t>(R));
-    const size_t sub[4] = {per, packed ? 0 : per, per, packed ? align(static_cast<size_t>(R)) : per};  // rc, rm, map, idx
-    constexpr size_t kHead = 2048;  // RoundInfo
-    const size_t need = kHead + tiles_bytes + 2 * (sub[0] + sub[1] + sub[2] + sub[3]);
-    EGPU_CUDA(ctx, grow(ctx->rounds_bytes, need, need, &ctx->d_rounds));
-    static_assert(sizeof(RoundInfo) <= kHead, "round info header");
-    char* base = static_cast<char*>(ctx->d_rounds);
-    RoundInfo* d_info = reinterpret_cast<RoundInfo*>(base);
-    unsigned int* d_tiles = reinterpret_cast<unsigned int*>(base + kHead);
+    RoundsScratch sc;
+    const int rcs = rounds_scratch(ctx, R, packed, &sc);
+    if (rcs != EGPU_OK) return rcs;
+    RoundInfo* d_info = sc.info;
+    unsigned int* d_tiles = sc.tiles;
     // current round's arrays (round 1: the caller's) and the next round's
     const int32_t* cur_rc = d_rc;
     const int32_t* cur_rm = d_rm;
     const int32_t* cur_map = nullptr;
     int32_t* cur_idx = d_idx;
     int64_t n = R;
-    int32_t* set[2][4];  // rc, rm (packed: none), map, idx
-    size_t off = kHead + tiles_bytes;
-    for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 4; ++b) {
-            set[a][b] = sub[b] ? reinterpret_cast<int32_t*>(base + off) : nullptr;
-            off += sub[b];
-        }
+    int32_t* (&set)[2][4] = sc.set;
     int which = 0;
     RoundInfo h{};
     auto idx8 = [](const int32_t* p) { return reinterpret_cast<signed char*>(const_cast<int32_t*>(p)); };
@@ -643,6 +672,84 @@ int launch_packed_rounds(egpu_ctx* ctx, const int32_t* d_words, int64_t R, int32
 constexpr int kRoundsNeeds = EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS;
 bool rounds_flags_ok(int flags, int64_t R) {
     return (flags & ~(kRoundsNeeds | EGPU_F_INPUTS_READY)) == 0 && (flags & kRoundsNeeds) == kRoundsNeeds && R < (1ll << 31);
+}
+
+// The flags EGPU_F_DEVICE_ROUNDS is valid with: all of kDeviceRoundsNeeds, optionally EGPU_F_PACKED and
+// EGPU_F_INPUTS_READY
+constexpr int kDeviceRoundsNeeds = EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS;
+bool device_rounds_flags_ok(int flags, int64_t R) {
+    return (flags & ~(kDeviceRoundsNeeds | EGPU_F_PACKED | EGPU_F_INPUTS_READY)) == 0 &&
+           (flags & kDeviceRoundsNeeds) == kDeviceRoundsNeeds && R < (1ll << 31);
+}
+
+// EGPU_F_DEVICE_ROUNDS: the rounds of run_rounds with no round limit, in ONE cooperative launch of
+// rounds_sorted_kernel / rounds_lut_kernel (egpu_scan.cuh) and without a host round trip: nothing
+// here waits for the device.  Rows in either format (see prefix_scan).  d_delta (may be NULL) receives
+// the demand committed over all rounds, d_table_out (may be NULL) the last round's table'.  Scratch is
+// the rounds scratch of run_rounds, sized before the launch.
+int launch_device_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx, long long* d_delta,
+                         int32_t* d_table_out, cudaStream_t s, RowFormat fmt) {
+    if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // no prefix-commit mode
+    const bool lut = lut_variant(ctx), packed = fmt == kRowsPacked;
+    const int bucket = d_bucket(ctx->D);
+    const auto& k = lut ? (packed ? kRoundsKernels<kRoundsLut, kRowsPacked> : kRoundsKernels<kRoundsLut, kRowsInt32>)[bucket]
+                        : (packed ? kRoundsKernels<kRoundsSorted, kRowsPacked> : kRoundsKernels<kRoundsSorted, kRowsInt32>)[bucket];
+    int per_sm = 0;
+    int rc = resident_ctas(ctx, k, ctx->rounds_ctas_per_sm[lut ? kRoundsLut : kRoundsSorted][packed][bucket], &per_sm);
+    if (rc != EGPU_OK) return rc;
+    // Grid: as many CTAs as round 1's scan wants at 8 rows per thread (the lone-launch rule of
+    // launch_snapshot_as), at most one resident wave (the grid barriers need every CTA resident) and at
+    // least one CTA per device (CTA d cuts device d).
+    if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
+    const int64_t wave = static_cast<int64_t>(ctx->sm_count) * per_sm;
+    const int64_t per_cta = static_cast<int64_t>(kRoundsThreads) * 2;  // 128-bit vectors of 4 rows
+    int64_t grid = ((R >> 2) + per_cta - 1) / per_cta;
+    if (grid > wave) grid = wave;
+    if (grid < ctx->D) grid = ctx->D;
+    if (grid > wave) return EGPU_ERR_STATE;  // fewer resident CTAs than devices: not on an H100
+    // every allocation before the launch, so that a failure commits nothing
+    RoundsScratch sc;
+    rc = rounds_scratch(ctx, R, packed, &sc);
+    if (rc != EGPU_OK) return rc;
+    const size_t sums_bytes = sizeof(unsigned long long) * 2 * kMaxD * static_cast<size_t>(grid);
+    EGPU_CUDA(ctx, grow(ctx->tile_bytes, sums_bytes, sums_bytes, &ctx->d_tile_sums));
+    if (!ctx->d_prefix_out) EGPU_CUDA(ctx, cudaMalloc(&ctx->d_prefix_out, sizeof(PrefixOut) + sizeof(long long) * 2 * kMaxD));
+    RoundsCtl* ctl = reinterpret_cast<RoundsCtl*>(reinterpret_cast<char*>(ctx->d_rounds) + kRoundsCtlOff);
+    if (ctx->rounds_ctl_bytes != ctx->rounds_bytes) {  // fresh scratch: the barrier words start at zero
+        EGPU_CUDA(ctx, cudaMemsetAsync(ctl, 0, sizeof(RoundsCtl), s));
+        ctx->rounds_ctl_bytes = ctx->rounds_bytes;
+    }
+    RoundsArgs a;
+    std::memset(&a, 0, sizeof a);
+    a.rc = d_rc;
+    a.rm = packed ? nullptr : d_rm;
+    a.R = static_cast<long long>(R);
+    a.idx = d_idx;
+    a.delta_out = d_delta;
+    a.table_out = d_table_out;
+    a.tile_sums = ctx->d_tile_sums;
+    a.pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
+    a.total = sc.info->delta;
+    a.deferred = &sc.info->deferred;
+    a.tile_count = sc.tiles;
+    std::memcpy(a.set, sc.set, sizeof a.set);
+    a.ctl = ctl;
+    a.lut = ctx->d_lut;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.blockDim = dim3(static_cast<unsigned>(k.threads));
+    cfg.dynamicSmemBytes = k.smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;  // the runtime refuses a grid it cannot co-schedule
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, k.fn, ctx->d_state, a));
+    ctx->launches += 1;
+    ctx->prev_is_scan = false;
+    ctx->lut_dirty = !lut;  // the lookup kernels leave d_lut built from the table they committed
+    return EGPU_OK;
 }
 
 // Prefix-commit over row shards (one rank per GPU, rank-major row order).  Two exchange
@@ -756,7 +863,8 @@ extern "C" {
 // 1.7: + EGPU_F_PACKED prefix-commit on egpu_bestfit_batch / egpu_bestfit_batch_dev (additive)
 // 1.8: + EGPU_F_ROUNDS, packed prefix-commit rounds on the same two entry points (additive)
 // 1.9: + EGPU_F_PACKED on egpu_bestfit_batch_shard_dev, _shard_lag_dev and _shard_prefix_dev (additive)
-int egpu_abi_version(void) { return 1009; }
+// 1.10: + EGPU_F_DEVICE_ROUNDS, rounds in one launch on egpu_bestfit_batch / egpu_bestfit_batch_dev (additive)
+int egpu_abi_version(void) { return 1010; }
 
 const char* egpu_strerror(int code) {
     switch (code) {
@@ -969,9 +1077,12 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32
     // EGPU_F_PACKED: prefix-commit only, d_req_core = words, d_req_mem NULL, d_out_idx = int8 indices.
     // Without it a NULL d_req_mem (R > 0) stays refused, so words are never read as int32 arrays.
     // EGPU_F_ROUNDS: that, committing, to the fixed point; synchronises the stream.
+    // EGPU_F_DEVICE_ROUNDS: rounds to the fixed point in either format, in one launch, asynchronous.
     const bool packed = (flags & EGPU_F_PACKED) != 0;
     const bool rounds = (flags & EGPU_F_ROUNDS) != 0;
-    if (!ctx || R < 0 || (rounds && !rounds_flags_ok(flags, R))) return EGPU_ERR_INVALID;
+    const bool device_rounds = (flags & EGPU_F_DEVICE_ROUNDS) != 0;
+    if (!ctx || R < 0 || (device_rounds ? !device_rounds_flags_ok(flags, R) : rounds && !rounds_flags_ok(flags, R)))
+        return EGPU_ERR_INVALID;
     if (packed ? (!(flags & EGPU_F_PREFIX_COMMIT) || d_req_mem || !rows_ok(R, {d_req_core, d_out_idx}))
                : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
         return EGPU_ERR_INVALID;
@@ -979,6 +1090,9 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
+    if (device_rounds)
+        return launch_device_rounds(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, s,
+                                    packed ? kRowsPacked : kRowsInt32);
     if (rounds) {
         long long total[2 * kMaxD];
         rc = launch_packed_rounds(ctx, d_req_core, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, total, s);
@@ -1119,7 +1233,9 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     const bool prefix = (commit & EGPU_F_PREFIX_COMMIT) != 0;
     const bool packed = (commit & EGPU_F_PACKED) != 0;
     const bool rounds = (commit & EGPU_F_ROUNDS) != 0;
-    if (!ctx || R < 0 || (rounds && !rounds_flags_ok(commit, R))) return EGPU_ERR_INVALID;
+    const bool device_rounds = (commit & EGPU_F_DEVICE_ROUNDS) != 0;
+    if (!ctx || R < 0 || (device_rounds ? !device_rounds_flags_ok(commit, R) : rounds && !rounds_flags_ok(commit, R)))
+        return EGPU_ERR_INVALID;
     if (packed ? (!prefix || req_mem || (R > 0 && (!req_core || !out_idx))) : (R > 0 && (!req_core || !req_mem || !out_idx)))
         return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
@@ -1127,6 +1243,33 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     int rc = enter(ctx, kNeedsTable, nullptr, &s);
     if (rc != EGPU_OK) return rc;
     const int D = ctx->D;
+    if (device_rounds) {  // one launch, staged through HBM: int32 8 bytes per row in and 4 out, packed 4 in and 1 out
+        rc = ensure_staging(ctx, R > 0 ? R : 1);
+        if (rc != EGPU_OK) return rc;
+        if (R > 0) {
+            EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
+            if (!packed) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
+        }
+        rc = launch_device_rounds(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, s,
+                                  packed ? kRowsPacked : kRowsInt32);
+        if (rc != EGPU_OK) return rc;
+        const size_t idx_bytes = packed ? sizeof(int8_t) : sizeof(int32_t);
+        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, idx_bytes * R, cudaMemcpyDeviceToHost, s));
+        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
+        unsigned long long timeouts = 0;
+        EGPU_CUDA(ctx, cudaMemcpyAsync(&timeouts, reinterpret_cast<char*>(ctx->d_state) + offsetof(DevState, rounds_timeouts),
+                                       sizeof timeouts, cudaMemcpyDeviceToHost, s));
+        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
+        if (timeouts != ctx->rounds_timeouts_seen) {  // this launch, or a _dev launch since the last check, gave up
+            ctx->rounds_timeouts_seen = timeouts;
+            std::snprintf(ctx->last_err, sizeof ctx->last_err,
+                          "EGPU_F_DEVICE_ROUNDS: a grid barrier waited more than 2 s and the launch gave up (%llu so far)", timeouts);
+            return EGPU_ERR_CUDA;
+        }
+        if (out_delta_core) std::memcpy(out_delta_core, ctx->h_delta, sizeof(int64_t) * D);
+        if (out_delta_mem) std::memcpy(out_delta_mem, ctx->h_delta + D, sizeof(int64_t) * D);
+        return EGPU_OK;
+    }
     if (rounds) {  // packed rounds to the fixed point, staged through HBM: 4 bytes per row in, 1 out
         long long total[2 * kMaxD];
         rc = ensure_staging(ctx, R > 0 ? R : 1);

@@ -24,6 +24,8 @@ enum PackedFamily { kPackedSortedMulti, kPackedLutMulti, kPackedFamilies };
 enum PackedContigFamily { kPackedSortedContig, kPackedLutContig, kPackedContigFamilies };
 // The packed sharded scans (round-robin tiles; egpu_bestfit_batch_shard[_lag]_dev with EGPU_F_PACKED), per D bucket
 enum PackedSnapFamily { kPackedSortedSnap, kPackedLutSnap, kPackedSnapFamilies };
+// The one-launch rounds (EGPU_F_DEVICE_ROUNDS), per row format and D bucket
+enum DeviceRoundsFamily { kRoundsSorted, kRoundsLut, kRoundsFamilies };
 
 struct egpu_ctx {
     std::mutex mu;
@@ -31,6 +33,7 @@ struct egpu_ctx {
     int packed_ctas_per_sm[kPackedFamilies][4] = {};  // ... and of each packed multi-batch kernel
     int packed_contig_ctas_per_sm[kPackedContigFamilies][4] = {};  // ... and of each packed prefix-commit scan
     int packed_snap_ctas_per_sm[kPackedSnapFamilies][4] = {};  // ... and of each packed sharded scan
+    int rounds_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each one-launch rounds kernel ([family][packed][bucket])
     void* h_qtable = nullptr;         // pinned host image of that table (the part of DevState before `peer`)
     DevState* d_qstate = nullptr;     // scratch table of egpu_bestfit_query (the context's own table is not touched)
     unsigned long long* h_gate = nullptr;      // pinned: start gates the host has opened (egpu_peer_gate_open)
@@ -40,6 +43,8 @@ struct egpu_ctx {
     void* d_prefix_out = nullptr;     // PrefixOut
     void* d_rounds = nullptr;         // scratch of egpu_bestfit_batch_rounds (grow-only)
     size_t rounds_bytes = 0;
+    size_t rounds_ctl_bytes = 0;      // rounds_bytes when the grid-barrier words in d_rounds were last zeroed
+    unsigned long long rounds_timeouts_seen = 0;  // DevState::rounds_timeouts as the host form last read it
     DevLut* d_lut = nullptr;
     XchgBuf* d_xchg = nullptr;        // this rank's exchange buffer (exported to the peers over CUDA IPC)
     void* peer_open[kMaxRanks] = {};  // peers' buffers as opened here (nullptr for own rank)

@@ -344,12 +344,10 @@ __device__ __forceinline__ void epilogue_publish(const unsigned long long* wacc,
     if (tid == 0) ep.ticket = 0u;
 }
 
-// Demand sums -> global running sums -> (last CTA) delta / table' publication.
+// Lane-private demand sums -> per-warp sums in s.sWarpAcc (core of device d at [warp][d], mem at
+// [warp][DT + d]); the caller synchronises the CTA before it reads them.
 template <int DT, int THREADS>
-__device__ __forceinline__ void snapshot_epilogue(SnapSmem<DT, THREADS>& s, DevState* st, int D,
-                                                  long long* __restrict__ delta_out,
-                                                  int32_t* __restrict__ table_out, int flags, const EpiCtl& ec,
-                                                  unsigned long long* __restrict__ tile_sums = nullptr) {
+__device__ __forceinline__ void hist_to_warp_sums(SnapSmem<DT, THREADS>& s, int D) {
     const int tid = threadIdx.x;
     const int lane = tid & 31;
     const int warp = tid >> 5;
@@ -367,6 +365,15 @@ __device__ __forceinline__ void snapshot_epilogue(SnapSmem<DT, THREADS>& s, DevS
             s.sWarpAcc[warp][DT + d] = static_cast<unsigned long long>(sl) + (static_cast<unsigned long long>(sh) << 19);
         }
     }
+}
+
+// Demand sums -> global running sums -> (last CTA) delta / table' publication.
+template <int DT, int THREADS>
+__device__ __forceinline__ void snapshot_epilogue(SnapSmem<DT, THREADS>& s, DevState* st, int D,
+                                                  long long* __restrict__ delta_out,
+                                                  int32_t* __restrict__ table_out, int flags, const EpiCtl& ec,
+                                                  unsigned long long* __restrict__ tile_sums = nullptr) {
+    hist_to_warp_sums<DT, THREADS>(s, D);
     __syncthreads();
     epilogue_publish<THREADS / 32>(&s.sWarpAcc[0][0], 2 * DT, 0, DT, s.sFc, s.sFm, s.sPosDev, &s.sLast, st, D, delta_out,
                                    table_out, flags, ec, tile_sums);
@@ -387,13 +394,29 @@ __device__ __forceinline__ uint32_t packed_request_word(uint32_t pw) {
 // and the demand sums are the same code.
 enum RowFormat { kRowsInt32, kRowsPacked };
 
+// How a scan reads its request rows (and the lookup scan its table).  kLoadStream: the streaming
+// ld.global.nc of every standalone scan, for rows nothing in the launch writes.  kLoadCoherent:
+// ld.global.cg, for rows another CTA of the SAME launch may have written (the compacted rows and the
+// rebuilt lookup table of rounds_*_kernel): the non-coherent path could return a stale line.
+enum RowLoad { kLoadStream, kLoadCoherent };
+template <RowLoad LD>
+__device__ __forceinline__ int4 ld_rows_v4(const int4* p) {
+    if constexpr (LD == kLoadStream) return ld_stream_v4(p);
+    else return __ldcg(p);
+}
+template <RowLoad LD, class T>
+__device__ __forceinline__ T ld_row(const T* p) {
+    if constexpr (LD == kLoadStream) return *p;
+    else return __ldcg(p);
+}
+
 // The scan of one batch by one CTA: tile `tile` of `n_tiles` (in a single-batch launch the grid's
 // CTAs are the tiles; in a multi-batch launch every batch has its own run of tiles).
 // CONTIG = false: vectors are dealt round-robin over the batch's tiles (the product mapping).
 // CONTIG = true (prefix-commit mode): tile b scans the contiguous rows of "tile" b and the
 // epilogue leaves its per-device sums in tile_sums[b][*]; everything else is the same code.
 // Returns D.  Leaves the demand sums in s.hist; the caller runs snapshot_epilogue.
-template <int DT, int THREADS, bool CONTIG, RowFormat FMT = kRowsInt32>
+template <int DT, int THREADS, bool CONTIG, RowFormat FMT = kRowsInt32, RowLoad LD = kLoadStream>
 __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevState* __restrict__ st,
                                                 const int32_t* __restrict__ req_core, const int32_t* __restrict__ req_mem,
                                                 long long R, int32_t* __restrict__ out_idx, int tile_i, int n_tiles) {
@@ -422,12 +445,12 @@ __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevSta
     int4 c0 = make_int4(0, 0, 0, 0), m0 = c0, c1 = c0, m1 = c0;
     bool has0 = v < nvec, has1 = (v + stride) < nvec;
     if (has0) {
-        c0 = ld_stream_v4(vc + v);
-        if constexpr (!packed) m0 = ld_stream_v4(vm + v);
+        c0 = ld_rows_v4<LD>(vc + v);
+        if constexpr (!packed) m0 = ld_rows_v4<LD>(vm + v);
     }
     if (has1) {
-        c1 = ld_stream_v4(vc + (v + stride));
-        if constexpr (!packed) m1 = ld_stream_v4(vm + (v + stride));
+        c1 = ld_rows_v4<LD>(vc + (v + stride));
+        if constexpr (!packed) m1 = ld_rows_v4<LD>(vm + (v + stride));
     }
 
     // sorted table rows: uniform loads straight into registers, no barrier
@@ -477,12 +500,12 @@ __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevSta
         const bool nhas0 = vn < nvec, nhas1 = (vn + stride) < nvec;
         int4 nc0 = make_int4(0, 0, 0, 0), nm0 = nc0, nc1 = nc0, nm1 = nc0;
         if (nhas0) {
-            nc0 = ld_stream_v4(vc + vn);
-            if constexpr (!packed) nm0 = ld_stream_v4(vm + vn);
+            nc0 = ld_rows_v4<LD>(vc + vn);
+            if constexpr (!packed) nm0 = ld_rows_v4<LD>(vm + vn);
         }
         if (nhas1) {
-            nc1 = ld_stream_v4(vc + (vn + stride));
-            if constexpr (!packed) nm1 = ld_stream_v4(vm + (vn + stride));
+            nc1 = ld_rows_v4<LD>(vc + (vn + stride));
+            if constexpr (!packed) nm1 = ld_rows_v4<LD>(vm + (vn + stride));
         }
         if constexpr (packed) {
             st_stream_u32(vo8 + v, decide4_words(c0));
@@ -500,9 +523,10 @@ __device__ __forceinline__ int sorted_scan_rows(SnapSmem<DT, THREADS>& s, DevSta
     if (tile_i == (CONTIG ? n_tiles - 1 : 0) && tid < static_cast<int>(R & 3)) {
         const long long r = ((R >> 2) << 2) + tid;
         if constexpr (packed)
-            reinterpret_cast<signed char*>(out_idx)[r] = static_cast<signed char>(decide_word(reinterpret_cast<const uint32_t*>(req_core)[r]));
+            reinterpret_cast<signed char*>(out_idx)[r] =
+                static_cast<signed char>(decide_word(ld_row<LD>(reinterpret_cast<const uint32_t*>(req_core) + r)));
         else
-            out_idx[r] = decide(req_core[r], req_mem[r]);
+            out_idx[r] = decide(ld_row<LD>(req_core + r), ld_row<LD>(req_mem + r));
     }
     return D;
 }
@@ -782,9 +806,8 @@ bestfit_grid_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_c
 // fine for D = 8 (HBM-bound), ALU-bound by 4x at D = 64.  The lookup form needs two
 // shared-memory reads and ~25 instructions per request whatever D is.
 
-// Builds DevLut from the sorted view in DevState.  One CTA; runs after every table change.
-__global__ void __launch_bounds__(256)
-lut_build_kernel(const DevState* __restrict__ st, DevLut* __restrict__ lut) {
+// Builds DevLut from the sorted view in DevState.  One CTA of >= 128 threads; runs after every table change.
+__device__ __forceinline__ void lut_build_cta(const DevState* __restrict__ st, DevLut* __restrict__ lut) {
     __shared__ uint32_t sFm[kMaxD], sFcs[kMaxD], sV[kMaxD + 4];
     __shared__ int sFirst[kMaxD], sRidx[kMaxD], sNv, sBlocks;
     __shared__ uint8_t sA[kLutStride * kLutStride];  // a[srow][rank]: first device at or after srow with ridx >= rank
@@ -865,6 +888,11 @@ lut_build_kernel(const DevState* __restrict__ st, DevLut* __restrict__ lut) {
     }
 }
 
+__global__ void __launch_bounds__(256)
+lut_build_kernel(const DevState* __restrict__ st, DevLut* __restrict__ lut) {
+    lut_build_cta(st, lut);
+}
+
 // Demand sums of the lookup scan.  64-bit shared-memory adds compile to CAS loops on sm_90a
 // (ATOMS.CAST.SPIN.64) and lane-private 64-bit sums cost 16.6 KB per warp; what is used instead is
 // native 32-bit ATOMS.ADD: two UNCONDITIONAL adds per request - word 0 = core | (mem >> 16) << 20,
@@ -903,7 +931,7 @@ __device__ __forceinline__ void unpack_request(uint32_t pw, int32_t& core, int32
 // Leaves the warp sums in sm.sWarpAcc; the caller synchronises and runs epilogue_publish.
 // Packed rows (FMT = kRowsPacked) are decoded into the int32 form as they are loaded; the trip is the
 // same two 4-row vectors per lane, so kLutFlushTrips holds for both formats.
-template <int THREADS, bool CONTIG, RowFormat FMT = kRowsInt32>
+template <int THREADS, bool CONTIG, RowFormat FMT = kRowsInt32, RowLoad LD = kLoadStream>
 __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __restrict__ st,
                                              const int32_t* __restrict__ req_core, const int32_t* __restrict__ req_mem,
                                              long long R, int32_t* __restrict__ out_idx, const DevLut* __restrict__ glut,
@@ -937,25 +965,25 @@ __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __r
     bool has0 = v < nvec, has1 = (v + stride) < nvec;
     if (has0) {
         if constexpr (packed) {
-            unpack4(ld_stream_v4(vc + v), c0, m0);
+            unpack4(ld_rows_v4<LD>(vc + v), c0, m0);
         } else {
-            c0 = ld_stream_v4(vc + v);
-            m0 = ld_stream_v4(vm + v);
+            c0 = ld_rows_v4<LD>(vc + v);
+            m0 = ld_rows_v4<LD>(vm + v);
         }
     }
     if (has1) {
         if constexpr (packed) {
-            unpack4(ld_stream_v4(vc + (v + stride)), c1, m1);
+            unpack4(ld_rows_v4<LD>(vc + (v + stride)), c1, m1);
         } else {
-            c1 = ld_stream_v4(vc + (v + stride));
-            m1 = ld_stream_v4(vm + (v + stride));
+            c1 = ld_rows_v4<LD>(vc + (v + stride));
+            m1 = ld_rows_v4<LD>(vm + (v + stride));
         }
     }
     // shared-memory tile of the lookup tables (15 KB, L2-resident source)
     {
         const uint4* src = reinterpret_cast<const uint4*>(glut);
         uint4* dst = reinterpret_cast<uint4*>(&sm.lut);
-        for (int i = tid; i < static_cast<int>(sizeof(DevLut) / 16); i += THREADS) dst[i] = src[i];
+        for (int i = tid; i < static_cast<int>(sizeof(DevLut) / 16); i += THREADS) dst[i] = ld_row<LD>(src + i);
     }
     const int D = st->D;
     {  // zero this warp's 32-bit tables
@@ -1042,18 +1070,18 @@ __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __r
         int4 nc0 = make_int4(-1, -1, -1, -1), nm0 = nc0, nc1 = nc0, nm1 = nc0;
         if (nhas0) {
             if constexpr (packed) {
-                unpack4(ld_stream_v4(vc + vn), nc0, nm0);
+                unpack4(ld_rows_v4<LD>(vc + vn), nc0, nm0);
             } else {
-                nc0 = ld_stream_v4(vc + vn);
-                nm0 = ld_stream_v4(vm + vn);
+                nc0 = ld_rows_v4<LD>(vc + vn);
+                nm0 = ld_rows_v4<LD>(vm + vn);
             }
         }
         if (nhas1) {
             if constexpr (packed) {
-                unpack4(ld_stream_v4(vc + (vn + stride)), nc1, nm1);
+                unpack4(ld_rows_v4<LD>(vc + (vn + stride)), nc1, nm1);
             } else {
-                nc1 = ld_stream_v4(vc + (vn + stride));
-                nm1 = ld_stream_v4(vm + (vn + stride));
+                nc1 = ld_rows_v4<LD>(vc + (vn + stride));
+                nm1 = ld_rows_v4<LD>(vm + (vn + stride));
             }
         }
         // no branch around the lookups (lanes past the end carry infeasible requests): the eight
@@ -1079,12 +1107,12 @@ __device__ __forceinline__ int lut_scan_rows(LutSmem<THREADS>& sm, DevState* __r
         const long long r = ((R >> 2) << 2) + lane;
         if constexpr (packed) {
             int32_t c = -1, m = -1;
-            if (mine) unpack_request(reinterpret_cast<const uint32_t*>(req_core)[r], c, m);
+            if (mine) unpack_request(ld_row<LD>(reinterpret_cast<const uint32_t*>(req_core) + r), c, m);
             const uint32_t dev = lookup(c, m);
             if (mine) reinterpret_cast<signed char*>(out_idx)[r] = static_cast<signed char>(dev);
             add1(dev, c, m);
         } else {
-            const int32_t c = mine ? req_core[r] : -1, m = mine ? req_mem[r] : -1;
+            const int32_t c = mine ? ld_row<LD>(req_core + r) : -1, m = mine ? ld_row<LD>(req_mem + r) : -1;
             const uint32_t dev = lookup(c, m);
             if (mine) out_idx[r] = static_cast<int32_t>(static_cast<int8_t>(dev));
             add1(dev, c, m);
@@ -1546,8 +1574,8 @@ prefix_cut_packed_shard_kernel(const DevState* __restrict__ st, const signed cha
                                 n_tiles, tile_sums, out, base);
 }
 
-__global__ void __launch_bounds__(256)
-prefix_apply_kernel(const PrefixOut* __restrict__ pf, int D, long long R, int32_t* __restrict__ idx) {
+// Rewrite of the deferred indices, a grid-stride loop over the launch's CTAs.
+__device__ __forceinline__ void prefix_apply_rows(const PrefixOut* __restrict__ pf, int D, long long R, int32_t* __restrict__ idx) {
     __shared__ long long sCut[kMaxD];
     if (threadIdx.x < kMaxD) sCut[threadIdx.x] = threadIdx.x < D ? pf->cut[threadIdx.x] : 0;
     __syncthreads();
@@ -1558,10 +1586,15 @@ prefix_apply_kernel(const PrefixOut* __restrict__ pf, int D, long long R, int32_
     }
 }
 
-// prefix_apply_kernel on int8 indices (16-byte aligned): four of them per 32-bit word and thread,
-// rewritten only when one of them is deferred; the R % 4 tail rows by the first threads of block 0.
 __global__ void __launch_bounds__(256)
-prefix_apply_packed_kernel(const PrefixOut* __restrict__ pf, int D, long long R, signed char* __restrict__ idx) {
+prefix_apply_kernel(const PrefixOut* __restrict__ pf, int D, long long R, int32_t* __restrict__ idx) {
+    prefix_apply_rows(pf, D, R, idx);
+}
+
+// prefix_apply_rows on int8 indices (16-byte aligned): four of them per 32-bit word and thread,
+// rewritten only when one of them is deferred; the R % 4 tail rows by the first threads of block 0.
+__device__ __forceinline__ void prefix_apply_packed_rows(const PrefixOut* __restrict__ pf, int D, long long R,
+                                                         signed char* __restrict__ idx) {
     __shared__ long long sCut[kMaxD];
     if (threadIdx.x < kMaxD) sCut[threadIdx.x] = threadIdx.x < D ? pf->cut[threadIdx.x] : 0;
     __syncthreads();
@@ -1585,9 +1618,14 @@ prefix_apply_packed_kernel(const PrefixOut* __restrict__ pf, int D, long long R,
     }
 }
 
-__global__ void __launch_bounds__(kMaxD)
-prefix_finalize_kernel(DevState* __restrict__ st, const PrefixOut* __restrict__ pf, long long* __restrict__ delta_out,
-                       int32_t* __restrict__ table_out, int commit) {
+__global__ void __launch_bounds__(256)
+prefix_apply_packed_kernel(const PrefixOut* __restrict__ pf, int D, long long R, signed char* __restrict__ idx) {
+    prefix_apply_packed_rows(pf, D, R, idx);
+}
+
+// delta / table' of the committed rows; commit installs table' and re-sorts.  One CTA of >= kMaxD threads.
+__device__ __forceinline__ void prefix_finalize_cta(DevState* __restrict__ st, const PrefixOut* __restrict__ pf,
+                                                    long long* __restrict__ delta_out, int32_t* __restrict__ table_out, int commit) {
     __shared__ int32_t sFc[kMaxD], sFm[kMaxD], sPosDev[kMaxD];
     const int D = st->D;
     const int d = threadIdx.x;
@@ -1612,6 +1650,12 @@ prefix_finalize_kernel(DevState* __restrict__ st, const PrefixOut* __restrict__ 
         }
     }
     if (commit) resort_table_cta(st, D, sFc, sFm, sPosDev, d);
+}
+
+__global__ void __launch_bounds__(kMaxD)
+prefix_finalize_kernel(DevState* __restrict__ st, const PrefixOut* __restrict__ pf, long long* __restrict__ delta_out,
+                       int32_t* __restrict__ table_out, int commit) {
+    prefix_finalize_cta(st, pf, delta_out, table_out, commit);
 }
 
 // Prefix-commit across GPUs (spec 2.5 "rank-major across shards").  The global row order is
@@ -1687,9 +1731,10 @@ __device__ __forceinline__ unsigned int deferred_mask_packed(const signed char* 
 }
 
 template <RowFormat FMT>
-__device__ __forceinline__ void deferred_count_cta(const int32_t* __restrict__ idx, long long n, unsigned int* __restrict__ tile_count) {
+__device__ __forceinline__ void deferred_count_cta(const int32_t* __restrict__ idx, long long n, unsigned int* __restrict__ tile_count,
+                                                   unsigned int tile) {
     __shared__ unsigned int sWarp[8];
-    const long long r0 = static_cast<long long>(blockIdx.x) * kCompactTile + 4ll * threadIdx.x;
+    const long long r0 = static_cast<long long>(tile) * kCompactTile + 4ll * threadIdx.x;
     unsigned int c = 0;
     if constexpr (FMT == kRowsPacked) {
         c = __popc(deferred_mask_packed(reinterpret_cast<const signed char*>(idx), r0, n));
@@ -1703,18 +1748,18 @@ __device__ __forceinline__ void deferred_count_cta(const int32_t* __restrict__ i
     if (threadIdx.x == 0) {
         unsigned int t = 0;
         for (int w = 0; w < 8; ++w) t += sWarp[w];
-        tile_count[blockIdx.x] = t;
+        tile_count[tile] = t;
     }
 }
 
 __global__ void __launch_bounds__(256)
 deferred_count_kernel(const int32_t* __restrict__ idx, long long n, unsigned int* __restrict__ tile_count) {
-    deferred_count_cta<kRowsInt32>(idx, n, tile_count);
+    deferred_count_cta<kRowsInt32>(idx, n, tile_count, blockIdx.x);
 }
 
 __global__ void __launch_bounds__(256)
 deferred_count_packed_kernel(const signed char* __restrict__ idx, long long n, unsigned int* __restrict__ tile_count) {
-    deferred_count_cta<kRowsPacked>(reinterpret_cast<const int32_t*>(idx), n, tile_count);
+    deferred_count_cta<kRowsPacked>(reinterpret_cast<const int32_t*>(idx), n, tile_count, blockIdx.x);
 }
 
 // exclusive scan of the tile counts in place; one CTA walks them 1024 at a time
@@ -1759,11 +1804,11 @@ template <RowFormat FMT>
 __device__ __forceinline__ void deferred_scatter_cta(const int32_t* __restrict__ idx, const int32_t* __restrict__ rc,
                                                      const int32_t* __restrict__ rm, const int32_t* __restrict__ map, long long n,
                                                      const unsigned int* __restrict__ tile_off, int32_t* __restrict__ out_rc,
-                                                     int32_t* __restrict__ out_rm, int32_t* __restrict__ out_map) {
+                                                     int32_t* __restrict__ out_rm, int32_t* __restrict__ out_map, unsigned int tile) {
     constexpr bool packed = FMT == kRowsPacked;
     __shared__ unsigned int sWarp[8];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long r0 = static_cast<long long>(blockIdx.x) * kCompactTile + 4ll * threadIdx.x;
+    const long long r0 = static_cast<long long>(tile) * kCompactTile + 4ll * threadIdx.x;
     bool f[4];
     unsigned int c = 0;
     if constexpr (packed) {
@@ -1786,7 +1831,7 @@ __device__ __forceinline__ void deferred_scatter_cta(const int32_t* __restrict__
     }
     if (lane == 31) sWarp[warp] = x;
     __syncthreads();
-    unsigned int pos = tile_off[blockIdx.x] + x - c;
+    unsigned int pos = tile_off[tile] + x - c;
     for (int w = 0; w < warp; ++w) pos += sWarp[w];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -1804,7 +1849,7 @@ deferred_scatter_kernel(const int32_t* __restrict__ idx, const int32_t* __restri
                         const int32_t* __restrict__ map /* nullptr: the rows are the caller's own */, long long n,
                         const unsigned int* __restrict__ tile_off, int32_t* __restrict__ out_rc, int32_t* __restrict__ out_rm,
                         int32_t* __restrict__ out_map) {
-    deferred_scatter_cta<kRowsInt32>(idx, rc, rm, map, n, tile_off, out_rc, out_rm, out_map);
+    deferred_scatter_cta<kRowsInt32>(idx, rc, rm, map, n, tile_off, out_rc, out_rm, out_map, blockIdx.x);
 }
 
 // the deferred rows' words (and caller's rows) of int8 indices idx into dense out_words / out_map
@@ -1814,7 +1859,7 @@ deferred_scatter_packed_kernel(const signed char* __restrict__ idx, const uint32
                                const unsigned int* __restrict__ tile_off, uint32_t* __restrict__ out_words,
                                int32_t* __restrict__ out_map) {
     deferred_scatter_cta<kRowsPacked>(reinterpret_cast<const int32_t*>(idx), reinterpret_cast<const int32_t*>(words), nullptr, map, n,
-                                      tile_off, reinterpret_cast<int32_t*>(out_words), nullptr, out_map);
+                                      tile_off, reinterpret_cast<int32_t*>(out_words), nullptr, out_map, blockIdx.x);
 }
 
 // a later round's answers (device, -1 or still -2) back to the caller's rows
@@ -1844,6 +1889,251 @@ __global__ void __launch_bounds__(256)
 round_writeback_packed_kernel(const signed char* __restrict__ idx_k, const int32_t* __restrict__ map, long long n,
                               signed char* __restrict__ out_idx) {
     round_writeback_rows<kRowsPacked>(reinterpret_cast<const int32_t*>(idx_k), map, n, reinterpret_cast<int32_t*>(out_idx));
+}
+
+// =============================================================================
+// Rounds in one launch (EGPU_F_DEVICE_ROUNDS): the rounds above, host loop and all, as one
+// persistent grid
+// =============================================================================
+//
+// One resident wave (cooperative launch: the runtime refuses a grid it cannot co-schedule) runs
+// every round.  A round is six phases separated by grid barriers:
+//   1. CONTIG scan of the round's rows, tile b = CTA b, per-tile sums (round 1 reads the caller's
+//      arrays, later rounds the compacted scratch set);
+//   2. the cut of device d by CTA d < D (prefix_cut_cta);
+//   3. deferred indices -> -2 by every CTA; CTA 0 adds the committed demand to the running totals,
+//      commits and re-sorts the table, writes table' and (lookup kernels) rebuilds the lookup table;
+//   4. a later round's indices back to the caller's rows, deferred rows counted per 1024-row tile;
+//   5. CTA 0 turns the counts into offsets; every CTA reads the total and leaves if it is 0;
+//   6. the deferred rows, in order, into the other scratch set.
+// Everything a phase reads that another CTA wrote in this launch is read with coherent loads
+// (kLoadCoherent scans, plain or .cg loads elsewhere; never the non-coherent path).
+constexpr int kRoundsThreads = 256;
+constexpr unsigned long long kRoundsBarrierTimeoutNs = 2000000000ull;  // the ~2 s bound of every device wait
+
+// Grid-barrier words of a rounds launch, in the context's rounds scratch.  Zero when allocated, and
+// every launch leaves them zero (except gen, which only counts up).
+struct RoundsCtl {
+    unsigned int arrive;  // CTAs at the current barrier
+    unsigned int gen;     // barriers completed: the word a waiting CTA watches
+    unsigned int abort;   // a CTA gave up waiting: every CTA leaves at its next barrier
+    unsigned int exited;  // CTAs that have left the launch; the last one re-zeroes arrive, abort and exited
+};
+
+struct RoundsArgs {
+    const int32_t* rc;             // round 1: the caller's rows (packed: the words)
+    const int32_t* rm;             // ... and mem (packed: nullptr)
+    long long R;
+    int32_t* idx;                  // the caller's indices (packed: int8)
+    long long* delta_out;          // int64[2*D] or nullptr: demand committed over all rounds
+    int32_t* table_out;            // int32[3*D] or nullptr: the last round's table'
+    unsigned long long* tile_sums; // [grid][2*kMaxD]
+    PrefixOut* pf;
+    long long* total;              // [2*kMaxD]: demand committed so far, core [0, D), mem [D, 2D)
+    unsigned long long* deferred;  // rows the last round deferred
+    unsigned int* tile_count;      // per compaction tile: deferred rows, then their exclusive offsets
+    int32_t* set[2][4];            // two scratch sets: rows (packed: words), mem (packed: none), caller's row, index
+    RoundsCtl* ctl;
+    DevLut* lut;                   // lookup kernels: rebuilt at the start and after every commit
+};
+
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+// Grid-wide barrier.  Thread 0 of each CTA releases the CTA's writes and arrives; the last to arrive
+// re-arms the counter and publishes the next generation, the others spin on it with acquire loads.
+// A spin gives up after ~2 s: the first CTA to give up counts the timeout in DevState::rounds_timeouts
+// and raises ctl->abort, and from then on every barrier returns false (the caller leaves).  `gen` is
+// thread 0's copy of the generation.
+__device__ __forceinline__ bool grid_barrier(RoundsCtl* ctl, DevState* st, unsigned int& gen, int* sOk) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        bool ok = true;
+        fence_acq_rel_gpu();  // release: this CTA's writes, ordered before thread 0 by the CTA barrier
+        if (atomicAdd(&ctl->arrive, 1u) == gridDim.x - 1) {
+            atomicExch(&ctl->arrive, 0u);
+            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(&ctl->gen), "r"(gen + 1) : "memory");
+        } else {
+            const unsigned long long t0 = globaltimer_ns();
+            for (;;) {
+                unsigned int g;
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(g) : "l"(&ctl->gen) : "memory");
+                if (g != gen) break;
+                if (*reinterpret_cast<volatile unsigned int*>(&ctl->abort)) {
+                    ok = false;
+                    break;
+                }
+                if (globaltimer_ns() - t0 > kRoundsBarrierTimeoutNs) {
+                    if (atomicExch(&ctl->abort, 1u) == 0u) atomicAdd(&st->rounds_timeouts, 1ull);
+                    ok = false;
+                    break;
+                }
+                __nanosleep(32);
+            }
+        }
+        gen += 1;
+        fence_acq_rel_gpu();  // acquire: the other CTAs' writes before their arrivals
+        if (*reinterpret_cast<volatile unsigned int*>(&ctl->abort)) ok = false;
+        *sOk = ok;
+    }
+    __syncthreads();
+    return *sOk != 0;
+}
+
+// A CTA leaves the launch; the last one re-arms the barrier words for the next launch.
+__device__ __forceinline__ void rounds_exit(RoundsCtl* ctl) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        fence_acq_rel_gpu();
+        if (atomicAdd(&ctl->exited, 1u) == gridDim.x - 1) {
+            *reinterpret_cast<volatile unsigned int*>(&ctl->arrive) = 0u;
+            *reinterpret_cast<volatile unsigned int*>(&ctl->abort) = 0u;
+            *reinterpret_cast<volatile unsigned int*>(&ctl->exited) = 0u;
+        }
+    }
+}
+
+// Per-device sums of tile `tile` from the per-warp sums in shared memory (the layout of
+// epilogue_publish), for the cut.  Called by all threads after a __syncthreads().
+template <int WARPS>
+__device__ __forceinline__ void tile_sums_store(const unsigned long long* wacc, int wstride, int core_off, int mem_off, int D,
+                                                unsigned long long* tile_sums, unsigned int tile) {
+    const int tid = threadIdx.x;
+    if (tid < 2 * D) {
+        const int j = tid < D ? core_off + tid : mem_off + (tid - D);
+        unsigned long long tot = 0;
+#pragma unroll
+        for (int w = 0; w < WARPS; ++w) tot += wacc[w * wstride + j];
+        tile_sums[static_cast<size_t>(tile) * 2 * kMaxD + (tid < D ? tid : kMaxD + (tid - D))] = tot;
+    }
+}
+
+// Exclusive offsets of n_tiles compaction tiles in place, and their total.  One CTA of kRoundsThreads.
+__device__ __forceinline__ void tile_offsets_cta(unsigned int* count, long long n_tiles, unsigned long long* total) {
+    __shared__ unsigned long long sh[2 * (kRoundsThreads / 32)];
+    unsigned long long carry = 0;
+    for (long long t0 = 0; t0 < n_tiles; t0 += kRoundsThreads) {
+        const long long t = t0 + threadIdx.x;
+        unsigned long long c = t < n_tiles ? __ldcg(count + t) : 0u, z = 0, tc, tz;
+        block_scan2<kRoundsThreads>(c, z, sh, tc, tz);
+        if (t < n_tiles) count[t] = static_cast<unsigned int>(carry + c);
+        carry += tc;
+    }
+    if (threadIdx.x == 0) *total = carry;
+}
+
+// Every round of one call, by one CTA of the persistent grid.  scan(rc, rm, n, idx, tile, n_tiles) is
+// phase 1: the CONTIG scan of tile `tile` and its per-tile sums.  The cut, rewrite and write-back bodies
+// read blockIdx.x / gridDim.x as the standalone kernels do: here that is CTA b of the G-CTA grid (G >= D).
+template <RowFormat FMT, bool LUT, class Scan>
+__device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Scan&& scan) {
+    __shared__ int sOk;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int tid = threadIdx.x;
+    unsigned int gen = 0;
+    if (tid == 0) gen = *reinterpret_cast<volatile unsigned int*>(&a.ctl->gen);
+    const int D = st->D;
+    bool ok = true;
+    if (b == 0) {
+        if (tid < 2 * kMaxD) a.total[tid] = 0;
+        // the table may have changed since the lookup table was last built (a replayed graph does not
+        // see the host's bookkeeping): build it from the table as it is now
+        if constexpr (LUT) lut_build_cta(st, a.lut);
+    }
+    if constexpr (LUT) ok = grid_barrier(a.ctl, st, gen, &sOk);
+    const int32_t* rc = a.rc;
+    const int32_t* rm = a.rm;
+    const int32_t* map = nullptr;
+    int32_t* idx = a.idx;
+    long long n = a.R;
+    int which = 0;
+    while (ok) {
+        scan(rc, rm, n, idx, b, G);  // 1
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (static_cast<int>(b) < D)  // 2
+            prefix_cut_cta<FMT>(st, idx, rc, rm, n, static_cast<int>(G), a.tile_sums, a.pf, nullptr);
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if constexpr (FMT == kRowsPacked)  // 3
+            prefix_apply_packed_rows(a.pf, D, n, reinterpret_cast<signed char*>(idx));
+        else
+            prefix_apply_rows(a.pf, D, n, idx);
+        if (b == 0) {
+            prefix_finalize_cta(st, a.pf, nullptr, a.table_out, 1);
+            if (tid < D) {
+                a.total[tid] += __ldcg(&a.pf->committed_c[tid]);
+                a.total[D + tid] += __ldcg(&a.pf->committed_m[tid]);
+            }
+            if constexpr (LUT) {
+                __syncthreads();  // resort_table_cta's stores of the sorted view, read by every thread of the build
+                lut_build_cta(st, a.lut);
+            }
+        }
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (map) round_writeback_rows<FMT>(idx, map, n, a.idx);  // 4
+        const long long tiles = (n + kCompactTile - 1) / kCompactTile;
+        for (long long t = b; t < tiles; t += G) {
+            deferred_count_cta<FMT>(idx, n, a.tile_count, static_cast<unsigned int>(t));
+            __syncthreads();
+        }
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (b == 0) tile_offsets_cta(a.tile_count, tiles, a.deferred);  // 5
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        const unsigned long long left = __ldcg(a.deferred);
+        if (left == 0) {
+            if (b == 0 && a.delta_out && tid < 2 * D) a.delta_out[tid] = a.total[tid];
+            break;
+        }
+        int32_t* const n_rc = which ? a.set[1][0] : a.set[0][0];  // 6
+        int32_t* const n_rm = which ? a.set[1][1] : a.set[0][1];
+        int32_t* const n_map = which ? a.set[1][2] : a.set[0][2];
+        int32_t* const n_idx = which ? a.set[1][3] : a.set[0][3];
+        for (long long t = b; t < tiles; t += G) {
+            deferred_scatter_cta<FMT>(idx, rc, rm, map, n, a.tile_count, n_rc, n_rm, n_map, static_cast<unsigned int>(t));
+            __syncthreads();
+        }
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        rc = n_rc;
+        rm = n_rm;
+        map = n_map;
+        idx = n_idx;
+        n = static_cast<long long>(left);
+        which ^= 1;
+    }
+    rounds_exit(a.ctl);
+}
+
+// The register scan's rounds: SnapSmem<DT, kRoundsThreads> of dynamic shared memory.
+template <int DT, RowFormat FMT>
+__global__ void __launch_bounds__(kRoundsThreads, 1)
+rounds_sorted_kernel(DevState* st, const __grid_constant__ RoundsArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& s = *reinterpret_cast<SnapSmem<DT, kRoundsThreads>*>(smem_raw);
+    rounds_cta<FMT, false>(st, a, [&](const int32_t* rc, const int32_t* rm, long long n, int32_t* idx, unsigned int tile,
+                                      unsigned int tiles) {
+        const int D = sorted_scan_rows<DT, kRoundsThreads, true, FMT, kLoadCoherent>(s, st, rc, rm, n, idx, static_cast<int>(tile),
+                                                                                     static_cast<int>(tiles));
+        hist_to_warp_sums<DT, kRoundsThreads>(s, D);
+        __syncthreads();
+        tile_sums_store<kRoundsThreads / 32>(&s.sWarpAcc[0][0], 2 * DT, 0, DT, D, a.tile_sums, tile);
+    });
+}
+
+// The lookup scan's rounds: LutSmem<kRoundsThreads> of dynamic shared memory.
+template <RowFormat FMT>
+__global__ void __launch_bounds__(kRoundsThreads, 1)
+rounds_lut_kernel(DevState* st, const __grid_constant__ RoundsArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& sm = *reinterpret_cast<LutSmem<kRoundsThreads>*>(smem_raw);
+    rounds_cta<FMT, true>(st, a, [&](const int32_t* rc, const int32_t* rm, long long n, int32_t* idx, unsigned int tile,
+                                     unsigned int tiles) {
+        const int D = lut_scan_rows<kRoundsThreads, true, FMT, kLoadCoherent>(sm, st, rc, rm, n, idx, a.lut, static_cast<int>(tile),
+                                                                              static_cast<int>(tiles));
+        __syncthreads();
+        tile_sums_store<kRoundsThreads / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, D, a.tile_sums, tile);
+    });
 }
 
 }  // namespace egpu

@@ -125,6 +125,14 @@ extern "C" {
                                     (egpu_bestfit_batch_rounds on packed words, no round limit); see
                                     egpu_bestfit_batch_dev.  egpu_bestfit_batches_dev refuses it. */
 
+#define EGPU_F_DEVICE_ROUNDS 128 /* egpu_bestfit_batch / egpu_bestfit_batch_dev only, and only as
+                                    EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS
+                                    [| EGPU_F_PACKED] [| EGPU_F_INPUTS_READY]: rounds to the fixed point, int32 or
+                                    packed, in ONE launch with no host round trip per round; the _dev form does
+                                    not synchronise its stream.  See egpu_bestfit_batch_dev.  The value is 128,
+                                    not 64: callers were told that EGPU_F_ROUNDS with bit 64 is refused, and it
+                                    still is.  Bit 64 is unassigned. */
+
 /* kernel variants for the snapshot scan (egpu_set_variant) */
 #define EGPU_VARIANT_AUTO    0   /* SORTED for D <= 16, LUT above */
 #define EGPU_VARIANT_GRID    1   /* direct (device x request) score grid, min over packed keys */
@@ -157,7 +165,8 @@ int  egpu_set_variant(egpu_ctx* ctx, int variant);
  * start gate, host registration, 1.5 preferred allocation for many container requests from flat ID
  * buffers, 1.6 EGPU_F_PACKED multi-batch launches, 1.7 EGPU_F_PACKED prefix-commit on egpu_bestfit_batch and
  * egpu_bestfit_batch_dev, 1.8 EGPU_F_ROUNDS packed rounds on the same two, 1.9 EGPU_F_PACKED on
- * egpu_bestfit_batch_shard_dev, egpu_bestfit_batch_shard_lag_dev and egpu_bestfit_batch_shard_prefix_dev); a
+ * egpu_bestfit_batch_shard_dev, egpu_bestfit_batch_shard_lag_dev and egpu_bestfit_batch_shard_prefix_dev,
+ * 1.10 EGPU_F_DEVICE_ROUNDS rounds in one launch on egpu_bestfit_batch and egpu_bestfit_batch_dev); a
  * caller built against 1.0 keeps working. */
 int  egpu_abi_version(void);
 
@@ -179,7 +188,10 @@ int egpu_table_size(egpu_ctx* ctx);
  * EGPU_F_PREFIX_COMMIT, and with it EGPU_F_PACKED (packed prefix-commit: see egpu_bestfit_batch_dev;
  * the words are staged through HBM, 4 bytes per row in and 1 out), and with those and EGPU_F_COMMIT,
  * EGPU_F_ROUNDS (packed rounds to the fixed point, staged the same way; out_delta_* receive the demand
- * committed over all rounds). */
+ * committed over all rounds), and with EGPU_F_ROUNDS, EGPU_F_DEVICE_ROUNDS (rounds in one launch, int32
+ * or packed: staged through HBM, int32 8 bytes per row in and 4 out, packed 4 in and 1 out; one launch
+ * and one synchronisation; returns EGPU_ERR_CUDA, with egpu_last_error saying so, when a device-rounds
+ * launch on this context gave up at a grid barrier since the previous host-form call). */
 int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core,
                        const int32_t* req_mem, int64_t R, int32_t* out_idx,
                        int64_t* out_delta_core, int64_t* out_delta_mem,
@@ -268,7 +280,27 @@ int  egpu_host_unregister(egpu_ctx* ctx, void* p);
  * allocation failure returns EGPU_ERR_NOMEM with nothing committed.  R = 0 is the packed prefix-commit
  * with R = 0.  EGPU_ERR_STATE under EGPU_VARIANT_GRID.  EGPU_ERR_INVALID, before anything is launched
  * or written: EGPU_F_ROUNDS with any other combination of flags, R >= 2^31, and everything packed
- * prefix-commit refuses. */
+ * prefix-commit refuses.
+ *
+ * Rounds in one launch (flags EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS
+ * [| EGPU_F_PACKED] [| EGPU_F_INPUTS_READY], the last accepted and without effect): the semantics of
+ * egpu_bestfit_batch_rounds_dev with no round limit - every index ends as a device or -1, never
+ * EGPU_IDX_DEFERRED, sticky oversubscription flags are kept - on int32 arrays (d_req_core, d_req_mem,
+ * int32 d_out_idx) or, with EGPU_F_PACKED, on the arguments of packed prefix-commit (words, NULL
+ * d_req_mem, int8 indices).  ASYNCHRONOUS on `stream`, with no synchronisation: every round runs in one
+ * persistent launch, so the call can sit in a pipelined stream.  d_delta (may be NULL) receives the
+ * demand committed over all rounds, int64[2*D]; d_table_out (may be NULL) the last round's table',
+ * oversub words 0; the committed table is installed in stream order.  R = 0 writes zero sums and
+ * table' = the current table.  Scratch is that of the rounds (32 bytes per request int32, 18 packed),
+ * kept by the context and allocated before the launch: an allocation failure returns EGPU_ERR_NOMEM
+ * with nothing committed.  Calls that share a context's scratch (all prefix-commit and rounds calls)
+ * must be ordered on one stream, or by the caller.  The launch is cooperative: the runtime refuses a
+ * grid it cannot keep resident rather than letting it wait.  Every wait inside the launch gives up
+ * after about 2 s; a launch that gave up leaves the rows it did not finish at EGPU_IDX_DEFERRED and is
+ * reported by the next host-form call with EGPU_F_DEVICE_ROUNDS (EGPU_ERR_CUDA).  EGPU_ERR_STATE under
+ * EGPU_VARIANT_GRID.  EGPU_ERR_INVALID, before anything is launched or written: EGPU_F_DEVICE_ROUNDS
+ * with any other combination of flags, R >= 2^31, NULL or misaligned arrays with R > 0, a non-NULL
+ * d_req_mem with EGPU_F_PACKED and a NULL one without it. */
 int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core,
                            const int32_t* d_req_mem, int64_t R,
                            int32_t* d_out_idx, int64_t* d_delta,
