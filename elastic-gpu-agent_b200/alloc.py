@@ -315,6 +315,21 @@ class BestFitAllocator:
         rc = self._lib.egpu_bestfit_batches_dev(self._h, arr, len(arr), flags, _stream(stream))
         self._check(rc, "egpu_bestfit_batches_dev")
 
+    def bestfit_batches_rounds_device_dev(self, batches, packed: bool = False, stream: int | None = None):
+        """egpu_bestfit_batches_dev with EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS:
+        up to 64 batches placed in order in one launch, each committed to its fixed point against the table the
+        batches before it left (what K bestfit_rounds_device_dev calls on one stream give), asynchronous on
+        `stream`.  `batches`: tuples as make_batches takes (packed=False) or as make_packed_batches takes
+        (packed=True), or the array either returns.  Per batch, d_delta receives the demand that batch committed
+        and d_table_out its last round's table'."""
+        if isinstance(batches, C.Array):
+            arr = batches
+        else:
+            arr = self.make_packed_batches(batches) if packed else self.make_batches(batches)
+        flags = L.F_PREFIX_COMMIT | L.F_COMMIT | L.F_ROUNDS | L.F_DEVICE_ROUNDS | (L.F_PACKED if packed else 0)
+        rc = self._lib.egpu_bestfit_batches_dev(self._h, arr, len(arr), flags, _stream(stream))
+        self._check(rc, "egpu_bestfit_batches_dev")
+
     def bestfit_batches_shard_dev(self, batches, first_step: int, stream: int | None = None, inputs_ready: bool = False,
                                   apply: bool = False):
         """K sharded steps in one launch: batch k = exchange step first_step + k.  apply: the CTAs that complete a

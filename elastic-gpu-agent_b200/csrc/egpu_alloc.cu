@@ -116,6 +116,19 @@ template <int F, RowFormat FMT>
 constexpr decltype(rounds_kernel<F, FMT, 0>()) kRoundsKernels[4] = {rounds_kernel<F, FMT, 0>(), rounds_kernel<F, FMT, 1>(),
                                                                    rounds_kernel<F, FMT, 2>(), rounds_kernel<F, FMT, 3>()};
 
+// ... and their multi-batch twins (egpu_bestfit_batches_dev with EGPU_F_DEVICE_ROUNDS): same CTAs and shared memory
+template <int F, RowFormat FMT, int B>
+constexpr auto rounds_multi_kernel() {
+    constexpr int DT = 8 << B;
+    if constexpr (F == kRoundsSorted)
+        return kernel(rounds_sorted_multi_kernel<DT, FMT>, kRoundsThreads, sizeof(SnapSmem<DT, kRoundsThreads>));
+    else return kernel(rounds_lut_multi_kernel<FMT>, kRoundsThreads, sizeof(LutSmem<kRoundsThreads>));
+}
+template <int F, RowFormat FMT>
+constexpr decltype(rounds_multi_kernel<F, FMT, 0>()) kRoundsMultiKernels[4] = {
+    rounds_multi_kernel<F, FMT, 0>(), rounds_multi_kernel<F, FMT, 1>(), rounds_multi_kernel<F, FMT, 2>(),
+    rounds_multi_kernel<F, FMT, 3>()};
+
 // Resident CTAs per SM of kernel k; `cached` is its entry in the context's occupancy cache.  The
 // first use on a context opts in to the kernel's dynamic shared memory and asks the occupancy.
 template <class Fn>
@@ -684,22 +697,37 @@ bool device_rounds_flags_ok(int flags, int64_t R) {
 
 // EGPU_F_DEVICE_ROUNDS: the rounds of run_rounds with no round limit, in ONE cooperative launch of
 // rounds_sorted_kernel / rounds_lut_kernel (egpu_scan.cuh) and without a host round trip: nothing
-// here waits for the device.  Rows in either format (see prefix_scan).  d_delta (may be NULL) receives
-// the demand committed over all rounds, d_table_out (may be NULL) the last round's table'.  Scratch is
-// the rounds scratch of run_rounds, sized before the launch.
-int launch_device_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx, long long* d_delta,
-                         int32_t* d_table_out, cudaStream_t s, RowFormat fmt) {
+// here waits for the device.  Rows in either format (see prefix_scan).  Per batch, d_delta (may be NULL)
+// receives the demand committed over all rounds, d_table_out (may be NULL) the last round's table'.
+// Scratch is the rounds scratch of run_rounds, sized before the launch.
+// multi (egpu_bestfit_batches_dev): the K batches of `bs`, each to its fixed point against the table the
+// batches before it committed, in one launch of the multi-batch twins; grid and scratch are those of the
+// largest batch.  Otherwise bs[0] alone (K = 1) in the single-batch kernels.
+int launch_device_rounds(egpu_ctx* ctx, const egpu_batch* bs, int K, bool multi, cudaStream_t s, RowFormat fmt) {
     if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // no prefix-commit mode
     const bool lut = lut_variant(ctx), packed = fmt == kRowsPacked;
-    const int bucket = d_bucket(ctx->D);
+    const int bucket = d_bucket(ctx->D), fam = lut ? kRoundsLut : kRoundsSorted;
+    int64_t R = 0;
+    for (int b = 0; b < K; ++b) R = std::max<int64_t>(R, bs[b].R);
+    if (multi) {  // two batches sharing an output: the later one would overwrite the earlier one's
+        Range* mine = ctx->multi_ranges;
+        for (int b = 0; b < K; ++b)
+            batch_ranges(mine + 3 * b, bs[b].d_out_idx, bs[b].R, packed ? sizeof(int8_t) : sizeof(int32_t), bs[b].d_delta,
+                         bs[b].d_table_out, ctx->D);
+        if (prepare_ranges(mine, 3 * K) < 0) return EGPU_ERR_INVALID;
+    }
     const auto& k = lut ? (packed ? kRoundsKernels<kRoundsLut, kRowsPacked> : kRoundsKernels<kRoundsLut, kRowsInt32>)[bucket]
                         : (packed ? kRoundsKernels<kRoundsSorted, kRowsPacked> : kRoundsKernels<kRoundsSorted, kRowsInt32>)[bucket];
+    const auto& km = lut ? (packed ? kRoundsMultiKernels<kRoundsLut, kRowsPacked> : kRoundsMultiKernels<kRoundsLut, kRowsInt32>)[bucket]
+                         : (packed ? kRoundsMultiKernels<kRoundsSorted, kRowsPacked>
+                                   : kRoundsMultiKernels<kRoundsSorted, kRowsInt32>)[bucket];
     int per_sm = 0;
-    int rc = resident_ctas(ctx, k, ctx->rounds_ctas_per_sm[lut ? kRoundsLut : kRoundsSorted][packed][bucket], &per_sm);
+    int rc = multi ? resident_ctas(ctx, km, ctx->rounds_multi_ctas_per_sm[fam][packed][bucket], &per_sm)
+                   : resident_ctas(ctx, k, ctx->rounds_ctas_per_sm[fam][packed][bucket], &per_sm);
     if (rc != EGPU_OK) return rc;
     // Grid: as many CTAs as round 1's scan wants at 8 rows per thread (the lone-launch rule of
-    // launch_snapshot_as), at most one resident wave (the grid barriers need every CTA resident) and at
-    // least one CTA per device (CTA d cuts device d).
+    // launch_snapshot_as; of the largest batch), at most one resident wave (the grid barriers need every
+    // CTA resident) and at least one CTA per device (CTA d cuts device d).
     if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
     const int64_t wave = static_cast<int64_t>(ctx->sm_count) * per_sm;
     const int64_t per_cta = static_cast<int64_t>(kRoundsThreads) * 2;  // 128-bit vectors of 4 rows
@@ -721,12 +749,12 @@ int launch_device_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm
     }
     RoundsArgs a;
     std::memset(&a, 0, sizeof a);
-    a.rc = d_rc;
-    a.rm = packed ? nullptr : d_rm;
-    a.R = static_cast<long long>(R);
-    a.idx = d_idx;
-    a.delta_out = d_delta;
-    a.table_out = d_table_out;
+    a.rc = bs[0].d_req_core;
+    a.rm = packed ? nullptr : bs[0].d_req_mem;
+    a.R = static_cast<long long>(bs[0].R);
+    a.idx = bs[0].d_out_idx;
+    a.delta_out = reinterpret_cast<long long*>(bs[0].d_delta);
+    a.table_out = bs[0].d_table_out;
     a.tile_sums = ctx->d_tile_sums;
     a.pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
     a.total = sc.info->delta;
@@ -738,14 +766,25 @@ int launch_device_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(static_cast<unsigned>(grid));
     cfg.blockDim = dim3(static_cast<unsigned>(k.threads));
-    cfg.dynamicSmemBytes = k.smem;
+    cfg.dynamicSmemBytes = multi ? km.smem : k.smem;
     cfg.stream = s;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeCooperative;  // the runtime refuses a grid it cannot co-schedule
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, k.fn, ctx->d_state, a));
+    if (multi) {
+        RoundsMultiArgs m;
+        std::memset(&m, 0, sizeof m);
+        m.a = a;
+        for (int b = 0; b < K; ++b)
+            m.b[b] = {bs[b].d_req_core, packed ? nullptr : bs[b].d_req_mem, static_cast<long long>(bs[b].R), bs[b].d_out_idx,
+                      reinterpret_cast<long long*>(bs[b].d_delta), bs[b].d_table_out};
+        m.K = K;
+        EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, km.fn, ctx->d_state, m));
+    } else {
+        EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, k.fn, ctx->d_state, a));
+    }
     ctx->launches += 1;
     ctx->prev_is_scan = false;
     ctx->lut_dirty = !lut;  // the lookup kernels leave d_lut built from the table they committed
@@ -864,7 +903,8 @@ extern "C" {
 // 1.8: + EGPU_F_ROUNDS, packed prefix-commit rounds on the same two entry points (additive)
 // 1.9: + EGPU_F_PACKED on egpu_bestfit_batch_shard_dev, _shard_lag_dev and _shard_prefix_dev (additive)
 // 1.10: + EGPU_F_DEVICE_ROUNDS, rounds in one launch on egpu_bestfit_batch / egpu_bestfit_batch_dev (additive)
-int egpu_abi_version(void) { return 1010; }
+// 1.11: + EGPU_F_DEVICE_ROUNDS on egpu_bestfit_batches_dev, K batches placed in order in one launch (additive)
+int egpu_abi_version(void) { return 1011; }
 
 const char* egpu_strerror(int code) {
     switch (code) {
@@ -1090,9 +1130,10 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
-    if (device_rounds)
-        return launch_device_rounds(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, s,
-                                    packed ? kRowsPacked : kRowsInt32);
+    if (device_rounds) {
+        const egpu_batch one{d_req_core, d_req_mem, R, d_out_idx, d_delta, d_table_out};
+        return launch_device_rounds(ctx, &one, 1, false, s, packed ? kRowsPacked : kRowsInt32);
+    }
     if (rounds) {
         long long total[2 * kMaxD];
         rc = launch_packed_rounds(ctx, d_req_core, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, total, s);
@@ -1122,13 +1163,19 @@ static int check_batches(const egpu_batch* batches, int32_t K, bool packed = fal
 }
 
 int egpu_bestfit_batches_dev(egpu_ctx* ctx, const egpu_batch* batches, int32_t K, int flags, void* stream) {
-    if (!ctx || (flags & ~(EGPU_F_INPUTS_READY | EGPU_F_PACKED))) return EGPU_ERR_INVALID;
-    int rc = check_batches(batches, K, (flags & EGPU_F_PACKED) != 0);
+    // EGPU_F_DEVICE_ROUNDS (with exactly the flags of the single-batch call): the batches placed in order,
+    // each committed to its fixed point, in one launch.  Otherwise a snapshot of every batch.
+    const bool device_rounds = (flags & EGPU_F_DEVICE_ROUNDS) != 0;
+    if (!ctx || (device_rounds ? !device_rounds_flags_ok(flags, 0) : (flags & ~(EGPU_F_INPUTS_READY | EGPU_F_PACKED)) != 0))
+        return EGPU_ERR_INVALID;
+    const bool packed = (flags & EGPU_F_PACKED) != 0;
+    int rc = check_batches(batches, K, packed);
     if (rc != EGPU_OK) return rc;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
+    if (device_rounds) return launch_device_rounds(ctx, batches, K, true, s, packed ? kRowsPacked : kRowsInt32);
     return launch_multi(ctx, batches, K, flags, s, 0);
 }
 
@@ -1250,8 +1297,8 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
             EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
             if (!packed) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
         }
-        rc = launch_device_rounds(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, s,
-                                  packed ? kRowsPacked : kRowsInt32);
+        const egpu_batch one{ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, reinterpret_cast<int64_t*>(ctx->d_delta), nullptr};
+        rc = launch_device_rounds(ctx, &one, 1, false, s, packed ? kRowsPacked : kRowsInt32);
         if (rc != EGPU_OK) return rc;
         const size_t idx_bytes = packed ? sizeof(int8_t) : sizeof(int32_t);
         if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, idx_bytes * R, cudaMemcpyDeviceToHost, s));

@@ -2025,11 +2025,52 @@ __device__ __forceinline__ void tile_offsets_cta(unsigned int* count, long long 
     if (threadIdx.x == 0) *total = carry;
 }
 
+// One batch of a multi-batch rounds launch: the batch fields of RoundsArgs.
+struct RoundsBatch {
+    const int32_t* rc;
+    const int32_t* rm;
+    long long R;
+    int32_t* idx;
+    long long* delta_out;
+    int32_t* table_out;
+};
+
+// A multi-batch rounds launch (egpu_bestfit_batches_dev with EGPU_F_DEVICE_ROUNDS): the scratch, barrier
+// words and lookup table of `a` (whose batch fields are batch 0's), and K batches placed in order.
+struct RoundsMultiArgs {
+    RoundsArgs a;
+    RoundsBatch b[kMultiMax];
+    int K;
+};
+static_assert(sizeof(DevState*) + sizeof(RoundsMultiArgs) <= 4096, "descriptors + the scalar arguments must fit the 4 KB kernel-parameter space");
+
 // Every round of one call, by one CTA of the persistent grid.  scan(rc, rm, n, idx, tile, n_tiles) is
 // phase 1: the CONTIG scan of tile `tile` and its per-tile sums.  The cut, rewrite and write-back bodies
 // read blockIdx.x / gridDim.x as the standalone kernels do: here that is CTA b of the G-CTA grid (G >= D).
-template <RowFormat FMT, bool LUT, class Scan>
-__device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Scan&& scan) {
+//
+// MULTI: the rounds of batch 0, then of batch 1 against the table batch 0 committed, and so on to batch
+// K - 1 (batch k's table_out and delta_out are list[k]'s).  At batch k's fixed point every CTA takes batch
+// k + 1 as round 1 of a fresh call, with no extra grid barrier.  The boundary is the boundary between two
+// rounds without phase 6 and its barrier, and nothing that crosses it needs them:
+//   - total: only CTA 0 touches it; each thread reads (delta_out) and then zeroes its own words, and the
+//     next adds to them come in phase 3, after two grid barriers;
+//   - deferred: read by every CTA after barrier 5; CTA 0 next writes it in phase 5 of batch k + 1, and no
+//     CTA passes barrier 1 before every CTA has read it;
+//   - tile_sums: last read in phase 2 of batch k's last round, next written in phase 1 of batch k + 1:
+//     barriers 2 to 5 lie between;
+//   - PrefixOut: last read in phase 3, next written in phase 2 of batch k + 1: barriers 3, 4, 5 and 1;
+//   - tile_count: last read in phase 5 (CTA 0), next written in phase 4 of batch k + 1;
+//   - the scratch sets: last read in phases 1 to 4 of batch k's last round, next written in phase 6 of
+//     batch k + 1's round 1, at least five barriers later;
+//   - the indices: batch k's are complete at barrier 4 (write-back); batch k + 1 writes its own, which
+//     the launcher has checked do not overlap batch k's outputs.
+// The committed table (and the lookup table, built from it by CTA 0 in phase 3) is read in phase 1 of
+// batch k + 1 as in any later round, behind barrier 3.  Everything one CTA writes that another reads in
+// the launch keeps coherent loads.  The lookup table is built once at the start and after every commit,
+// as in a single call: never per batch.
+template <RowFormat FMT, bool LUT, bool MULTI = false, class Scan>
+__device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Scan&& scan, const RoundsBatch* list = nullptr,
+                                           int K = 1) {
     __shared__ int sOk;
     const unsigned int b = blockIdx.x, G = gridDim.x;
     const int tid = threadIdx.x;
@@ -2050,6 +2091,7 @@ __device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Sc
     int32_t* idx = a.idx;
     long long n = a.R;
     int which = 0;
+    [[maybe_unused]] int k = 0;  // MULTI: the batch these rounds place
     while (ok) {
         scan(rc, rm, n, idx, b, G);  // 1
         if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
@@ -2061,7 +2103,7 @@ __device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Sc
         else
             prefix_apply_rows(a.pf, D, n, idx);
         if (b == 0) {
-            prefix_finalize_cta(st, a.pf, nullptr, a.table_out, 1);
+            prefix_finalize_cta(st, a.pf, nullptr, MULTI ? list[k].table_out : a.table_out, 1);
             if (tid < D) {
                 a.total[tid] += __ldcg(&a.pf->committed_c[tid]);
                 a.total[D + tid] += __ldcg(&a.pf->committed_m[tid]);
@@ -2072,7 +2114,7 @@ __device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Sc
             }
         }
         if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
-        if (map) round_writeback_rows<FMT>(idx, map, n, a.idx);  // 4
+        if (map) round_writeback_rows<FMT>(idx, map, n, MULTI ? list[k].idx : a.idx);  // 4
         const long long tiles = (n + kCompactTile - 1) / kCompactTile;
         for (long long t = b; t < tiles; t += G) {
             deferred_count_cta<FMT>(idx, n, a.tile_count, static_cast<unsigned int>(t));
@@ -2083,7 +2125,24 @@ __device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Sc
         if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
         const unsigned long long left = __ldcg(a.deferred);
         if (left == 0) {
-            if (b == 0 && a.delta_out && tid < 2 * D) a.delta_out[tid] = a.total[tid];
+            if constexpr (MULTI) {
+                long long* const delta_out = list[k].delta_out;
+                if (b == 0 && tid < 2 * kMaxD) {
+                    if (delta_out && tid < 2 * D) delta_out[tid] = a.total[tid];
+                    a.total[tid] = 0;
+                }
+                if (++k < K) {  // the next batch, round 1 on its own arrays (see the boundary note above)
+                    rc = list[k].rc;
+                    rm = list[k].rm;
+                    map = nullptr;
+                    idx = list[k].idx;
+                    n = list[k].R;
+                    which = 0;
+                    continue;
+                }
+            } else {
+                if (b == 0 && a.delta_out && tid < 2 * D) a.delta_out[tid] = a.total[tid];
+            }
             break;
         }
         int32_t* const n_rc = which ? a.set[1][0] : a.set[0][0];  // 6
@@ -2134,6 +2193,45 @@ rounds_lut_kernel(DevState* st, const __grid_constant__ RoundsArgs a) {
         __syncthreads();
         tile_sums_store<kRoundsThreads / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, D, a.tile_sums, tile);
     });
+}
+
+// The multi-batch twins of the two kernels above: the same scans, K batches placed in order.  The
+// register twins keep the residency of their single-batch kernel: 2 CTAs per SM at D <= 8, and in the
+// packed format up to D = 32 (those fit 128 registers), 1 elsewhere.
+template <int DT, RowFormat FMT>
+constexpr int kRoundsMultiMinCtas = (DT == 8 || (FMT == kRowsPacked && DT <= 32)) ? 2 : 1;
+
+template <int DT, RowFormat FMT>
+__global__ void __launch_bounds__(kRoundsThreads, (kRoundsMultiMinCtas<DT, FMT>))
+rounds_sorted_multi_kernel(DevState* st, const __grid_constant__ RoundsMultiArgs m) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& s = *reinterpret_cast<SnapSmem<DT, kRoundsThreads>*>(smem_raw);
+    rounds_cta<FMT, false, true>(
+        st, m.a,
+        [&](const int32_t* rc, const int32_t* rm, long long n, int32_t* idx, unsigned int tile, unsigned int tiles) {
+            const int D = sorted_scan_rows<DT, kRoundsThreads, true, FMT, kLoadCoherent>(s, st, rc, rm, n, idx, static_cast<int>(tile),
+                                                                                         static_cast<int>(tiles));
+            hist_to_warp_sums<DT, kRoundsThreads>(s, D);
+            __syncthreads();
+            tile_sums_store<kRoundsThreads / 32>(&s.sWarpAcc[0][0], 2 * DT, 0, DT, D, m.a.tile_sums, tile);
+        },
+        m.b, m.K);
+}
+
+template <RowFormat FMT>
+__global__ void __launch_bounds__(kRoundsThreads, 1)
+rounds_lut_multi_kernel(DevState* st, const __grid_constant__ RoundsMultiArgs m) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& sm = *reinterpret_cast<LutSmem<kRoundsThreads>*>(smem_raw);
+    rounds_cta<FMT, true, true>(
+        st, m.a,
+        [&](const int32_t* rc, const int32_t* rm, long long n, int32_t* idx, unsigned int tile, unsigned int tiles) {
+            const int D = lut_scan_rows<kRoundsThreads, true, FMT, kLoadCoherent>(sm, st, rc, rm, n, idx, m.a.lut, static_cast<int>(tile),
+                                                                                  static_cast<int>(tiles));
+            __syncthreads();
+            tile_sums_store<kRoundsThreads / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, D, m.a.tile_sums, tile);
+        },
+        m.b, m.K);
 }
 
 }  // namespace egpu

@@ -123,13 +123,16 @@ extern "C" {
                                     EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS
                                     [| EGPU_F_INPUTS_READY]: packed prefix-commit rounds to the fixed point
                                     (egpu_bestfit_batch_rounds on packed words, no round limit); see
-                                    egpu_bestfit_batch_dev.  egpu_bestfit_batches_dev refuses it. */
+                                    egpu_bestfit_batch_dev.  egpu_bestfit_batches_dev refuses it except in
+                                    the flag set of EGPU_F_DEVICE_ROUNDS. */
 
-#define EGPU_F_DEVICE_ROUNDS 128 /* egpu_bestfit_batch / egpu_bestfit_batch_dev only, and only as
+#define EGPU_F_DEVICE_ROUNDS 128 /* egpu_bestfit_batch / egpu_bestfit_batch_dev / egpu_bestfit_batches_dev only,
+                                    and only as
                                     EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS
                                     [| EGPU_F_PACKED] [| EGPU_F_INPUTS_READY]: rounds to the fixed point, int32 or
-                                    packed, in ONE launch with no host round trip per round; the _dev form does
-                                    not synchronise its stream.  See egpu_bestfit_batch_dev.  The value is 128,
+                                    packed, in ONE launch with no host round trip per round; the _dev forms do
+                                    not synchronise their stream.  See egpu_bestfit_batch_dev (one batch) and
+                                    egpu_bestfit_batches_dev (batches placed in order).  The value is 128,
                                     not 64: callers were told that EGPU_F_ROUNDS with bit 64 is refused, and it
                                     still is.  Bit 64 is unassigned. */
 
@@ -166,7 +169,8 @@ int  egpu_set_variant(egpu_ctx* ctx, int variant);
  * buffers, 1.6 EGPU_F_PACKED multi-batch launches, 1.7 EGPU_F_PACKED prefix-commit on egpu_bestfit_batch and
  * egpu_bestfit_batch_dev, 1.8 EGPU_F_ROUNDS packed rounds on the same two, 1.9 EGPU_F_PACKED on
  * egpu_bestfit_batch_shard_dev, egpu_bestfit_batch_shard_lag_dev and egpu_bestfit_batch_shard_prefix_dev,
- * 1.10 EGPU_F_DEVICE_ROUNDS rounds in one launch on egpu_bestfit_batch and egpu_bestfit_batch_dev); a
+ * 1.10 EGPU_F_DEVICE_ROUNDS rounds in one launch on egpu_bestfit_batch and egpu_bestfit_batch_dev,
+ * 1.11 EGPU_F_DEVICE_ROUNDS on egpu_bestfit_batches_dev: K batches placed in order in one launch); a
  * caller built against 1.0 keeps working. */
 int  egpu_abi_version(void);
 
@@ -312,8 +316,8 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core,
  * exactly what K separate non-committing calls would produce; only the launch latency, ramp and
  * tail are paid once instead of K times (at R = 1 M that fixed cost is about a third of a lone
  * launch; at R <= 100 k it is nearly all of it).  Asynchronous on `stream`.  flags:
- * EGPU_F_INPUTS_READY only (a multi-batch launch never commits: install a table' with
- * egpu_table_set or a committing single-batch call).  Outputs of different batches must not
+ * EGPU_F_INPUTS_READY only for a snapshot launch, which never commits; the one committing form is
+ * the flag set of the rounds in one launch (below).  Outputs of different batches must not
  * overlap (EGPU_ERR_INVALID).  Batches may have different R (R = 0 allowed).
  *
  * Packed batches (flags EGPU_F_PACKED, alone or with EGPU_F_INPUTS_READY): every batch of the call
@@ -328,7 +332,33 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core,
  * EGPU_VARIANT_GRID - and outputs of different batches must not overlap: an index array covers R
  * bytes.  Without the flag a batch with R > 0 and a NULL d_req_mem is refused, so packed batches
  * handed over without it are never read as int32 arrays.  egpu_bestfit_batches_shard_dev refuses
- * the flag. */
+ * the flag.
+ *
+ * Batches placed in order, each to the fixed point, in one launch (flags EGPU_F_PREFIX_COMMIT |
+ * EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS [| EGPU_F_PACKED] [| EGPU_F_INPUTS_READY], the
+ * last accepted and without effect): batch k runs the rounds in one launch of egpu_bestfit_batch_dev
+ * against the table batches 0..k-1 committed, so the result is, bit for bit, what K consecutive
+ * egpu_bestfit_batch_dev calls with the same flags give when issued on one stream in batch order (an
+ * ordered admission queue: FIFO, or priority tiers placed one after the other).  This is not one rounds
+ * call on the concatenated batches, whose round 1 would let a later batch take the device an earlier
+ * batch's deferred row gets in its round 2.  Every index ends as a device or -1; sticky
+ * oversubscription flags are kept.  Per batch, d_delta (may be NULL) receives the demand that batch
+ * committed over its rounds, int64[2*D], and d_table_out (may be NULL) the table' of its last round,
+ * oversub words 0; an empty batch (R = 0) writes zero sums and table' = the table its predecessors left.
+ * The rows are int32 arrays, or with EGPU_F_PACKED the packed batch layout above (words, NULL
+ * d_req_mem, int8 indices).  ONE launch (egpu_launch_count + 1), ASYNCHRONOUS on `stream` with no
+ * synchronisation; the committed table is installed in stream order, and the call replays from a
+ * CUDA graph (a replay after egpu_table_set starts from the new table).  Scratch is the rounds scratch
+ * of egpu_bestfit_batch_dev, sized by the largest batch before the launch: an allocation failure
+ * returns EGPU_ERR_NOMEM with nothing committed.  Every wait inside the launch gives up after about
+ * 2 s, counted as for egpu_bestfit_batch_dev and reported by the next host-form call with
+ * EGPU_F_DEVICE_ROUNDS (EGPU_ERR_CUDA); then the batch in progress keeps its unfinished rows at
+ * EGPU_IDX_DEFERRED, and the batches after it are not reached: their indices, d_delta and d_table_out
+ * are left unwritten.  EGPU_ERR_STATE under EGPU_VARIANT_GRID, EGPU_ERR_NO_TABLE without a table.
+ * EGPU_ERR_INVALID, before anything is launched or written: EGPU_F_DEVICE_ROUNDS with any other
+ * combination of flags, K outside 1..64, a batch with R >= 2^31, NULL or misaligned arrays with R > 0,
+ * a non-NULL d_req_mem with EGPU_F_PACKED and a NULL one without it, outputs of two batches that
+ * overlap.  egpu_bestfit_batches_shard_dev refuses these flags. */
 #define EGPU_MAX_BATCHES 64
 typedef struct egpu_batch {
     const int32_t* d_req_core;   /* EGPU_F_PACKED: the packed words */
