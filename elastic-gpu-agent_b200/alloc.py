@@ -271,6 +271,16 @@ class BestFitAllocator:
                                               _stream(stream))
         self._check(rc, "egpu_bestfit_batch_dev")
 
+    def bestfit_packed_dev(self, d_words: int, R: int, d_idx8: int, d_delta: int = 0, d_table_out: int = 0,
+                           stream: int | None = None, commit: bool = False, inputs_ready: bool = False):
+        """egpu_bestfit_batch_packed_dev: the snapshot of R packed words (uint32 in, int8 indices out, both
+        16-byte aligned), asynchronous on `stream`; pipelines with the other scans under inputs_ready."""
+        flags = (L.F_COMMIT if commit else 0) | (L.F_INPUTS_READY if inputs_ready else 0)
+        rc = self._lib.egpu_bestfit_batch_packed_dev(self._h, C.c_void_p(d_words), int(R), C.c_void_p(d_idx8),
+                                                     C.c_void_p(d_delta or None), C.c_void_p(d_table_out or None), flags,
+                                                     _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_packed_dev")
+
     def bestfit_packed_prefix_dev(self, d_words: int, R: int, d_idx8: int, d_delta: int = 0, d_table_out: int = 0,
                                   commit: bool = False, stream: int | None = None, rounds: bool = False):
         """egpu_bestfit_batch_dev with EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT: R packed words in, R int8

@@ -1573,8 +1573,18 @@ int egpu_bestfit_batch_packed_dev(egpu_ctx* ctx, const uint32_t* d_req_packed, i
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
-    return launch_packed(ctx, d_req_packed, R, reinterpret_cast<signed char*>(d_out_idx8), reinterpret_cast<long long*>(d_delta),
-                         d_table_out, flags, s, 16);
+    // The grid variant has no packed snapshot scan, and the snapshot scans index at most EGPU_MAX_ROWS rows:
+    // those calls keep the warp-chunk scan of the host call, fully ordered.
+    if (ctx->variant == EGPU_VARIANT_GRID || R > kMaxRows)
+        return launch_packed(ctx, d_req_packed, R, reinterpret_cast<signed char*>(d_out_idx8), reinterpret_cast<long long*>(d_delta),
+                             d_table_out, flags, s, 16);
+    // Otherwise the round-robin packed scan of the sharded calls, in the variant's scan (register scan up to
+    // D = 16 under AUTO, lookup scan above), pipelined under EGPU_F_INPUTS_READY as the int32 call is.  Other
+    // flag bits are ignored: callers may pass them, and EGPU_F_PREFIX_COMMIT must not turn this into prefix-commit.
+    Snapshot a{reinterpret_cast<const int32_t*>(d_req_packed), nullptr, R, reinterpret_cast<int32_t*>(d_out_idx8),
+               reinterpret_cast<long long*>(d_delta), d_table_out, flags & (EGPU_F_COMMIT | EGPU_F_INPUTS_READY)};
+    a.packed = true;
+    return launch_snapshot(ctx, a, s);
 }
 
 int egpu_bestfit_batch_packed(egpu_ctx* ctx, const uint32_t* req_packed, int64_t R, int8_t* out_idx8,

@@ -234,6 +234,17 @@ int egpu_bestfit_batch_rounds_dev(egpu_ctx* ctx, const int32_t* d_req_core,
 #define EGPU_PACKED_INVALID 0xFFFFFFFFu
 int egpu_bestfit_batch_packed(egpu_ctx* ctx, const uint32_t* req_packed, int64_t R, int8_t* out_idx8,
                               int64_t* out_delta_core, int64_t* out_delta_mem, int commit);
+/* The same snapshot on device buffers, asynchronous on `stream` as egpu_bestfit_batch_dev: d_req_packed R
+ * words, d_out_idx8 R int8 indices (both 16-byte aligned when R > 0), d_delta int64[2*D] and d_table_out
+ * int32[3*D] (either may be NULL).  flags: EGPU_F_COMMIT (table' replaces the current table) and
+ * EGPU_F_INPUTS_READY (as in egpu_bestfit_batch_dev: consecutive non-committing scans of this context on one
+ * stream - packed, int32, multi-batch or sharded - may overlap); every other bit is ignored, so
+ * EGPU_F_PREFIX_COMMIT does not select prefix-commit here.  The scan follows egpu_set_variant as the int32
+ * scan does: the register scan for D <= 16 and the lookup scan above under EGPU_VARIANT_AUTO.  Under
+ * EGPU_VARIANT_GRID, and for R > EGPU_MAX_ROWS, the call runs the fully ordered scan of
+ * egpu_bestfit_batch_packed instead; the outputs are the same either way.  EGPU_ERR_INVALID: NULL or
+ * misaligned words or indices with R > 0, R < 0, and (as in egpu_bestfit_batch_dev) indices, sums and
+ * table' that overlap each other. */
 int egpu_bestfit_batch_packed_dev(egpu_ctx* ctx, const uint32_t* d_req_packed, int64_t R,
                                   int8_t* d_out_idx8, int64_t* d_delta, int32_t* d_table_out,
                                   int flags, void* stream);
