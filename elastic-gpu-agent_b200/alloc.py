@@ -350,6 +350,21 @@ class BestFitAllocator:
                                                       int(first_step), _stream(stream))
         self._check(rc, "egpu_bestfit_batches_shard_dev")
 
+    def bestfit_batches_shard_prefix_dev(self, batches, first_step: int, commit: bool = False, packed: bool = False,
+                                         stream: int | None = None):
+        """egpu_bestfit_batches_shard_dev with EGPU_F_PREFIX_COMMIT: K rank-major prefix-commits over row shards in
+        one launch, batch k on exchange steps first_step + 2k and first_step + 2k + 1 (what K bestfit_shard_prefix_dev
+        calls on one stream give).  Per batch, d_delta receives this rank's committed demand and d_table_out the table
+        minus every rank's committed demand; commit installs it before the next batch.  `batches`: tuples as
+        make_batches takes (packed=False) or as make_packed_batches takes (packed=True), or the array either returns."""
+        if isinstance(batches, C.Array):
+            arr = batches
+        else:
+            arr = self.make_packed_batches(batches) if packed else self.make_batches(batches)
+        flags = L.F_PREFIX_COMMIT | (L.F_COMMIT if commit else 0) | (L.F_PACKED if packed else 0)
+        rc = self._lib.egpu_bestfit_batches_shard_dev(self._h, arr, len(arr), flags, int(first_step), _stream(stream))
+        self._check(rc, "egpu_bestfit_batches_shard_dev")
+
     def query(self, free_core, free_mem, req_core, req_mem) -> np.ndarray:
         """egpu_bestfit_query: score against the table given here; the context's own table is untouched."""
         fc, fm, rc_, rm_ = _i32(free_core), _i32(free_mem), _i32(req_core), _i32(req_mem)

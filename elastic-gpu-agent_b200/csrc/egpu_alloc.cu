@@ -129,6 +129,20 @@ constexpr decltype(rounds_multi_kernel<F, FMT, 0>()) kRoundsMultiKernels[4] = {
     rounds_multi_kernel<F, FMT, 0>(), rounds_multi_kernel<F, FMT, 1>(), rounds_multi_kernel<F, FMT, 2>(),
     rounds_multi_kernel<F, FMT, 3>()};
 
+// The sharded prefix-commit of K batches in one launch (egpu_bestfit_batches_shard_dev with EGPU_F_PREFIX_COMMIT):
+// the scans, CTAs and shared memory of the multi-batch rounds kernels
+template <int F, RowFormat FMT, int B>
+constexpr auto shard_prefix_kernel() {
+    constexpr int DT = 8 << B;
+    if constexpr (F == kRoundsSorted)
+        return kernel(shard_prefix_multi_sorted_kernel<DT, FMT>, kRoundsThreads, sizeof(SnapSmem<DT, kRoundsThreads>));
+    else return kernel(shard_prefix_multi_lut_kernel<FMT>, kRoundsThreads, sizeof(LutSmem<kRoundsThreads>));
+}
+template <int F, RowFormat FMT>
+constexpr decltype(shard_prefix_kernel<F, FMT, 0>()) kShardPrefixKernels[4] = {
+    shard_prefix_kernel<F, FMT, 0>(), shard_prefix_kernel<F, FMT, 1>(), shard_prefix_kernel<F, FMT, 2>(),
+    shard_prefix_kernel<F, FMT, 3>()};
+
 // Resident CTAs per SM of kernel k; `cached` is its entry in the context's occupancy cache.  The
 // first use on a context opts in to the kernel's dynamic shared memory and asks the occupancy.
 template <class Fn>
@@ -570,7 +584,10 @@ struct RoundInfo {
 // round are at most R.  Packed: two sets of (words, caller's row, int8 index), 9 bytes per row each.
 constexpr size_t kRoundsHead = 2048;
 constexpr size_t kRoundsCtlOff = 1536;
-static_assert(sizeof(RoundInfo) <= kRoundsCtlOff && kRoundsCtlOff + sizeof(RoundsCtl) <= kRoundsHead, "rounds scratch head");
+constexpr size_t kShardStopOff = 1792;  // the stop word of the multi-batch sharded prefix-commit (ShardPrefixArgs::stop)
+static_assert(sizeof(RoundInfo) <= kRoundsCtlOff && kRoundsCtlOff + sizeof(RoundsCtl) <= kShardStopOff &&
+                  kShardStopOff + sizeof(unsigned int) <= kRoundsHead,
+              "rounds scratch head");
 struct RoundsScratch {
     RoundInfo* info;
     unsigned int* tiles;
@@ -593,6 +610,17 @@ int rounds_scratch(egpu_ctx* ctx, int64_t R, bool packed, RoundsScratch* out) {
             out->set[a][b] = sub[b] ? reinterpret_cast<int32_t*>(base + off) : nullptr;
             off += sub[b];
         }
+    return EGPU_OK;
+}
+
+// The grid-barrier words of the persistent launches, in the head of the rounds scratch (rounds_scratch first)
+int rounds_ctl(egpu_ctx* ctx, cudaStream_t s, RoundsCtl** out) {
+    RoundsCtl* ctl = reinterpret_cast<RoundsCtl*>(reinterpret_cast<char*>(ctx->d_rounds) + kRoundsCtlOff);
+    if (ctx->rounds_ctl_bytes != ctx->rounds_bytes) {  // fresh scratch: the barrier words start at zero
+        EGPU_CUDA(ctx, cudaMemsetAsync(ctl, 0, sizeof(RoundsCtl), s));
+        ctx->rounds_ctl_bytes = ctx->rounds_bytes;
+    }
+    *out = ctl;
     return EGPU_OK;
 }
 
@@ -695,6 +723,51 @@ bool device_rounds_flags_ok(int flags, int64_t R) {
            (flags & kDeviceRoundsNeeds) == kDeviceRoundsNeeds && R < (1ll << 31);
 }
 
+// Grid of a persistent launch (the one-launch rounds, the multi-batch sharded prefix-commit) of kernel k over
+// batches of at most R rows: as many CTAs as round 1's CONTIG scan wants at 8 rows per thread (the lone-launch
+// rule of launch_snapshot_as), at most one resident wave (the grid barriers need every CTA resident) and at
+// least one CTA per device (CTA d cuts device d).  Also sizes the tile sums and PrefixOut for that grid, so
+// that, with the caller's own scratch, everything is allocated before the launch and a failure commits nothing.
+// `cached` is the kernel's entry in the context's occupancy cache.
+template <class Fn>
+int persistent_grid(egpu_ctx* ctx, const Kernel<Fn>& k, int& cached, int64_t R, int64_t* grid_out) {
+    int per_sm = 0;
+    const int rc = resident_ctas(ctx, k, cached, &per_sm);
+    if (rc != EGPU_OK) return rc;
+    if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
+    const int64_t wave = static_cast<int64_t>(ctx->sm_count) * per_sm;
+    const int64_t per_cta = static_cast<int64_t>(kRoundsThreads) * 2;  // 128-bit vectors of 4 rows
+    int64_t grid = ((R >> 2) + per_cta - 1) / per_cta;
+    if (grid > wave) grid = wave;
+    if (grid < ctx->D) grid = ctx->D;
+    if (grid > wave) return EGPU_ERR_STATE;  // fewer resident CTAs than devices: not on an H100
+    const size_t sums_bytes = sizeof(unsigned long long) * 2 * kMaxD * static_cast<size_t>(grid);
+    EGPU_CUDA(ctx, grow(ctx->tile_bytes, sums_bytes, sums_bytes, &ctx->d_tile_sums));
+    if (!ctx->d_prefix_out) EGPU_CUDA(ctx, cudaMalloc(&ctx->d_prefix_out, sizeof(PrefixOut) + sizeof(long long) * 2 * kMaxD));
+    *grid_out = grid;
+    return EGPU_OK;
+}
+
+// The cooperative launch of a persistent kernel on `grid` CTAs (persistent_grid): the runtime refuses a grid it
+// cannot co-schedule rather than letting its barriers wait.
+template <class Fn, class A>
+int launch_persistent(egpu_ctx* ctx, const Kernel<Fn>& k, int64_t grid, cudaStream_t s, const A& args) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.blockDim = dim3(static_cast<unsigned>(k.threads));
+    cfg.dynamicSmemBytes = k.smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, k.fn, ctx->d_state, args));
+    ctx->launches += 1;
+    ctx->prev_is_scan = false;
+    return EGPU_OK;
+}
+
 // EGPU_F_DEVICE_ROUNDS: the rounds of run_rounds with no round limit, in ONE cooperative launch of
 // rounds_sorted_kernel / rounds_lut_kernel (egpu_scan.cuh) and without a host round trip: nothing
 // here waits for the device.  Rows in either format (see prefix_scan).  Per batch, d_delta (may be NULL)
@@ -721,32 +794,16 @@ int launch_device_rounds(egpu_ctx* ctx, const egpu_batch* bs, int K, bool multi,
     const auto& km = lut ? (packed ? kRoundsMultiKernels<kRoundsLut, kRowsPacked> : kRoundsMultiKernels<kRoundsLut, kRowsInt32>)[bucket]
                          : (packed ? kRoundsMultiKernels<kRoundsSorted, kRowsPacked>
                                    : kRoundsMultiKernels<kRoundsSorted, kRowsInt32>)[bucket];
-    int per_sm = 0;
-    int rc = multi ? resident_ctas(ctx, km, ctx->rounds_multi_ctas_per_sm[fam][packed][bucket], &per_sm)
-                   : resident_ctas(ctx, k, ctx->rounds_ctas_per_sm[fam][packed][bucket], &per_sm);
+    int64_t grid = 0;
+    int rc = multi ? persistent_grid(ctx, km, ctx->rounds_multi_ctas_per_sm[fam][packed][bucket], R, &grid)
+                   : persistent_grid(ctx, k, ctx->rounds_ctas_per_sm[fam][packed][bucket], R, &grid);
     if (rc != EGPU_OK) return rc;
-    // Grid: as many CTAs as round 1's scan wants at 8 rows per thread (the lone-launch rule of
-    // launch_snapshot_as; of the largest batch), at most one resident wave (the grid barriers need every
-    // CTA resident) and at least one CTA per device (CTA d cuts device d).
-    if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
-    const int64_t wave = static_cast<int64_t>(ctx->sm_count) * per_sm;
-    const int64_t per_cta = static_cast<int64_t>(kRoundsThreads) * 2;  // 128-bit vectors of 4 rows
-    int64_t grid = ((R >> 2) + per_cta - 1) / per_cta;
-    if (grid > wave) grid = wave;
-    if (grid < ctx->D) grid = ctx->D;
-    if (grid > wave) return EGPU_ERR_STATE;  // fewer resident CTAs than devices: not on an H100
-    // every allocation before the launch, so that a failure commits nothing
     RoundsScratch sc;
     rc = rounds_scratch(ctx, R, packed, &sc);
     if (rc != EGPU_OK) return rc;
-    const size_t sums_bytes = sizeof(unsigned long long) * 2 * kMaxD * static_cast<size_t>(grid);
-    EGPU_CUDA(ctx, grow(ctx->tile_bytes, sums_bytes, sums_bytes, &ctx->d_tile_sums));
-    if (!ctx->d_prefix_out) EGPU_CUDA(ctx, cudaMalloc(&ctx->d_prefix_out, sizeof(PrefixOut) + sizeof(long long) * 2 * kMaxD));
-    RoundsCtl* ctl = reinterpret_cast<RoundsCtl*>(reinterpret_cast<char*>(ctx->d_rounds) + kRoundsCtlOff);
-    if (ctx->rounds_ctl_bytes != ctx->rounds_bytes) {  // fresh scratch: the barrier words start at zero
-        EGPU_CUDA(ctx, cudaMemsetAsync(ctl, 0, sizeof(RoundsCtl), s));
-        ctx->rounds_ctl_bytes = ctx->rounds_bytes;
-    }
+    RoundsCtl* ctl = nullptr;
+    rc = rounds_ctl(ctx, s, &ctl);
+    if (rc != EGPU_OK) return rc;
     RoundsArgs a;
     std::memset(&a, 0, sizeof a);
     a.rc = bs[0].d_req_core;
@@ -763,16 +820,6 @@ int launch_device_rounds(egpu_ctx* ctx, const egpu_batch* bs, int K, bool multi,
     std::memcpy(a.set, sc.set, sizeof a.set);
     a.ctl = ctl;
     a.lut = ctx->d_lut;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(grid));
-    cfg.blockDim = dim3(static_cast<unsigned>(k.threads));
-    cfg.dynamicSmemBytes = multi ? km.smem : k.smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;  // the runtime refuses a grid it cannot co-schedule
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     if (multi) {
         RoundsMultiArgs m;
         std::memset(&m, 0, sizeof m);
@@ -781,12 +828,11 @@ int launch_device_rounds(egpu_ctx* ctx, const egpu_batch* bs, int K, bool multi,
             m.b[b] = {bs[b].d_req_core, packed ? nullptr : bs[b].d_req_mem, static_cast<long long>(bs[b].R), bs[b].d_out_idx,
                       reinterpret_cast<long long*>(bs[b].d_delta), bs[b].d_table_out};
         m.K = K;
-        EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, km.fn, ctx->d_state, m));
+        rc = launch_persistent(ctx, km, grid, s, m);
     } else {
-        EGPU_CUDA(ctx, cudaLaunchKernelEx(&cfg, k.fn, ctx->d_state, a));
+        rc = launch_persistent(ctx, k, grid, s, a);
     }
-    ctx->launches += 1;
-    ctx->prev_is_scan = false;
+    if (rc != EGPU_OK) return rc;
     ctx->lut_dirty = !lut;  // the lookup kernels leave d_lut built from the table they committed
     return EGPU_OK;
 }
@@ -821,6 +867,55 @@ int launch_prefix_commit_shard(egpu_ctx* ctx, const int32_t* d_rc, const int32_t
     ctx->launches += 5;
     ctx->prev_is_scan = false;
     if (user_flags & EGPU_F_COMMIT) ctx->lut_dirty = true;
+    return EGPU_OK;
+}
+
+// K sharded prefix-commits in ONE cooperative launch of shard_prefix_multi_sorted_kernel /
+// shard_prefix_multi_lut_kernel (egpu_scan.cuh): batch k is launch_prefix_commit_shard with
+// step = first_step + 2k, scored against the table batch k - 1 left (with commit, the one it installed).
+// Grid: persistent_grid of the largest batch; scratch: the tile sums, PrefixOut and the head of the rounds
+// scratch (barrier words, stop word), all allocated before the launch.
+int launch_shard_prefix_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, bool commit, uint64_t first_step, cudaStream_t s,
+                              RowFormat fmt) {
+    if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // no prefix-commit mode
+    const bool lut = lut_variant(ctx), packed = fmt == kRowsPacked;
+    const int bucket = d_bucket(ctx->D), fam = lut ? kRoundsLut : kRoundsSorted;
+    int64_t R = 0;
+    Range* mine = ctx->multi_ranges;
+    for (int b = 0; b < K; ++b) {
+        R = std::max<int64_t>(R, bs[b].R);
+        batch_ranges(mine + 3 * b, bs[b].d_out_idx, bs[b].R, packed ? sizeof(int8_t) : sizeof(int32_t), bs[b].d_delta,
+                     bs[b].d_table_out, ctx->D);
+    }
+    if (prepare_ranges(mine, 3 * K) < 0) return EGPU_ERR_INVALID;  // the later batch would overwrite the earlier one's outputs
+    const auto& k = lut ? (packed ? kShardPrefixKernels<kRoundsLut, kRowsPacked> : kShardPrefixKernels<kRoundsLut, kRowsInt32>)[bucket]
+                        : (packed ? kShardPrefixKernels<kRoundsSorted, kRowsPacked>
+                                  : kShardPrefixKernels<kRoundsSorted, kRowsInt32>)[bucket];
+    int64_t grid = 0;
+    int rc = persistent_grid(ctx, k, ctx->shard_prefix_ctas_per_sm[fam][packed][bucket], R, &grid);
+    if (rc != EGPU_OK) return rc;
+    RoundsScratch sc;
+    rc = rounds_scratch(ctx, 0, packed, &sc);  // the head only
+    if (rc != EGPU_OK) return rc;
+    ShardPrefixArgs a;
+    std::memset(&a, 0, sizeof a);
+    rc = rounds_ctl(ctx, s, &a.ctl);
+    if (rc != EGPU_OK) return rc;
+    for (int b = 0; b < K; ++b)
+        a.b[b] = {bs[b].d_req_core, packed ? nullptr : bs[b].d_req_mem, static_cast<long long>(bs[b].R), bs[b].d_out_idx,
+                  reinterpret_cast<long long*>(bs[b].d_delta), bs[b].d_table_out};
+    a.tile_sums = ctx->d_tile_sums;
+    a.pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
+    a.stop = reinterpret_cast<unsigned int*>(static_cast<char*>(ctx->d_rounds) + kShardStopOff);
+    a.lut = ctx->d_lut;
+    a.first_step_plus1 = first_step + 1;
+    a.K = K;
+    a.commit = commit ? 1 : 0;
+    rc = launch_persistent(ctx, k, grid, s, a);
+    if (rc != EGPU_OK) return rc;
+    // the lookup kernel leaves d_lut built from the table it last scored against or installed
+    if (lut) ctx->lut_dirty = false;
+    else if (commit) ctx->lut_dirty = true;
     return EGPU_OK;
 }
 
@@ -904,6 +999,8 @@ extern "C" {
 // 1.9: + EGPU_F_PACKED on egpu_bestfit_batch_shard_dev, _shard_lag_dev and _shard_prefix_dev (additive)
 // 1.10: + EGPU_F_DEVICE_ROUNDS, rounds in one launch on egpu_bestfit_batch / egpu_bestfit_batch_dev (additive)
 // 1.11: + EGPU_F_DEVICE_ROUNDS on egpu_bestfit_batches_dev, K batches placed in order in one launch (additive)
+//       + EGPU_F_PREFIX_COMMIT on egpu_bestfit_batches_shard_dev, K sharded prefix-commits in one launch (a newly
+//         accepted flag set on an existing entry point; the version stays 1011, which callers and tests pin)
 int egpu_abi_version(void) { return 1011; }
 
 const char* egpu_strerror(int code) {
@@ -1181,13 +1278,23 @@ int egpu_bestfit_batches_dev(egpu_ctx* ctx, const egpu_batch* batches, int32_t K
 
 int egpu_bestfit_batches_shard_dev(egpu_ctx* ctx, const egpu_batch* batches, int32_t K, int flags, uint64_t first_step,
                                    void* stream) {
-    if (!ctx || (flags & ~(EGPU_F_INPUTS_READY | EGPU_F_APPLY)) || first_step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    int rc = check_batches(batches, K);
+    // EGPU_F_PREFIX_COMMIT [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: K sharded prefix-commits in order, in one launch, on
+    // exchange steps first_step .. first_step + 2K - 1.  Otherwise K sharded snapshot steps.
+    const bool prefix = (flags & EGPU_F_PREFIX_COMMIT) != 0;
+    const bool packed = (flags & EGPU_F_PACKED) != 0;
+    if (!ctx || first_step >= (1ull << 47) ||
+        (flags & ~(prefix ? EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_PACKED : EGPU_F_INPUTS_READY | EGPU_F_APPLY)))
+        return EGPU_ERR_INVALID;
+    int rc = check_batches(batches, K, packed);
     if (rc != EGPU_OK) return rc;
+    if (prefix && first_step + 2ull * static_cast<uint64_t>(K) > (1ull << 47)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
+    if (prefix)
+        return launch_shard_prefix_multi(ctx, batches, K, (flags & EGPU_F_COMMIT) != 0, first_step, s,
+                                         packed ? kRowsPacked : kRowsInt32);
     return launch_multi(ctx, batches, K, flags, s, first_step + 1);
 }
 

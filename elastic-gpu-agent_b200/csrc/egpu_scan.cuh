@@ -1317,12 +1317,12 @@ gate_kernel(DevState* __restrict__ st, const unsigned long long* __restrict__ ho
     }
 }
 
-// Without commit the steps are independent of each other (each is table - its own sum): the grid
-// has one CTA per step, so the waits overlap instead of queueing behind one another (the vectors of
-// all the steps of a multi-batch launch arrive at about the same time, when that launch drains).
-// With commit the steps apply on top of each other: one CTA walks them in order.
-__global__ void __launch_bounds__(kMaxD)
-apply_peers_kernel(DevState* __restrict__ st, unsigned long long first_step_plus1, int nsteps, ApplyOuts outs, int commit) {
+// Body of apply_peers_kernel: steps [k_begin, k_end) after first_step_plus1 by one CTA of >= kMaxD
+// threads; table_out(k) is step k's table' (may be nullptr).  false when a peer's vector did not
+// arrive within ~2 s: DevState::peer_timeout records it and the table is left alone.
+template <class Outs>
+__device__ __forceinline__ bool apply_peers_cta(DevState* __restrict__ st, unsigned long long first_step_plus1, int k_begin, int k_end,
+                                                Outs&& table_out, int commit) {
     __shared__ int32_t sFc[kMaxD], sFm[kMaxD], sPosDev[kMaxD];
     __shared__ int sOk;
     const int D = st->D;
@@ -1331,8 +1331,6 @@ apply_peers_kernel(DevState* __restrict__ st, unsigned long long first_step_plus
     // running table across the steps of this launch (only installed when commit is set)
     long long cur_c = d < D ? st->free_core[d] : 0, cur_m = d < D ? st->free_mem[d] : 0;
     int32_t sticky = 0;
-    const int k_begin = commit ? 0 : static_cast<int>(blockIdx.x);
-    const int k_end = commit ? nsteps : k_begin + 1;
     for (int k = k_begin; k < k_end; ++k) {
         const unsigned long long step_plus1 = first_step_plus1 + k;
         XchgRow* rows = st->peer.buf[me]->slot[(step_plus1 - 1) % kXchgSlots];
@@ -1343,15 +1341,15 @@ apply_peers_kernel(DevState* __restrict__ st, unsigned long long first_step_plus
         __syncthreads();
         if (!sOk) {
             if (d == 0) st->peer_timeout = step_plus1;
-            return;
+            return false;
         }
         if (d < D) {
             const long long nc = cur_c - dc, nm = cur_m - dm;
             const int32_t over = (nc < 0 || nm < 0) ? 1 : 0;
-            if (outs.table_out[k]) {
-                outs.table_out[k][d] = sat_i32(nc);
-                outs.table_out[k][D + d] = sat_i32(nm);
-                outs.table_out[k][2 * D + d] = over;
+            if (table_out(k)) {
+                table_out(k)[d] = sat_i32(nc);
+                table_out(k)[D + d] = sat_i32(nm);
+                table_out(k)[2 * D + d] = over;
             }
             if (commit) {  // the next step of this launch is applied on top of this one
                 cur_c = nc < 0 ? 0 : nc;
@@ -1370,8 +1368,19 @@ apply_peers_kernel(DevState* __restrict__ st, unsigned long long first_step_plus
         }
         resort_table_cta(st, D, sFc, sFm, sPosDev, d);
     }
+    return true;
 }
 
+// Without commit the steps are independent of each other (each is table - its own sum): the grid
+// has one CTA per step, so the waits overlap instead of queueing behind one another (the vectors of
+// all the steps of a multi-batch launch arrive at about the same time, when that launch drains).
+// With commit the steps apply on top of each other: one CTA walks them in order.
+__global__ void __launch_bounds__(kMaxD)
+apply_peers_kernel(DevState* __restrict__ st, unsigned long long first_step_plus1, int nsteps, ApplyOuts outs, int commit) {
+    const int k_begin = commit ? 0 : static_cast<int>(blockIdx.x);
+    const int k_end = commit ? nsteps : k_begin + 1;
+    apply_peers_cta(st, first_step_plus1, k_begin, k_end, [&](int k) { return outs.table_out[k]; }, commit);
+}
 
 // =============================================================================
 // Prefix-commit (spec 2.5): turn the snapshot choice into an allocation that never
@@ -1688,9 +1697,8 @@ prefix_base_kernel(DevState* __restrict__ st, unsigned long long step_plus1, lon
 
 // This rank's COMMITTED demand (after the cut) to every peer as exchange step `step`;
 // apply_peers_kernel of that step then makes table' = table - sum over ranks.  One CTA.
-__global__ void __launch_bounds__(kMaxD)
-prefix_push_kernel(DevState* __restrict__ st, const PrefixOut* __restrict__ pf, unsigned long long step_plus1,
-                   long long* __restrict__ delta_out) {
+__device__ __forceinline__ void prefix_push_cta(DevState* __restrict__ st, const PrefixOut* __restrict__ pf,
+                                                unsigned long long step_plus1, long long* __restrict__ delta_out) {
     const int D = st->D;
     const int d = threadIdx.x;
     if (d < D) {
@@ -1701,6 +1709,12 @@ prefix_push_kernel(DevState* __restrict__ st, const PrefixOut* __restrict__ pf, 
         }
         xchg_push(st, step_plus1, d, D, dc, dm);
     }
+}
+
+__global__ void __launch_bounds__(kMaxD)
+prefix_push_kernel(DevState* __restrict__ st, const PrefixOut* __restrict__ pf, unsigned long long step_plus1,
+                   long long* __restrict__ delta_out) {
+    prefix_push_cta(st, pf, step_plus1, delta_out);
 }
 
 // =============================================================================
@@ -2232,6 +2246,179 @@ rounds_lut_multi_kernel(DevState* st, const __grid_constant__ RoundsMultiArgs m)
             tile_sums_store<kRoundsThreads / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, D, m.a.tile_sums, tile);
         },
         m.b, m.K);
+}
+
+// =============================================================================
+// Sharded prefix-commit of K batches in one launch (egpu_bestfit_batches_shard_dev with
+// EGPU_F_PREFIX_COMMIT)
+// =============================================================================
+//
+// Batch k is one egpu_bestfit_batch_shard_prefix_dev call with step = first_step + 2k (the
+// pipeline of launch_prefix_commit_shard), batch k + 1 scored against the table batch k left.
+// One resident wave (cooperative launch), per batch three phases separated by grid barriers:
+//   1. CONTIG scan of the batch, tile b = CTA b, per-tile sums;
+//   2. CTA d < D: the batch's uncapped demand on device d (its column of the tile sums) to every
+//      rank as exchange step first_step + 2k, the lower ranks' demand on d from this rank's buffer
+//      (the base of prefix_base_kernel), then the cut of device d from that base (prefix_cut_cta);
+//   3. deferred indices -> -2 by every CTA; CTA 0 pushes the committed demand as step
+//      first_step + 2k + 1 and writes d_delta (prefix_push_cta), waits for every rank's committed
+//      demand and applies it (apply_peers_cta): table', and with commit the installed, re-sorted
+//      table and (lookup kernel) the rebuilt lookup table.
+// The single call needs a launch between the base and the cut; here they share CTA d, because
+// the exchange is word-granular: CTA d pushes and pulls only the two words of device d.
+// Across batches: tile_sums are last read in phase 2 and next written in phase 1 of the next
+// batch (barrier 3 between); PrefixOut is last read in phase 3 and next written in phase 2
+// (barriers 3 and 1).  Everything one CTA writes that another reads keeps coherent loads, as in
+// the rounds kernels.
+//
+// A wait that gives up ends the launch after the batch in progress; later batches are not written.
+// Until every CTA has passed barrier 2 the batch's rows hold the scan's device choices, which commit
+// nothing.  So when barrier 1 or 2 gives up (DevState::rounds_timeouts), or a base pull gave up
+// (DevState::peer_timeout; as in prefix_base_kernel, nothing of the batch commits), every CTA
+// rewrites the rows of its own CONTIG tile that chose a device to -2 and leaves: the batch's
+// d_delta, d_table_out and the table stay as they were.  No other CTA writes those rows before
+// barrier 2, so this needs no further wait.  The bounds of the two waits differ (2 s of
+// %globaltimer at a barrier, 4e9 SM cycles in a pull), so which of the two comes first does not
+// matter.  From barrier 2 on the rows are final when each CTA arrives at barrier 3: an apply that
+// gives up leaves the rows and d_delta written and the table alone, as apply_peers_kernel does
+// after the single call's rewrite (DevState::peer_timeout).
+struct ShardPrefixArgs {
+    RoundsBatch b[kMultiMax];         // delta_out: this rank's committed demand; table_out: table' of all ranks
+    unsigned long long* tile_sums;    // [grid][2*kMaxD]
+    PrefixOut* pf;
+    RoundsCtl* ctl;
+    unsigned int* stop;               // a wait gave up: every CTA leaves after the batch in progress
+    DevLut* lut;                      // lookup kernel: built at the start and after every commit
+    unsigned long long first_step_plus1;
+    int K;
+    int commit;
+};
+static_assert(sizeof(DevState*) + sizeof(ShardPrefixArgs) <= 4096, "descriptors + the scalar arguments must fit the 4 KB kernel-parameter space");
+
+template <RowFormat FMT, bool LUT, class Scan>
+__device__ __forceinline__ void shard_prefix_cta(DevState* st, const ShardPrefixArgs& a, Scan&& scan) {
+    __shared__ int sOk;
+    __shared__ long long sBase[2 * kMaxD];  // prefix_cut_cta's base: only device blockIdx.x's two words are read
+    __shared__ unsigned long long sh[2 * (kRoundsThreads / 32)];
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int tid = threadIdx.x;
+    unsigned int gen = 0;
+    if (tid == 0) gen = *reinterpret_cast<volatile unsigned int*>(&a.ctl->gen);
+    const int D = st->D;
+    if (b == 0) {
+        if (tid == 0) *reinterpret_cast<volatile unsigned int*>(a.stop) = 0u;  // next written in phase 2, behind barrier 1
+        // the table may have changed since the lookup table was last built (a replayed graph does not
+        // see the host's bookkeeping): build it from the table as it is now
+        if constexpr (LUT) lut_build_cta(st, a.lut);
+    }
+    // the rows of this CTA's CONTIG tile of `in` (the partition of the scans and of prefix_cut_cta) that chose a
+    // device -> -2: the way out of a batch that did not get past barrier 2 (see above)
+    auto defer_tile = [&](const RoundsBatch& in) {
+        const long long nvec = in.R >> 2;
+        const long long per = (nvec + G - 1) / G;
+        const long long lo = b * per * 4 < nvec * 4 ? b * per * 4 : nvec * 4;
+        const long long hi = b == G - 1 ? in.R : ((b + 1) * per * 4 < nvec * 4 ? (b + 1) * per * 4 : nvec * 4);
+        for (long long r = lo + tid; r < hi; r += kRoundsThreads) {
+            if constexpr (FMT == kRowsPacked) {
+                signed char* const idx8 = reinterpret_cast<signed char*>(in.idx);
+                if (__ldcg(idx8 + r) >= 0) idx8[r] = -2;
+            } else {
+                if (__ldcg(in.idx + r) >= 0) in.idx[r] = -2;
+            }
+        }
+    };
+    bool ok = true;
+    if constexpr (LUT) ok = grid_barrier(a.ctl, st, gen, &sOk);
+    for (int k = 0; ok && k < a.K; ++k) {
+        const RoundsBatch& in = a.b[k];
+        const unsigned long long push = a.first_step_plus1 + 2ull * static_cast<unsigned long long>(k);
+        scan(in.rc, in.rm, in.R, in.idx, b, G);  // 1
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) {
+            defer_tile(in);
+            break;
+        }
+        if (static_cast<int>(b) < D) {  // 2
+            const int d = static_cast<int>(b);
+            unsigned long long c = 0, m = 0, tc, tm;
+            for (unsigned int t = tid; t < G; t += kRoundsThreads) {
+                c += __ldcg(&a.tile_sums[static_cast<size_t>(t) * 2 * kMaxD + d]);
+                m += __ldcg(&a.tile_sums[static_cast<size_t>(t) * 2 * kMaxD + kMaxD + d]);
+            }
+            block_scan2<kRoundsThreads>(c, m, sh, tc, tm);
+            if (tid == 0) {
+                xchg_push(st, push, d, D, static_cast<long long>(tc), static_cast<long long>(tm));
+                const int world = st->peer.world, me = st->peer.rank;
+                long long bc = 0, bm = 0;
+                if (xchg_pull(st->peer.buf[me]->slot[(push - 1) % kXchgSlots], world, push, d, D, 0, me, bc, bm)) {
+                    sBase[d] = bc;
+                    sBase[kMaxD + d] = bm;
+                } else {  // a rank died: nothing of this batch commits (below), and the launch ends with it
+                    st->peer_timeout = push;
+                    sBase[d] = 1ll << 40;
+                    sBase[kMaxD + d] = 1ll << 40;
+                    atomicExch(a.stop, 1u);
+                }
+            }
+            __syncthreads();
+            prefix_cut_cta<FMT>(st, in.idx, in.rc, in.rm, in.R, static_cast<int>(G), a.tile_sums, a.pf, sBase);
+        }
+        // a base pull that gave up raised the stop word before its CTA arrived: every CTA that passes sees it
+        if (!grid_barrier(a.ctl, st, gen, &sOk) || *reinterpret_cast<volatile unsigned int*>(a.stop)) {
+            defer_tile(in);
+            break;
+        }
+        if constexpr (FMT == kRowsPacked)  // 3
+            prefix_apply_packed_rows(a.pf, D, in.R, reinterpret_cast<signed char*>(in.idx));
+        else
+            prefix_apply_rows(a.pf, D, in.R, in.idx);
+        if (b == 0) {
+            prefix_push_cta(st, a.pf, push + 1, in.delta_out);
+            if (apply_peers_cta(st, push + 1, 0, 1, [&](int) { return in.table_out; }, a.commit)) {
+                if constexpr (LUT) {
+                    if (a.commit) {
+                        __syncthreads();  // resort_table_cta's stores of the sorted view, read by every thread of the build
+                        lut_build_cta(st, a.lut);
+                    }
+                }
+            } else if (tid == 0) {
+                atomicExch(a.stop, 1u);
+            }
+        }
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (*reinterpret_cast<volatile unsigned int*>(a.stop)) break;
+    }
+    rounds_exit(a.ctl);
+}
+
+// The register scan's form: the scan of the multi-batch rounds kernels, at their residency.
+template <int DT, RowFormat FMT>
+__global__ void __launch_bounds__(kRoundsThreads, (kRoundsMultiMinCtas<DT, FMT>))
+shard_prefix_multi_sorted_kernel(DevState* st, const __grid_constant__ ShardPrefixArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& s = *reinterpret_cast<SnapSmem<DT, kRoundsThreads>*>(smem_raw);
+    shard_prefix_cta<FMT, false>(st, a, [&](const int32_t* rc, const int32_t* rm, long long n, int32_t* idx, unsigned int tile,
+                                            unsigned int tiles) {
+        const int D = sorted_scan_rows<DT, kRoundsThreads, true, FMT, kLoadCoherent>(s, st, rc, rm, n, idx, static_cast<int>(tile),
+                                                                                     static_cast<int>(tiles));
+        hist_to_warp_sums<DT, kRoundsThreads>(s, D);
+        __syncthreads();
+        tile_sums_store<kRoundsThreads / 32>(&s.sWarpAcc[0][0], 2 * DT, 0, DT, D, a.tile_sums, tile);
+    });
+}
+
+// The lookup scan's form.
+template <RowFormat FMT>
+__global__ void __launch_bounds__(kRoundsThreads, 1)
+shard_prefix_multi_lut_kernel(DevState* st, const __grid_constant__ ShardPrefixArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& sm = *reinterpret_cast<LutSmem<kRoundsThreads>*>(smem_raw);
+    shard_prefix_cta<FMT, true>(st, a, [&](const int32_t* rc, const int32_t* rm, long long n, int32_t* idx, unsigned int tile,
+                                           unsigned int tiles) {
+        const int D = lut_scan_rows<kRoundsThreads, true, FMT, kLoadCoherent>(sm, st, rc, rm, n, idx, a.lut, static_cast<int>(tile),
+                                                                              static_cast<int>(tiles));
+        __syncthreads();
+        tile_sums_store<kRoundsThreads / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, D, a.tile_sums, tile);
+    });
 }
 
 }  // namespace egpu

@@ -343,7 +343,7 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core,
  * EGPU_VARIANT_GRID - and outputs of different batches must not overlap: an index array covers R
  * bytes.  Without the flag a batch with R > 0 and a NULL d_req_mem is refused, so packed batches
  * handed over without it are never read as int32 arrays.  egpu_bestfit_batches_shard_dev refuses
- * the flag.
+ * the flag on its snapshot steps; it takes it only with EGPU_F_PREFIX_COMMIT (below).
  *
  * Batches placed in order, each to the fixed point, in one launch (flags EGPU_F_PREFIX_COMMIT |
  * EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS [| EGPU_F_PACKED] [| EGPU_F_INPUTS_READY], the
@@ -440,7 +440,39 @@ int egpu_table_apply_peers_dev(egpu_ctx* ctx, uint64_t step, int32_t* d_table_ou
 /* K sharded steps in one launch: batch k is exchange step first_step + k (egpu_bestfit_batches_dev
  * + the fused push of egpu_bestfit_batch_shard_dev).  Without EGPU_F_APPLY d_table_out of the
  * batches is ignored (table' comes from the apply calls); with it the exchange steps are consumed
- * by the launch itself and no apply call must follow. */
+ * by the launch itself and no apply call must follow.
+ *
+ * K sharded prefix-commits in one launch (flags EGPU_F_PREFIX_COMMIT [| EGPU_F_COMMIT] [| EGPU_F_PACKED]):
+ * batch k, in order for k = 0..K-1, is exactly one egpu_bestfit_batch_shard_prefix_dev call with
+ * step = first_step + 2k and the same flags; the result is, bit for bit, what K such calls issued on one
+ * stream give, and the call uses exchange steps first_step .. first_step + 2K - 1 (the caller advances
+ * by 2K).  Per batch: rows commit while the running demand of their device fits, counted over the whole
+ * shards of the lower ranks and this rank's earlier rows of that batch; the others get
+ * EGPU_IDX_DEFERRED.  d_delta (may be NULL) receives THIS rank's committed demand, int64[2*D];
+ * d_table_out (may be NULL) receives table - committed demand of all ranks, int32[3*D], identical on
+ * every rank (unlike the snapshot steps, it is written).  With EGPU_F_COMMIT that table is installed
+ * before batch k + 1 is scored; without it every batch is scored against the current table.  Never
+ * oversubscribes.  With EGPU_F_PACKED every batch is in the packed batch layout of
+ * egpu_bestfit_batches_dev (words, NULL d_req_mem, int8 indices).  The exchange vectors are those of
+ * the single call, so ranks may mix formats and may mix this launch with single calls.  ONE launch
+ * (egpu_launch_count + 1), ASYNCHRONOUS on `stream` with no synchronisation; it replays from a CUDA
+ * graph, and a replay after egpu_table_set starts from the new table.  It shares the prefix-commit and
+ * rounds scratch of the context: calls that use it must be ordered on one stream, or by the caller.
+ * Every wait inside the launch gives up after about 2 s: a peer vector that does not arrive is recorded
+ * as egpu_peer_last_timeout records it, a grid barrier is counted as for EGPU_F_DEVICE_ROUNDS.  The
+ * batches after the one in progress are then left unwritten.  If the wait was for the other ranks'
+ * uncapped demand (the base), or a grid barrier before the cut, the batch in progress commits nothing:
+ * every row of it that is not -1 is EGPU_IDX_DEFERRED, and its d_delta, d_table_out and the table are left
+ * as they were.  If it was for the committed demand (the apply), the batch's indices and d_delta are
+ * final and, as in the single call, its d_table_out and the table are left alone.  EGPU_ERR_STATE when the context is not attached to peers or under EGPU_VARIANT_GRID,
+ * EGPU_ERR_NO_TABLE without a table, EGPU_ERR_NOMEM (nothing committed) when scratch cannot be
+ * allocated.  EGPU_ERR_INVALID, before anything is launched or written: EGPU_F_APPLY or
+ * EGPU_F_INPUTS_READY with EGPU_F_PREFIX_COMMIT (this form always applies, and the single call refuses
+ * EGPU_F_INPUTS_READY too), EGPU_F_PACKED without EGPU_F_PREFIX_COMMIT, any EGPU_F_ROUNDS or
+ * EGPU_F_DEVICE_ROUNDS bit, first_step + 2K > 2^47, K outside 1..64, a batch with R >= 2^31, NULL or
+ * misaligned arrays with R > 0, a non-NULL d_req_mem with EGPU_F_PACKED and a NULL one without it,
+ * outputs of two batches that overlap.  This is a newly accepted flag set on an existing entry point:
+ * egpu_abi_version() stays 1011. */
 int egpu_bestfit_batches_shard_dev(egpu_ctx* ctx, const egpu_batch* batches, int32_t K, int flags,
                                    uint64_t first_step, void* stream);
 /* Start gate for a sharded sequence.  egpu_peer_gate_dev enqueues a one-warp kernel that
