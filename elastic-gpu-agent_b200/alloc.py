@@ -431,6 +431,20 @@ class BestFitAllocator:
                                                            _stream(stream))
         self._check(rc, "egpu_bestfit_batch_shard_prefix_dev")
 
+    def bestfit_shard_rounds_dev(self, d_core: int, d_mem: int, R: int, d_idx: int, d_delta: int, d_table_out: int, step: int,
+                                 packed: bool = False, stream: int | None = None):
+        """egpu_bestfit_batch_shard_prefix_dev with EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS |
+        EGPU_F_DEVICE_ROUNDS [| EGPU_F_PACKED]: rounds to the fixed point over the ranks' shards (rank-major order) in
+        one launch, asynchronous on `stream`; consumes exchange steps `step` and `step + 1`, whatever the number of
+        rounds.  d_delta (int64[2*D]) receives this rank's demand committed over all rounds, d_table_out (int32[3*D])
+        the last round's table'; both may be 0.  packed: d_core holds the words, d_idx receives int8 indices and d_mem
+        is not passed (NULL)."""
+        flags = L.F_PREFIX_COMMIT | L.F_COMMIT | L.F_ROUNDS | L.F_DEVICE_ROUNDS | (L.F_PACKED if packed else 0)
+        rc = self._lib.egpu_bestfit_batch_shard_prefix_dev(self._h, C.c_void_p(d_core), None if packed else C.c_void_p(d_mem),
+                                                           int(R), C.c_void_p(d_idx), C.c_void_p(d_delta or None),
+                                                           C.c_void_p(d_table_out or None), flags, int(step), _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_shard_prefix_dev")
+
     def bestfit_shard_lag_dev(self, d_core: int, d_mem: int, R: int, d_idx: int, d_delta: int, step: int, lag: int,
                               d_table_out_lagged: int = 0, stream: int | None = None, inputs_ready: bool = False):
         rc = self._lib.egpu_bestfit_batch_shard_lag_dev(self._h, C.c_void_p(d_core), C.c_void_p(d_mem), int(R),

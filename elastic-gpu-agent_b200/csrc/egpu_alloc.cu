@@ -143,6 +143,20 @@ constexpr decltype(shard_prefix_kernel<F, FMT, 0>()) kShardPrefixKernels[4] = {
     shard_prefix_kernel<F, FMT, 0>(), shard_prefix_kernel<F, FMT, 1>(), shard_prefix_kernel<F, FMT, 2>(),
     shard_prefix_kernel<F, FMT, 3>()};
 
+// The sharded rounds to the fixed point in one launch (egpu_bestfit_batch_shard_prefix_dev with EGPU_F_DEVICE_ROUNDS):
+// the same scans, CTAs and shared memory
+template <int F, RowFormat FMT, int B>
+constexpr auto shard_rounds_kernel() {
+    constexpr int DT = 8 << B;
+    if constexpr (F == kRoundsSorted)
+        return kernel(shard_rounds_sorted_kernel<DT, FMT>, kRoundsThreads, sizeof(SnapSmem<DT, kRoundsThreads>));
+    else return kernel(shard_rounds_lut_kernel<FMT>, kRoundsThreads, sizeof(LutSmem<kRoundsThreads>));
+}
+template <int F, RowFormat FMT>
+constexpr decltype(shard_rounds_kernel<F, FMT, 0>()) kShardRoundsKernels[4] = {
+    shard_rounds_kernel<F, FMT, 0>(), shard_rounds_kernel<F, FMT, 1>(), shard_rounds_kernel<F, FMT, 2>(),
+    shard_rounds_kernel<F, FMT, 3>()};
+
 // Resident CTAs per SM of kernel k; `cached` is its entry in the context's occupancy cache.  The
 // first use on a context opts in to the kernel's dynamic shared memory and asks the occupancy.
 template <class Fn>
@@ -585,8 +599,9 @@ struct RoundInfo {
 constexpr size_t kRoundsHead = 2048;
 constexpr size_t kRoundsCtlOff = 1536;
 constexpr size_t kShardStopOff = 1792;  // the stop word of the multi-batch sharded prefix-commit (ShardPrefixArgs::stop)
+constexpr size_t kShardAgainOff = 1800;  // the again word of the sharded rounds (ShardRoundsArgs::again)
 static_assert(sizeof(RoundInfo) <= kRoundsCtlOff && kRoundsCtlOff + sizeof(RoundsCtl) <= kShardStopOff &&
-                  kShardStopOff + sizeof(unsigned int) <= kRoundsHead,
+                  kShardStopOff + sizeof(unsigned int) <= kShardAgainOff && kShardAgainOff + sizeof(unsigned int) <= kRoundsHead,
               "rounds scratch head");
 struct RoundsScratch {
     RoundInfo* info;
@@ -916,6 +931,51 @@ int launch_shard_prefix_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, bool c
     // the lookup kernel leaves d_lut built from the table it last scored against or installed
     if (lut) ctx->lut_dirty = false;
     else if (commit) ctx->lut_dirty = true;
+    return EGPU_OK;
+}
+
+// Sharded rounds to the fixed point in ONE cooperative launch of shard_rounds_sorted_kernel / shard_rounds_lut_kernel
+// (egpu_scan.cuh): launch_prefix_commit_shard on exchange steps `step` and `step + 1`, committing, then every later
+// round on the same two steps, until no rank has a deferred row.  Grid: persistent_grid of this rank's R; scratch:
+// the rounds scratch of launch_device_rounds, sized by R, and the barrier, stop and again words in its head, all
+// allocated before the launch.  Nothing here waits for the device.
+int launch_shard_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx, long long* d_delta,
+                        int32_t* d_table_out, uint64_t step, cudaStream_t s, RowFormat fmt) {
+    if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // no prefix-commit mode
+    const bool lut = lut_variant(ctx), packed = fmt == kRowsPacked;
+    const int bucket = d_bucket(ctx->D), fam = lut ? kRoundsLut : kRoundsSorted;
+    const auto& k = lut ? (packed ? kShardRoundsKernels<kRoundsLut, kRowsPacked> : kShardRoundsKernels<kRoundsLut, kRowsInt32>)[bucket]
+                        : (packed ? kShardRoundsKernels<kRoundsSorted, kRowsPacked>
+                                  : kShardRoundsKernels<kRoundsSorted, kRowsInt32>)[bucket];
+    int64_t grid = 0;
+    int rc = persistent_grid(ctx, k, ctx->shard_rounds_ctas_per_sm[fam][packed][bucket], R, &grid);
+    if (rc != EGPU_OK) return rc;
+    RoundsScratch sc;
+    rc = rounds_scratch(ctx, R, packed, &sc);
+    if (rc != EGPU_OK) return rc;
+    ShardRoundsArgs a;
+    std::memset(&a, 0, sizeof a);
+    rc = rounds_ctl(ctx, s, &a.a.ctl);
+    if (rc != EGPU_OK) return rc;
+    a.a.rc = d_rc;
+    a.a.rm = packed ? nullptr : d_rm;
+    a.a.R = static_cast<long long>(R);
+    a.a.idx = d_idx;
+    a.a.delta_out = d_delta;
+    a.a.table_out = d_table_out;
+    a.a.tile_sums = ctx->d_tile_sums;
+    a.a.pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
+    a.a.total = sc.info->delta;
+    a.a.deferred = &sc.info->deferred;
+    a.a.tile_count = sc.tiles;
+    std::memcpy(a.a.set, sc.set, sizeof a.a.set);
+    a.a.lut = ctx->d_lut;
+    a.stop = reinterpret_cast<unsigned int*>(static_cast<char*>(ctx->d_rounds) + kShardStopOff);
+    a.again = reinterpret_cast<unsigned int*>(static_cast<char*>(ctx->d_rounds) + kShardAgainOff);
+    a.step_plus1 = step + 1;
+    rc = launch_persistent(ctx, k, grid, s, a);
+    if (rc != EGPU_OK) return rc;
+    ctx->lut_dirty = !lut;  // the lookup kernel leaves d_lut built from the table it committed
     return EGPU_OK;
 }
 
@@ -1604,8 +1664,13 @@ int egpu_bestfit_batch_shard_dev(egpu_ctx* ctx, const int32_t* d_req_core, const
 int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                                         int32_t* d_out_idx, int64_t* d_delta, int32_t* d_table_out, int flags,
                                         uint64_t step, void* stream) {
+    // EGPU_F_ROUNDS / EGPU_F_DEVICE_ROUNDS only as the flag set of the one-launch rounds, without
+    // EGPU_F_INPUTS_READY: rounds to the fixed point over the shards, in one launch, on steps step and step + 1
     const bool packed = (flags & EGPU_F_PACKED) != 0;
-    if (!ctx || R < 0 || step >= (1ull << 47) || (flags & ~(EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT | EGPU_F_PACKED)))
+    const bool rounds = (flags & (EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS)) != 0;
+    if (!ctx || R < 0 || step >= (1ull << 47)) return EGPU_ERR_INVALID;
+    if (rounds ? (flags & ~EGPU_F_PACKED) != kDeviceRoundsNeeds || R >= (1ll << 31) || step + 2 > (1ull << 47)
+               : (flags & ~(EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT | EGPU_F_PACKED)) != 0)
         return EGPU_ERR_INVALID;
     if (packed ? (d_req_mem || !rows_ok(R, {d_req_core, d_out_idx})) : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
         return EGPU_ERR_INVALID;
@@ -1613,6 +1678,9 @@ int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
+    if (rounds)
+        return launch_shard_rounds(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out,
+                                   step, s, packed ? kRowsPacked : kRowsInt32);
     return launch_prefix_commit_shard(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta),
                                       d_table_out, flags, step, s, packed ? kRowsPacked : kRowsInt32);
 }

@@ -171,6 +171,40 @@ __device__ __forceinline__ bool xchg_pull_word(XchgRow* rows, int world, unsigne
     }
     return true;
 }
+// xchg_pull_word with two sums from the one pass that consumes the words: `lower` += ranks [0, g_hi), `all` +=
+// every rank.  A second pull could not get the other sum: the first one has zeroed the words.
+__device__ __forceinline__ bool xchg_pull_word_split(XchgRow* rows, int world, unsigned long long step_plus1, int w, int g_hi,
+                                                     long long& lower, long long& all) {
+    const unsigned long long tag = xchg_tag(step_plus1);
+    const long long t0 = clock64();
+    for (int gb = 0; gb < world; gb += kPullGroup) {
+        const int ng = world - gb < kPullGroup ? world - gb : kPullGroup;
+        unsigned int pending = (1u << ng) - 1u;
+        for (;;) {
+            unsigned long long w0[kPullGroup], w1[kPullGroup];
+#pragma unroll
+            for (int k = 0; k < kPullGroup; ++k) {
+                w0[k] = w1[k] = 0ull;
+                if ((pending >> k) & 1u)
+                    asm volatile("ld.volatile.global.v2.u64 {%0, %1}, [%2];" : "=l"(w0[k]), "=l"(w1[k]) : "l"(&rows[gb + k].ll[2 * w]) : "memory");
+            }
+#pragma unroll
+            for (int k = 0; k < kPullGroup; ++k) {
+                if (((pending >> k) & 1u) && (w0[k] >> 32) == tag && (w1[k] >> 32) == tag) {
+                    const long long x = static_cast<long long>((w0[k] & 0xffffffffull) | (w1[k] << 32));
+                    all += x;
+                    if (gb + k < g_hi) lower += x;
+                    asm volatile("st.volatile.global.v2.u64 [%0], {%1, %1};" ::"l"(&rows[gb + k].ll[2 * w]), "l"(0ull) : "memory");
+                    pending &= ~(1u << k);
+                }
+            }
+            if (!pending) break;
+            if (clock64() - t0 > 4000000000ll) return false;
+            __nanosleep(40);
+        }
+    }
+    return true;
+}
 // thread d < D: the two values for device d (words d and D + d) of every rank; see xchg_pull_word
 __device__ __forceinline__ bool xchg_pull(XchgRow* rows, int world, unsigned long long step_plus1, int d, int D, int g_lo, int g_hi,
                                           long long& dc, long long& dm) {
@@ -2418,6 +2452,233 @@ shard_prefix_multi_lut_kernel(DevState* st, const __grid_constant__ ShardPrefixA
                                                                               static_cast<int>(tiles));
         __syncthreads();
         tile_sums_store<kRoundsThreads / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, D, a.tile_sums, tile);
+    });
+}
+
+// =============================================================================
+// Rounds to the fixed point over row shards in one launch (egpu_bestfit_batch_shard_prefix_dev with
+// EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS)
+// =============================================================================
+//
+// The batch is the concatenation of the ranks' shards in rank order, and the result is that of
+// egpu_bestfit_batch_rounds on it.  Round 1 is the sharded prefix-commit of the caller's rows.  Round j + 1
+// re-submits, rank-major, the rows round j deferred against the table round j committed: each rank compacts its
+// own deferred rows in order, so the concatenation of the compacted shards is the compacted batch.  One resident
+// wave (cooperative launch) runs the loop of rounds_cta with its phases 2 and 3 replaced by shard_prefix_cta's:
+//   1. CONTIG scan of the round's rows, tile b = CTA b, per-tile sums;
+//   2. CTA d < D: this rank's uncapped demand on device d to every rank as exchange step `step`, then every rank's
+//      word d in ONE pull (xchg_pull_word_split): the lower ranks' sum is the base of the cut, the sum of all ranks
+//      decides whether another round follows (below); then the cut of device d (prefix_cut_cta);
+//   3. deferred indices -> -2 by every CTA; CTA 0 pushes this rank's committed demand as step + 1 (prefix_push_cta),
+//      adds it to the running totals and applies every rank's with commit (apply_peers_cta): the installed,
+//      re-sorted table, table' in the last round only, and (lookup kernel) the rebuilt lookup table;
+//   4. a later round's indices back to the caller's rows.  The last round ends here, CTA 0 writing d_delta;
+//      otherwise the deferred rows are counted per 1024-row tile;
+//   5. CTA 0 turns the counts into offsets and their total;
+//   6. this rank's deferred rows, in order, into the other scratch set (none: its next round has n = 0 rows).
+//
+// Termination, decided from the same data on every rank with no exchange of its own.  Demands are non-negative,
+// so spec 2.5's cut keeps a prefix of device d's rows in the global order: a row on d is deferred on some rank iff
+// the all-rank uncapped demand on d exceeds free_core[d] or free_mem[d].  Every rank pulls exactly those words and
+// holds the same table, so every rank takes the same decision, whether or not it deferred rows itself; a rank
+// with none runs the next round on n = 0 rows (it pushes zero vectors, pulls and applies).  Every round commits
+// at least one row - the first row in the global order on an overflowing device fits by itself, since the scan
+// chose that device for it - so the rounds end.
+//
+// Every round reuses steps `step` and `step + 1`, slots and tags unchanged.  A rank pushes round j + 1's `step`
+// words only after its round-j apply has pulled every rank's `step + 1` words; each peer pushed those after its
+// barrier 2, which follows its own pulls of round j's `step` words (which zero them).  The same holds for
+// `step + 1` a phase later: a rank pushes round j + 1's after its barrier 2 of round j + 1, behind its pulls of
+// round j + 1's `step` words, which every peer pushed after its round-j apply.  So no word is overwritten before
+// it is consumed (DESIGN.md §5).  The zeroing store is to the puller's own memory, where the peer's next store
+// lands, and the barrier's fence orders it before the puller's next push.
+//
+// The again word: CTA 0 zeroes it at the top of every round, CTAs d < D raise it in phase 2, every CTA reads it
+// after barrier 2.  Barrier 1 orders the reset before the raises; barriers 3 to 6 of round j separate its reads
+// from round j + 1's reset.  The stop word: zeroed by CTA 0 at the start, raised by a pull that gives up, read by
+// every CTA after barriers 2 and 3 (the raising CTA arrives at the barrier after its store).
+//
+// A wait that gives up ends the launch (a pull: DevState::peer_timeout; a grid barrier:
+// DevState::rounds_timeouts).  In round 1 before the cut - barrier 1, barrier 2 or a base pull - nothing commits:
+// every CTA rewrites the rows of its own CONTIG tile of the caller's rows that chose a device to -2 and leaves,
+// exactly as shard_prefix_cta does (d_delta, d_table_out and the table stay as they were).  After that the rounds
+// already applied stay installed and the rows not finished stay -2: a later round's answers reach the caller's
+// rows only in its phase 4, behind its apply.  If round 1's apply gives up, its rows stay as its cut left them
+// and the table is left alone, as in the single prefix call.  d_delta and d_table_out are written at the fixed
+// point only.
+struct ShardRoundsArgs {
+    RoundsArgs a;                   // rows, outputs, scratch, barrier words and lookup table of the one-launch rounds
+    unsigned int* stop;             // a pull gave up: every CTA leaves at its next check
+    unsigned int* again;            // some device's all-rank demand exceeds its capacity: another round follows
+    unsigned long long step_plus1;  // `step` + 1; the committed demand travels as step + 1
+};
+static_assert(sizeof(DevState*) + sizeof(ShardRoundsArgs) <= 4096, "descriptors + the scalar arguments must fit the 4 KB kernel-parameter space");
+
+template <RowFormat FMT, bool LUT, class Scan>
+__device__ __forceinline__ void shard_rounds_cta(DevState* st, const ShardRoundsArgs& s, Scan&& scan) {
+    __shared__ int sOk;
+    __shared__ long long sBase[2 * kMaxD];  // prefix_cut_cta's base: only device blockIdx.x's two words are read
+    __shared__ unsigned long long sh[2 * (kRoundsThreads / 32)];
+    const RoundsArgs& a = s.a;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int tid = threadIdx.x;
+    unsigned int gen = 0;
+    if (tid == 0) gen = *reinterpret_cast<volatile unsigned int*>(&a.ctl->gen);
+    const int D = st->D;
+    volatile unsigned int* const stop = s.stop;
+    volatile unsigned int* const again = s.again;
+    if (b == 0) {
+        if (tid < 2 * kMaxD) a.total[tid] = 0;
+        if (tid == 0) *stop = 0u;  // next written in phase 2, behind barrier 1
+        // the table may have changed since the lookup table was last built (a replayed graph does not
+        // see the host's bookkeeping): build it from the table as it is now
+        if constexpr (LUT) lut_build_cta(st, a.lut);
+    }
+    // round 1's way out before the cut: the rows of this CTA's CONTIG tile of the caller's rows (the partition of
+    // the scans and of prefix_cut_cta) that chose a device -> -2
+    auto defer_tile = [&]() {
+        const long long nvec = a.R >> 2;
+        const long long per = (nvec + G - 1) / G;
+        const long long lo = b * per * 4 < nvec * 4 ? b * per * 4 : nvec * 4;
+        const long long hi = b == G - 1 ? a.R : ((b + 1) * per * 4 < nvec * 4 ? (b + 1) * per * 4 : nvec * 4);
+        for (long long r = lo + tid; r < hi; r += kRoundsThreads) {
+            if constexpr (FMT == kRowsPacked) {
+                signed char* const idx8 = reinterpret_cast<signed char*>(a.idx);
+                if (__ldcg(idx8 + r) >= 0) idx8[r] = -2;
+            } else {
+                if (__ldcg(a.idx + r) >= 0) a.idx[r] = -2;
+            }
+        }
+    };
+    bool ok = true;
+    if constexpr (LUT) ok = grid_barrier(a.ctl, st, gen, &sOk);
+    const int32_t* rc = a.rc;
+    const int32_t* rm = a.rm;
+    const int32_t* map = nullptr;  // nullptr in round 1: the rows are the caller's own
+    int32_t* idx = a.idx;
+    long long n = a.R;
+    int which = 0;
+    while (ok) {
+        if (b == 0 && tid == 0) *again = 0u;
+        scan(rc, rm, n, idx, b, G);  // 1
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) {
+            if (!map) defer_tile();
+            break;
+        }
+        if (static_cast<int>(b) < D) {  // 2
+            const int d = static_cast<int>(b);
+            unsigned long long c = 0, m = 0, tc, tm;
+            for (unsigned int t = tid; t < G; t += kRoundsThreads) {
+                c += __ldcg(&a.tile_sums[static_cast<size_t>(t) * 2 * kMaxD + d]);
+                m += __ldcg(&a.tile_sums[static_cast<size_t>(t) * 2 * kMaxD + kMaxD + d]);
+            }
+            block_scan2<kRoundsThreads>(c, m, sh, tc, tm);
+            if (tid == 0) {
+                xchg_push(st, s.step_plus1, d, D, static_cast<long long>(tc), static_cast<long long>(tm));
+                const int world = st->peer.world, me = st->peer.rank;
+                XchgRow* rows = st->peer.buf[me]->slot[(s.step_plus1 - 1) % kXchgSlots];
+                long long bc = 0, bm = 0, ac = 0, am = 0;
+                if (xchg_pull_word_split(rows, world, s.step_plus1, d, me, bc, ac) &&
+                    xchg_pull_word_split(rows, world, s.step_plus1, D + d, me, bm, am)) {
+                    sBase[d] = bc;
+                    sBase[kMaxD + d] = bm;
+                    if (ac > __ldcg(&st->free_core[d]) || am > __ldcg(&st->free_mem[d])) *again = 1u;
+                } else {  // a rank died: nothing of this round commits, and the launch ends with it
+                    st->peer_timeout = s.step_plus1;
+                    sBase[d] = 1ll << 40;
+                    sBase[kMaxD + d] = 1ll << 40;
+                    atomicExch(s.stop, 1u);
+                }
+            }
+            __syncthreads();
+            prefix_cut_cta<FMT>(st, idx, rc, rm, n, static_cast<int>(G), a.tile_sums, a.pf, sBase);
+        }
+        if (!grid_barrier(a.ctl, st, gen, &sOk) || *stop) {
+            if (!map) defer_tile();
+            break;
+        }
+        const bool last = *again == 0u;
+        if constexpr (FMT == kRowsPacked)  // 3
+            prefix_apply_packed_rows(a.pf, D, n, reinterpret_cast<signed char*>(idx));
+        else
+            prefix_apply_rows(a.pf, D, n, idx);
+        if (b == 0) {
+            prefix_push_cta(st, a.pf, s.step_plus1 + 1, nullptr);
+            if (tid < D) {
+                a.total[tid] += __ldcg(&a.pf->committed_c[tid]);
+                a.total[D + tid] += __ldcg(&a.pf->committed_m[tid]);
+            }
+            if (apply_peers_cta(st, s.step_plus1 + 1, 0, 1, [&](int) { return last ? a.table_out : nullptr; }, 1)) {
+                if constexpr (LUT) {
+                    __syncthreads();  // resort_table_cta's stores of the sorted view, read by every thread of the build
+                    lut_build_cta(st, a.lut);
+                }
+            } else if (tid == 0) {
+                atomicExch(s.stop, 1u);
+            }
+        }
+        if (!grid_barrier(a.ctl, st, gen, &sOk) || *stop) break;
+        if (map) round_writeback_rows<FMT>(idx, map, n, a.idx);  // 4
+        if (last) {
+            if (b == 0 && a.delta_out && tid < 2 * D) a.delta_out[tid] = a.total[tid];
+            break;
+        }
+        const long long tiles = (n + kCompactTile - 1) / kCompactTile;
+        for (long long t = b; t < tiles; t += G) {
+            deferred_count_cta<FMT>(idx, n, a.tile_count, static_cast<unsigned int>(t));
+            __syncthreads();
+        }
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (b == 0) tile_offsets_cta(a.tile_count, tiles, a.deferred);  // 5
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        const unsigned long long left = __ldcg(a.deferred);
+        int32_t* const n_rc = which ? a.set[1][0] : a.set[0][0];  // 6
+        int32_t* const n_rm = which ? a.set[1][1] : a.set[0][1];
+        int32_t* const n_map = which ? a.set[1][2] : a.set[0][2];
+        int32_t* const n_idx = which ? a.set[1][3] : a.set[0][3];
+        for (long long t = b; t < tiles; t += G) {
+            deferred_scatter_cta<FMT>(idx, rc, rm, map, n, a.tile_count, n_rc, n_rm, n_map, static_cast<unsigned int>(t));
+            __syncthreads();
+        }
+        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        rc = n_rc;
+        rm = n_rm;
+        map = n_map;
+        idx = n_idx;
+        n = static_cast<long long>(left);
+        which ^= 1;
+    }
+    rounds_exit(a.ctl);
+}
+
+// The register scan's form: the scan of the one-launch rounds, at the residency of the multi-batch twins.
+template <int DT, RowFormat FMT>
+__global__ void __launch_bounds__(kRoundsThreads, (kRoundsMultiMinCtas<DT, FMT>))
+shard_rounds_sorted_kernel(DevState* st, const __grid_constant__ ShardRoundsArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& s = *reinterpret_cast<SnapSmem<DT, kRoundsThreads>*>(smem_raw);
+    shard_rounds_cta<FMT, false>(st, a, [&](const int32_t* rc, const int32_t* rm, long long n, int32_t* idx, unsigned int tile,
+                                            unsigned int tiles) {
+        const int D = sorted_scan_rows<DT, kRoundsThreads, true, FMT, kLoadCoherent>(s, st, rc, rm, n, idx, static_cast<int>(tile),
+                                                                                     static_cast<int>(tiles));
+        hist_to_warp_sums<DT, kRoundsThreads>(s, D);
+        __syncthreads();
+        tile_sums_store<kRoundsThreads / 32>(&s.sWarpAcc[0][0], 2 * DT, 0, DT, D, a.a.tile_sums, tile);
+    });
+}
+
+// The lookup scan's form.
+template <RowFormat FMT>
+__global__ void __launch_bounds__(kRoundsThreads, 1)
+shard_rounds_lut_kernel(DevState* st, const __grid_constant__ ShardRoundsArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& sm = *reinterpret_cast<LutSmem<kRoundsThreads>*>(smem_raw);
+    shard_rounds_cta<FMT, true>(st, a, [&](const int32_t* rc, const int32_t* rm, long long n, int32_t* idx, unsigned int tile,
+                                           unsigned int tiles) {
+        const int D = lut_scan_rows<kRoundsThreads, true, FMT, kLoadCoherent>(sm, st, rc, rm, n, idx, a.a.lut, static_cast<int>(tile),
+                                                                              static_cast<int>(tiles));
+        __syncthreads();
+        tile_sums_store<kRoundsThreads / 32>(&sm.sWarpAcc[0][0], 2 * kMaxD, 0, kMaxD, D, a.a.tile_sums, tile);
     });
 }
 

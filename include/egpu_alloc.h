@@ -123,16 +123,19 @@ extern "C" {
                                     EGPU_F_PACKED | EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS
                                     [| EGPU_F_INPUTS_READY]: packed prefix-commit rounds to the fixed point
                                     (egpu_bestfit_batch_rounds on packed words, no round limit); see
-                                    egpu_bestfit_batch_dev.  egpu_bestfit_batches_dev refuses it except in
-                                    the flag set of EGPU_F_DEVICE_ROUNDS. */
+                                    egpu_bestfit_batch_dev.  egpu_bestfit_batches_dev and
+                                    egpu_bestfit_batch_shard_prefix_dev refuse it except in the flag set of
+                                    EGPU_F_DEVICE_ROUNDS. */
 
-#define EGPU_F_DEVICE_ROUNDS 128 /* egpu_bestfit_batch / egpu_bestfit_batch_dev / egpu_bestfit_batches_dev only,
-                                    and only as
+#define EGPU_F_DEVICE_ROUNDS 128 /* egpu_bestfit_batch / egpu_bestfit_batch_dev / egpu_bestfit_batches_dev and
+                                    egpu_bestfit_batch_shard_prefix_dev only, and only as
                                     EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS
                                     [| EGPU_F_PACKED] [| EGPU_F_INPUTS_READY]: rounds to the fixed point, int32 or
                                     packed, in ONE launch with no host round trip per round; the _dev forms do
                                     not synchronise their stream.  See egpu_bestfit_batch_dev (one batch) and
-                                    egpu_bestfit_batches_dev (batches placed in order).  The value is 128,
+                                    egpu_bestfit_batches_dev (batches placed in order).  Also accepted by
+                                    egpu_bestfit_batch_shard_prefix_dev, as that flag set without
+                                    EGPU_F_INPUTS_READY: rounds over row shards (see there).  The value is 128,
                                     not 64: callers were told that EGPU_F_ROUNDS with bit 64 is refused, and it
                                     still is.  Bit 64 is unassigned. */
 
@@ -502,7 +505,43 @@ int64_t egpu_peer_gate_timeouts(egpu_ctx* ctx);
  * flags EGPU_F_PACKED [| EGPU_F_PREFIX_COMMIT] [| EGPU_F_COMMIT]: the same on packed words, with the
  * arguments and refusals of the packed sharded scan (egpu_bestfit_batch_shard_dev above); d_out_idx
  * receives int8 indices: device, -1 or EGPU_IDX_DEFERRED.  The exchange steps carry the same vectors
- * as in the int32 call.  EGPU_ERR_STATE under EGPU_VARIANT_GRID (in either format). */
+ * as in the int32 call.  EGPU_ERR_STATE under EGPU_VARIANT_GRID (in either format).
+ *
+ * Rounds to the fixed point over row shards in one launch (flags EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT |
+ * EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS [| EGPU_F_PACKED]): the result is, bit for bit, egpu_bestfit_batch_rounds
+ * with no round limit on the concatenation of the ranks' shards in rank order - every rank's slice of the indices
+ * and the table every rank ends with.  Round 1 is the prefix-commit above, committing; round j + 1 re-submits,
+ * rank-major, the rows round j deferred against the table round j committed.  Every index ends as a device or -1,
+ * never EGPU_IDX_DEFERRED; sticky oversubscription flags are kept.  d_delta (may be NULL) receives THIS rank's
+ * demand committed over all rounds, int64[2*D]; d_table_out (may be NULL) the last round's table', int32[3*D] with
+ * the oversub words 0, identical on every rank; the committed table is installed in stream order.  If every rank
+ * passes R = 0 the call writes zero sums and table' = the current table.  The rows are int32 arrays or, with
+ * EGPU_F_PACKED, the packed arguments above (words, NULL d_req_mem, int8 indices).
+ * Exchange steps: the call uses `step` and `step + 1`, as the prefix call does, whatever the number of rounds
+ * (every round reuses the two), so the caller advances by 2.  Every rank must issue this call with the same
+ * `step`; R may differ between ranks, and a rank with no deferred rows left still takes part in every round.  A
+ * rank that issues the plain prefix call on that step instead is a usage error: its peers give up after about 2 s.
+ * ONE launch (egpu_launch_count + 1), ASYNCHRONOUS on `stream` with no synchronisation; it replays from a CUDA
+ * graph, and a replay after egpu_table_set starts from the new table.  The launch is cooperative: the runtime
+ * refuses a grid it cannot keep resident rather than letting it wait.  Scratch is the rounds scratch of
+ * egpu_bestfit_batch_dev with EGPU_F_DEVICE_ROUNDS, sized by this rank's R and allocated before the launch: an
+ * allocation failure returns EGPU_ERR_NOMEM with nothing committed.  The call shares that scratch with every
+ * prefix-commit and rounds call of the context, so they must be ordered on one stream, or by the caller.
+ * Timeouts: every wait inside the launch gives up after about 2 s and ends the launch.  A pull that gives up is
+ * recorded as egpu_peer_last_timeout reports it; a grid barrier that gives up is counted and reported by the next
+ * host-form call with EGPU_F_DEVICE_ROUNDS (EGPU_ERR_CUDA).  If the wait is in round 1 before the cut (the other
+ * ranks' uncapped demand, or a grid barrier), nothing commits: every row that chose a device is
+ * EGPU_IDX_DEFERRED, and the table, d_delta and d_table_out are left as they were, as in the multi-batch form of
+ * egpu_bestfit_batches_shard_dev.  If it is round 1's apply, the rows stay as its cut left them and the table is
+ * left alone, as in the prefix call.  In a later round the rounds already applied stay installed and the rows not
+ * finished stay EGPU_IDX_DEFERRED.  d_delta and d_table_out are written at the fixed point only.
+ * EGPU_ERR_STATE when the context is not attached to peers or under EGPU_VARIANT_GRID, EGPU_ERR_NO_TABLE without a
+ * table.  EGPU_ERR_INVALID, before anything is launched or written: EGPU_F_ROUNDS or EGPU_F_DEVICE_ROUNDS in any
+ * other combination (EGPU_F_INPUTS_READY or EGPU_F_APPLY with them among it), step + 2 > 2^47, R >= 2^31, NULL or
+ * misaligned arrays with R > 0, a non-NULL d_req_mem with EGPU_F_PACKED and a NULL one without it.  This is a
+ * newly accepted flag set on an existing entry point: egpu_abi_version() stays 1011.  The K-batch form
+ * (egpu_bestfit_batches_shard_dev) does not take these flags; K calls on one stream give K batches, one launch
+ * each. */
 int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core,
                                         const int32_t* d_req_mem, int64_t R,
                                         int32_t* d_out_idx, int64_t* d_delta,
