@@ -876,7 +876,12 @@ extern "C" int egpu_table_restore_flat(egpu_ctx* ctx, const char* ids_flat, cons
                                        int32_t* out_table, int32_t* out_status) {
     if (!ctx || !out_table || !cap_core || !cap_mem || D < 1 || D > EGPU_MAX_DEVICES || n_sets < 0 || n_ids < 0)
         return EGPU_ERR_INVALID;
-    if (flags & ~(EGPU_RESTORE_VERIFY | EGPU_RESTORE_INSTALL)) return EGPU_ERR_INVALID;
+    if (flags & ~(EGPU_RESTORE_VERIFY | EGPU_RESTORE_INSTALL | EGPU_RESTORE_CHARGE | EGPU_RESTORE_RELEASE))
+        return EGPU_ERR_INVALID;
+    // CHARGE / RELEASE: the entries' usage against the context's current table (DESIGN.md §2.7)
+    const int delta = flags & (EGPU_RESTORE_CHARGE | EGPU_RESTORE_RELEASE);
+    if (delta == (EGPU_RESTORE_CHARGE | EGPU_RESTORE_RELEASE) || (delta && (flags & EGPU_RESTORE_INSTALL)))
+        return EGPU_ERR_INVALID;
     for (int d = 0; d < D; ++d) {
         if (cap_core[d] < 0 || cap_core[d] > EGPU_CORE_MAX) return EGPU_ERR_INVALID;
         if (cap_mem[d] < 0 || cap_mem[d] > EGPU_MEM_MAX) return EGPU_ERR_INVALID;
@@ -905,10 +910,13 @@ extern "C" int egpu_table_restore_flat(egpu_ctx* ctx, const char* ids_flat, cons
         if (link_offsets[n_sets] > 0 && !link_gpu) return EGPU_ERR_INVALID;
     }
     std::lock_guard<std::mutex> g(ctx->mu);
+    if (delta && !ctx->has_table) return EGPU_ERR_NO_TABLE;
+    if (delta && D != ctx->D) return EGPU_ERR_INVALID;
     EGPU_CUDA(ctx, cudaSetDevice(ctx->dev));
     cudaStream_t s = ctx->stream;
     std::vector<int32_t> table(static_cast<size_t>(3) * D, 0);
     std::vector<int32_t> status(static_cast<size_t>(n_sets), EGPU_REC_OK);
+    unsigned long long usage[2 * kMaxD] = {0};  // CHARGE / RELEASE: [core 0..63, mem 64..127]
     if (n_sets == 0) {
         for (int d = 0; d < D; ++d) table[d] = cap_core[d], table[D + d] = cap_mem[d];
     } else {
@@ -941,18 +949,57 @@ extern "C" int egpu_table_restore_flat(egpu_ctx* ctx, const char* ids_flat, cons
             reinterpret_cast<const uint32_t*>(b + o_stored), reinterpret_cast<const int32_t*>(b + o_res),
             reinterpret_cast<const long long*>(b + o_loff), reinterpret_cast<const int32_t*>(b + o_lgpu), D,
             reinterpret_cast<unsigned long long*>(b + o_usage), reinterpret_cast<int32_t*>(b + o_status));
-        restore_table_kernel<<<1, kMaxD, 0, s>>>(reinterpret_cast<const int32_t*>(b + o_cap),
-                                                 reinterpret_cast<const unsigned long long*>(b + o_usage), D,
-                                                 reinterpret_cast<int32_t*>(b + o_table));
-        ctx->launches += 2;
+        ctx->launches += 1;
+        if (delta) {
+            // 2 x 64 sums against a table of at most 64 rows: read back, applied below
+            EGPU_CUDA(ctx, cudaMemcpyAsync(usage, b + o_usage, sizeof usage, cudaMemcpyDeviceToHost, s));
+        } else {
+            restore_table_kernel<<<1, kMaxD, 0, s>>>(reinterpret_cast<const int32_t*>(b + o_cap),
+                                                     reinterpret_cast<const unsigned long long*>(b + o_usage), D,
+                                                     reinterpret_cast<int32_t*>(b + o_table));
+            ctx->launches += 1;
+            EGPU_CUDA(ctx, cudaMemcpyAsync(table.data(), b + o_table, 4 * 3 * static_cast<size_t>(D), cudaMemcpyDeviceToHost, s));
+        }
         EGPU_CUDA(ctx, cudaGetLastError());
         EGPU_CUDA(ctx, cudaMemcpyAsync(status.data(), b + o_status, 4 * n_sets, cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaMemcpyAsync(table.data(), b + o_table, 4 * 3 * static_cast<size_t>(D), cudaMemcpyDeviceToHost, s));
         EGPU_CUDA(ctx, cudaStreamSynchronize(s));
+    }
+    if (delta) {
+        // the current table, read as egpu_table_get reads it: the context's stream is idle (synchronised
+        // above, or nothing was enqueued), and ctx->mu keeps every other call of this context out until
+        // the result is installed
+        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
+        EGPU_CUDA(ctx, cudaMemcpy(ctx->h_table, ctx->d_state, sizeof(int32_t) * 3 * kMaxD, cudaMemcpyDeviceToHost));
+        const int32_t* cur = ctx->h_table;
+        for (int d = 0; d < D; ++d) {
+            const long long uc = static_cast<long long>(usage[d]), um = static_cast<long long>(usage[kMaxD + d]);
+            const int32_t ov = cur[2 * kMaxD + d];
+            if (delta == EGPU_RESTORE_CHARGE) {
+                // max(max(a, 0) - u, 0) = max(a - u, 0) for u >= 0: charging a restored table is restoring the union
+                const long long c = cur[d] - uc, m = cur[kMaxD + d] - um;
+                table[d] = c < 0 ? 0 : static_cast<int32_t>(c);
+                table[D + d] = m < 0 ? 0 : static_cast<int32_t>(m);
+                table[2 * D + d] = (ov || c < 0 || m < 0) ? 1 : 0;
+                continue;
+            }
+            const long long c = cur[d] + uc, m = cur[kMaxD + d] + um;
+            const char* why = nullptr;
+            if ((uc || um) && ov) why = "is oversubscribed: the stored table lost the deficit; restore the node instead";
+            else if ((uc || um) && (c > cap_core[d] || m > cap_mem[d]))
+                why = "would exceed its capacity: more is released than is in use";
+            if (why) {
+                std::snprintf(ctx->last_err, sizeof ctx->last_err, "egpu_table_restore: release on device %d %s", d, why);
+                return EGPU_ERR_STATE;
+            }
+            table[d] = static_cast<int32_t>(c);
+            table[D + d] = static_cast<int32_t>(m);
+            table[2 * D + d] = ov;
+        }
     }
     std::memcpy(out_table, table.data(), sizeof(int32_t) * 3 * static_cast<size_t>(D));
     if (out_status && n_sets) std::memcpy(out_status, status.data(), sizeof(int32_t) * static_cast<size_t>(n_sets));
     // the installed table keeps the oversubscription flags, as a committing batch's table does (DESIGN.md §2.4)
-    if (flags & EGPU_RESTORE_INSTALL) return egpu_table_set_locked(ctx, table.data(), table.data() + D, table.data() + 2 * D, D);
+    if ((flags & EGPU_RESTORE_INSTALL) || delta)
+        return egpu_table_set_locked(ctx, table.data(), table.data() + D, table.data() + 2 * D, D);
     return EGPU_OK;
 }

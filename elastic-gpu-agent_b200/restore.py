@@ -14,6 +14,8 @@ REC_OK, REC_EMPTY, REC_FOREIGN, REC_NO_LINK, REC_HASH_MISMATCH = range(5)
 REC_STATUS_COUNT = 5
 RESTORE_VERIFY = 1
 RESTORE_INSTALL = 2
+RESTORE_CHARGE = 4
+RESTORE_RELEASE = 8
 RESOURCE_CORE, RESOURCE_MEM, RESOURCE_FOREIGN = 0, 1, -1
 
 
@@ -21,10 +23,17 @@ def _i32(a):
     return np.ascontiguousarray(a, dtype=np.int32)
 
 
-def restore_table(alloc, records, links, cap_core, cap_mem, verify: bool = True, install: bool = False):
+def _flags(verify, install, charge, release):
+    return ((RESTORE_VERIFY if verify else 0) | (RESTORE_INSTALL if install else 0) | (RESTORE_CHARGE if charge else 0)
+            | (RESTORE_RELEASE if release else 0))
+
+
+def restore_table(alloc, records, links, cap_core, cap_mem, verify: bool = True, install: bool = False,
+                  charge: bool = False, release: bool = False):
     """egpu_table_restore.  records: iterable of (key bytes, value bytes) as bucket.ForEach yields
-    them; links: iterable of (file name, readlink target).  Returns (free_core, free_mem, oversub,
-    counts[5], record_status[n_records])."""
+    them; links: iterable of (file name, readlink target).  charge / release apply the records'
+    usage to the context's current table instead (EGPU_RESTORE_CHARGE / EGPU_RESTORE_RELEASE).
+    Returns (free_core, free_mem, oversub, counts[5], record_status[n_records])."""
     records = [(bytes(k), bytes(v)) for k, v in records]
     links = [(n.encode() if isinstance(n, str) else bytes(n), t.encode() if isinstance(t, str) else bytes(t))
              for n, t in links]
@@ -40,7 +49,7 @@ def restore_table(alloc, records, links, cap_core, cap_mem, verify: bool = True,
     table = np.zeros(3 * D, dtype=np.int32)
     counts = np.zeros(REC_STATUS_COUNT, dtype=np.int64)
     rstat = np.zeros(max(1, n), dtype=np.int32)
-    flags = (RESTORE_VERIFY if verify else 0) | (RESTORE_INSTALL if install else 0)
+    flags = _flags(verify, install, charge, release)
     rc = L.load().egpu_table_restore(alloc.handle, keys, C.c_void_p(klen.ctypes.data), vals, C.c_void_p(vlen.ctypes.data), n,
                                      names, targets, nl, C.c_void_p(cc.ctypes.data), C.c_void_p(cm.ctypes.data), D, flags,
                                      C.c_void_p(table.ctypes.data), C.c_void_p(counts.ctypes.data),
@@ -51,10 +60,10 @@ def restore_table(alloc, records, links, cap_core, cap_mem, verify: bool = True,
 
 
 def restore_table_flat(alloc, sets, hashes, resources, links, cap_core, cap_mem, verify: bool = True,
-                       install: bool = False):
+                       install: bool = False, charge: bool = False, release: bool = False):
     """egpu_table_restore_flat.  sets: list of ID lists; hashes: stored 8-hex strings; resources:
-    RESOURCE_* per set; links: per set, the list of GPU indices of its symlinks (-1 = absent).
-    Returns (free_core, free_mem, oversub, status[n_sets])."""
+    RESOURCE_* per set; links: per set, the list of GPU indices of its symlinks (-1 = absent);
+    charge / release as in restore_table.  Returns (free_core, free_mem, oversub, status[n_sets])."""
     from .devhash import flatten
     flat, id_off, set_off = flatten(sets)
     n_sets = len(sets)
@@ -70,7 +79,7 @@ def restore_table_flat(alloc, sets, hashes, resources, links, cap_core, cap_mem,
     D = cc.size
     table = np.zeros(3 * D, dtype=np.int32)
     status = np.zeros(max(1, n_sets), dtype=np.int32)
-    flags = (RESTORE_VERIFY if verify else 0) | (RESTORE_INSTALL if install else 0)
+    flags = _flags(verify, install, charge, release)
     rc = L.load().egpu_table_restore_flat(alloc.handle, C.c_char_p(flat), C.c_void_p(id_off.ctypes.data), len(id_off) - 1,
                                           C.c_void_p(set_off.ctypes.data), n_sets, C.c_char_p(h8),
                                           C.c_void_p(res.ctypes.data), C.c_void_p(loff.ctypes.data),

@@ -61,6 +61,35 @@ extern "C" {
                                   with out_table's oversubscription flags: they stay set until the next
                                   egpu_table_set, as after a committing batch */
 
+/* Charge and release (DESIGN.md §2.7).  The caller's own stored records are the ledger: these flags
+ * apply a few of them to the context's CURRENT table instead of rebuilding it from all of them.
+ * U = the usage of the given entries, by the rule above and with the same per-entry statuses (only
+ * EGPU_REC_OK entries count, in either direction; EGPU_RESTORE_VERIFY is optional, as for a restore).
+ *   EGPU_RESTORE_CHARGE   free' = max(free - U, 0), oversub' = oversub | (free - U < 0), per device
+ *                         and dimension: charging B on the table a restore of A installed gives exactly
+ *                         the table a restore of A and B installs, flags included.  For placements this
+ *                         context did not commit itself (the scheduler's pick, stored by PreStartContainer).
+ *   EGPU_RESTORE_RELEASE  free' = free + U, flags unchanged: releasing B, a part of A, gives exactly the
+ *                         table a restore of A without B installs.  For the records GC is about to delete.
+ *                         All or nothing: refused with EGPU_ERR_STATE, installing and writing nothing, when
+ *                         on some device d with U[d] > 0 the sticky oversubscription flag is set (the stored
+ *                         table saturated at 0 and the deficit is lost: restore the node instead) or
+ *                         free + U > cap_core / cap_mem (more is released than is in use).
+ * Either one installs its result as EGPU_RESTORE_INSTALL does (sorted view, lookup tables rebuilt
+ * before the next lookup scan) and writes it to out_table.  Refused with EGPU_ERR_INVALID before
+ * anything is launched: both together, either with EGPU_RESTORE_INSTALL, D other than the context's
+ * table size; EGPU_ERR_NO_TABLE without a table.  n_sets = 0 leaves the table as it is and writes it
+ * to out_table.
+ * Ordering: the current table is read as egpu_table_get reads it, after the context's stream is
+ * synchronised and under the context's lock, and the result is installed before the lock is released,
+ * as EGPU_RESTORE_INSTALL and egpu_table_set install theirs.  So every host-buffer call and every _dev
+ * call on the context's own stream is counted; a committing _dev call on another stream must have
+ * completed (synchronise that stream first), or one of the two changes is lost.
+ * egpu_abi_version() stays 1011: these are newly accepted flags on existing entry points, as in
+ * ABI 1.9-1.11; a library that predates them refuses them with EGPU_ERR_INVALID. */
+#define EGPU_RESTORE_CHARGE  4
+#define EGPU_RESTORE_RELEASE 8
+
 /* Already-parsed form.  Entries = device-ID sets in the layout of egpu_device_hash_batch:
  *   ids_flat / id_offsets[n_ids + 1] / set_offsets[n_sets + 1]
  *   set_hash8     [n_sets * 8]   the stored Hash, 8 lowercase hex characters, no NUL
