@@ -38,6 +38,9 @@ F_APPLY = 8
 F_PACKED = 16
 F_ROUNDS = 32
 F_DEVICE_ROUNDS = 128
+F_RELEASE = 256
+REL_FLAGGED = 1
+REL_EXCEEDS = 2
 IDX_DEFERRED = -2
 
 EV_ALLOC = 0
@@ -116,6 +119,7 @@ def load() -> C.CDLL:
         "egpu_peer_gate_dev": (C.c_int, [vp, vp]),
         "egpu_peer_gate_open": (C.c_int, [vp]),
         "egpu_peer_gate_timeouts": (C.c_int64, [vp]),
+        "egpu_release_refusals": (C.c_int64, [vp]),
         "egpu_bestfit_query": (C.c_int, [vp, i32p, i32p, C.c_int32, vp, vp, C.c_int64, vp]),
         "egpu_device_hash_batch": (C.c_int, [vp, vp, vp, C.c_int64, vp, C.c_int64, vp, vp]),
         "egpu_device_hash": (C.c_int, [vp, vp, C.c_int64, vp]),

@@ -292,6 +292,49 @@ class BestFitAllocator:
                                               _stream(stream))
         self._check(rc, "egpu_bestfit_batch_dev")
 
+    # -- release: give placed rows' capacity back by index -----------------------
+    def release_dev(self, d_core: int, d_mem: int, R: int, d_idx: int, d_delta: int = 0, d_table_out: int = 0,
+                    commit: bool = False, packed: bool = False, stream: int | None = None):
+        """egpu_bestfit_batch_dev with EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: the R rows give back what
+        they hold on the devices in d_idx (read, never written), all or nothing, in one launch, asynchronous on
+        `stream`.  d_delta (int64[2*D]) receives the sums, d_table_out (int32[3*D]) table + sums (refused: the
+        table) and the per-device reason words; both may be 0.  commit=False is a dry run.  packed: d_core holds
+        the words, d_idx int8 indices and d_mem is not passed (NULL)."""
+        flags = L.F_RELEASE | (L.F_COMMIT if commit else 0) | (L.F_PACKED if packed else 0)
+        rc = self._lib.egpu_bestfit_batch_dev(self._h, C.c_void_p(d_core), None if packed else C.c_void_p(d_mem), int(R),
+                                              C.c_void_p(d_idx), C.c_void_p(d_delta or None), C.c_void_p(d_table_out or None),
+                                              flags, _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_dev")
+
+    def release(self, req_core, req_mem, idx, commit: bool = True, packed: bool = False):
+        """egpu_bestfit_batch with EGPU_F_RELEASE: host arrays, staged through HBM.  Returns (released_core
+        int64[D], released_mem int64[D]); raises EgpuError (ERR_STATE, naming the first offending device) when the
+        release was refused, with the sums in the exception's `released`.  packed: req_core holds the packed words,
+        req_mem is None and idx int8."""
+        rc_ = np.ascontiguousarray(req_core, dtype=np.uint32 if packed else np.int32)
+        rm_ = None if packed else _i32(req_mem)
+        ix = np.ascontiguousarray(idx, dtype=np.int8 if packed else np.int32)
+        if rc_.ndim != 1 or ix.shape != rc_.shape or (rm_ is not None and rm_.shape != rc_.shape):
+            raise L.EgpuError(L.ERR_INVALID, "release")
+        D = self._lib.egpu_table_size(self._h)
+        if D < 0:
+            raise L.EgpuError(D, "egpu_table_size")
+        dc = np.zeros(D, dtype=np.int64)
+        dm = np.zeros(D, dtype=np.int64)
+        flags = L.F_RELEASE | (L.F_COMMIT if commit else 0) | (L.F_PACKED if packed else 0)
+        rc = self._lib.egpu_bestfit_batch(self._h, _ptr(rc_), None if packed else _ptr(rm_), rc_.size, _ptr(ix), _ptr(dc),
+                                          _ptr(dm), flags)
+        if rc != L.OK:
+            err = L.EgpuError(rc, "egpu_bestfit_batch", self._lib.egpu_last_error(self._h).decode())
+            err.released = (dc, dm)
+            raise err
+        return dc, dm
+
+    @property
+    def release_refusals(self) -> int:
+        """egpu_release_refusals: release launches of this context refused on the device (synchronises it)."""
+        return int(self._lib.egpu_release_refusals(self._h))
+
     @staticmethod
     def make_batches(batches):
         """(d_core, d_mem, R, d_idx, d_delta, d_table_out) tuples -> the egpu_batch array of the C ABI

@@ -1005,6 +1005,60 @@ int launch_packed(egpu_ctx* ctx, const uint32_t* d_req, int64_t R, signed char* 
     return EGPU_OK;
 }
 
+// The release kernels (EGPU_F_RELEASE), per row format and D bucket: the register scans' CTA sizes and SnapSmem,
+// whose lane-private accumulators they reuse at every D (DESIGN.md 4.1h)
+template <RowFormat FMT, int B>
+constexpr auto release_kernel() {
+    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
+    return kernel(release_rows_kernel<DT, T, FMT>, T, sizeof(SnapSmem<DT, T>));
+}
+template <RowFormat FMT>
+constexpr decltype(release_kernel<FMT, 0>()) kReleaseKernels[4] = {release_kernel<FMT, 0>(), release_kernel<FMT, 1>(),
+                                                                  release_kernel<FMT, 2>(), release_kernel<FMT, 3>()};
+
+// The flags EGPU_F_RELEASE is valid with: itself, optionally EGPU_F_COMMIT and EGPU_F_PACKED
+bool release_flags_ok(int flags, int64_t R) {
+    return (flags & ~(EGPU_F_RELEASE | EGPU_F_COMMIT | EGPU_F_PACKED)) == 0 && R < (1ll << 31);
+}
+
+// EGPU_F_RELEASE (spec 2.8): the R rows (d_rc, d_rm) give back what they hold on device d_idx[r], all or
+// nothing, in one launch of release_rows_kernel.  Rows in either format (see prefix_scan); the indices are
+// read, never written.  d_delta (may be NULL) receives the sums, d_table_out (may be NULL) table + sums or,
+// refused, the table, and the per-device reason words; EGPU_F_COMMIT installs an accepted result.  An ordinary
+// launch, fully ordered behind everything on the stream, whatever the context's scan variant.  Grid: the
+// lone-launch rule of launch_snapshot_as (8 rows per thread, one resident wave, two from 16 Mi rows).
+int launch_release(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, const int32_t* d_idx, long long* d_delta,
+                   int32_t* d_table_out, int user_flags, cudaStream_t s, RowFormat fmt) {
+    const bool packed = fmt == kRowsPacked, commit = (user_flags & EGPU_F_COMMIT) != 0;
+    const int bucket = d_bucket(ctx->D);
+    const auto& k = (packed ? kReleaseKernels<kRowsPacked> : kReleaseKernels<kRowsInt32>)[bucket];
+    int per_sm = 0;
+    const int rc = resident_ctas(ctx, k, ctx->release_ctas_per_sm[packed][bucket], &per_sm);
+    if (rc != EGPU_OK) return rc;
+    Range mine[3];
+    batch_ranges(mine, nullptr, 0, 0, d_delta, d_table_out, ctx->D);
+    if (prepare_ranges(mine, 3) < 0) return EGPU_ERR_INVALID;  // the sums and table' overlap
+    const int rpt = ctx->rows_per_thread > 0 ? ctx->rows_per_thread : 8;
+    const int64_t per_cta = static_cast<int64_t>(k.threads) * ((rpt + 3) / 4);
+    int64_t want = ((R >> 2) + per_cta - 1) / per_cta;
+    if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
+    const int64_t cap = static_cast<int64_t>(ctx->sm_count) * per_sm * (R >= (16ll << 20) ? 2 : 1);
+    if (want > cap) want = cap;
+    if (want < 1) want = 1;
+    // lane-private sums hold 2^19 rows per lane (kAccShift)
+    if (R / (want * k.threads) + 8 >= (1ll << 19)) return EGPU_ERR_INVALID;
+    k.fn<<<static_cast<unsigned>(want), k.threads, k.smem, s>>>(ctx->d_state, d_rc, d_rm, static_cast<long long>(R), d_idx, d_delta,
+                                                                d_table_out, commit ? kFlagCommit : 0,
+                                                                static_cast<int>(ctx->seq % kEpiSlots));
+    EGPU_CUDA(ctx, cudaGetLastError());
+    ctx->launches += 1;
+    ctx->seq += 1;
+    new_group(ctx);
+    ctx->prev_is_scan = false;
+    if (commit) ctx->lut_dirty = true;  // a refused launch leaves the table as it was: a rebuild is harmless
+    return EGPU_OK;
+}
+
 // staging of the host-buffer entry points: three arrays of at least `rows` int32, doubling
 int ensure_staging(egpu_ctx* ctx, int64_t rows) {
     const size_t need = sizeof(int32_t) * static_cast<size_t>(rows);
@@ -1278,15 +1332,21 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32
     const bool packed = (flags & EGPU_F_PACKED) != 0;
     const bool rounds = (flags & EGPU_F_ROUNDS) != 0;
     const bool device_rounds = (flags & EGPU_F_DEVICE_ROUNDS) != 0;
-    if (!ctx || R < 0 || (device_rounds ? !device_rounds_flags_ok(flags, R) : rounds && !rounds_flags_ok(flags, R)))
+    // EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: the rows give back what they hold on d_out_idx, which is read.
+    const bool release = (flags & EGPU_F_RELEASE) != 0;
+    if (!ctx || R < 0 ||
+        (release ? !release_flags_ok(flags, R) : device_rounds ? !device_rounds_flags_ok(flags, R) : rounds && !rounds_flags_ok(flags, R)))
         return EGPU_ERR_INVALID;
-    if (packed ? (!(flags & EGPU_F_PREFIX_COMMIT) || d_req_mem || !rows_ok(R, {d_req_core, d_out_idx}))
+    if (packed ? ((!release && !(flags & EGPU_F_PREFIX_COMMIT)) || d_req_mem || !rows_ok(R, {d_req_core, d_out_idx}))
                : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
         return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
+    if (release)
+        return launch_release(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags, s,
+                              packed ? kRowsPacked : kRowsInt32);
     if (device_rounds) {
         const egpu_batch one{d_req_core, d_req_mem, R, d_out_idx, d_delta, d_table_out};
         return launch_device_rounds(ctx, &one, 1, false, s, packed ? kRowsPacked : kRowsInt32);
@@ -1384,6 +1444,21 @@ int64_t egpu_peer_gate_timeouts(egpu_ctx* ctx) {
     return static_cast<int64_t>(v);
 }
 
+int64_t egpu_release_refusals(egpu_ctx* ctx) {
+    if (!ctx) return EGPU_ERR_INVALID;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    if (cudaSetDevice(ctx->dev) != cudaSuccess) return EGPU_ERR_CUDA;
+    unsigned long long v = 0;
+    // every stream, the non-blocking ones too: the launches counted may sit on any of them
+    if (cudaDeviceSynchronize() != cudaSuccess ||
+        cudaMemcpy(&v, reinterpret_cast<char*>(ctx->d_state) + offsetof(DevState, release_refusals), sizeof v,
+                   cudaMemcpyDeviceToHost) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return EGPU_ERR_CUDA;
+    }
+    return static_cast<int64_t>(v);
+}
+
 int egpu_peer_gate_open(egpu_ctx* ctx) {
     if (!ctx) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
@@ -1448,15 +1523,44 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
     const bool packed = (commit & EGPU_F_PACKED) != 0;
     const bool rounds = (commit & EGPU_F_ROUNDS) != 0;
     const bool device_rounds = (commit & EGPU_F_DEVICE_ROUNDS) != 0;
-    if (!ctx || R < 0 || (device_rounds ? !device_rounds_flags_ok(commit, R) : rounds && !rounds_flags_ok(commit, R)))
+    const bool release = (commit & EGPU_F_RELEASE) != 0;  // out_idx is an input: the devices the rows were placed on
+    if (!ctx || R < 0 ||
+        (release ? !release_flags_ok(commit, R) : device_rounds ? !device_rounds_flags_ok(commit, R) : rounds && !rounds_flags_ok(commit, R)))
         return EGPU_ERR_INVALID;
-    if (packed ? (!prefix || req_mem || (R > 0 && (!req_core || !out_idx))) : (R > 0 && (!req_core || !req_mem || !out_idx)))
+    if (packed ? ((!release && !prefix) || req_mem || (R > 0 && (!req_core || !out_idx)))
+               : (R > 0 && (!req_core || !req_mem || !out_idx)))
         return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, nullptr, &s);
     if (rc != EGPU_OK) return rc;
     const int D = ctx->D;
+    if (release) {  // one launch, rows and indices staged through HBM: int32 12 bytes per row in, packed 5; nothing per row out
+        rc = ensure_staging(ctx, R > 0 ? R : 1);
+        if (rc != EGPU_OK) return rc;
+        if (R > 0) {
+            EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
+            if (!packed) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
+            EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_idx, out_idx, (packed ? sizeof(int8_t) : sizeof(int32_t)) * R, cudaMemcpyHostToDevice, s));
+        }
+        rc = launch_release(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, ctx->d_table_out, commit, s,
+                            packed ? kRowsPacked : kRowsInt32);
+        if (rc != EGPU_OK) return rc;
+        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
+        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_table, ctx->d_table_out, sizeof(int32_t) * 3 * D, cudaMemcpyDeviceToHost, s));
+        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
+        if (out_delta_core) std::memcpy(out_delta_core, ctx->h_delta, sizeof(int64_t) * D);
+        if (out_delta_mem) std::memcpy(out_delta_mem, ctx->h_delta + D, sizeof(int64_t) * D);
+        for (int d = 0; d < D; ++d) {
+            const int32_t reason = ctx->h_table[2 * D + d];
+            if (!reason) continue;
+            std::snprintf(ctx->last_err, sizeof ctx->last_err, "EGPU_F_RELEASE refused, nothing released: device %d %s", d,
+                          reason == EGPU_REL_FLAGGED ? "is oversubscribed (EGPU_REL_FLAGGED)"
+                                                     : "would hold more than the domain allows (EGPU_REL_EXCEEDS)");
+            return EGPU_ERR_STATE;
+        }
+        return EGPU_OK;
+    }
     if (device_rounds) {  // one launch, staged through HBM: int32 8 bytes per row in and 4 out, packed 4 in and 1 out
         rc = ensure_staging(ctx, R > 0 ? R : 1);
         if (rc != EGPU_OK) return rc;

@@ -37,7 +37,8 @@ struct egpu_ctx {
     int rounds_multi_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each multi-batch one-launch rounds kernel
     int shard_prefix_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each multi-batch sharded prefix-commit kernel
     int shard_rounds_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each sharded one-launch rounds kernel
-    void* h_qtable = nullptr;         // pinned host image of that table (the part of DevState before `peer`)
+    int release_ctas_per_sm[2][4] = {};  // ... and of each release kernel ([packed][bucket])
+    void* h_qtable = nullptr;        // pinned host image of that table (the part of DevState before `peer`)
     DevState* d_qstate = nullptr;     // scratch table of egpu_bestfit_query (the context's own table is not touched)
     unsigned long long* h_gate = nullptr;      // pinned: start gates the host has opened (egpu_peer_gate_open)
     unsigned long long* h_gate_dev = nullptr;  // its device-visible alias

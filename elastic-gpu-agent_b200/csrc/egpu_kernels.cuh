@@ -116,6 +116,7 @@ struct DevState {
     unsigned long long gate_epoch;        // start gates passed so far (egpu_peer_gate_dev)
     unsigned long long gate_timeouts;     // ... of which gave up waiting (~2 s) for the host or a peer
     unsigned long long rounds_timeouts;   // one-launch rounds (EGPU_F_DEVICE_ROUNDS) whose grid barrier gave up (~2 s)
+    unsigned long long release_refusals;  // release launches (EGPU_F_RELEASE) that were refused on the device
 };
 constexpr int kEpiSlots = 32;      // ring used by pipelined launches; slot 32 is spare
 constexpr int kPipeGroupMax = 24;  // at most this many launches between two fully ordered ones

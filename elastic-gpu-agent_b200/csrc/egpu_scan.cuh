@@ -2682,4 +2682,179 @@ shard_rounds_lut_kernel(DevState* st, const __grid_constant__ ShardRoundsArgs a)
     });
 }
 
+// =============================================================================
+// Release (EGPU_F_RELEASE, DESIGN.md §2.8): give placed rows' capacity back by index
+// =============================================================================
+//
+// A streaming per-device reduction with no scan: row r holds (core, mem) on device idx[r] when
+// 0 <= idx[r] < D and the request is in the spec's domain, and nothing otherwise.  12 bytes per row
+// are read (int32) or 5 (packed) and none written.  The rows are dealt as sorted_scan_rows deals
+// them (128-bit streaming loads, round-robin over the CTAs, the R % 4 tail in CTA 0) and summed
+// in the register scan's lane-private accumulators, at every D: row 0 absorbs the rows that hold
+// nothing, so the update is unconditional.  The last CTA to arrive accepts or refuses the whole
+// call and, when committing, installs table + sums.
+
+// per-device reason words of a release (EGPU_REL_* of include/egpu_alloc.h)
+constexpr int32_t kRelFlagged = 1;  // the device is oversubscribed: its true deficit was lost at 0
+constexpr int32_t kRelExceeds = 2;  // free + released would leave the spec's domain
+
+// four int8 indices of the packed format in one 32-bit load
+__device__ __forceinline__ uint32_t ld_stream_u32(const uint32_t* p) {
+    uint32_t r;
+    asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(r) : "l"(p));
+    return r;
+}
+
+template <int DT, int THREADS, RowFormat FMT>
+__global__ void __launch_bounds__(THREADS)
+release_rows_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_core, const int32_t* __restrict__ req_mem,
+                    long long R, const int32_t* __restrict__ idx, long long* __restrict__ delta_out,
+                    int32_t* __restrict__ table_out, int flags, int slot) {
+    static_assert(THREADS >= 2 * kMaxD, "the epilogue gives every sum a thread");
+    constexpr bool packed = FMT == kRowsPacked;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    auto& s = *reinterpret_cast<SnapSmem<DT, THREADS>*>(smem_raw);
+    const int tid = threadIdx.x;
+    const int lane = tid & 31;
+    const int warp = tid >> 5;
+    const int4* __restrict__ vc = reinterpret_cast<const int4*>(req_core);  // packed: 4 words per vector
+    const int4* __restrict__ vm = reinterpret_cast<const int4*>(req_mem);
+    const int4* __restrict__ vi = reinterpret_cast<const int4*>(idx);
+    const uint32_t* __restrict__ vi8 = reinterpret_cast<const uint32_t*>(idx);  // packed: 4 int8 indices per vector
+    const int nvec = static_cast<int>(R >> 2);
+    const int stride = static_cast<int>(gridDim.x) * THREADS;
+    int v = static_cast<int>(blockIdx.x) * THREADS + tid;
+
+    int4 c0 = make_int4(0, 0, 0, 0), m0 = c0, i0 = c0, c1 = c0, m1 = c0, i1 = c0;
+    bool has0 = v < nvec, has1 = (v + stride) < nvec;
+    auto load = [&](int at, int4& c, int4& m, int4& i) {
+        c = ld_stream_v4(vc + at);
+        if constexpr (packed) {
+            i.x = static_cast<int32_t>(ld_stream_u32(vi8 + at));
+        } else {
+            m = ld_stream_v4(vm + at);
+            i = ld_stream_v4(vi + at);
+        }
+    };
+    if (has0) load(v, c0, m0, i0);
+    if (has1) load(v + stride, c1, m1, i1);
+
+    const uint32_t D = static_cast<uint32_t>(st->D);
+    hist_zero<DT, THREADS>(s, warp, lane);
+    __syncwarp();
+
+    // the row test is folded into the accumulator row: -1 (row 0) for a row that holds nothing
+    auto add = [&](int32_t core, int32_t mem, int32_t d) {
+        const bool holds = static_cast<uint32_t>(d) < D && static_cast<uint32_t>(core) <= static_cast<uint32_t>(kCoreMax) &&
+                           static_cast<uint32_t>(mem) <= static_cast<uint32_t>(kMemMax);
+        hist_add<DT, THREADS>(s, warp, lane, holds ? d : -1, core, mem);
+    };
+    // packed: a word below (kCoreMax + 1) << 18 is below 2^25 with core <= 100, which is the set packed_request_word
+    // leaves feasible; a byte index is a device iff it is below D as an unsigned byte (D <= 64)
+    auto add_word = [&](uint32_t pw, uint32_t d8) {
+        const bool holds = d8 < D && pw < (static_cast<uint32_t>(kCoreMax + 1) << 18);
+        hist_add<DT, THREADS>(s, warp, lane, holds ? static_cast<int32_t>(d8) : -1, static_cast<int32_t>((pw >> 18) & 127u),
+                              static_cast<int32_t>(pw & 0x3FFFFu));
+    };
+    auto add4 = [&](const int4& c, const int4& m, const int4& i) {
+        if constexpr (packed) {
+            const uint32_t b = static_cast<uint32_t>(i.x);
+            add_word(static_cast<uint32_t>(c.x), b & 0xffu);
+            add_word(static_cast<uint32_t>(c.y), (b >> 8) & 0xffu);
+            add_word(static_cast<uint32_t>(c.z), (b >> 16) & 0xffu);
+            add_word(static_cast<uint32_t>(c.w), b >> 24);
+        } else {
+            add(c.x, m.x, i.x);
+            add(c.y, m.y, i.y);
+            add(c.z, m.z, i.z);
+            add(c.w, m.w, i.w);
+        }
+    };
+
+    while (has0) {
+        const int vn = v + 2 * stride;
+        const bool nhas0 = vn < nvec, nhas1 = (vn + stride) < nvec;
+        int4 nc0 = make_int4(0, 0, 0, 0), nm0 = nc0, ni0 = nc0, nc1 = nc0, nm1 = nc0, ni1 = nc0;
+        if (nhas0) load(vn, nc0, nm0, ni0);
+        if (nhas1) load(vn + stride, nc1, nm1, ni1);
+        add4(c0, m0, i0);
+        if (has1) add4(c1, m1, i1);
+        v = vn;
+        has0 = nhas0;
+        has1 = nhas1;
+        c0 = nc0; m0 = nm0; i0 = ni0; c1 = nc1; m1 = nm1; i1 = ni1;
+    }
+    // ragged tail: R % 4 rows, scalar loads that stay inside the arrays
+    if (blockIdx.x == 0 && tid < static_cast<int>(R & 3)) {
+        const long long r = ((R >> 2) << 2) + tid;
+        if constexpr (packed)
+            add_word(reinterpret_cast<const uint32_t*>(req_core)[r], reinterpret_cast<const unsigned char*>(idx)[r]);
+        else
+            add(req_core[r], req_mem[r], idx[r]);
+    }
+
+    // The general committing epilogue: every CTA adds its sums to the launch's slot (red.global.add.u64),
+    // orders them before its arrival ticket, and the last CTA to arrive owns the decision.
+    const int Di = static_cast<int>(D);
+    hist_to_warp_sums<DT, THREADS>(s, Di);
+    __syncthreads();
+    DevState::EpiSlot& ep = st->epi[slot];
+    if (tid < 2 * Di) {
+        const int j = tid < Di ? tid : DT + (tid - Di);
+        unsigned long long tot = 0;
+#pragma unroll
+        for (int w = 0; w < THREADS / 32; ++w) tot += s.sWarpAcc[w][j];
+        if (tot) atomicAdd(&ep.acc[tid < Di ? tid : kMaxD + (tid - Di)], tot);
+        fence_acq_rel_gpu();
+    }
+    __syncthreads();
+    if (tid == 0) s.sLast = atomicAdd(&ep.ticket, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!s.sLast) return;
+    fence_acq_rel_gpu();  // acquire: the other CTAs' sums, published before their tickets
+
+    // All or nothing: a touched device that is flagged, or that the sums would take out of the domain,
+    // refuses the whole call.  The context does not know a device's memory capacity, so the memory bound
+    // is the domain's.
+    long long uc = 0, um = 0;
+    int32_t fc = 0, fm = 0, reason = 0;
+    if (tid < Di) {
+        volatile unsigned long long* acc = ep.acc;
+        uc = static_cast<long long>(acc[tid]);
+        um = static_cast<long long>(acc[kMaxD + tid]);
+        acc[tid] = 0ull;
+        acc[kMaxD + tid] = 0ull;
+        fc = st->free_core[tid];
+        fm = st->free_mem[tid];
+        if (uc > 0 || um > 0)
+            reason = st->oversub[tid] ? kRelFlagged : (fc + uc > kCoreMax || fm + um > kMemMax) ? kRelExceeds : 0;
+    }
+    const bool refused = __syncthreads_or(reason) != 0;
+    const bool install = !refused && (flags & kFlagCommit);
+    if (tid < Di) {
+        const int32_t nc = refused ? fc : static_cast<int32_t>(fc + uc);
+        const int32_t nm = refused ? fm : static_cast<int32_t>(fm + um);
+        if (delta_out) {
+            delta_out[tid] = uc;
+            delta_out[Di + tid] = um;
+        }
+        if (table_out) {
+            table_out[tid] = nc;
+            table_out[Di + tid] = nm;
+            table_out[2 * Di + tid] = reason;
+        }
+        if (install) {  // the sticky oversubscription flags stay as they are
+            st->free_core[tid] = nc;
+            st->free_mem[tid] = nm;
+            s.sFc[tid] = nc;
+            s.sFm[tid] = nm;
+        }
+    }
+    if (install) resort_table_cta(st, Di, s.sFc, s.sFm, s.sPosDev, tid);
+    if (tid == 0) {
+        ep.ticket = 0u;
+        if (refused) st->release_refusals += 1;  // launches of a context are ordered: one writer at a time
+    }
+}
+
 }  // namespace egpu

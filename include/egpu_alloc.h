@@ -139,6 +139,21 @@ extern "C" {
                                     not 64: callers were told that EGPU_F_ROUNDS with bit 64 is refused, and it
                                     still is.  Bit 64 is unassigned. */
 
+#define EGPU_F_RELEASE      256  /* egpu_bestfit_batch / egpu_bestfit_batch_dev only, and only as
+                                    EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: the rows give back the
+                                    capacity they hold on the devices in the index array, which is an INPUT, all
+                                    or nothing, in one launch; see egpu_bestfit_batch_dev.  Any other bit with it
+                                    is EGPU_ERR_INVALID.  egpu_bestfit_batches_dev, egpu_bestfit_batches_shard_dev,
+                                    egpu_bestfit_batch_shard_dev and egpu_bestfit_batch_shard_prefix_dev refuse it;
+                                    egpu_bestfit_batch_packed_dev and egpu_bestfit_batch_shard_lag_dev ignore it, as
+                                    they ignore every bit they never checked.  Until this flag was defined the two
+                                    calls that take it ignored bit 256 when no rounds bit came with it; it is now
+                                    defined, and with it set only EGPU_F_COMMIT commits.  Bit 64 stays unassigned. */
+
+/* per-device reason words of a refused release: the third block of d_table_out */
+#define EGPU_REL_FLAGGED     1   /* rows are held on a device whose oversubscription flag is set */
+#define EGPU_REL_EXCEEDS     2   /* free + released would exceed EGPU_CORE_MAX or EGPU_MEM_MAX on the device */
+
 /* kernel variants for the snapshot scan (egpu_set_variant) */
 #define EGPU_VARIANT_AUTO    0   /* SORTED for D <= 16, LUT above */
 #define EGPU_VARIANT_GRID    1   /* direct (device x request) score grid, min over packed keys */
@@ -198,7 +213,9 @@ int egpu_table_size(egpu_ctx* ctx);
  * committed over all rounds), and with EGPU_F_ROUNDS, EGPU_F_DEVICE_ROUNDS (rounds in one launch, int32
  * or packed: staged through HBM, int32 8 bytes per row in and 4 out, packed 4 in and 1 out; one launch
  * and one synchronisation; returns EGPU_ERR_CUDA, with egpu_last_error saying so, when a device-rounds
- * launch on this context gave up at a grid barrier since the previous host-form call). */
+ * launch on this context gave up at a grid barrier since the previous host-form call).  `commit` also takes
+ * EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED] (release: see egpu_bestfit_batch_dev): out_idx is then an
+ * input, and the call returns EGPU_ERR_STATE when the release was refused. */
 int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core,
                        const int32_t* req_mem, int64_t R, int32_t* out_idx,
                        int64_t* out_delta_core, int64_t* out_delta_mem,
@@ -318,7 +335,37 @@ int  egpu_host_unregister(egpu_ctx* ctx, void* p);
  * reported by the next host-form call with EGPU_F_DEVICE_ROUNDS (EGPU_ERR_CUDA).  EGPU_ERR_STATE under
  * EGPU_VARIANT_GRID.  EGPU_ERR_INVALID, before anything is launched or written: EGPU_F_DEVICE_ROUNDS
  * with any other combination of flags, R >= 2^31, NULL or misaligned arrays with R > 0, a non-NULL
- * d_req_mem with EGPU_F_PACKED and a NULL one without it. */
+ * d_req_mem with EGPU_F_PACKED and a NULL one without it.
+ *
+ * Release (flags EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]; DESIGN.md 2.8): the R rows give back what
+ * they hold, by index, in ONE launch (egpu_launch_count + 1).  d_out_idx is READ, never written: it is the index
+ * array a committing call produced for these rows, or any subset or concatenation of such rows.  Row r holds
+ * (core, mem) on device d_out_idx[r] iff 0 <= d_out_idx[r] < D, 0 <= core <= EGPU_CORE_MAX and 0 <= mem <=
+ * EGPU_MEM_MAX; every other row (-1, EGPU_IDX_DEFERRED, any other index, an out-of-domain request) holds nothing
+ * and is skipped, so the output of a rounds or prefix-commit call can be handed back unfiltered.  U[d] = the int64
+ * sums over the rows held on d; a device is touched iff U_core[d] > 0 or U_mem[d] > 0.  The call is REFUSED, as a
+ * whole, iff some touched device has its oversubscription flag set (EGPU_REL_FLAGGED: saturation at 0 lost its
+ * true deficit) or free + U would exceed EGPU_CORE_MAX or EGPU_MEM_MAX there (EGPU_REL_EXCEEDS).  The context does
+ * not know a device's memory capacity: the memory bound is the domain bound only, and a caller who wants a
+ * capacity check runs the call without EGPU_F_COMMIT and compares d_table_out with its capacities.  Rows that are
+ * truly held on unflagged devices are never refused; a refusal means a double release, foreign rows or an
+ * oversubscribed device.  Written whether accepted or refused: d_delta (may be NULL) = U, int64[2*D]; d_table_out
+ * (may be NULL) = free + U when accepted and the current table when refused, int32[2*D], followed by D reason
+ * words: 0, EGPU_REL_FLAGGED or EGPU_REL_EXCEEDS (any non-zero word: refused).  With EGPU_F_COMMIT an accepted
+ * free + U becomes the table, in stream order; the sticky oversubscription flags stay as they are.  Without it
+ * nothing is installed (dry run).  A refused launch changes nothing but d_delta, d_table_out and
+ * egpu_release_refusals.  With EGPU_F_PACKED the rows are the arguments of packed prefix-commit (words, NULL
+ * d_req_mem, int8 indices); a word >= 2^25 or with core 101..127 holds nothing.  R = 0 is accepted: zero sums and
+ * d_table_out = the current table.  ASYNCHRONOUS on `stream`, fully ordered behind what the stream holds, and it
+ * replays from a CUDA graph.  It does not depend on the scan variant: it works under EGPU_VARIANT_GRID too.
+ * EGPU_ERR_NO_TABLE without a table.  EGPU_ERR_INVALID, before anything is launched or written: any other bit
+ * with EGPU_F_RELEASE (EGPU_F_INPUTS_READY, EGPU_F_PREFIX_COMMIT, EGPU_F_ROUNDS, EGPU_F_DEVICE_ROUNDS and
+ * EGPU_F_APPLY among them), R >= 2^31, NULL or misaligned arrays with R > 0, a non-NULL d_req_mem with
+ * EGPU_F_PACKED and a NULL one without it, d_delta and d_table_out that overlap.  The host form
+ * egpu_bestfit_batch takes the same flags in `commit`, reads out_idx, stages rows and indices through HBM (12
+ * bytes per row in, packed 5, none out), and returns EGPU_ERR_STATE when the release was refused, with
+ * egpu_last_error naming the first offending device and the reason; out_delta_* are written either way.  This is
+ * a newly accepted flag set on existing entry points: egpu_abi_version() stays 1011. */
 int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core,
                            const int32_t* d_req_mem, int64_t R,
                            int32_t* d_out_idx, int64_t* d_delta,
@@ -491,6 +538,9 @@ int egpu_bestfit_batches_shard_dev(egpu_ctx* ctx, const egpu_batch* batches, int
 int egpu_peer_gate_dev(egpu_ctx* ctx, void* stream);
 int egpu_peer_gate_open(egpu_ctx* ctx);
 int64_t egpu_peer_gate_timeouts(egpu_ctx* ctx);
+/* Release launches (EGPU_F_RELEASE) of this context that were refused on the device, since creation.  An
+ * asynchronous caller that passes a NULL d_table_out reads its refusals here.  Synchronises the device. */
+int64_t egpu_release_refusals(egpu_ctx* ctx);
 /* Prefix-commit (EGPU_F_PREFIX_COMMIT semantics, see egpu_bestfit_batch) over row shards.
  * The batch is the concatenation of the ranks' shards in rank order; request r of rank g
  * commits iff the running demand of its device over ALL earlier rows - the whole shards of
