@@ -488,6 +488,21 @@ class BestFitAllocator:
                                                            C.c_void_p(d_table_out or None), flags, int(step), _stream(stream))
         self._check(rc, "egpu_bestfit_batch_shard_prefix_dev")
 
+    def release_shard_dev(self, d_core: int, d_mem: int, R: int, d_idx: int, d_delta: int = 0, d_table_out: int = 0, *, step: int,
+                          commit: bool = True, packed: bool = False, stream: int | None = None):
+        """egpu_bestfit_batch_shard_prefix_dev with EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: this rank's R
+        rows give back what they hold on the devices in d_idx (read, never written); the result is the single-GPU
+        release of the concatenation of every rank's rows, all or nothing, in one launch, asynchronous on `stream`.
+        Consumes ONE exchange step, `step`, which every rank passes (with R = 0 too).  d_delta (int64[2*D]) receives
+        this rank's sums, d_table_out (int32[3*D]) table + every rank's sums (refused: the table) and the per-device
+        reason words, the same on every rank; both may be 0.  commit=False is a dry run.  packed: d_core holds the
+        words, d_idx int8 indices and d_mem is not passed (NULL)."""
+        flags = L.F_RELEASE | (L.F_COMMIT if commit else 0) | (L.F_PACKED if packed else 0)
+        rc = self._lib.egpu_bestfit_batch_shard_prefix_dev(self._h, C.c_void_p(d_core), None if packed else C.c_void_p(d_mem),
+                                                           int(R), C.c_void_p(d_idx), C.c_void_p(d_delta or None),
+                                                           C.c_void_p(d_table_out or None), flags, int(step), _stream(stream))
+        self._check(rc, "egpu_bestfit_batch_shard_prefix_dev")
+
     def bestfit_shard_lag_dev(self, d_core: int, d_mem: int, R: int, d_idx: int, d_delta: int, step: int, lag: int,
                               d_table_out_lagged: int = 0, stream: int | None = None, inputs_ready: bool = False):
         rc = self._lib.egpu_bestfit_batch_shard_lag_dev(self._h, C.c_void_p(d_core), C.c_void_p(d_mem), int(R),

@@ -1006,15 +1006,16 @@ int launch_packed(egpu_ctx* ctx, const uint32_t* d_req, int64_t R, signed char* 
 }
 
 // The release kernels (EGPU_F_RELEASE), per row format and D bucket: the register scans' CTA sizes and SnapSmem,
-// whose lane-private accumulators they reuse at every D (DESIGN.md 4.1h)
-template <RowFormat FMT, int B>
+// whose lane-private accumulators they reuse at every D (DESIGN.md 4.1h).  SHARD: the sharded form, whose last
+// CTA exchanges the sums with the peers before it decides.
+template <RowFormat FMT, bool SHARD, int B>
 constexpr auto release_kernel() {
     constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
-    return kernel(release_rows_kernel<DT, T, FMT>, T, sizeof(SnapSmem<DT, T>));
+    return kernel(release_rows_kernel<DT, T, FMT, SHARD>, T, sizeof(SnapSmem<DT, T>));
 }
-template <RowFormat FMT>
-constexpr decltype(release_kernel<FMT, 0>()) kReleaseKernels[4] = {release_kernel<FMT, 0>(), release_kernel<FMT, 1>(),
-                                                                  release_kernel<FMT, 2>(), release_kernel<FMT, 3>()};
+template <RowFormat FMT, bool SHARD>
+constexpr decltype(release_kernel<FMT, SHARD, 0>()) kReleaseKernels[4] = {
+    release_kernel<FMT, SHARD, 0>(), release_kernel<FMT, SHARD, 1>(), release_kernel<FMT, SHARD, 2>(), release_kernel<FMT, SHARD, 3>()};
 
 // The flags EGPU_F_RELEASE is valid with: itself, optionally EGPU_F_COMMIT and EGPU_F_PACKED
 bool release_flags_ok(int flags, int64_t R) {
@@ -1027,13 +1028,16 @@ bool release_flags_ok(int flags, int64_t R) {
 // refused, the table, and the per-device reason words; EGPU_F_COMMIT installs an accepted result.  An ordinary
 // launch, fully ordered behind everything on the stream, whatever the context's scan variant.  Grid: the
 // lone-launch rule of launch_snapshot_as (8 rows per thread, one resident wave, two from 16 Mi rows).
+// step_plus1 (egpu_bestfit_batch_shard_prefix_dev): the rows are this rank's shard, and the decision is taken on
+// every rank's sums, exchanged under step step_plus1 - 1 in the last CTA; 0 for one GPU.
 int launch_release(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, const int32_t* d_idx, long long* d_delta,
-                   int32_t* d_table_out, int user_flags, cudaStream_t s, RowFormat fmt) {
-    const bool packed = fmt == kRowsPacked, commit = (user_flags & EGPU_F_COMMIT) != 0;
+                   int32_t* d_table_out, int user_flags, cudaStream_t s, RowFormat fmt, uint64_t step_plus1) {
+    const bool packed = fmt == kRowsPacked, commit = (user_flags & EGPU_F_COMMIT) != 0, shard = step_plus1 != 0;
     const int bucket = d_bucket(ctx->D);
-    const auto& k = (packed ? kReleaseKernels<kRowsPacked> : kReleaseKernels<kRowsInt32>)[bucket];
+    const auto& k = (shard ? (packed ? kReleaseKernels<kRowsPacked, true> : kReleaseKernels<kRowsInt32, true>)
+                           : (packed ? kReleaseKernels<kRowsPacked, false> : kReleaseKernels<kRowsInt32, false>))[bucket];
     int per_sm = 0;
-    const int rc = resident_ctas(ctx, k, ctx->release_ctas_per_sm[packed][bucket], &per_sm);
+    const int rc = resident_ctas(ctx, k, (shard ? ctx->release_shard_ctas_per_sm : ctx->release_ctas_per_sm)[packed][bucket], &per_sm);
     if (rc != EGPU_OK) return rc;
     Range mine[3];
     batch_ranges(mine, nullptr, 0, 0, d_delta, d_table_out, ctx->D);
@@ -1049,7 +1053,7 @@ int launch_release(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int6
     if (R / (want * k.threads) + 8 >= (1ll << 19)) return EGPU_ERR_INVALID;
     k.fn<<<static_cast<unsigned>(want), k.threads, k.smem, s>>>(ctx->d_state, d_rc, d_rm, static_cast<long long>(R), d_idx, d_delta,
                                                                 d_table_out, commit ? kFlagCommit : 0,
-                                                                static_cast<int>(ctx->seq % kEpiSlots));
+                                                                static_cast<int>(ctx->seq % kEpiSlots), step_plus1);
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
     ctx->seq += 1;
@@ -1346,7 +1350,7 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32
     if (rc != EGPU_OK) return rc;
     if (release)
         return launch_release(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags, s,
-                              packed ? kRowsPacked : kRowsInt32);
+                              packed ? kRowsPacked : kRowsInt32, 0);
     if (device_rounds) {
         const egpu_batch one{d_req_core, d_req_mem, R, d_out_idx, d_delta, d_table_out};
         return launch_device_rounds(ctx, &one, 1, false, s, packed ? kRowsPacked : kRowsInt32);
@@ -1544,7 +1548,7 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
             EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_idx, out_idx, (packed ? sizeof(int8_t) : sizeof(int32_t)) * R, cudaMemcpyHostToDevice, s));
         }
         rc = launch_release(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, ctx->d_table_out, commit, s,
-                            packed ? kRowsPacked : kRowsInt32);
+                            packed ? kRowsPacked : kRowsInt32, 0);
         if (rc != EGPU_OK) return rc;
         EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
         EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_table, ctx->d_table_out, sizeof(int32_t) * 3 * D, cudaMemcpyDeviceToHost, s));
@@ -1769,12 +1773,16 @@ int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core
                                         int32_t* d_out_idx, int64_t* d_delta, int32_t* d_table_out, int flags,
                                         uint64_t step, void* stream) {
     // EGPU_F_ROUNDS / EGPU_F_DEVICE_ROUNDS only as the flag set of the one-launch rounds, without
-    // EGPU_F_INPUTS_READY: rounds to the fixed point over the shards, in one launch, on steps step and step + 1
+    // EGPU_F_INPUTS_READY: rounds to the fixed point over the shards, in one launch, on steps step and step + 1.
+    // EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: this rank's rows give back what they hold on d_out_idx
+    // (read, never written), decided on every rank's sums, in one launch, on step `step`
     const bool packed = (flags & EGPU_F_PACKED) != 0;
     const bool rounds = (flags & (EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS)) != 0;
+    const bool release = (flags & EGPU_F_RELEASE) != 0;
     if (!ctx || R < 0 || step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    if (rounds ? (flags & ~EGPU_F_PACKED) != kDeviceRoundsNeeds || R >= (1ll << 31) || step + 2 > (1ull << 47)
-               : (flags & ~(EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT | EGPU_F_PACKED)) != 0)
+    if (release ? !release_flags_ok(flags, R)
+        : rounds ? (flags & ~EGPU_F_PACKED) != kDeviceRoundsNeeds || R >= (1ll << 31) || step + 2 > (1ull << 47)
+                 : (flags & ~(EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT | EGPU_F_PACKED)) != 0)
         return EGPU_ERR_INVALID;
     if (packed ? (d_req_mem || !rows_ok(R, {d_req_core, d_out_idx})) : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
         return EGPU_ERR_INVALID;
@@ -1782,6 +1790,9 @@ int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
+    if (release)
+        return launch_release(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags, s,
+                              packed ? kRowsPacked : kRowsInt32, step + 1);
     if (rounds)
         return launch_shard_rounds(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out,
                                    step, s, packed ? kRowsPacked : kRowsInt32);

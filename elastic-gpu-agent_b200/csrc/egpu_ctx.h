@@ -38,6 +38,7 @@ struct egpu_ctx {
     int shard_prefix_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each multi-batch sharded prefix-commit kernel
     int shard_rounds_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each sharded one-launch rounds kernel
     int release_ctas_per_sm[2][4] = {};  // ... and of each release kernel ([packed][bucket])
+    int release_shard_ctas_per_sm[2][4] = {};  // ... and of each sharded release kernel ([packed][bucket])
     void* h_qtable = nullptr;        // pinned host image of that table (the part of DevState before `peer`)
     DevState* d_qstate = nullptr;     // scratch table of egpu_bestfit_query (the context's own table is not touched)
     unsigned long long* h_gate = nullptr;      // pinned: start gates the host has opened (egpu_peer_gate_open)

@@ -2693,6 +2693,12 @@ shard_rounds_lut_kernel(DevState* st, const __grid_constant__ ShardRoundsArgs a)
 // in the register scan's lane-private accumulators, at every D: row 0 absorbs the rows that hold
 // nothing, so the update is unconditional.  The last CTA to arrive accepts or refuses the whole
 // call and, when committing, installs table + sums.
+//
+// SHARD (egpu_bestfit_batch_shard_prefix_dev): the rows are this rank's shard of the release.  The
+// last CTA pushes this rank's sums under exchange step step_plus1 - 1, pulls every rank's sums of
+// that step and decides on their total, so every rank whose table is the same decides the same way
+// and installs the same table; d_delta keeps this rank's own sums.  A pull that gives up (~2 s, a
+// rank died) skips the decision, table' and the install and records the step in peer_timeout.
 
 // per-device reason words of a release (EGPU_REL_* of include/egpu_alloc.h)
 constexpr int32_t kRelFlagged = 1;  // the device is oversubscribed: its true deficit was lost at 0
@@ -2705,11 +2711,11 @@ __device__ __forceinline__ uint32_t ld_stream_u32(const uint32_t* p) {
     return r;
 }
 
-template <int DT, int THREADS, RowFormat FMT>
+template <int DT, int THREADS, RowFormat FMT, bool SHARD>
 __global__ void __launch_bounds__(THREADS)
 release_rows_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_core, const int32_t* __restrict__ req_mem,
                     long long R, const int32_t* __restrict__ idx, long long* __restrict__ delta_out,
-                    int32_t* __restrict__ table_out, int flags, int slot) {
+                    int32_t* __restrict__ table_out, int flags, int slot, unsigned long long step_plus1) {
     static_assert(THREADS >= 2 * kMaxD, "the epilogue gives every sum a thread");
     constexpr bool packed = FMT == kRowsPacked;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -2826,7 +2832,35 @@ release_rows_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_c
         acc[kMaxD + tid] = 0ull;
         fc = st->free_core[tid];
         fm = st->free_mem[tid];
-        if (uc > 0 || um > 0)
+        if constexpr (!SHARD)
+            if (uc > 0 || um > 0)
+                reason = st->oversub[tid] ? kRelFlagged : (fc + uc > kCoreMax || fm + um > kMemMax) ? kRelExceeds : 0;
+    }
+    const long long own_c = uc, own_m = um;  // this rank's sums: d_delta
+    if constexpr (SHARD) {
+        // thread d pushes this rank's (U_core[d], U_mem[d]) to every rank, then pulls every rank's words of the
+        // step (its own included) into (uc, um): both pull groups from world 5 up.  It has pushed before it waits
+        // and no push waits for anything, so there is no cycle.
+        bool ok = true;
+        if (tid < Di) {
+            const int world = st->peer.world;
+            xchg_push(st, step_plus1, tid, Di, own_c, own_m);
+            uc = um = 0;
+            ok = xchg_pull(st->peer.buf[st->peer.rank]->slot[(step_plus1 - 1) % kXchgSlots], world, step_plus1, tid, Di, 0, world,
+                           uc, um);
+        }
+        if (__syncthreads_or(!ok)) {  // a rank died: no decision, no table', no install
+            if (tid < Di && delta_out) {
+                delta_out[tid] = own_c;
+                delta_out[Di + tid] = own_m;
+            }
+            if (tid == 0) {
+                st->peer_timeout = step_plus1;
+                ep.ticket = 0u;
+            }
+            return;
+        }
+        if (tid < Di && (uc > 0 || um > 0))
             reason = st->oversub[tid] ? kRelFlagged : (fc + uc > kCoreMax || fm + um > kMemMax) ? kRelExceeds : 0;
     }
     const bool refused = __syncthreads_or(reason) != 0;
@@ -2835,8 +2869,8 @@ release_rows_kernel(DevState* __restrict__ st, const int32_t* __restrict__ req_c
         const int32_t nc = refused ? fc : static_cast<int32_t>(fc + uc);
         const int32_t nm = refused ? fm : static_cast<int32_t>(fm + um);
         if (delta_out) {
-            delta_out[tid] = uc;
-            delta_out[Di + tid] = um;
+            delta_out[tid] = own_c;
+            delta_out[Di + tid] = own_m;
         }
         if (table_out) {
             table_out[tid] = nc;

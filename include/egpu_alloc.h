@@ -139,12 +139,14 @@ extern "C" {
                                     not 64: callers were told that EGPU_F_ROUNDS with bit 64 is refused, and it
                                     still is.  Bit 64 is unassigned. */
 
-#define EGPU_F_RELEASE      256  /* egpu_bestfit_batch / egpu_bestfit_batch_dev only, and only as
+#define EGPU_F_RELEASE      256  /* egpu_bestfit_batch / egpu_bestfit_batch_dev and
+                                    egpu_bestfit_batch_shard_prefix_dev only, and only as
                                     EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: the rows give back the
                                     capacity they hold on the devices in the index array, which is an INPUT, all
-                                    or nothing, in one launch; see egpu_bestfit_batch_dev.  Any other bit with it
-                                    is EGPU_ERR_INVALID.  egpu_bestfit_batches_dev, egpu_bestfit_batches_shard_dev,
-                                    egpu_bestfit_batch_shard_dev and egpu_bestfit_batch_shard_prefix_dev refuse it;
+                                    or nothing, in one launch; see egpu_bestfit_batch_dev, and
+                                    egpu_bestfit_batch_shard_prefix_dev for the release over row shards.  Any other
+                                    bit with it is EGPU_ERR_INVALID.  egpu_bestfit_batches_dev,
+                                    egpu_bestfit_batches_shard_dev and egpu_bestfit_batch_shard_dev refuse it;
                                     egpu_bestfit_batch_packed_dev and egpu_bestfit_batch_shard_lag_dev ignore it, as
                                     they ignore every bit they never checked.  Until this flag was defined the two
                                     calls that take it ignored bit 256 when no rounds bit came with it; it is now
@@ -591,7 +593,36 @@ int64_t egpu_release_refusals(egpu_ctx* ctx);
  * misaligned arrays with R > 0, a non-NULL d_req_mem with EGPU_F_PACKED and a NULL one without it.  This is a
  * newly accepted flag set on an existing entry point: egpu_abi_version() stays 1011.  The K-batch form
  * (egpu_bestfit_batches_shard_dev) does not take these flags; K calls on one stream give K batches, one launch
- * each. */
+ * each.
+ *
+ * Release over row shards (flags EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]; DESIGN.md 2.8): each rank
+ * passes its own rows and index array - typically the slice of the indices this rank's sharded placement call
+ * produced - with the row rule and the packed arguments of the single-GPU release (egpu_bestfit_batch_dev): the
+ * index array is READ, never written, and rows that hold nothing are skipped.  The result is, bit for bit, the
+ * single-GPU release of the concatenation of every rank's rows against the table the ranks share: U = the int64 sum
+ * over the ranks of each rank's U_g, the same all-or-nothing test on every touched device (EGPU_REL_FLAGGED,
+ * EGPU_REL_EXCEEDS), and the same install of free + U, re-sorted, with the sticky flags kept.  The decision is taken
+ * from each rank's own table: ranks whose tables are equal, as every sharded call keeps them, decide the same way
+ * and install the same table; a caller who installed different tables on different ranks gets no guarantee.
+ * Written whether accepted or refused: d_delta (may be NULL) = THIS rank's U_g, int64[2*D]; d_table_out (may be
+ * NULL) = free + U when accepted and the current table when refused, int32[2*D], followed by the D reason words,
+ * identical on every rank.  With EGPU_F_COMMIT an accepted result is installed on every rank in stream order.  A
+ * refused launch changes nothing but d_delta, d_table_out and egpu_release_refusals, which each rank counts for
+ * itself.  Exchange steps: the call uses ONE step, `step`, so the caller advances by 1.  Every rank must issue the
+ * call with the same `step`, and every rank launches, with R = 0 too (it contributes zero sums).  A rank that
+ * issues a different call on that step (a prefix call, say) is a usage error: its peers give up after about 2 s.
+ * ONE launch (egpu_launch_count + 1), ASYNCHRONOUS on `stream`, fully ordered behind what the stream holds; it
+ * replays from a CUDA graph and does not depend on the scan variant (it works under EGPU_VARIANT_GRID too).
+ * Timeout: a peer whose sums do not arrive makes the launch give up after about 2 s; d_delta is written, d_table_out
+ * and the table are left as they were, no refusal is counted, and egpu_peer_last_timeout reports step + 1.  The
+ * ranks' tables may then differ (a peer may have installed the release): the caller re-installs a table on every
+ * rank (egpu_table_set).  EGPU_ERR_STATE when the context is not attached to peers, EGPU_ERR_NO_TABLE without a
+ * table.  EGPU_ERR_INVALID, before anything is launched or written: any other bit with EGPU_F_RELEASE
+ * (EGPU_F_PREFIX_COMMIT, EGPU_F_ROUNDS, EGPU_F_DEVICE_ROUNDS, EGPU_F_INPUTS_READY and EGPU_F_APPLY among them),
+ * R >= 2^31, step >= 2^47, NULL or misaligned arrays with R > 0, a non-NULL d_req_mem with EGPU_F_PACKED and a
+ * NULL one without it, d_delta and d_table_out that overlap.  This is a newly accepted flag set on an existing entry
+ * point: egpu_abi_version() stays 1011.  egpu_bestfit_batches_shard_dev, egpu_bestfit_batch_shard_dev,
+ * egpu_bestfit_batches_dev and egpu_bestfit_batch_shard_lag_dev keep their handling of EGPU_F_RELEASE. */
 int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core,
                                         const int32_t* d_req_mem, int64_t R,
                                         int32_t* d_out_idx, int64_t* d_delta,
