@@ -207,14 +207,59 @@ bool lut_variant(const egpu_ctx* ctx) {
     return ctx->variant == EGPU_VARIANT_LUT || (ctx->variant == EGPU_VARIANT_AUTO && ctx->D > 16);
 }
 
-// the lookup scans read ctx->d_lut: rebuild it on the launching stream after the table changed
-int refresh_lut(egpu_ctx* ctx, cudaStream_t s) {
-    if (!ctx->lut_dirty) return EGPU_OK;
+// Stream capture (CUDA graphs).  A launch captured into a graph runs at every replay, not now, against whatever
+// table the context holds then; so the host bookkeeping of a captured launch must not change as if it had run
+// (DESIGN.md 2.9):
+//  - a captured lookup scan rebuilds d_lut inside the graph when it is stale (once per capture), and lut_dirty is
+//    left as it was: the next eager lookup scan still rebuilds it;
+//  - a captured launch that may rewrite the table and leaves d_lut alone is followed, inside the graph, by a
+//    rebuild of d_lut, so that a replay leaves d_lut built from the table it installed; lut_dirty is left as it was;
+//  - scans pipeline only behind scans of the same capture, or eagerly behind eager ones: a captured scan is never
+//    the eager predecessor of the next launch; the epilogue rings still advance, so that slots stay distinct.
+// capture_id: the capture sequence `s` belongs to (bit 63 set), 0 when it is not capturing.
+unsigned long long capture_id(cudaStream_t s) {
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    unsigned long long id = 0;
+    if (cudaStreamGetCaptureInfo(s, &st, &id) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return 0;
+    }
+    return st == cudaStreamCaptureStatusActive ? (id | (1ull << 63)) : 0;
+}
+
+int launch_lut_build(egpu_ctx* ctx, cudaStream_t s) {
     lut_build_kernel<<<1, 256, 0, s>>>(ctx->d_state, ctx->d_lut);
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
-    ctx->lut_dirty = false;
     ctx->prev_is_scan = false;
+    return EGPU_OK;
+}
+
+// the lookup scans read ctx->d_lut: rebuild it on the launching stream after the table changed
+int refresh_lut(egpu_ctx* ctx, cudaStream_t s) {
+    const unsigned long long cap = capture_id(s);
+    if (!ctx->lut_dirty || (cap && ctx->lut_capture == cap)) return EGPU_OK;
+    const int rc = launch_lut_build(ctx, s);
+    if (rc != EGPU_OK) return rc;
+    if (cap) ctx->lut_capture = cap;
+    else ctx->lut_dirty = false;
+    return EGPU_OK;
+}
+
+// After a launch on `s` that may rewrite the table.  lut_built: the launch itself leaves d_lut built from the
+// table it leaves (the persistent lookup kernels).  Eagerly: mark d_lut stale (or, lut_built, current).  Captured:
+// rebuild it inside the graph (see capture_id).
+int table_changed(egpu_ctx* ctx, cudaStream_t s, bool lut_built = false) {
+    const unsigned long long cap = capture_id(s);
+    if (!cap) {
+        ctx->lut_dirty = !lut_built;
+        return EGPU_OK;
+    }
+    if (!lut_built) {
+        const int rc = launch_lut_build(ctx, s);
+        if (rc != EGPU_OK) return rc;
+    }
+    ctx->lut_capture = cap;  // the graph's later lookup scans read the tables it rebuilt
     return EGPU_OK;
 }
 
@@ -305,9 +350,11 @@ void new_group(egpu_ctx* ctx) {
 //    flight to pipe_group + 1 < kEpiSlots, and the epi_multi slots of those launches and this
 //    one's `batches` (0 for a single-batch launch) stay within half of that ring.
 // Otherwise the launch is fully ordered and opens a new group.
-int order_scan(egpu_ctx* ctx, int user_flags, bool eligible, int batches, cudaStream_t s, const Range* mine, int n_mine) {
+// `cap`: the launch's capture_id; the previous launch must belong to the same capture, or both be eager.
+int order_scan(egpu_ctx* ctx, int user_flags, bool eligible, int batches, cudaStream_t s, const Range* mine, int n_mine,
+               unsigned long long cap) {
     int flags = 0;
-    const bool pipelined = (user_flags & EGPU_F_INPUTS_READY) && eligible && ctx->prev_is_scan && !ctx->prev_changes_table &&
+    const bool pipelined = (user_flags & EGPU_F_INPUTS_READY) && eligible && ctx->prev_capture == cap && ctx->prev_is_scan && !ctx->prev_changes_table &&
                            ctx->prev_stream == s && ctx->group_len > 0 && !overlaps_inflight(ctx->inflight, mine, n_mine);
     if (pipelined) {
         flags |= kFlagLateWait;
@@ -330,11 +377,13 @@ int order_scan(egpu_ctx* ctx, int user_flags, bool eligible, int batches, cudaSt
 }
 
 // Bookkeeping of a scan launched under order_scan: `batches` = 0 for a single-batch launch (one
-// epilogue slot of the seq ring), K for a multi-batch one (K slots of the mseq ring).
-void record_scan(egpu_ctx* ctx, cudaStream_t s, const Range* mine, int n_mine, int batches, bool changes_table) {
+// epilogue slot of the seq ring), K for a multi-batch one (K slots of the mseq ring); `cap` its capture_id.
+void record_scan(egpu_ctx* ctx, cudaStream_t s, const Range* mine, int n_mine, int batches, bool changes_table,
+                 unsigned long long cap) {
     ctx->launches += 1;
     if (batches) ctx->mseq += static_cast<uint64_t>(batches);
     else ctx->seq += 1;
+    ctx->prev_capture = cap;
     ctx->range_tmp.resize(ctx->inflight.size() + static_cast<size_t>(n_mine));
     std::merge(ctx->inflight.begin(), ctx->inflight.end(), mine, mine + n_mine, ctx->range_tmp.begin(),
                [](const Range& a, const Range& b) { return a.lo < b.lo; });
@@ -383,8 +432,9 @@ int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_
     const int n_mine = prepare_ranges(mine, 3);
     if (n_mine < 0) return EGPU_ERR_INVALID;  // two of this launch's own outputs overlap
     const bool commit = (a.user_flags & EGPU_F_COMMIT) != 0;
+    const unsigned long long captured = capture_id(s);
     const int flags = kFlagFinalize | (commit ? kFlagCommit : 0) |
-                      order_scan(ctx, a.user_flags, !grid_variant && !a.contig && !commit, 0, s, mine, n_mine);
+                      order_scan(ctx, a.user_flags, !grid_variant && !a.contig && !commit, 0, s, mine, n_mine, captured);
     const unsigned long long slot = (ctx->seq % kEpiSlots) | (a.push_step_plus1 << 8) | (static_cast<unsigned long long>(a.lag) << 56);
 
     // Grid: one resident wave at most.  A lone launch wants every SM pulling at once
@@ -429,9 +479,8 @@ int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_
         rc = launch_pdl(ctx, k, want, s, ctx->d_state, a.rc, a.rm, static_cast<long long>(a.R), a.idx, a.delta, a.table_out, flags,
                         slot, tile_sums);
     if (rc != EGPU_OK) return rc;
-    if (commit) ctx->lut_dirty = true;
-    record_scan(ctx, s, mine, n_mine, 0, commit);
-    return EGPU_OK;
+    record_scan(ctx, s, mine, n_mine, 0, commit, captured);
+    return commit ? table_changed(ctx, s) : EGPU_OK;
 }
 
 // One scan of one batch against the context's table, in the kernel the context's variant picks.
@@ -486,8 +535,9 @@ int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, 
     }
     const int n_mine = prepare_ranges(mine, 3 * K);
     if (n_mine < 0) return EGPU_ERR_INVALID;  // two batches of one launch share an output: their order would be undefined
+    const unsigned long long captured = capture_id(s);
     const int flags = kFlagFinalize | ((push_base && (user_flags & EGPU_F_APPLY)) ? kFlagApplyNow : 0) |
-                      order_scan(ctx, user_flags, true, K, s, mine, n_mine);
+                      order_scan(ctx, user_flags, true, K, s, mine, n_mine, captured);
 
     // Tiles per batch.  Batches below 512 Ki rows: enough CTAs that a thread has >= multi_rpt rows,
     // at most the resident capacity of the GPU (one wave: there, every extra CTA costs an epilogue
@@ -529,7 +579,7 @@ int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, 
     else
         rc = launch_pdl(ctx, k, n_ctas, s, ctx->d_state, args, tiles_extra, flags, slot_base, push_base);
     if (rc != EGPU_OK) return rc;
-    record_scan(ctx, s, mine, n_mine, K, false);
+    record_scan(ctx, s, mine, n_mine, K, false, captured);
     return EGPU_OK;
 }
 
@@ -576,8 +626,7 @@ int launch_prefix_commit(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 3;
     ctx->prev_is_scan = false;
-    if (user_flags & EGPU_F_COMMIT) ctx->lut_dirty = true;
-    return EGPU_OK;
+    return (user_flags & EGPU_F_COMMIT) ? table_changed(ctx, s) : EGPU_OK;
 }
 
 // Rounds of committing prefix-commit until nothing is deferred (spec 2.5, "rounds").  Round 1
@@ -848,8 +897,7 @@ int launch_device_rounds(egpu_ctx* ctx, const egpu_batch* bs, int K, bool multi,
         rc = launch_persistent(ctx, k, grid, s, a);
     }
     if (rc != EGPU_OK) return rc;
-    ctx->lut_dirty = !lut;  // the lookup kernels leave d_lut built from the table they committed
-    return EGPU_OK;
+    return table_changed(ctx, s, lut);  // the lookup kernels leave d_lut built from the table they committed
 }
 
 // Prefix-commit over row shards (one rank per GPU, rank-major row order).  Two exchange
@@ -881,8 +929,7 @@ int launch_prefix_commit_shard(egpu_ctx* ctx, const int32_t* d_rc, const int32_t
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 5;
     ctx->prev_is_scan = false;
-    if (user_flags & EGPU_F_COMMIT) ctx->lut_dirty = true;
-    return EGPU_OK;
+    return (user_flags & EGPU_F_COMMIT) ? table_changed(ctx, s) : EGPU_OK;
 }
 
 // K sharded prefix-commits in ONE cooperative launch of shard_prefix_multi_sorted_kernel /
@@ -929,9 +976,7 @@ int launch_shard_prefix_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, bool c
     rc = launch_persistent(ctx, k, grid, s, a);
     if (rc != EGPU_OK) return rc;
     // the lookup kernel leaves d_lut built from the table it last scored against or installed
-    if (lut) ctx->lut_dirty = false;
-    else if (commit) ctx->lut_dirty = true;
-    return EGPU_OK;
+    return (lut || commit) ? table_changed(ctx, s, lut) : EGPU_OK;
 }
 
 // Sharded rounds to the fixed point in ONE cooperative launch of shard_rounds_sorted_kernel / shard_rounds_lut_kernel
@@ -975,8 +1020,7 @@ int launch_shard_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm,
     a.step_plus1 = step + 1;
     rc = launch_persistent(ctx, k, grid, s, a);
     if (rc != EGPU_OK) return rc;
-    ctx->lut_dirty = !lut;  // the lookup kernel leaves d_lut built from the table it committed
-    return EGPU_OK;
+    return table_changed(ctx, s, lut);  // the lookup kernel leaves d_lut built from the table it committed
 }
 
 // Packed-format scan: always a fully ordered launch (it serves the synchronous host path).
@@ -1001,8 +1045,7 @@ int launch_packed(egpu_ctx* ctx, const uint32_t* d_req, int64_t R, signed char* 
     ctx->seq += 1;
     new_group(ctx);
     ctx->prev_is_scan = false;  // the int32 scans do not pipeline behind this one
-    if (flags & kFlagCommit) ctx->lut_dirty = true;
-    return EGPU_OK;
+    return (flags & kFlagCommit) ? table_changed(ctx, s) : EGPU_OK;
 }
 
 // The release kernels (EGPU_F_RELEASE), per row format and D bucket: the register scans' CTA sizes and SnapSmem,
@@ -1059,8 +1102,7 @@ int launch_release(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int6
     ctx->seq += 1;
     new_group(ctx);
     ctx->prev_is_scan = false;
-    if (commit) ctx->lut_dirty = true;  // a refused launch leaves the table as it was: a rebuild is harmless
-    return EGPU_OK;
+    return commit ? table_changed(ctx, s) : EGPU_OK;  // a refused launch leaves the table as it was: a rebuild is harmless
 }
 
 // staging of the host-buffer entry points: three arrays of at least `rows` int32, doubling
@@ -1826,16 +1868,13 @@ int egpu_table_apply_peers_multi_dev(egpu_ctx* ctx, uint64_t first_step, int nst
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
-    if (commit) {
-        ctx->lut_dirty = true;
-        ctx->prev_is_scan = false;  // the next scan must see the new table
-    }
+    if (commit) ctx->prev_is_scan = false;  // the next scan must see the new table
     ApplyOuts outs;
     for (int k = 0; k < kApplyMax; ++k) outs.table_out[k] = (d_table_outs && k < nsteps) ? d_table_outs[k] : nullptr;
     apply_peers_kernel<<<commit ? 1 : nsteps, kMaxD, 0, s>>>(ctx->d_state, first_step + 1, nsteps, outs, commit);
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
-    return EGPU_OK;
+    return commit ? table_changed(ctx, s) : EGPU_OK;
 }
 
 int egpu_table_apply_peers_dev(egpu_ctx* ctx, uint64_t step, int32_t* d_table_out, int commit, void* stream) {
@@ -1916,12 +1955,11 @@ int egpu_table_apply_deltas_dev(egpu_ctx* ctx, const int64_t* d_deltas, int G, i
     const int rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
     ctx->prev_is_scan = false;
-    if (commit) ctx->lut_dirty = true;
     apply_deltas_kernel<<<1, kMaxD, 0, s>>>(ctx->d_state, reinterpret_cast<const long long*>(d_deltas), G,
                                             d_table_out, commit);
     EGPU_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
-    return EGPU_OK;
+    return commit ? table_changed(ctx, s) : EGPU_OK;
 }
 
 int egpu_synth_requests_dev(egpu_ctx* ctx, int dist, uint64_t seed, int64_t first_row, int64_t R,

@@ -56,6 +56,7 @@ struct egpu_ctx {
     int world = 1, rank = 0;
     bool attached = false;
     bool lut_dirty = true;            // table changed since the lookup tables were built
+    unsigned long long lut_capture = 0;  // the capture (capture_id) whose graph rebuilds them after its last table change
     int dev = -1;
     int sm_count = 132;  // H100 SXM; egpu_ctx_create reads the device's own count
     cudaStream_t stream = nullptr;
@@ -80,6 +81,7 @@ struct egpu_ctx {
     bool prev_is_scan = false;        // the last kernel this context launched was a snapshot scan ...
     bool prev_changes_table = false;  // ... and it may rewrite the table (commit)
     cudaStream_t prev_stream = nullptr;
+    unsigned long long prev_capture = 0;  // ... and the capture it was recorded in (capture_id), 0 = eager
     uint64_t seq = 0;                 // scans launched (epilogue slot = seq mod kEpiSlots)
     int group_len = 0;                // launches since (and including) the last fully ordered one
     int group_mbatches = 0;           // ... and the epi_multi slots (batches of multi-batch launches) they hold

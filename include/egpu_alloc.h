@@ -287,7 +287,16 @@ int  egpu_host_unregister(egpu_ctx* ctx, void* p);
 
 /* ---- snapshot mode, device buffers (bench / multi-GPU plumbing) -------- */
 
-/* Asynchronous on `stream` (a cudaStream_t passed as void*; NULL = the
+/* CUDA graphs (DESIGN.md 2.9): a _dev call captured into a graph changes nothing at capture time; it runs at
+ * every replay against the table the context holds then.  A captured call that may rewrite the table is followed
+ * inside the graph by a rebuild of the lookup tables (one more node than the eager call's launches), so eager calls
+ * after a replay read the table it left.  A captured lookup scan rebuilds them inside the graph only when they were
+ * stale at capture: after changing the table outside the graph (egpu_table_set, an eager commit), run one eager
+ * lookup scan before the next replay of such a graph.  EGPU_F_INPUTS_READY pipelines captured scans behind scans of
+ * the same capture only: never behind an eager launch, nor an eager one behind them.
+ * Calls that synchronise a stream (the host forms, the rounds with EGPU_F_ROUNDS alone) cannot be captured.
+ *
+ * Asynchronous on `stream` (a cudaStream_t passed as void*; NULL = the
  * context's own non-blocking stream — to name the legacy default stream pass
  * cudaStreamLegacy, not 0).  d_delta is int64[2*D]: core sums then mem sums; it
  * is overwritten, not accumulated.  d_table_out (may be NULL) receives

@@ -129,6 +129,43 @@ def restore(records, links, cap_core, cap_mem, verify: bool = True):
     return free_c, free_m, over, counts, rstat
 
 
+# ---- EGPU_RESTORE_CHARGE / EGPU_RESTORE_RELEASE: a few records applied to a live table -----------------
+BIG = 1 << 40
+
+
+class Refused(Exception):
+    """EGPU_RESTORE_RELEASE refused (EGPU_ERR_STATE); args[0] is the first offending device"""
+
+
+def usage(records, links, D, verify=True):
+    """(use_core[D], use_mem[D], counts[5], record_status) of the records, by the restore rule: what a
+    restore against an unbounded capacity takes away"""
+    fc, fm, _, counts, rstat = restore(records, links, [BIG] * D, [BIG] * D, verify=verify)
+    return [BIG - x for x in fc], [BIG - x for x in fm], counts, rstat
+
+
+def charge(table, records, links, verify=True):
+    """table = (free_core, free_mem, oversub): free' = max(free - U, 0), oversub' = oversub | (free - U < 0).
+    Returns (table', counts, record_status)."""
+    fc, fm, ov = table
+    uc, um, counts, rstat = usage(records, links, len(fc), verify)
+    c = [f - u for f, u in zip(fc, uc)]
+    m = [f - u for f, u in zip(fm, um)]
+    return ([max(x, 0) for x in c], [max(x, 0) for x in m],
+            [int(bool(o) or x < 0 or y < 0) for o, x, y in zip(ov, c, m)]), counts, rstat
+
+
+def release(table, records, links, cap_core, cap_mem, verify=True):
+    """free' = free + U, flags unchanged, all or nothing: raises Refused on the first touched device that is
+    oversubscribed or would exceed its capacity.  Returns (table', counts, record_status)."""
+    fc, fm, ov = table
+    uc, um, counts, rstat = usage(records, links, len(fc), verify)
+    for d in range(len(fc)):
+        if (uc[d] or um[d]) and (ov[d] or fc[d] + uc[d] > cap_core[d] or fm[d] + um[d] > cap_mem[d]):
+            raise Refused(d)
+    return ([f + u for f, u in zip(fc, uc)], [f + u for f, u in zip(fm, um)], list(ov)), counts, rstat
+
+
 def marshal_record(namespace: str, name: str, containers: dict):
     """(key, value) as the reference writes them: PodInfo.Key() / Val() (pkg/types/pod.go:51-58).
     containers: {container: (ids, resource_name) | None}.  json.Marshal sorts map keys, writes the

@@ -4,8 +4,8 @@ EGPU_RESTORE_RELEASE on egpu_table_restore[_flat] (include/egpu_restore.h, DESIG
 The property every test below comes back to: with T(A) the table a full restore of the record set A
 installs, CHARGE(B) on T(A) is exactly T(A + B), flags included, and RELEASE(B) for B a part of A is
 exactly T(A - B) whenever it is accepted; it is always accepted when no device B touches is
-oversubscribed.  The CPU restatement here is built on the restore oracle (oracle/restore_py.py): the
-usage U of a set is what a restore against an unbounded capacity takes away.
+oversubscribed.  The CPU restatement is built on the restore oracle (oracle/restore_py.py: usage, charge,
+release): the usage U of a set is what a restore against an unbounded capacity takes away.
 """
 import ctypes as C
 import os
@@ -15,44 +15,12 @@ import numpy as np
 import pytest
 
 from oracle import restore_py as R
+from oracle.restore_py import Refused, charge, release, usage
 from restore_util import persisted_state
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BIG = 1 << 40
 MEM_MAX = (1 << 18) - 1
 OTHER = "example.com/other-gpu"
-
-
-# ---- the restatement --------------------------------------------------------------------------------
-class Refused(Exception):
-    """RELEASE refused with EGPU_ERR_STATE"""
-
-
-def usage(records, links, D, verify=True):
-    """(use_core[D], use_mem[D], counts[5], record_status) of the records, by the restore rule"""
-    fc, fm, _, counts, rstat = R.restore(records, links, [BIG] * D, [BIG] * D, verify=verify)
-    return [BIG - x for x in fc], [BIG - x for x in fm], counts, rstat
-
-
-def charge(table, records, links, verify=True):
-    """free' = max(free - U, 0), oversub' = oversub | (free - U < 0)"""
-    fc, fm, ov = table
-    uc, um, counts, rstat = usage(records, links, len(fc), verify)
-    c = [f - u for f, u in zip(fc, uc)]
-    m = [f - u for f, u in zip(fm, um)]
-    return ([max(x, 0) for x in c], [max(x, 0) for x in m],
-            [int(bool(o) or x < 0 or y < 0) for o, x, y in zip(ov, c, m)]), counts, rstat
-
-
-def release(table, records, links, cap_core, cap_mem, verify=True):
-    """free' = free + U, all or nothing: refused on a touched device that is oversubscribed or would
-    exceed its capacity"""
-    fc, fm, ov = table
-    uc, um, counts, rstat = usage(records, links, len(fc), verify)
-    for d in range(len(fc)):
-        if (uc[d] or um[d]) and (ov[d] or fc[d] + uc[d] > cap_core[d] or fm[d] + um[d] > cap_mem[d]):
-            raise Refused(d)
-    return ([f + u for f, u in zip(fc, uc)], [f + u for f, u in zip(fm, um)], list(ov)), counts, rstat
 
 
 def full(records, links, cap_core, cap_mem, verify=True):
