@@ -7,8 +7,9 @@ directory name carries a hyphen; the sibling shim package maps it).
 """
 from . import synth  # noqa: F401
 from ._lib import (EgpuError, LIB_PATH, VARIANT_AUTO, VARIANT_GRID, VARIANT_SORTED, VARIANT_LUT,  # noqa: F401
-                   EV_ALLOC, EV_FREE, load, strerror)
+                   EV_ALLOC, EV_FREE, EV_RELEASE, load, strerror)
 from .alloc import BestFitAllocator  # noqa: F401
 
 __all__ = ["BestFitAllocator", "EgpuError", "synth", "load", "strerror", "LIB_PATH",
-           "VARIANT_AUTO", "VARIANT_GRID", "VARIANT_SORTED", "VARIANT_LUT", "EV_ALLOC", "EV_FREE"]
+           "VARIANT_AUTO", "VARIANT_GRID", "VARIANT_SORTED", "VARIANT_LUT", "EV_ALLOC", "EV_FREE",
+           "EV_RELEASE"]

@@ -45,6 +45,7 @@ IDX_DEFERRED = -2
 
 EV_ALLOC = 0
 EV_FREE = 1
+EV_RELEASE = 3
 
 
 MAX_BATCHES = 64

@@ -558,6 +558,9 @@ class BestFitAllocator:
 
     # -- sequential mode ------------------------------------------------------
     def replay(self, kind, a, b):
+        """egpu_replay: events in order against the current table; returns out_idx int32[E].  A release event
+        (EV_RELEASE) carries the device in `a` and pack_requests(core, mem) in `b` (uint32 words are read as
+        int32); it gives back a placement made before this call, or comes back -1 and changes nothing."""
         k, a_, b_ = _i32(kind), _i32(a), _i32(b)
         if not (k.shape == a_.shape == b_.shape) or k.ndim != 1:
             raise L.EgpuError(L.ERR_INVALID, "replay")

@@ -2013,13 +2013,18 @@ int egpu_replay(egpu_ctx* ctx, const int32_t* kind, const int32_t* a, const int3
     ctx->prev_is_scan = false;
     ctx->lut_dirty = true;
     if (ctx->D <= 32 && E <= kReplaySmemEvents && ctx->replay_variant == 2) {
-        // two warps: decode off the chain, lane = device on it (default wherever it applies)
+        // two warps: decode off the chain, lane = device on it (default wherever it applies); the release path
+        // only for streams that hold a release event
         const size_t smem2 = static_cast<size_t>((E + 15) & ~15ll);
         if (!ctx->replay2_configured) {
-            EGPU_CUDA(ctx, cudaFuncSetAttribute(replay2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kReplaySmemEvents));
+            EGPU_CUDA(ctx, cudaFuncSetAttribute(replay2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kReplaySmemEvents));
+            EGPU_CUDA(ctx, cudaFuncSetAttribute(replay2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kReplaySmemEvents));
             ctx->replay2_configured = true;
         }
-        replay2_kernel<<<1, 64, smem2, s>>>(ctx->d_state, d_kind, d_a, d_b, E, d_out);
+        if (std::find(kind, kind + E, EGPU_EV_RELEASE) != kind + E)
+            replay2_kernel<true><<<1, 64, smem2, s>>>(ctx->d_state, d_kind, d_a, d_b, E, d_out);
+        else
+            replay2_kernel<false><<<1, 64, smem2, s>>>(ctx->d_state, d_kind, d_a, d_b, E, d_out);
     } else if (ctx->D <= 8 && !ctx->replay_general)
         replay8_kernel<<<1, 32, smem, s>>>(ctx->d_state, d_kind, d_a, d_b, E, d_out, d_live);
     else

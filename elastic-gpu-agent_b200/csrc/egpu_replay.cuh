@@ -58,7 +58,14 @@ __global__ void synth_requests_kernel(int dist, unsigned long long seed, long lo
 // with CREDUX.MIN (__reduce_min_sync).  `live` (device currently held by each
 // ALLOC event, -1 otherwise) sits in shared memory when it fits, else in HBM;
 // only lane 0 touches it, so program order gives consistency.
+//
+// RELEASE(d, word) (DESIGN.md §2.6) gives back a placement made before the call.  Its bound is the device's
+// "room": the domain bound minus the table minus what this call's live ALLOCs hold, i.e. the room the device had
+// when the call started less the releases accepted since.  ALLOC and FREE move capacity between the table and
+// the live ALLOCs and leave the room as it is, so only a RELEASE changes it, and a later FREE can never push
+// the table past the domain.  The oversubscription flags are read once: replay never changes them.
 constexpr int kReplaySmemEvents = 200 * 1024;
+constexpr uint32_t kReleaseWordEnd = 101u << 18;  // packed words below this hold a request in the domain
 
 __global__ void __launch_bounds__(32)
 replay_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, const int32_t* __restrict__ ev_a,
@@ -73,6 +80,8 @@ replay_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, const
     int32_t fm0 = d0 < D ? st->free_mem[d0] : -1;
     int32_t fc1 = d1 < D ? st->free_core[d1] : -1;
     int32_t fm1 = d1 < D ? st->free_mem[d1] : -1;
+    int32_t rc0 = kCoreMax - fc0, rm0 = kMemMax - fm0, rc1 = kCoreMax - fc1, rm1 = kMemMax - fm1;  // room
+    const bool ov0 = d0 < D && st->oversub[d0] != 0, ov1 = d1 < D && st->oversub[d1] != 0;
 
     for (long long base = 0; base < E; base += 32) {
         const long long i = base + lane;
@@ -109,6 +118,21 @@ replay_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, const
                     if (res == d1) { fc1 -= aj; fm1 -= bj; }
                 }
                 if (lane == 0) live[base + j] = static_cast<signed char>(res);
+            } else if (kj == 3) {  // RELEASE: device aj, packed request bj; the lane that holds aj decides
+                // (its `live` entry is never read: a FREE only reads the entries of ALLOC events)
+                const bool ok = static_cast<uint32_t>(aj) < static_cast<uint32_t>(D) &&
+                                static_cast<uint32_t>(bj) < kReleaseWordEnd;
+                const int32_t c = bj >> 18, m = bj & kMemMax;
+                bool hit = false;
+                if (ok && aj == d0 && (bj == 0 || !ov0) && c <= rc0 && m <= rm0) {
+                    fc0 += c; fm0 += m; rc0 -= c; rm0 -= m;
+                    hit = true;
+                }
+                if (ok && aj == d1 && (bj == 0 || !ov1) && c <= rc1 && m <= rm1) {
+                    fc1 += c; fm1 += m; rc1 -= c; rm1 -= m;
+                    hit = true;
+                }
+                res = __ballot_sync(0xffffffffu, hit) ? aj : -1;
             } else {
                 const bool tv = __shfl_sync(0xffffffffu, static_cast<int>(tvalid), j) != 0;
                 const int32_t taj = __shfl_sync(0xffffffffu, ta, j);
@@ -154,11 +178,18 @@ replay8_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, cons
     signed char* live = (E <= kReplaySmemEvents) ? reinterpret_cast<signed char*>(smem_raw) : live_global;
     const int lane = threadIdx.x;
     const int D = st->D;
-    uint32_t K[8];
+    uint32_t K[8], room[8];  // room: packed like K (guards, room in core and mem), without the device
+    uint32_t ov_mask = 0;
 #pragma unroll
-    for (int d = 0; d < 8; ++d)
-        K[d] = d < D ? (pack_table_word(st->free_core[d], st->free_mem[d]) | static_cast<uint32_t>(d)) : kPadWord;
+    for (int d = 0; d < 8; ++d) {
+        const int32_t fc = d < D ? st->free_core[d] : 0, fm = d < D ? st->free_mem[d] : 0;
+        K[d] = d < D ? (pack_table_word(fc, fm) | static_cast<uint32_t>(d)) : kPadWord;
+        room[d] = pack_table_word(kCoreMax - fc, kMemMax - fm);
+        ov_mask |= (d < D && st->oversub[d] != 0) ? 1u << d : 0u;
+    }
 
+    // t: a FREE's target (an earlier ALLOC) with qt its request word; a RELEASE's device with q its request word,
+    // -1 when the release holds nothing or sits on a flagged device.  Otherwise -1.
     auto fetch = [&](long long i, int32_t& k, uint32_t& q, uint32_t& qt, int32_t& t) {
         k = -1; q = 0; qt = 0; t = -1;
         if (i < E) {
@@ -168,6 +199,10 @@ replay8_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, cons
             if (k == 1 && a >= 0 && a < i && kind[a] == 0) {  // FREE of an earlier ALLOC: fetch its request now
                 t = a;
                 qt = pack_request_word(ev_a[a], ev_b[a]);
+            } else if (k == 3 && static_cast<uint32_t>(a) < static_cast<uint32_t>(D) &&
+                       static_cast<uint32_t>(b) < kReleaseWordEnd && (b == 0 || !((ov_mask >> a) & 1u))) {
+                t = a;
+                q = pack_request_word(b >> 18, b & kMemMax);
             }
         }
     };
@@ -201,6 +236,16 @@ replay8_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, cons
                     for (int d = 0; d < 8; ++d) K[d] = (w[d] == best) ? w[d] : K[d];
                 }
                 if (lane == 0) live[base + j] = static_cast<signed char>(res);
+            } else if (kj == 3) {  // RELEASE: accepted iff the request fits the device's room
+                const int32_t dev = __shfl_sync(0xffffffffu, ct, j);
+#pragma unroll
+                for (int d = 0; d < 8; ++d) {
+                    const uint32_t w = room[d] - q;
+                    const bool hit = d == dev && (w & kGuards) == kGuards;
+                    K[d] = hit ? K[d] + q : K[d];
+                    room[d] = hit ? w : room[d];
+                    res = hit ? d : res;
+                }
             } else {
                 const int32_t t = __shfl_sync(0xffffffffu, ct, j);
                 const uint32_t qt = __shfl_sync(0xffffffffu, cqt, j);
@@ -248,11 +293,18 @@ replay8_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, cons
 // device a FREE releases reaches the other lanes through one shuffle.  (All lanes keeping `live` redundantly -
 // same address, same value - saved that shuffle, 40 against 48 ns per event, but is a formal shared-memory race
 // that racecheck reports; warp barriers around a single writer: 80 ns; `if (lane == 0)` as a branch: 87 ns.)
+// kRelease: the stream holds RELEASE events (the host looks before the launch).  Warp 1 decodes them (domain,
+// device, flag) as well; warp 0 tests the request word against the room word of the device's lane, which is the
+// ALLOC test on another word, and adds it back as a FREE does.  Without them the kernel is the chain above, unchanged:
+// the release path costs every event about ten instructions and a VOTE, 6.5 -> 7.7 ms on cfg5.
 constexpr int kReplayChunk = 256;
 struct ReplayRing {
-    uint4 ev[2][kReplayChunk];   // x = request word (ALLOC: its own; FREE: its target's), y = FREE target event or -1, z = kind
+    // x = request word (ALLOC, RELEASE: its own; FREE: its target's), y = FREE target event or -1, z = kind,
+    // w = RELEASE device or -1
+    uint4 ev[2][kReplayChunk];
     int32_t res[2][kReplayChunk];
 };
+template <bool kRelease>
 __global__ void __launch_bounds__(64)
 replay2_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, const int32_t* __restrict__ ev_a,
                const int32_t* __restrict__ ev_b, long long E, int32_t* __restrict__ out_idx) {
@@ -263,14 +315,17 @@ replay2_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, cons
     const uint32_t live_base = static_cast<uint32_t>(__cvta_generic_to_shared(smem_raw));  // `live`: int8 per event
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int D = st->D;
-    uint32_t K = lane < D ? (pack_table_word(st->free_core[lane], st->free_mem[lane]) | static_cast<uint32_t>(lane)) : kPadWord;
+    const int32_t fc = lane < D ? st->free_core[lane] : 0, fm = lane < D ? st->free_mem[lane] : 0;
+    uint32_t K = lane < D ? (pack_table_word(fc, fm) | static_cast<uint32_t>(lane)) : kPadWord;
+    uint32_t room = pack_table_word(kCoreMax - fc, kMemMax - fm);
+    const uint32_t ov_mask = kRelease ? __ballot_sync(0xffffffffu, lane < D && st->oversub[lane] != 0) : 0u;
     const long long n_chunks = (E + kReplayChunk - 1) / kReplayChunk;
 
     auto decode = [&](long long c) {  // warp 1
         const long long base = c * kReplayChunk;
         for (int j = lane; j < kReplayChunk; j += 32) {
             const long long i = base + j;
-            uint4 e = make_uint4(0u, 0xFFFFFFFFu, 2u, 0u);  // past the end: a no-op kind
+            uint4 e = make_uint4(0u, 0xFFFFFFFFu, 2u, 0xFFFFFFFFu);  // past the end: a no-op kind
             if (i < E) {
                 const int32_t k = kind[i], a = ev_a[i], b = ev_b[i];
                 e.z = static_cast<uint32_t>(k);
@@ -279,6 +334,10 @@ replay2_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, cons
                 } else if (k == 1 && a >= 0 && a < i && kind[a] == 0) {  // FREE of an earlier ALLOC
                     e.y = static_cast<uint32_t>(a);
                     e.x = pack_request_word(ev_a[a], ev_b[a]);
+                } else if (kRelease && k == 3 && static_cast<uint32_t>(a) < static_cast<uint32_t>(D) &&
+                           static_cast<uint32_t>(b) < kReleaseWordEnd && (b == 0 || !((ov_mask >> a) & 1u))) {
+                    e.w = static_cast<uint32_t>(a);  // RELEASE of a request in the domain, on an unflagged device
+                    e.x = pack_request_word(b >> 18, b & kMemMax);
                 }
             }
             ring.ev[c & 1][j] = e;
@@ -306,7 +365,7 @@ replay2_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, cons
                 const uint4 e = nxt;
                 nxt = evs[(j + 1) & (kReplayChunk - 1)];  // one event ahead: its read latency is off the chain
                 // Branch-free: one warp alone pays a pipeline refill for every taken branch, which cost more
-                // than the work it skipped.  Both kinds are computed, the event's kind selects.
+                // than the work it skipped.  Every kind's update is computed, the event's kind selects.
                 const bool is_alloc = e.z == 0u;
                 const int32_t t = static_cast<int32_t>(e.y);            // FREE target (an earlier ALLOC) or -1
                 // `live` belongs to lane 0 alone (reads and writes in its program order: nothing to race with);
@@ -324,9 +383,21 @@ replay2_kernel(DevState* __restrict__ st, const int32_t* __restrict__ kind, cons
                 const uint32_t best = __reduce_min_sync(0xffffffffu, key);
                 const int32_t a_res = best == 0xFFFFFFFFu ? -1 : static_cast<int32_t>(best & 31u);
                 const int32_t tdev = t >= 0 ? tdev_raw : -1;
-                const int32_t res = is_alloc ? a_res : tdev;
+                int32_t res;
+                bool add = lane == tdev;  // FREE: this lane takes its target's request back
+                if constexpr (kRelease) {
+                    // RELEASE: the device's lane takes the word back iff it fits its room (-1 on every other event)
+                    const uint32_t w_room = room - e.x;
+                    const bool rel = lane == static_cast<int32_t>(e.w) && (~w_room & kGuards) == 0u;
+                    room = rel ? w_room : room;
+                    const int32_t rel_res = __ballot_sync(0xffffffffu, rel) != 0u ? static_cast<int32_t>(e.w) : -1;
+                    res = is_alloc ? a_res : max(tdev, rel_res);
+                    add = add || rel;
+                } else {
+                    res = is_alloc ? a_res : tdev;
+                }
                 const uint32_t k_alloc = (w == best) ? w : K;
-                const uint32_t k_free = (lane == tdev) ? K + e.x : K;
+                const uint32_t k_free = add ? K + e.x : K;
                 K = is_alloc ? k_alloc : k_free;
                 {
                     const int32_t mine = is_alloc ? a_res : -1;

@@ -87,8 +87,9 @@ extern "C" {
 #define EGPU_ERR_UNSAT       (-8)   /* preferred allocation cannot be satisfied */
 
 /* event kinds for egpu_replay */
-#define EGPU_EV_ALLOC 0
-#define EGPU_EV_FREE  1
+#define EGPU_EV_ALLOC   0
+#define EGPU_EV_FREE    1
+#define EGPU_EV_RELEASE 3   /* gives back a placement made before the call; 2 stays a no-op */
 
 /* flags of egpu_bestfit_batch_dev */
 #define EGPU_F_COMMIT        1   /* table' replaces the current table */
@@ -676,7 +677,20 @@ int egpu_synth_requests_dev(egpu_ctx* ctx, int dist, uint64_t seed,
  * kind[i] = EGPU_EV_FREE : a[i] = index of the ALLOC event to release
  *                          -> out_idx[i] = device released, or -1 when that
  *                          event is not a live allocation (not an ALLOC, not
- *                          earlier than i, infeasible, or already freed). */
+ *                          earlier than i, infeasible, or already freed).
+ * kind[i] = EGPU_EV_RELEASE: a[i] = device, b[i] = EGPU_PACK_REQUEST(core, mem) read as int32: gives back a
+ *                          placement made before this call (an earlier call's ALLOC, a batch row, a restored
+ *                          record), with no ledger in the library: the caller keeps (device, request).
+ *                          -> out_idx[i] = a[i] when accepted, else -1 and nothing changes.  Accepted iff,
+ *                          on the table as events 0..i-1 left it: 0 <= a[i] < D; 0 <= b[i] < 2^25 with
+ *                          core <= EGPU_CORE_MAX; the device's oversubscription flag is clear unless the
+ *                          request is (0, 0) (EGPU_REL_FLAGGED); and free + live + request stays within
+ *                          EGPU_CORE_MAX and EGPU_MEM_MAX on the device (EGPU_REL_EXCEEDS), where live is
+ *                          what this call's ALLOC events still hold there: its FREE events may give that
+ *                          back later.  The decision is per event: a release that EGPU_F_RELEASE refuses as
+ *                          a batch can be a stream whose first events are accepted.  The flags never change.
+ * Every other kind is a no-op with out_idx[i] = -1, and so is an EGPU_EV_FREE whose target is not an
+ * EGPU_EV_ALLOC.  EGPU_EV_RELEASE is a newly accepted input: egpu_abi_version() stays 1011. */
 int egpu_replay(egpu_ctx* ctx, const int32_t* kind, const int32_t* a,
                 const int32_t* b, int64_t E, int32_t* out_idx);
 
