@@ -178,6 +178,31 @@ __device__ __forceinline__ uint32_t pack_request_word(int32_t core, int32_t mem)
     return (c << 24) + (m << 5);
 }
 
+// First feasible sorted position; kNoCand (DT <= 32) or DT (DT = 64) when there is none.
+// Per (request, row) pair: one subtract (IMAD.IADD or IADD3, ptxas balances the FMA and
+// ALU pipes), one 3-input LOP3 ((t ^ G) & M, both masks in registers), half a VIMNMX3.
+template <int N>
+__device__ __forceinline__ uint32_t first_feasible32(const uint32_t* K, uint32_t q, uint32_t gx, uint32_t gm) {
+    uint32_t best = kNoCand;
+#pragma unroll
+    for (int j = 0; j < N; j += 2) {
+        const uint32_t c0 = ((K[j] - q) ^ gx) & gm;
+        const uint32_t c1 = ((K[j + 1] - q) ^ gx) & gm;
+        best = __vimin3_u32(best, c0, c1);
+    }
+    return best;  // 0..N-1, or >= 32
+}
+template <int DT>
+__device__ __forceinline__ uint32_t first_feasible(const uint32_t (&K)[DT], uint32_t q, uint32_t gx, uint32_t gm) {
+    if constexpr (DT <= 32) {
+        return first_feasible32<DT>(K, q, gx, gm);  // 0..DT-1, or kNoCand (= 32): the tile maps both ranges
+    } else {  // positions are stored mod 32: two halves
+        const uint32_t lo = first_feasible32<32>(K, q, gx, gm);
+        const uint32_t hi = first_feasible32<DT - 32>(K + 32, q, gx, gm);
+        return lo < 32u ? lo : (hi < 32u ? 32u + hi : static_cast<uint32_t>(DT));
+    }
+}
+
 // streaming 128-bit accesses: read-once / write-once data stays out of L1
 __device__ __forceinline__ int4 ld_stream_v4(const int32_t* p) {
     int4 r;

@@ -1,0 +1,118 @@
+"""Best fit of many pending requests against many capacity tables in one launch: the PyTorch operator
+`egpu::bestfit_tables` (DESIGN.md §2.10).
+
+A scheduler scores every pending pod against every node's device table; this does all N x P pairs in
+one CUDA launch on the current stream instead of N `egpu_bestfit_query` calls.  The kernel lives in
+csrc/egpu_tables.cu and is built by __graft_entry__.build() as lib/libegpu_tables.so; it is separate
+from libegpu_alloc.so and its C ABI, reads no context and writes no table.  Importing this module does
+not load the library; the first call (or `load()`) does, and a missing library raises: there is no
+fallback.
+"""
+from __future__ import annotations
+
+import os
+
+import torch
+
+_HERE = os.path.dirname(os.path.abspath(__file__))
+LIB_PATH = os.path.join(_HERE, "lib", "libegpu_tables.so")
+
+MAX_DEVICES = 64
+CORE_MAX = 100
+MEM_MAX = (1 << 18) - 1
+NO_KEY = 0x7FFFFFFF  # key of a pair with no feasible device
+
+_loaded = False
+
+
+def load() -> None:
+    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables) and the operator's fake implementation."""
+    global _loaded
+    if _loaded:
+        return
+    if not os.path.exists(LIB_PATH):
+        raise ImportError(
+            f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.")
+    torch.ops.load_library(LIB_PATH)
+    torch.library.register_fake("egpu::bestfit_tables")(_fake)
+    _loaded = True
+
+
+def check_args(free_core, free_mem, d_valid, req_core, req_mem) -> None:
+    """The operator's checks on dtypes, contiguity, shapes and device (no data is read), in the operator's order:
+    RuntimeError for a dtype, layout or device, ValueError for a shape."""
+    names = ("free_core", "free_mem", "d_valid", "req_core", "req_mem")
+    ts = (free_core, free_mem, d_valid, req_core, req_mem)
+    for name, t in zip(names, ts):
+        if t.dtype != torch.int32:
+            raise RuntimeError(f"bestfit_tables: {name} must be int32, got {t.dtype}")
+        if not t.is_contiguous():
+            raise RuntimeError(f"bestfit_tables: {name} must be contiguous")
+    if free_core.dim() != 2 or free_mem.shape != free_core.shape:
+        raise ValueError(f"bestfit_tables: free_core and free_mem must both be [N, D], got {tuple(free_core.shape)} "
+                         f"and {tuple(free_mem.shape)}")
+    N, D = free_core.shape
+    if not 1 <= D <= MAX_DEVICES:
+        raise ValueError(f"bestfit_tables: D must be in [1, 64], got {D}")
+    if d_valid.dim() != 1 or d_valid.shape[0] != N:
+        raise ValueError(f"bestfit_tables: d_valid must be [N] = [{N}], got {tuple(d_valid.shape)}")
+    if req_core.dim() != 1 or req_mem.shape != req_core.shape:
+        raise ValueError(f"bestfit_tables: req_core and req_mem must both be [P], got {tuple(req_core.shape)} "
+                         f"and {tuple(req_mem.shape)}")
+    if N >= 2**31 or req_core.shape[0] >= 2**31:
+        raise ValueError(f"bestfit_tables: N and P must be below 2^31, got {N} and {req_core.shape[0]}")
+    dev = free_core.device
+    for t in ts:
+        if t.device.type != "cuda" or t.device != dev:
+            raise RuntimeError(f"bestfit_tables: every tensor must be on one CUDA device, got {t.device} and {dev}")
+
+
+def check_tables(free_core, free_mem, d_valid) -> None:
+    """ValueError unless every table is in §2.1's domain: 1 <= d_valid[n] <= D, and the first d_valid[n] devices of
+    table n have free_core in [0, 100] and free_mem in [0, 2^18 - 1].  Reads the data: one host round trip."""
+    D = free_core.shape[1]
+    dv = d_valid.to(torch.int64)
+    live = torch.arange(D, device=free_core.device)[None, :] < dv[:, None]
+    out = (free_core < 0) | (free_core > CORE_MAX) | (free_mem < 0) | (free_mem > MEM_MAX)
+    bad_dv = int(((dv < 1) | (dv > D)).sum())
+    bad_rows = int((live & out).any(dim=1).sum())
+    if bad_dv:
+        raise ValueError(f"bestfit_tables: {bad_dv} table(s) with d_valid outside [1, {D}]")
+    if bad_rows:
+        raise ValueError(f"bestfit_tables: {bad_rows} table(s) outside the domain (free_core in [0, 100], "
+                         f"free_mem in [0, 2^18 - 1] on the first d_valid devices)")
+
+
+def _fake(free_core, free_mem, d_valid, req_core, req_mem):
+    check_args(free_core, free_mem, d_valid, req_core, req_mem)
+    N, P = free_core.shape[0], req_core.shape[0]
+    return (free_core.new_empty((N, P), dtype=torch.int8), free_core.new_empty((N, P), dtype=torch.int32))
+
+
+def bestfit_tables(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.Tensor,
+                   req_core: torch.Tensor, req_mem: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Score P requests against N capacity tables in one launch (DESIGN.md §2.10).
+
+    free_core, free_mem: int32[N, D], 1 <= D <= 64; table n holds its first d_valid[n] devices (int32[N],
+    1 <= d_valid[n] <= D), each with free_core in [0, 100] (percent) and free_mem in [0, 2^18 - 1] (MiB).
+    req_core, req_mem: int32[P].  All contiguous, on one CUDA device.
+
+    Returns (idx int8[N, P], key int32[N, P]).  idx[n, p] is the device egpu_bestfit_query would choose for
+    request p against table n alone: the feasible device (core <= free_core, mem <= free_mem, both >= 0) with
+    the smallest (free_core - core, free_mem - mem, d), or -1.  key[n, p] is that order packed as
+    (lc << 24) | (lm << 6) | d, the leftovers of the chosen device, so nodes can be ranked by it directly;
+    it is 0x7fffffff when idx is -1.  A request outside the domain (negative, core > 100, mem >= 2^18) is
+    -1 everywhere.  N = 0 or P = 0 gives empty outputs.
+
+    Stateless: no context is read and no table written; no demand sums.  Asynchronous on the current stream.
+    Shapes, dtypes, layout and device are checked before any launch (ValueError for a shape, RuntimeError
+    otherwise).  Eagerly, this function also checks the tables' domain and d_valid (ValueError), which
+    reads them back; during CUDA-graph capture or torch.compile tracing it cannot, and the operator
+    answers -1 (key 0x7fffffff) for every request against a table outside the domain.
+    """
+    load()
+    check_args(free_core, free_mem, d_valid, req_core, req_mem)
+    if not torch.compiler.is_compiling() and not torch.cuda.is_current_stream_capturing():
+        check_tables(free_core, free_mem, d_valid)
+    return torch.ops.egpu.bestfit_tables(free_core, free_mem, d_valid, req_core, req_mem)
