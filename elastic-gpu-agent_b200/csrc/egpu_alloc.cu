@@ -15,7 +15,6 @@
 #include <cstdlib>
 #include <algorithm>
 #include <cstring>
-#include <initializer_list>
 #include <mutex>
 #include <new>
 #include <vector>
@@ -38,129 +37,82 @@ constexpr int64_t kMaxRows = (1ll << 31) - 1;  // EGPU_MAX_ROWS
 
 int d_bucket(int D) { return D <= 8 ? 0 : D <= 16 ? 1 : D <= 32 ? 2 : 3; }
 
-// ---- kernel table: one kernel per scan family and D bucket ----
+RowFormat row_format(int flags) { return (flags & EGPU_F_PACKED) ? kRowsPacked : kRowsInt32; }
+
+// ---- kernel tables: one kernel per family, row format and D bucket ----
 template <class Fn>
 struct Kernel {
     Fn fn;
     int threads;
     size_t smem;  // dynamic shared memory
+    int slot;     // its entry in egpu_ctx::ctas_per_sm
 };
 template <class Fn>
-constexpr Kernel<Fn> kernel(Fn fn, int threads, size_t smem) { return {fn, threads, smem}; }
+constexpr Kernel<Fn> kernel(Fn fn, int threads, size_t smem) { return {fn, threads, smem, 0}; }
 
-// The register scans run 256 threads up to D = 32 and 128 at D = 64; the lookup scan is one
-// kernel for every D.
-template <int F, int B>
+// Kernel of family F for rows in format FMT in bucket B.  The register scans run 256 threads up to D = 32 and 128 at
+// D = 64; the lookup scan is one kernel for every D.  Packed rows run in the packed twin of a scan (P ? twin : int32
+// kernel): same CTA size, shared memory and kernel type.  The grid scan reads int32 rows only, the warp-chunk scan
+// (kScanPacked) packed words only.  The one-launch kernels run kRoundsThreads per CTA in every bucket, with the register
+// scan's SnapSmem or the lookup scan's LutSmem of that CTA size.  The release kernels reuse the register scans' CTA sizes
+// and lane-private accumulators at every D (DESIGN.md 4.1h); the sharded one's last CTA exchanges the sums with the
+// peers before it decides.
+template <int F, RowFormat FMT, int B>
 constexpr auto family_kernel() {
-    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
+    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256, RT = kRoundsThreads;
     constexpr size_t snap = sizeof(SnapSmem<DT, T>), lut = sizeof(LutSmem<256>);
-    if constexpr (F == kScanSorted) return kernel(bestfit_sorted_kernel<DT, T, false>, T, snap);
-    else if constexpr (F == kScanSortedContig) return kernel(bestfit_sorted_kernel<DT, T, true>, T, snap);
+    constexpr size_t rsnap = sizeof(SnapSmem<DT, RT>), rlut = sizeof(LutSmem<RT>);
+    constexpr bool P = FMT == kRowsPacked;
+    static_assert(F != kScanGrid || !P, "the grid scan has no packed form");
+    static_assert(F != kScanPacked || P, "the warp-chunk scan reads packed words");
+    if constexpr (F == kScanSorted) return kernel(P ? bestfit_sorted_packed_snap_kernel<DT, T> : bestfit_sorted_kernel<DT, T, false>, T, snap);
+    else if constexpr (F == kScanSortedContig) return kernel(P ? bestfit_sorted_packed_contig_kernel<DT, T> : bestfit_sorted_kernel<DT, T, true>, T, snap);
     else if constexpr (F == kScanGrid) return kernel(bestfit_grid_kernel<DT, T>, T, snap);
-    else if constexpr (F == kScanLut) return kernel(bestfit_lut_kernel<256, false>, 256, lut);
-    else if constexpr (F == kScanLutContig) return kernel(bestfit_lut_kernel<256, true>, 256, lut);
-    else if constexpr (F == kScanSortedMulti) return kernel(bestfit_sorted_multi_kernel<DT, T>, T, snap);
-    else if constexpr (F == kScanLutMulti) return kernel(bestfit_lut_multi_kernel<256>, 256, lut);
-    else return kernel(bestfit_sorted_packed_kernel<DT, T>, T, snap);
+    else if constexpr (F == kScanLut) return kernel(P ? bestfit_lut_packed_snap_kernel<256> : bestfit_lut_kernel<256, false>, 256, lut);
+    else if constexpr (F == kScanLutContig) return kernel(P ? bestfit_lut_packed_contig_kernel<256> : bestfit_lut_kernel<256, true>, 256, lut);
+    else if constexpr (F == kScanSortedMulti) return kernel(P ? bestfit_sorted_packed_multi_kernel<DT, T> : bestfit_sorted_multi_kernel<DT, T>, T, snap);
+    else if constexpr (F == kScanLutMulti) return kernel(P ? bestfit_lut_packed_multi_kernel<256> : bestfit_lut_multi_kernel<256>, 256, lut);
+    else if constexpr (F == kScanPacked) return kernel(bestfit_sorted_packed_kernel<DT, T>, T, snap);
+    else if constexpr (F == kRoundsSorted) return kernel(rounds_sorted_kernel<DT, FMT>, RT, rsnap);
+    else if constexpr (F == kRoundsLut) return kernel(rounds_lut_kernel<FMT>, RT, rlut);
+    else if constexpr (F == kRoundsMultiSorted) return kernel(rounds_sorted_multi_kernel<DT, FMT>, RT, rsnap);
+    else if constexpr (F == kRoundsMultiLut) return kernel(rounds_lut_multi_kernel<FMT>, RT, rlut);
+    else if constexpr (F == kShardPrefixSorted) return kernel(shard_prefix_multi_sorted_kernel<DT, FMT>, RT, rsnap);
+    else if constexpr (F == kShardPrefixLut) return kernel(shard_prefix_multi_lut_kernel<FMT>, RT, rlut);
+    else if constexpr (F == kShardRoundsSorted) return kernel(shard_rounds_sorted_kernel<DT, FMT>, RT, rsnap);
+    else if constexpr (F == kShardRoundsLut) return kernel(shard_rounds_lut_kernel<FMT>, RT, rlut);
+    else if constexpr (F == kRelease) return kernel(release_rows_kernel<DT, T, FMT, false>, T, snap);
+    else {
+        static_assert(F == kReleaseShard, "a family without kernels");
+        return kernel(release_rows_kernel<DT, T, FMT, true>, T, snap);
+    }
 }
-template <int F>
-constexpr decltype(family_kernel<F, 0>()) kKernels[4] = {family_kernel<F, 0>(), family_kernel<F, 1>(), family_kernel<F, 2>(),
-                                                         family_kernel<F, 3>()};
-
-// The packed multi-batch kernels: the same CTA sizes and shared memory as the int32 multi-batch
-// kernels of their bucket, and the same kernel types, so a launcher takes either table.
-template <int P, int B>
-constexpr auto packed_kernel() {
-    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
-    if constexpr (P == kPackedSortedMulti) return kernel(bestfit_sorted_packed_multi_kernel<DT, T>, T, sizeof(SnapSmem<DT, T>));
-    else return kernel(bestfit_lut_packed_multi_kernel<256>, 256, sizeof(LutSmem<256>));
-}
-template <int P>
-constexpr decltype(packed_kernel<P, 0>()) kPackedKernels[4] = {packed_kernel<P, 0>(), packed_kernel<P, 1>(), packed_kernel<P, 2>(),
-                                                               packed_kernel<P, 3>()};
-
-// The packed prefix-commit scans: twins of the CONTIG kernels of their bucket, same CTA sizes,
-// shared memory and kernel types.
-template <int P, int B>
-constexpr auto packed_contig_kernel() {
-    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
-    if constexpr (P == kPackedSortedContig) return kernel(bestfit_sorted_packed_contig_kernel<DT, T>, T, sizeof(SnapSmem<DT, T>));
-    else return kernel(bestfit_lut_packed_contig_kernel<256>, 256, sizeof(LutSmem<256>));
-}
-template <int P>
-constexpr decltype(packed_contig_kernel<P, 0>()) kPackedContigKernels[4] = {packed_contig_kernel<P, 0>(), packed_contig_kernel<P, 1>(),
-                                                                            packed_contig_kernel<P, 2>(), packed_contig_kernel<P, 3>()};
-
-// The packed sharded scans: twins of the round-robin single-batch kernels of their bucket, same CTA
-// sizes, shared memory and kernel types.
-template <int P, int B>
-constexpr auto packed_snap_kernel() {
-    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
-    if constexpr (P == kPackedSortedSnap) return kernel(bestfit_sorted_packed_snap_kernel<DT, T>, T, sizeof(SnapSmem<DT, T>));
-    else return kernel(bestfit_lut_packed_snap_kernel<256>, 256, sizeof(LutSmem<256>));
-}
-template <int P>
-constexpr decltype(packed_snap_kernel<P, 0>()) kPackedSnapKernels[4] = {packed_snap_kernel<P, 0>(), packed_snap_kernel<P, 1>(),
-                                                                        packed_snap_kernel<P, 2>(), packed_snap_kernel<P, 3>()};
-
-// The one-launch rounds kernels (EGPU_F_DEVICE_ROUNDS): kRoundsThreads per CTA in every bucket, the
-// register scan's SnapSmem or the lookup scan's LutSmem of that CTA size, one kernel type for all.
 template <int F, RowFormat FMT, int B>
-constexpr auto rounds_kernel() {
-    constexpr int DT = 8 << B;
-    if constexpr (F == kRoundsSorted)
-        return kernel(rounds_sorted_kernel<DT, FMT>, kRoundsThreads, sizeof(SnapSmem<DT, kRoundsThreads>));
-    else return kernel(rounds_lut_kernel<FMT>, kRoundsThreads, sizeof(LutSmem<kRoundsThreads>));
+constexpr auto table_entry() {
+    auto k = family_kernel<F, FMT, B>();
+    k.slot = (F * 2 + FMT) * 4 + B;
+    return k;
 }
+// The table of family F in format FMT, one kernel per D bucket
 template <int F, RowFormat FMT>
-constexpr decltype(rounds_kernel<F, FMT, 0>()) kRoundsKernels[4] = {rounds_kernel<F, FMT, 0>(), rounds_kernel<F, FMT, 1>(),
-                                                                   rounds_kernel<F, FMT, 2>(), rounds_kernel<F, FMT, 3>()};
+constexpr decltype(family_kernel<F, FMT, 0>()) kKernels[4] = {table_entry<F, FMT, 0>(), table_entry<F, FMT, 1>(),
+                                                              table_entry<F, FMT, 2>(), table_entry<F, FMT, 3>()};
 
-// ... and their multi-batch twins (egpu_bestfit_batches_dev with EGPU_F_DEVICE_ROUNDS): same CTAs and shared memory
-template <int F, RowFormat FMT, int B>
-constexpr auto rounds_multi_kernel() {
-    constexpr int DT = 8 << B;
-    if constexpr (F == kRoundsSorted)
-        return kernel(rounds_sorted_multi_kernel<DT, FMT>, kRoundsThreads, sizeof(SnapSmem<DT, kRoundsThreads>));
-    else return kernel(rounds_lut_multi_kernel<FMT>, kRoundsThreads, sizeof(LutSmem<kRoundsThreads>));
+// The kernel a launcher runs for the context's D: family F, or G when `alt` (the lookup scan, the sharded release), in
+// row format fmt.  The one place a launcher's run-time choice of table is made.
+template <int F, int G = F>
+const auto& select_kernel(const egpu_ctx* ctx, bool alt, RowFormat fmt) {
+    const int b = d_bucket(ctx->D);
+    if constexpr (F == kScanGrid) return kKernels<F, kRowsInt32>[b];  // no packed form: launch_snapshot refuses packed rows
+    else if (fmt == kRowsPacked) return alt ? kKernels<G, kRowsPacked>[b] : kKernels<F, kRowsPacked>[b];
+    else return alt ? kKernels<G, kRowsInt32>[b] : kKernels<F, kRowsInt32>[b];
 }
-template <int F, RowFormat FMT>
-constexpr decltype(rounds_multi_kernel<F, FMT, 0>()) kRoundsMultiKernels[4] = {
-    rounds_multi_kernel<F, FMT, 0>(), rounds_multi_kernel<F, FMT, 1>(), rounds_multi_kernel<F, FMT, 2>(),
-    rounds_multi_kernel<F, FMT, 3>()};
 
-// The sharded prefix-commit of K batches in one launch (egpu_bestfit_batches_shard_dev with EGPU_F_PREFIX_COMMIT):
-// the scans, CTAs and shared memory of the multi-batch rounds kernels
-template <int F, RowFormat FMT, int B>
-constexpr auto shard_prefix_kernel() {
-    constexpr int DT = 8 << B;
-    if constexpr (F == kRoundsSorted)
-        return kernel(shard_prefix_multi_sorted_kernel<DT, FMT>, kRoundsThreads, sizeof(SnapSmem<DT, kRoundsThreads>));
-    else return kernel(shard_prefix_multi_lut_kernel<FMT>, kRoundsThreads, sizeof(LutSmem<kRoundsThreads>));
-}
-template <int F, RowFormat FMT>
-constexpr decltype(shard_prefix_kernel<F, FMT, 0>()) kShardPrefixKernels[4] = {
-    shard_prefix_kernel<F, FMT, 0>(), shard_prefix_kernel<F, FMT, 1>(), shard_prefix_kernel<F, FMT, 2>(),
-    shard_prefix_kernel<F, FMT, 3>()};
-
-// The sharded rounds to the fixed point in one launch (egpu_bestfit_batch_shard_prefix_dev with EGPU_F_DEVICE_ROUNDS):
-// the same scans, CTAs and shared memory
-template <int F, RowFormat FMT, int B>
-constexpr auto shard_rounds_kernel() {
-    constexpr int DT = 8 << B;
-    if constexpr (F == kRoundsSorted)
-        return kernel(shard_rounds_sorted_kernel<DT, FMT>, kRoundsThreads, sizeof(SnapSmem<DT, kRoundsThreads>));
-    else return kernel(shard_rounds_lut_kernel<FMT>, kRoundsThreads, sizeof(LutSmem<kRoundsThreads>));
-}
-template <int F, RowFormat FMT>
-constexpr decltype(shard_rounds_kernel<F, FMT, 0>()) kShardRoundsKernels[4] = {
-    shard_rounds_kernel<F, FMT, 0>(), shard_rounds_kernel<F, FMT, 1>(), shard_rounds_kernel<F, FMT, 2>(),
-    shard_rounds_kernel<F, FMT, 3>()};
-
-// Resident CTAs per SM of kernel k; `cached` is its entry in the context's occupancy cache.  The
-// first use on a context opts in to the kernel's dynamic shared memory and asks the occupancy.
+// Resident CTAs per SM of kernel k.  The first use on a context opts in to the kernel's dynamic shared memory and
+// asks the occupancy; the answer stays in the context's occupancy cache.
 template <class Fn>
-int resident_ctas(egpu_ctx* ctx, const Kernel<Fn>& k, int& cached, int* per_sm) {
+int resident_ctas(egpu_ctx* ctx, const Kernel<Fn>& k, int* per_sm) {
+    int& cached = ctx->ctas_per_sm[k.slot];
     if (cached == 0) {
         EGPU_CUDA(ctx, cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(k.smem)));
         int m = 0;
@@ -169,11 +121,6 @@ int resident_ctas(egpu_ctx* ctx, const Kernel<Fn>& k, int& cached, int* per_sm) 
     }
     *per_sm = cached;
     return EGPU_OK;
-}
-// ... of family F's kernel for D devices
-template <int F>
-int resident_ctas(egpu_ctx* ctx, int D, int* per_sm) {
-    return resident_ctas(ctx, kKernels<F>[d_bucket(D)], ctx->scan_ctas_per_sm[F][d_bucket(D)], per_sm);
 }
 
 // Programmatic dependent launch: the kernel may be scheduled while its predecessor on the stream
@@ -325,6 +272,32 @@ bool overlaps_inflight(const std::vector<Range>& f, const Range* r, int n) {
     }
     return false;
 }
+// the device descriptor of one batch: of the multi-batch scans, and of the persistent kernels
+void set_desc(BatchDesc& d, const int32_t* rc, const int32_t* rm, long long R, int32_t* idx, long long* delta, int32_t* table_out) {
+    d = {rc, rm, idx, delta, table_out, R};
+}
+void set_desc(RoundsBatch& d, const int32_t* rc, const int32_t* rm, long long R, int32_t* idx, long long* delta, int32_t* table_out) {
+    d = {rc, rm, R, idx, delta, table_out};
+}
+// K batches of `bs` in format fmt as device descriptors `out` (packed: no mem array; table_out false: no table'), and
+// their outputs in ctx->multi_ranges, prepared.  Returns the number of ranges, or -1 when two batches share an output
+// (their order would be undefined); *max_r = the largest R.
+template <class Desc>
+int batch_descs(egpu_ctx* ctx, const egpu_batch* bs, int K, RowFormat fmt, bool table_out, Desc* out, int64_t* max_r) {
+    const bool packed = fmt == kRowsPacked;
+    Range* mine = ctx->multi_ranges;
+    *max_r = 0;
+    for (int b = 0; b < K; ++b) {
+        const egpu_batch& in = bs[b];
+        long long* delta = reinterpret_cast<long long*>(in.d_delta);
+        int32_t* tab = table_out ? in.d_table_out : nullptr;
+        set_desc(out[b], in.d_req_core, packed ? nullptr : in.d_req_mem, in.R, in.d_out_idx, delta, tab);
+        batch_ranges(mine + 3 * b, in.d_out_idx, in.R, packed ? sizeof(int8_t) : sizeof(int32_t), delta, tab, ctx->D);
+        *max_r = std::max<int64_t>(*max_r, in.R);
+    }
+    return prepare_ranges(mine, 3 * K);
+}
+
 void new_group(egpu_ctx* ctx) {
     ctx->group_len = 0;
     ctx->group_mbatches = 0;
@@ -415,13 +388,9 @@ struct Snapshot {
 template <int F>
 int launch_snapshot_as(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_tiles_out) {
     constexpr bool lut = F == kScanLut || F == kScanLutContig, grid_variant = F == kScanGrid;
-    constexpr int P = lut ? kPackedLutContig : kPackedSortedContig, Q = lut ? kPackedLutSnap : kPackedSortedSnap;
-    const int bucket = d_bucket(ctx->D);
-    const auto& k = !a.packed ? kKernels<F>[bucket] : a.contig ? kPackedContigKernels<P>[bucket] : kPackedSnapKernels<Q>[bucket];
-    int& cached = !a.packed ? ctx->scan_ctas_per_sm[F][bucket]
-                            : a.contig ? ctx->packed_contig_ctas_per_sm[P][bucket] : ctx->packed_snap_ctas_per_sm[Q][bucket];
+    const auto& k = select_kernel<F>(ctx, false, a.packed ? kRowsPacked : kRowsInt32);
     int per_sm = 0;
-    int rc = resident_ctas(ctx, k, cached, &per_sm);
+    int rc = resident_ctas(ctx, k, &per_sm);
     if (rc != EGPU_OK) return rc;
     if (lut) {
         rc = refresh_lut(ctx, s);
@@ -505,12 +474,10 @@ int launch_snapshot(egpu_ctx* ctx, const Snapshot& a, cudaStream_t s, int* n_til
 template <int F>
 int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, cudaStream_t s, unsigned long long push_base) {
     constexpr bool lut = F == kScanLutMulti;
-    constexpr int P = lut ? kPackedLutMulti : kPackedSortedMulti;
-    const bool packed = (user_flags & EGPU_F_PACKED) != 0;
-    const int bucket = d_bucket(ctx->D);
-    const auto& k = packed ? kPackedKernels<P>[bucket] : kKernels<F>[bucket];
+    const RowFormat fmt = row_format(user_flags);
+    const auto& k = select_kernel<F>(ctx, false, fmt);
     int per_sm = 0;
-    int rc = resident_ctas(ctx, k, packed ? ctx->packed_ctas_per_sm[P][bucket] : ctx->scan_ctas_per_sm[F][bucket], &per_sm);
+    int rc = resident_ctas(ctx, k, &per_sm);
     if (rc != EGPU_OK) return rc;
     if (lut) {
         rc = refresh_lut(ctx, s);
@@ -520,21 +487,10 @@ int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, 
     std::memset(&args, 0, sizeof args);
     Range* mine = ctx->multi_ranges;
     int64_t max_r = 0;
-    for (int b = 0; b < K; ++b) {
-        const egpu_batch& in = bs[b];
-        BatchDesc& d = args.b[b];
-        d.rc = in.d_req_core;
-        d.rm = in.d_req_mem;
-        d.idx = in.d_out_idx;
-        d.delta = reinterpret_cast<long long*>(in.d_delta);
-        // sharded: table' comes from an apply call, or (EGPU_F_APPLY) from the batch's own last CTA
-        d.table_out = (push_base && !(user_flags & EGPU_F_APPLY)) ? nullptr : in.d_table_out;
-        d.R = in.R;
-        if (in.R > max_r) max_r = in.R;
-        batch_ranges(mine + 3 * b, d.idx, d.R, packed ? sizeof(int8_t) : sizeof(int32_t), d.delta, d.table_out, ctx->D);
-    }
-    const int n_mine = prepare_ranges(mine, 3 * K);
-    if (n_mine < 0) return EGPU_ERR_INVALID;  // two batches of one launch share an output: their order would be undefined
+    // sharded: table' comes from an apply call, or (EGPU_F_APPLY) from the batch's own last CTA
+    const bool table_out = !push_base || (user_flags & EGPU_F_APPLY);
+    const int n_mine = batch_descs(ctx, bs, K, fmt, table_out, args.b, &max_r);
+    if (n_mine < 0) return EGPU_ERR_INVALID;
     const unsigned long long captured = capture_id(s);
     const int flags = kFlagFinalize | ((push_base && (user_flags & EGPU_F_APPLY)) ? kFlagApplyNow : 0) |
                       order_scan(ctx, user_flags, true, K, s, mine, n_mine, captured);
@@ -551,7 +507,7 @@ int launch_multi_as(egpu_ctx* ctx, const egpu_batch* bs, int K, int user_flags, 
     // fastest of 20 / 28, 32 / 40 and 48 / 56.  Measured on an H100: DESIGN.md 4.1e.
     const int64_t nvec = max_r >> 2;
     const bool small = max_r < (512ll << 10);
-    const int64_t rpt = small ? ctx->multi_rpt : packed ? (lut ? 56 : 48) : (lut ? 28 : 20);
+    const int64_t rpt = small ? ctx->multi_rpt : fmt == kRowsPacked ? (lut ? 56 : 48) : (lut ? 28 : 20);
     const int64_t per_cta = static_cast<int64_t>(k.threads) * ((rpt + 3) / 4);
     int64_t tiles = (nvec + per_cta - 1) / per_cta;
     if (tiles < 1) tiles = 1;
@@ -688,6 +644,33 @@ int rounds_ctl(egpu_ctx* ctx, cudaStream_t s, RoundsCtl** out) {
     return EGPU_OK;
 }
 
+// The RoundsArgs of a one-launch rounds kernel whose (first) batch is b, in format fmt: allocates the rounds scratch
+// for R rows and zeroes fresh barrier words on s (rounds_scratch, rounds_ctl); the context's tile sums, PrefixOut and
+// lookup tables.
+int rounds_args(egpu_ctx* ctx, const egpu_batch& b, int64_t R, RowFormat fmt, cudaStream_t s, RoundsArgs* a) {
+    const bool packed = fmt == kRowsPacked;
+    RoundsScratch sc;
+    int rc = rounds_scratch(ctx, R, packed, &sc);
+    if (rc != EGPU_OK) return rc;
+    std::memset(a, 0, sizeof *a);
+    rc = rounds_ctl(ctx, s, &a->ctl);
+    if (rc != EGPU_OK) return rc;
+    a->rc = b.d_req_core;
+    a->rm = packed ? nullptr : b.d_req_mem;
+    a->R = static_cast<long long>(b.R);
+    a->idx = b.d_out_idx;
+    a->delta_out = reinterpret_cast<long long*>(b.d_delta);
+    a->table_out = b.d_table_out;
+    a->tile_sums = ctx->d_tile_sums;
+    a->pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
+    a->total = sc.info->delta;
+    a->deferred = &sc.info->deferred;
+    a->tile_count = sc.tiles;
+    std::memcpy(a->set, sc.set, sizeof a->set);
+    a->lut = ctx->d_lut;
+    return EGPU_OK;
+}
+
 int run_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx, int max_rounds,
                long long* total_delta /* host [2*D] */, int32_t* rounds_out, int64_t* left_out, cudaStream_t s,
                RowFormat fmt = kRowsInt32, int32_t* d_table_out = nullptr) {
@@ -787,16 +770,41 @@ bool device_rounds_flags_ok(int flags, int64_t R) {
            (flags & kDeviceRoundsNeeds) == kDeviceRoundsNeeds && R < (1ll << 31);
 }
 
+// The flags EGPU_F_RELEASE is valid with: itself, optionally EGPU_F_COMMIT and EGPU_F_PACKED
+bool release_flags_ok(int flags, int64_t R) {
+    return (flags & ~(EGPU_F_RELEASE | EGPU_F_COMMIT | EGPU_F_PACKED)) == 0 && R < (1ll << 31);
+}
+
+// What egpu_bestfit_batch[_dev] does
+enum BatchOp { kOpSnapshot, kOpPrefix, kOpRounds, kOpDeviceRounds, kOpRelease };
+
+// The operation of egpu_bestfit_batch[_dev]'s flags for R rows; false when the flags are refused.  Without
+// EGPU_F_RELEASE, EGPU_F_DEVICE_ROUNDS or EGPU_F_ROUNDS other bits are ignored, except that EGPU_F_PACKED needs
+// EGPU_F_PREFIX_COMMIT.
+bool batch_op(int flags, int64_t R, BatchOp* op) {
+    *op = (flags & EGPU_F_RELEASE)         ? kOpRelease
+          : (flags & EGPU_F_DEVICE_ROUNDS) ? kOpDeviceRounds
+          : (flags & EGPU_F_ROUNDS)        ? kOpRounds
+          : (flags & EGPU_F_PREFIX_COMMIT) ? kOpPrefix
+                                           : kOpSnapshot;
+    switch (*op) {
+        case kOpRelease: return release_flags_ok(flags, R);
+        case kOpDeviceRounds: return device_rounds_flags_ok(flags, R);
+        case kOpRounds: return rounds_flags_ok(flags, R);
+        case kOpPrefix: return true;
+        default: return !(flags & EGPU_F_PACKED);
+    }
+}
+
 // Grid of a persistent launch (the one-launch rounds, the multi-batch sharded prefix-commit) of kernel k over
 // batches of at most R rows: as many CTAs as round 1's CONTIG scan wants at 8 rows per thread (the lone-launch
 // rule of launch_snapshot_as), at most one resident wave (the grid barriers need every CTA resident) and at
 // least one CTA per device (CTA d cuts device d).  Also sizes the tile sums and PrefixOut for that grid, so
 // that, with the caller's own scratch, everything is allocated before the launch and a failure commits nothing.
-// `cached` is the kernel's entry in the context's occupancy cache.
 template <class Fn>
-int persistent_grid(egpu_ctx* ctx, const Kernel<Fn>& k, int& cached, int64_t R, int64_t* grid_out) {
+int persistent_grid(egpu_ctx* ctx, const Kernel<Fn>& k, int64_t R, int64_t* grid_out) {
     int per_sm = 0;
-    const int rc = resident_ctas(ctx, k, cached, &per_sm);
+    const int rc = resident_ctas(ctx, k, &per_sm);
     if (rc != EGPU_OK) return rc;
     if (ctx->ctas_per_sm_cap > 0 && ctx->ctas_per_sm_cap < per_sm) per_sm = ctx->ctas_per_sm_cap;
     const int64_t wave = static_cast<int64_t>(ctx->sm_count) * per_sm;
@@ -842,55 +850,23 @@ int launch_persistent(egpu_ctx* ctx, const Kernel<Fn>& k, int64_t grid, cudaStre
 // largest batch.  Otherwise bs[0] alone (K = 1) in the single-batch kernels.
 int launch_device_rounds(egpu_ctx* ctx, const egpu_batch* bs, int K, bool multi, cudaStream_t s, RowFormat fmt) {
     if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // no prefix-commit mode
-    const bool lut = lut_variant(ctx), packed = fmt == kRowsPacked;
-    const int bucket = d_bucket(ctx->D), fam = lut ? kRoundsLut : kRoundsSorted;
-    int64_t R = 0;
-    for (int b = 0; b < K; ++b) R = std::max<int64_t>(R, bs[b].R);
+    const bool lut = lut_variant(ctx);
+    RoundsMultiArgs m;
+    int64_t R = bs[0].R;
     if (multi) {  // two batches sharing an output: the later one would overwrite the earlier one's
-        Range* mine = ctx->multi_ranges;
-        for (int b = 0; b < K; ++b)
-            batch_ranges(mine + 3 * b, bs[b].d_out_idx, bs[b].R, packed ? sizeof(int8_t) : sizeof(int32_t), bs[b].d_delta,
-                         bs[b].d_table_out, ctx->D);
-        if (prepare_ranges(mine, 3 * K) < 0) return EGPU_ERR_INVALID;
+        std::memset(&m, 0, sizeof m);
+        if (batch_descs(ctx, bs, K, fmt, true, m.b, &R) < 0) return EGPU_ERR_INVALID;
     }
-    const auto& k = lut ? (packed ? kRoundsKernels<kRoundsLut, kRowsPacked> : kRoundsKernels<kRoundsLut, kRowsInt32>)[bucket]
-                        : (packed ? kRoundsKernels<kRoundsSorted, kRowsPacked> : kRoundsKernels<kRoundsSorted, kRowsInt32>)[bucket];
-    const auto& km = lut ? (packed ? kRoundsMultiKernels<kRoundsLut, kRowsPacked> : kRoundsMultiKernels<kRoundsLut, kRowsInt32>)[bucket]
-                         : (packed ? kRoundsMultiKernels<kRoundsSorted, kRowsPacked>
-                                   : kRoundsMultiKernels<kRoundsSorted, kRowsInt32>)[bucket];
+    const auto& k = select_kernel<kRoundsSorted, kRoundsLut>(ctx, lut, fmt);
+    const auto& km = select_kernel<kRoundsMultiSorted, kRoundsMultiLut>(ctx, lut, fmt);
     int64_t grid = 0;
-    int rc = multi ? persistent_grid(ctx, km, ctx->rounds_multi_ctas_per_sm[fam][packed][bucket], R, &grid)
-                   : persistent_grid(ctx, k, ctx->rounds_ctas_per_sm[fam][packed][bucket], R, &grid);
-    if (rc != EGPU_OK) return rc;
-    RoundsScratch sc;
-    rc = rounds_scratch(ctx, R, packed, &sc);
-    if (rc != EGPU_OK) return rc;
-    RoundsCtl* ctl = nullptr;
-    rc = rounds_ctl(ctx, s, &ctl);
+    int rc = multi ? persistent_grid(ctx, km, R, &grid) : persistent_grid(ctx, k, R, &grid);
     if (rc != EGPU_OK) return rc;
     RoundsArgs a;
-    std::memset(&a, 0, sizeof a);
-    a.rc = bs[0].d_req_core;
-    a.rm = packed ? nullptr : bs[0].d_req_mem;
-    a.R = static_cast<long long>(bs[0].R);
-    a.idx = bs[0].d_out_idx;
-    a.delta_out = reinterpret_cast<long long*>(bs[0].d_delta);
-    a.table_out = bs[0].d_table_out;
-    a.tile_sums = ctx->d_tile_sums;
-    a.pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
-    a.total = sc.info->delta;
-    a.deferred = &sc.info->deferred;
-    a.tile_count = sc.tiles;
-    std::memcpy(a.set, sc.set, sizeof a.set);
-    a.ctl = ctl;
-    a.lut = ctx->d_lut;
+    rc = rounds_args(ctx, bs[0], R, fmt, s, &a);
+    if (rc != EGPU_OK) return rc;
     if (multi) {
-        RoundsMultiArgs m;
-        std::memset(&m, 0, sizeof m);
         m.a = a;
-        for (int b = 0; b < K; ++b)
-            m.b[b] = {bs[b].d_req_core, packed ? nullptr : bs[b].d_req_mem, static_cast<long long>(bs[b].R), bs[b].d_out_idx,
-                      reinterpret_cast<long long*>(bs[b].d_delta), bs[b].d_table_out};
         m.K = K;
         rc = launch_persistent(ctx, km, grid, s, m);
     } else {
@@ -940,32 +916,21 @@ int launch_prefix_commit_shard(egpu_ctx* ctx, const int32_t* d_rc, const int32_t
 int launch_shard_prefix_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, bool commit, uint64_t first_step, cudaStream_t s,
                               RowFormat fmt) {
     if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // no prefix-commit mode
-    const bool lut = lut_variant(ctx), packed = fmt == kRowsPacked;
-    const int bucket = d_bucket(ctx->D), fam = lut ? kRoundsLut : kRoundsSorted;
-    int64_t R = 0;
-    Range* mine = ctx->multi_ranges;
-    for (int b = 0; b < K; ++b) {
-        R = std::max<int64_t>(R, bs[b].R);
-        batch_ranges(mine + 3 * b, bs[b].d_out_idx, bs[b].R, packed ? sizeof(int8_t) : sizeof(int32_t), bs[b].d_delta,
-                     bs[b].d_table_out, ctx->D);
-    }
-    if (prepare_ranges(mine, 3 * K) < 0) return EGPU_ERR_INVALID;  // the later batch would overwrite the earlier one's outputs
-    const auto& k = lut ? (packed ? kShardPrefixKernels<kRoundsLut, kRowsPacked> : kShardPrefixKernels<kRoundsLut, kRowsInt32>)[bucket]
-                        : (packed ? kShardPrefixKernels<kRoundsSorted, kRowsPacked>
-                                  : kShardPrefixKernels<kRoundsSorted, kRowsInt32>)[bucket];
-    int64_t grid = 0;
-    int rc = persistent_grid(ctx, k, ctx->shard_prefix_ctas_per_sm[fam][packed][bucket], R, &grid);
-    if (rc != EGPU_OK) return rc;
-    RoundsScratch sc;
-    rc = rounds_scratch(ctx, 0, packed, &sc);  // the head only
-    if (rc != EGPU_OK) return rc;
+    const bool lut = lut_variant(ctx);
     ShardPrefixArgs a;
     std::memset(&a, 0, sizeof a);
+    int64_t R = 0;
+    // the later batch would overwrite the earlier one's outputs
+    if (batch_descs(ctx, bs, K, fmt, true, a.b, &R) < 0) return EGPU_ERR_INVALID;
+    const auto& k = select_kernel<kShardPrefixSorted, kShardPrefixLut>(ctx, lut, fmt);
+    int64_t grid = 0;
+    int rc = persistent_grid(ctx, k, R, &grid);
+    if (rc != EGPU_OK) return rc;
+    RoundsScratch sc;
+    rc = rounds_scratch(ctx, 0, fmt == kRowsPacked, &sc);  // the head only
+    if (rc != EGPU_OK) return rc;
     rc = rounds_ctl(ctx, s, &a.ctl);
     if (rc != EGPU_OK) return rc;
-    for (int b = 0; b < K; ++b)
-        a.b[b] = {bs[b].d_req_core, packed ? nullptr : bs[b].d_req_mem, static_cast<long long>(bs[b].R), bs[b].d_out_idx,
-                  reinterpret_cast<long long*>(bs[b].d_delta), bs[b].d_table_out};
     a.tile_sums = ctx->d_tile_sums;
     a.pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
     a.stop = reinterpret_cast<unsigned int*>(static_cast<char*>(ctx->d_rounds) + kShardStopOff);
@@ -984,37 +949,17 @@ int launch_shard_prefix_multi(egpu_ctx* ctx, const egpu_batch* bs, int K, bool c
 // round on the same two steps, until no rank has a deferred row.  Grid: persistent_grid of this rank's R; scratch:
 // the rounds scratch of launch_device_rounds, sized by R, and the barrier, stop and again words in its head, all
 // allocated before the launch.  Nothing here waits for the device.
-int launch_shard_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, int32_t* d_idx, long long* d_delta,
-                        int32_t* d_table_out, uint64_t step, cudaStream_t s, RowFormat fmt) {
+int launch_shard_rounds(egpu_ctx* ctx, const egpu_batch& b, uint64_t step, cudaStream_t s, RowFormat fmt) {
     if (ctx->variant == EGPU_VARIANT_GRID) return EGPU_ERR_STATE;  // no prefix-commit mode
-    const bool lut = lut_variant(ctx), packed = fmt == kRowsPacked;
-    const int bucket = d_bucket(ctx->D), fam = lut ? kRoundsLut : kRoundsSorted;
-    const auto& k = lut ? (packed ? kShardRoundsKernels<kRoundsLut, kRowsPacked> : kShardRoundsKernels<kRoundsLut, kRowsInt32>)[bucket]
-                        : (packed ? kShardRoundsKernels<kRoundsSorted, kRowsPacked>
-                                  : kShardRoundsKernels<kRoundsSorted, kRowsInt32>)[bucket];
+    const bool lut = lut_variant(ctx);
+    const auto& k = select_kernel<kShardRoundsSorted, kShardRoundsLut>(ctx, lut, fmt);
     int64_t grid = 0;
-    int rc = persistent_grid(ctx, k, ctx->shard_rounds_ctas_per_sm[fam][packed][bucket], R, &grid);
-    if (rc != EGPU_OK) return rc;
-    RoundsScratch sc;
-    rc = rounds_scratch(ctx, R, packed, &sc);
+    int rc = persistent_grid(ctx, k, b.R, &grid);
     if (rc != EGPU_OK) return rc;
     ShardRoundsArgs a;
     std::memset(&a, 0, sizeof a);
-    rc = rounds_ctl(ctx, s, &a.a.ctl);
+    rc = rounds_args(ctx, b, b.R, fmt, s, &a.a);
     if (rc != EGPU_OK) return rc;
-    a.a.rc = d_rc;
-    a.a.rm = packed ? nullptr : d_rm;
-    a.a.R = static_cast<long long>(R);
-    a.a.idx = d_idx;
-    a.a.delta_out = d_delta;
-    a.a.table_out = d_table_out;
-    a.a.tile_sums = ctx->d_tile_sums;
-    a.a.pf = static_cast<PrefixOut*>(ctx->d_prefix_out);
-    a.a.total = sc.info->delta;
-    a.a.deferred = &sc.info->deferred;
-    a.a.tile_count = sc.tiles;
-    std::memcpy(a.a.set, sc.set, sizeof a.a.set);
-    a.a.lut = ctx->d_lut;
     a.stop = reinterpret_cast<unsigned int*>(static_cast<char*>(ctx->d_rounds) + kShardStopOff);
     a.again = reinterpret_cast<unsigned int*>(static_cast<char*>(ctx->d_rounds) + kShardAgainOff);
     a.step_plus1 = step + 1;
@@ -1026,9 +971,9 @@ int launch_shard_rounds(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm,
 // Packed-format scan: always a fully ordered launch (it serves the synchronous host path).
 int launch_packed(egpu_ctx* ctx, const uint32_t* d_req, int64_t R, signed char* d_idx8, long long* d_delta,
                   int32_t* d_table_out, int user_flags, cudaStream_t s, int rows_per_thread) {
-    const auto& k = kKernels<kScanPacked>[d_bucket(ctx->D)];
+    const auto& k = kKernels<kScanPacked, kRowsPacked>[d_bucket(ctx->D)];
     int per_sm = 0;
-    int rc = resident_ctas<kScanPacked>(ctx, ctx->D, &per_sm);
+    int rc = resident_ctas(ctx, k, &per_sm);
     if (rc != EGPU_OK) return rc;
     const int64_t nchunk = R >> 9;  // 512 requests per warp trip
     const int64_t per_cta = static_cast<int64_t>(k.threads / 32) * ((rows_per_thread + 15) / 16);
@@ -1048,23 +993,6 @@ int launch_packed(egpu_ctx* ctx, const uint32_t* d_req, int64_t R, signed char* 
     return (flags & kFlagCommit) ? table_changed(ctx, s) : EGPU_OK;
 }
 
-// The release kernels (EGPU_F_RELEASE), per row format and D bucket: the register scans' CTA sizes and SnapSmem,
-// whose lane-private accumulators they reuse at every D (DESIGN.md 4.1h).  SHARD: the sharded form, whose last
-// CTA exchanges the sums with the peers before it decides.
-template <RowFormat FMT, bool SHARD, int B>
-constexpr auto release_kernel() {
-    constexpr int DT = 8 << B, T = B == 3 ? 128 : 256;
-    return kernel(release_rows_kernel<DT, T, FMT, SHARD>, T, sizeof(SnapSmem<DT, T>));
-}
-template <RowFormat FMT, bool SHARD>
-constexpr decltype(release_kernel<FMT, SHARD, 0>()) kReleaseKernels[4] = {
-    release_kernel<FMT, SHARD, 0>(), release_kernel<FMT, SHARD, 1>(), release_kernel<FMT, SHARD, 2>(), release_kernel<FMT, SHARD, 3>()};
-
-// The flags EGPU_F_RELEASE is valid with: itself, optionally EGPU_F_COMMIT and EGPU_F_PACKED
-bool release_flags_ok(int flags, int64_t R) {
-    return (flags & ~(EGPU_F_RELEASE | EGPU_F_COMMIT | EGPU_F_PACKED)) == 0 && R < (1ll << 31);
-}
-
 // EGPU_F_RELEASE (spec 2.8): the R rows (d_rc, d_rm) give back what they hold on device d_idx[r], all or
 // nothing, in one launch of release_rows_kernel.  Rows in either format (see prefix_scan); the indices are
 // read, never written.  d_delta (may be NULL) receives the sums, d_table_out (may be NULL) table + sums or,
@@ -1075,12 +1003,10 @@ bool release_flags_ok(int flags, int64_t R) {
 // every rank's sums, exchanged under step step_plus1 - 1 in the last CTA; 0 for one GPU.
 int launch_release(egpu_ctx* ctx, const int32_t* d_rc, const int32_t* d_rm, int64_t R, const int32_t* d_idx, long long* d_delta,
                    int32_t* d_table_out, int user_flags, cudaStream_t s, RowFormat fmt, uint64_t step_plus1) {
-    const bool packed = fmt == kRowsPacked, commit = (user_flags & EGPU_F_COMMIT) != 0, shard = step_plus1 != 0;
-    const int bucket = d_bucket(ctx->D);
-    const auto& k = (shard ? (packed ? kReleaseKernels<kRowsPacked, true> : kReleaseKernels<kRowsInt32, true>)
-                           : (packed ? kReleaseKernels<kRowsPacked, false> : kReleaseKernels<kRowsInt32, false>))[bucket];
+    const bool commit = (user_flags & EGPU_F_COMMIT) != 0;
+    const auto& k = select_kernel<kRelease, kReleaseShard>(ctx, step_plus1 != 0, fmt);
     int per_sm = 0;
-    const int rc = resident_ctas(ctx, k, (shard ? ctx->release_shard_ctas_per_sm : ctx->release_ctas_per_sm)[packed][bucket], &per_sm);
+    const int rc = resident_ctas(ctx, k, &per_sm);
     if (rc != EGPU_OK) return rc;
     Range mine[3];
     batch_ranges(mine, nullptr, 0, 0, d_delta, d_table_out, ctx->D);
@@ -1116,12 +1042,53 @@ int ensure_staging(egpu_ctx* ctx, int64_t rows) {
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-// device row arrays of an entry point: present when there are rows, 16-byte aligned (the scans
-// move 128-bit vectors)
-bool rows_ok(int64_t R, std::initializer_list<const void*> arrays) {
-    for (const void* p : arrays)
-        if ((R > 0 && !p) || !aligned16(p)) return false;
-    return true;
+// The row arrays of an entry point in format fmt: present when there are rows and, device arrays, 16-byte aligned
+// (the scans move 128-bit vectors).  Packed rows are words in rc with rm NULL, so that packed rows handed over
+// without EGPU_F_PACKED (rm NULL, R > 0) are refused rather than read as int32 arrays.
+bool arrays_ok(RowFormat fmt, int64_t R, const void* rc, const void* rm, const void* idx, bool device = true) {
+    auto ok = [&](const void* p) { return (R <= 0 || p) && (!device || aligned16(p)); };
+    return ok(rc) && ok(idx) && (fmt == kRowsPacked ? !rm : ok(rm));
+}
+
+// Host forms: the caller's rows into the staging arrays (rm: NULL for packed rows; idx: only when the indices are
+// an input, idx_bytes each) ...
+int stage_in(egpu_ctx* ctx, cudaStream_t s, int64_t R, const void* rc, const void* rm, const void* idx, size_t idx_bytes) {
+    const int e = ensure_staging(ctx, R > 0 ? R : 1);
+    if (e != EGPU_OK) return e;
+    if (R > 0) {
+        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, rc, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
+        if (rm) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, rm, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
+        if (idx) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_idx, idx, idx_bytes * R, cudaMemcpyHostToDevice, s));
+    }
+    return EGPU_OK;
+}
+// ... and back, before the synchronisation: the indices (idx: NULL when they were an input) and, `sums`, the demand
+// sums into ctx->h_delta
+int stage_out(egpu_ctx* ctx, cudaStream_t s, int64_t R, void* idx, size_t idx_bytes, bool sums) {
+    if (idx && R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(idx, ctx->d_idx, idx_bytes * R, cudaMemcpyDeviceToHost, s));
+    if (sums) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * ctx->D, cudaMemcpyDeviceToHost, s));
+    return EGPU_OK;
+}
+// a call's demand sums (host, core then mem) into the caller's arrays, each of which may be NULL
+void sums_out(const egpu_ctx* ctx, const long long* sums, int64_t* core, int64_t* mem) {
+    if (core) std::memcpy(core, sums, sizeof(int64_t) * ctx->D);
+    if (mem) std::memcpy(mem, sums + ctx->D, sizeof(int64_t) * ctx->D);
+}
+
+// egpu_bestfit_batch[_dev] after their checks, on device arrays: the caller's, or the host form's staging.  total:
+// host int64[2*D], where the packed rounds leave the demand they committed over all rounds.
+int run_batch(egpu_ctx* ctx, BatchOp op, RowFormat fmt, const int32_t* rc, const int32_t* rm, int64_t R, int32_t* idx,
+              long long* delta, int32_t* table_out, int flags, cudaStream_t s, long long* total) {
+    switch (op) {
+        case kOpRelease: return launch_release(ctx, rc, rm, R, idx, delta, table_out, flags, s, fmt, 0);
+        case kOpDeviceRounds: {
+            const egpu_batch one{rc, rm, R, idx, reinterpret_cast<int64_t*>(delta), table_out};
+            return launch_device_rounds(ctx, &one, 1, false, s, fmt);
+        }
+        case kOpRounds: return launch_packed_rounds(ctx, rc, R, idx, delta, table_out, total, s);
+        case kOpPrefix: return launch_prefix_commit(ctx, rc, rm, R, idx, delta, table_out, flags, s, fmt);
+        default: return launch_snapshot(ctx, Snapshot{rc, rm, R, idx, delta, table_out, flags}, s);
+    }
 }
 
 // What an entry point needs of the context, each level including the ones before it.
@@ -1372,73 +1339,47 @@ int egpu_bestfit_batch_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32
                            int32_t* d_out_idx, int64_t* d_delta, int32_t* d_table_out, int flags,
                            void* stream) {
     // EGPU_F_PACKED: prefix-commit only, d_req_core = words, d_req_mem NULL, d_out_idx = int8 indices.
-    // Without it a NULL d_req_mem (R > 0) stays refused, so words are never read as int32 arrays.
     // EGPU_F_ROUNDS: that, committing, to the fixed point; synchronises the stream.
     // EGPU_F_DEVICE_ROUNDS: rounds to the fixed point in either format, in one launch, asynchronous.
-    const bool packed = (flags & EGPU_F_PACKED) != 0;
-    const bool rounds = (flags & EGPU_F_ROUNDS) != 0;
-    const bool device_rounds = (flags & EGPU_F_DEVICE_ROUNDS) != 0;
     // EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: the rows give back what they hold on d_out_idx, which is read.
-    const bool release = (flags & EGPU_F_RELEASE) != 0;
-    if (!ctx || R < 0 ||
-        (release ? !release_flags_ok(flags, R) : device_rounds ? !device_rounds_flags_ok(flags, R) : rounds && !rounds_flags_ok(flags, R)))
-        return EGPU_ERR_INVALID;
-    if (packed ? ((!release && !(flags & EGPU_F_PREFIX_COMMIT)) || d_req_mem || !rows_ok(R, {d_req_core, d_out_idx}))
-               : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
-        return EGPU_ERR_INVALID;
+    BatchOp op;
+    if (!ctx || R < 0 || !batch_op(flags, R, &op)) return EGPU_ERR_INVALID;
+    const RowFormat fmt = row_format(flags);
+    if (!arrays_ok(fmt, R, d_req_core, d_req_mem, d_out_idx)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
-    if (release)
-        return launch_release(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags, s,
-                              packed ? kRowsPacked : kRowsInt32, 0);
-    if (device_rounds) {
-        const egpu_batch one{d_req_core, d_req_mem, R, d_out_idx, d_delta, d_table_out};
-        return launch_device_rounds(ctx, &one, 1, false, s, packed ? kRowsPacked : kRowsInt32);
-    }
-    if (rounds) {
-        long long total[2 * kMaxD];
-        rc = launch_packed_rounds(ctx, d_req_core, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, total, s);
-        if (rc != EGPU_OK) return rc;
-        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
-        return EGPU_OK;
-    }
-    if (flags & EGPU_F_PREFIX_COMMIT)
-        return launch_prefix_commit(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out,
-                                    flags, s, packed ? kRowsPacked : kRowsInt32);
-    Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags};
-    return launch_snapshot(ctx, a, s);
-}
-
-// packed: d_req_core holds the words and d_req_mem must be NULL, so that a packed batch handed over
-// without EGPU_F_PACKED (d_req_mem NULL, R > 0) is refused rather than read as int32 arrays
-static int check_batches(const egpu_batch* batches, int32_t K, bool packed = false) {
-    if (!batches || K < 1 || K > EGPU_MAX_BATCHES) return EGPU_ERR_INVALID;
-    for (int k = 0; k < K; ++k) {
-        const egpu_batch& b = batches[k];
-        if (b.R < 0 || b.R > kMaxRows) return EGPU_ERR_INVALID;
-        if (packed ? (b.d_req_mem || !rows_ok(b.R, {b.d_req_core, b.d_out_idx}))
-                   : !rows_ok(b.R, {b.d_req_core, b.d_req_mem, b.d_out_idx}))
-            return EGPU_ERR_INVALID;
-    }
+    long long total[2 * kMaxD];
+    rc = run_batch(ctx, op, fmt, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags, s,
+                   total);
+    if (rc != EGPU_OK || op != kOpRounds) return rc;
+    EGPU_CUDA(ctx, cudaStreamSynchronize(s));
     return EGPU_OK;
 }
 
+// one check of every batch of a multi-batch call (see arrays_ok)
+static int check_batches(const egpu_batch* batches, int32_t K, RowFormat fmt) {
+    if (!batches || K < 1 || K > EGPU_MAX_BATCHES) return EGPU_ERR_INVALID;
+    for (int k = 0; k < K; ++k) {
+        const egpu_batch& b = batches[k];
+        if (b.R < 0 || b.R > kMaxRows || !arrays_ok(fmt, b.R, b.d_req_core, b.d_req_mem, b.d_out_idx)) return EGPU_ERR_INVALID;
+    }
+    return EGPU_OK;
+}
 int egpu_bestfit_batches_dev(egpu_ctx* ctx, const egpu_batch* batches, int32_t K, int flags, void* stream) {
     // EGPU_F_DEVICE_ROUNDS (with exactly the flags of the single-batch call): the batches placed in order,
     // each committed to its fixed point, in one launch.  Otherwise a snapshot of every batch.
     const bool device_rounds = (flags & EGPU_F_DEVICE_ROUNDS) != 0;
     if (!ctx || (device_rounds ? !device_rounds_flags_ok(flags, 0) : (flags & ~(EGPU_F_INPUTS_READY | EGPU_F_PACKED)) != 0))
         return EGPU_ERR_INVALID;
-    const bool packed = (flags & EGPU_F_PACKED) != 0;
-    int rc = check_batches(batches, K, packed);
+    int rc = check_batches(batches, K, row_format(flags));
     if (rc != EGPU_OK) return rc;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     rc = enter(ctx, kNeedsTable, stream, &s);
     if (rc != EGPU_OK) return rc;
-    if (device_rounds) return launch_device_rounds(ctx, batches, K, true, s, packed ? kRowsPacked : kRowsInt32);
+    if (device_rounds) return launch_device_rounds(ctx, batches, K, true, s, row_format(flags));
     return launch_multi(ctx, batches, K, flags, s, 0);
 }
 
@@ -1447,11 +1388,10 @@ int egpu_bestfit_batches_shard_dev(egpu_ctx* ctx, const egpu_batch* batches, int
     // EGPU_F_PREFIX_COMMIT [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: K sharded prefix-commits in order, in one launch, on
     // exchange steps first_step .. first_step + 2K - 1.  Otherwise K sharded snapshot steps.
     const bool prefix = (flags & EGPU_F_PREFIX_COMMIT) != 0;
-    const bool packed = (flags & EGPU_F_PACKED) != 0;
     if (!ctx || first_step >= (1ull << 47) ||
         (flags & ~(prefix ? EGPU_F_PREFIX_COMMIT | EGPU_F_COMMIT | EGPU_F_PACKED : EGPU_F_INPUTS_READY | EGPU_F_APPLY)))
         return EGPU_ERR_INVALID;
-    int rc = check_batches(batches, K, packed);
+    int rc = check_batches(batches, K, row_format(flags));
     if (rc != EGPU_OK) return rc;
     if (prefix && first_step + 2ull * static_cast<uint64_t>(K) > (1ull << 47)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
@@ -1459,8 +1399,7 @@ int egpu_bestfit_batches_shard_dev(egpu_ctx* ctx, const egpu_batch* batches, int
     rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
     if (prefix)
-        return launch_shard_prefix_multi(ctx, batches, K, (flags & EGPU_F_COMMIT) != 0, first_step, s,
-                                         packed ? kRowsPacked : kRowsInt32);
+        return launch_shard_prefix_multi(ctx, batches, K, (flags & EGPU_F_COMMIT) != 0, first_step, s, row_format(flags));
     return launch_multi(ctx, batches, K, flags, s, first_step + 1);
 }
 
@@ -1538,9 +1477,9 @@ int egpu_bestfit_query(egpu_ctx* ctx, const int32_t* free_core, const int32_t* f
     EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
     EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
     // the register scan whatever the context's variant: one table, used once - lookup tables would not pay
-    const auto& k = kKernels<kScanSorted>[d_bucket(D)];
+    const auto& k = kKernels<kScanSorted, kRowsInt32>[d_bucket(D)];
     int per_sm = 0;
-    rc = resident_ctas<kScanSorted>(ctx, D, &per_sm);
+    rc = resident_ctas(ctx, k, &per_sm);
     if (rc != EGPU_OK) return rc;
     const int64_t nvec = R >> 2;
     const int64_t per_cta = static_cast<int64_t>(k.threads) * 2;
@@ -1563,99 +1502,27 @@ int egpu_bestfit_query(egpu_ctx* ctx, const int32_t* free_core, const int32_t* f
 
 int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* req_mem, int64_t R,
                        int32_t* out_idx, int64_t* out_delta_core, int64_t* out_delta_mem, int commit) {
-    // `commit` carries EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT, and EGPU_F_PACKED with the latter:
-    // req_core = words, req_mem NULL, out_idx = int8 indices (as in egpu_bestfit_batch_dev)
-    const bool prefix = (commit & EGPU_F_PREFIX_COMMIT) != 0;
-    const bool packed = (commit & EGPU_F_PACKED) != 0;
-    const bool rounds = (commit & EGPU_F_ROUNDS) != 0;
-    const bool device_rounds = (commit & EGPU_F_DEVICE_ROUNDS) != 0;
-    const bool release = (commit & EGPU_F_RELEASE) != 0;  // out_idx is an input: the devices the rows were placed on
-    if (!ctx || R < 0 ||
-        (release ? !release_flags_ok(commit, R) : device_rounds ? !device_rounds_flags_ok(commit, R) : rounds && !rounds_flags_ok(commit, R)))
-        return EGPU_ERR_INVALID;
-    if (packed ? ((!release && !prefix) || req_mem || (R > 0 && (!req_core || !out_idx)))
-               : (R > 0 && (!req_core || !req_mem || !out_idx)))
-        return EGPU_ERR_INVALID;
+    // `commit` carries the flags of egpu_bestfit_batch_dev: EGPU_F_PACKED rows are req_core = words, req_mem NULL,
+    // out_idx = int8 indices; with EGPU_F_RELEASE out_idx is an input, the devices the rows were placed on
+    BatchOp op;
+    if (!ctx || R < 0 || !batch_op(commit, R, &op)) return EGPU_ERR_INVALID;
+    const RowFormat fmt = row_format(commit);
+    if (!arrays_ok(fmt, R, req_core, req_mem, out_idx, false)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, nullptr, &s);
     if (rc != EGPU_OK) return rc;
     const int D = ctx->D;
-    if (release) {  // one launch, rows and indices staged through HBM: int32 12 bytes per row in, packed 5; nothing per row out
-        rc = ensure_staging(ctx, R > 0 ? R : 1);
-        if (rc != EGPU_OK) return rc;
-        if (R > 0) {
-            EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-            if (!packed) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-            EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_idx, out_idx, (packed ? sizeof(int8_t) : sizeof(int32_t)) * R, cudaMemcpyHostToDevice, s));
-        }
-        rc = launch_release(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, ctx->d_table_out, commit, s,
-                            packed ? kRowsPacked : kRowsInt32, 0);
-        if (rc != EGPU_OK) return rc;
-        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_table, ctx->d_table_out, sizeof(int32_t) * 3 * D, cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
-        if (out_delta_core) std::memcpy(out_delta_core, ctx->h_delta, sizeof(int64_t) * D);
-        if (out_delta_mem) std::memcpy(out_delta_mem, ctx->h_delta + D, sizeof(int64_t) * D);
-        for (int d = 0; d < D; ++d) {
-            const int32_t reason = ctx->h_table[2 * D + d];
-            if (!reason) continue;
-            std::snprintf(ctx->last_err, sizeof ctx->last_err, "EGPU_F_RELEASE refused, nothing released: device %d %s", d,
-                          reason == EGPU_REL_FLAGGED ? "is oversubscribed (EGPU_REL_FLAGGED)"
-                                                     : "would hold more than the domain allows (EGPU_REL_EXCEEDS)");
-            return EGPU_ERR_STATE;
-        }
-        return EGPU_OK;
-    }
-    if (device_rounds) {  // one launch, staged through HBM: int32 8 bytes per row in and 4 out, packed 4 in and 1 out
-        rc = ensure_staging(ctx, R > 0 ? R : 1);
-        if (rc != EGPU_OK) return rc;
-        if (R > 0) {
-            EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-            if (!packed) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-        }
-        const egpu_batch one{ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, reinterpret_cast<int64_t*>(ctx->d_delta), nullptr};
-        rc = launch_device_rounds(ctx, &one, 1, false, s, packed ? kRowsPacked : kRowsInt32);
-        if (rc != EGPU_OK) return rc;
-        const size_t idx_bytes = packed ? sizeof(int8_t) : sizeof(int32_t);
-        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, idx_bytes * R, cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
-        unsigned long long timeouts = 0;
-        EGPU_CUDA(ctx, cudaMemcpyAsync(&timeouts, reinterpret_cast<char*>(ctx->d_state) + offsetof(DevState, rounds_timeouts),
-                                       sizeof timeouts, cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
-        if (timeouts != ctx->rounds_timeouts_seen) {  // this launch, or a _dev launch since the last check, gave up
-            ctx->rounds_timeouts_seen = timeouts;
-            std::snprintf(ctx->last_err, sizeof ctx->last_err,
-                          "EGPU_F_DEVICE_ROUNDS: a grid barrier waited more than 2 s and the launch gave up (%llu so far)", timeouts);
-            return EGPU_ERR_CUDA;
-        }
-        if (out_delta_core) std::memcpy(out_delta_core, ctx->h_delta, sizeof(int64_t) * D);
-        if (out_delta_mem) std::memcpy(out_delta_mem, ctx->h_delta + D, sizeof(int64_t) * D);
-        return EGPU_OK;
-    }
-    if (rounds) {  // packed rounds to the fixed point, staged through HBM: 4 bytes per row in, 1 out
-        long long total[2 * kMaxD];
-        rc = ensure_staging(ctx, R > 0 ? R : 1);
-        if (rc != EGPU_OK) return rc;
-        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-        rc = launch_packed_rounds(ctx, ctx->d_req_core, R, ctx->d_idx, nullptr, nullptr, total, s);
-        if (rc != EGPU_OK) return rc;
-        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, sizeof(int8_t) * R, cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
-        if (out_delta_core) std::memcpy(out_delta_core, total, sizeof(int64_t) * D);
-        if (out_delta_mem) std::memcpy(out_delta_mem, total + D, sizeof(int64_t) * D);
-        return EGPU_OK;
-    }
-    const int user_flags = (commit & EGPU_F_COMMIT) ? EGPU_F_COMMIT : 0;
-    // Zero-copy: when all three caller arrays are pinned (egpu_host_alloc or
+    const int user_flags = commit & EGPU_F_COMMIT;
+    // Zero-copy: when all three caller arrays of a snapshot are pinned (egpu_host_alloc or
     // cudaHostRegister) and 16-byte aligned, the scan reads the requests and writes
     // the indices straight across PCIe — one launch, no staging in HBM, reads and
     // writes overlap on the full-duplex link.  Demand sums land in pinned memory too.
-    const int32_t* zc = R > 0 && !prefix ? static_cast<const int32_t*>(mapped_alias(req_core)) : nullptr;
-    const int32_t* zm = R > 0 && !prefix ? static_cast<const int32_t*>(mapped_alias(req_mem)) : nullptr;
-    int32_t* zi = R > 0 && !prefix ? static_cast<int32_t*>(mapped_alias(out_idx)) : nullptr;
-    if (!prefix && zc && zm && zi && aligned16(zc) && aligned16(zm) && aligned16(zi) && !ctx->no_zero_copy) {
+    const bool mapped = R > 0 && op == kOpSnapshot;
+    const int32_t* zc = mapped ? static_cast<const int32_t*>(mapped_alias(req_core)) : nullptr;
+    const int32_t* zm = mapped ? static_cast<const int32_t*>(mapped_alias(req_mem)) : nullptr;
+    int32_t* zi = mapped ? static_cast<int32_t*>(mapped_alias(out_idx)) : nullptr;
+    if (zc && zm && zi && aligned16(zc) && aligned16(zm) && aligned16(zi) && !ctx->no_zero_copy) {
         // 64 rows per thread: few CTAs, many trips, so reads of later rows and writes of
         // earlier ones are on the link at the same time (PCIe is full duplex)
         Snapshot a{zc, zm, R, zi, ctx->h_delta_dev, nullptr, user_flags};
@@ -1663,24 +1530,43 @@ int egpu_bestfit_batch(egpu_ctx* ctx, const int32_t* req_core, const int32_t* re
         rc = launch_snapshot(ctx, a, s);
         if (rc != EGPU_OK) return rc;
         EGPU_CUDA(ctx, cudaStreamSynchronize(s));
-    } else {
-        rc = ensure_staging(ctx, R > 0 ? R : 1);
-        if (rc != EGPU_OK) return rc;
-        if (R > 0) {  // packed: 4 bytes per row in (the words, in d_req_core), 1 out
-            EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-            if (!packed) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-        }
-        rc = prefix ? launch_prefix_commit(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, user_flags, s,
-                                           packed ? kRowsPacked : kRowsInt32)
-                    : launch_snapshot(ctx, Snapshot{ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, ctx->d_delta, nullptr, user_flags}, s);
-        if (rc != EGPU_OK) return rc;
-        const size_t idx_bytes = packed ? sizeof(int8_t) : sizeof(int32_t);
-        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, idx_bytes * R, cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaStreamSynchronize(s));
+        sums_out(ctx, ctx->h_delta, out_delta_core, out_delta_mem);
+        return EGPU_OK;
     }
-    if (out_delta_core) std::memcpy(out_delta_core, ctx->h_delta, sizeof(int64_t) * D);
-    if (out_delta_mem) std::memcpy(out_delta_mem, ctx->h_delta + D, sizeof(int64_t) * D);
+    // Otherwise staged through HBM, per row int32 12 bytes in and 4 out (release: 12 in, nothing out), packed 4 in
+    // and 1 out (release: 5 in).  The packed rounds keep their sums on the host (d_delta NULL: no copy to the
+    // device); a release's table' carries the reason words of a refusal.
+    const bool release = op == kOpRelease;
+    const size_t idx_bytes = fmt == kRowsPacked ? sizeof(int8_t) : sizeof(int32_t);
+    rc = stage_in(ctx, s, R, req_core, req_mem, release ? out_idx : nullptr, idx_bytes);
+    if (rc != EGPU_OK) return rc;
+    long long total[2 * kMaxD];
+    rc = run_batch(ctx, op, fmt, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, op == kOpRounds ? nullptr : ctx->d_delta,
+                   release ? ctx->d_table_out : nullptr, user_flags, s, total);
+    if (rc != EGPU_OK) return rc;
+    rc = stage_out(ctx, s, R, release ? nullptr : out_idx, idx_bytes, op != kOpRounds);
+    if (rc != EGPU_OK) return rc;
+    if (release) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_table, ctx->d_table_out, sizeof(int32_t) * 3 * D, cudaMemcpyDeviceToHost, s));
+    unsigned long long timeouts = 0;
+    if (op == kOpDeviceRounds)
+        EGPU_CUDA(ctx, cudaMemcpyAsync(&timeouts, reinterpret_cast<char*>(ctx->d_state) + offsetof(DevState, rounds_timeouts),
+                                       sizeof timeouts, cudaMemcpyDeviceToHost, s));
+    EGPU_CUDA(ctx, cudaStreamSynchronize(s));
+    if (op == kOpDeviceRounds && timeouts != ctx->rounds_timeouts_seen) {  // this launch, or a _dev launch since the last check, gave up
+        ctx->rounds_timeouts_seen = timeouts;
+        std::snprintf(ctx->last_err, sizeof ctx->last_err,
+                      "EGPU_F_DEVICE_ROUNDS: a grid barrier waited more than 2 s and the launch gave up (%llu so far)", timeouts);
+        return EGPU_ERR_CUDA;
+    }
+    sums_out(ctx, op == kOpRounds ? total : ctx->h_delta, out_delta_core, out_delta_mem);
+    for (int d = 0; release && d < D; ++d) {
+        const int32_t reason = ctx->h_table[2 * D + d];
+        if (!reason) continue;
+        std::snprintf(ctx->last_err, sizeof ctx->last_err, "EGPU_F_RELEASE refused, nothing released: device %d %s", d,
+                      reason == EGPU_REL_FLAGGED ? "is oversubscribed (EGPU_REL_FLAGGED)"
+                                                 : "would hold more than the domain allows (EGPU_REL_EXCEEDS)");
+        return EGPU_ERR_STATE;
+    }
     return EGPU_OK;
 }
 
@@ -1688,27 +1574,22 @@ int egpu_bestfit_batch_rounds(egpu_ctx* ctx, const int32_t* req_core, const int3
                               int64_t* out_delta_core, int64_t* out_delta_mem, int32_t max_rounds, int32_t* out_rounds,
                               int64_t* out_deferred) {
     if (!ctx || R < 0 || R >= (1ll << 31) || max_rounds < 1) return EGPU_ERR_INVALID;
-    if (R > 0 && (!req_core || !req_mem || !out_idx)) return EGPU_ERR_INVALID;
+    if (!arrays_ok(kRowsInt32, R, req_core, req_mem, out_idx, false)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, nullptr, &s);
     if (rc != EGPU_OK) return rc;
-    rc = ensure_staging(ctx, R > 0 ? R : 1);
+    rc = stage_in(ctx, s, R, req_core, req_mem, nullptr, 0);
     if (rc != EGPU_OK) return rc;
-    if (R > 0) {
-        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_core, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_mem, req_mem, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
-    }
     long long total[2 * kMaxD];
     int32_t rounds = 0;
     int64_t left = 0;
     rc = run_rounds(ctx, ctx->d_req_core, ctx->d_req_mem, R, ctx->d_idx, max_rounds, total, &rounds, &left, s);
     if (rc != EGPU_OK) return rc;
-    if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx, ctx->d_idx, sizeof(int32_t) * R, cudaMemcpyDeviceToHost, s));
+    rc = stage_out(ctx, s, R, out_idx, sizeof(int32_t), false);
+    if (rc != EGPU_OK) return rc;
     EGPU_CUDA(ctx, cudaStreamSynchronize(s));
-    const int D = ctx->D;
-    if (out_delta_core) std::memcpy(out_delta_core, total, sizeof(int64_t) * D);
-    if (out_delta_mem) std::memcpy(out_delta_mem, total + D, sizeof(int64_t) * D);
+    sums_out(ctx, total, out_delta_core, out_delta_mem);
     if (out_rounds) *out_rounds = rounds;
     if (out_deferred) *out_deferred = left;
     return EGPU_OK;
@@ -1717,7 +1598,7 @@ int egpu_bestfit_batch_rounds(egpu_ctx* ctx, const int32_t* req_core, const int3
 int egpu_bestfit_batch_rounds_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
                                   int32_t* d_out_idx, int64_t* out_delta /* host [2*D] */, int32_t max_rounds,
                                   int32_t* out_rounds, int64_t* out_deferred, void* stream) {
-    if (!ctx || R < 0 || R >= (1ll << 31) || max_rounds < 1 || !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
+    if (!ctx || R < 0 || R >= (1ll << 31) || max_rounds < 1 || !arrays_ok(kRowsInt32, R, d_req_core, d_req_mem, d_out_idx))
         return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
@@ -1797,17 +1678,16 @@ int egpu_bestfit_batch_shard_dev(egpu_ctx* ctx, const int32_t* d_req_core, const
     // the commit happens in apply_peers; prefix-commit over shards has its own entry point;
     // step + 1 travels in 48 bits of the launch word.  EGPU_F_PACKED: words in d_req_core, d_req_mem
     // NULL, int8 indices (as in egpu_bestfit_batch_dev)
-    const bool packed = (flags & EGPU_F_PACKED) != 0;
+    const RowFormat fmt = row_format(flags);
     if (!ctx || R < 0 || (flags & ~(EGPU_F_INPUTS_READY | EGPU_F_PACKED)) || step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    if (packed ? (d_req_mem || !rows_ok(R, {d_req_core, d_out_idx})) : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
-        return EGPU_ERR_INVALID;
+    if (!arrays_ok(fmt, R, d_req_core, d_req_mem, d_out_idx)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
     Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), nullptr, flags};
     a.push_step_plus1 = step + 1;
-    a.packed = packed;
+    a.packed = fmt == kRowsPacked;
     return launch_snapshot(ctx, a, s);
 }
 
@@ -1818,7 +1698,7 @@ int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core
     // EGPU_F_INPUTS_READY: rounds to the fixed point over the shards, in one launch, on steps step and step + 1.
     // EGPU_F_RELEASE [| EGPU_F_COMMIT] [| EGPU_F_PACKED]: this rank's rows give back what they hold on d_out_idx
     // (read, never written), decided on every rank's sums, in one launch, on step `step`
-    const bool packed = (flags & EGPU_F_PACKED) != 0;
+    const RowFormat fmt = row_format(flags);
     const bool rounds = (flags & (EGPU_F_ROUNDS | EGPU_F_DEVICE_ROUNDS)) != 0;
     const bool release = (flags & EGPU_F_RELEASE) != 0;
     if (!ctx || R < 0 || step >= (1ull << 47)) return EGPU_ERR_INVALID;
@@ -1826,20 +1706,15 @@ int egpu_bestfit_batch_shard_prefix_dev(egpu_ctx* ctx, const int32_t* d_req_core
         : rounds ? (flags & ~EGPU_F_PACKED) != kDeviceRoundsNeeds || R >= (1ll << 31) || step + 2 > (1ull << 47)
                  : (flags & ~(EGPU_F_COMMIT | EGPU_F_PREFIX_COMMIT | EGPU_F_PACKED)) != 0)
         return EGPU_ERR_INVALID;
-    if (packed ? (d_req_mem || !rows_ok(R, {d_req_core, d_out_idx})) : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx}))
-        return EGPU_ERR_INVALID;
+    if (!arrays_ok(fmt, R, d_req_core, d_req_mem, d_out_idx)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
     if (rc != EGPU_OK) return rc;
-    if (release)
-        return launch_release(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out, flags, s,
-                              packed ? kRowsPacked : kRowsInt32, step + 1);
-    if (rounds)
-        return launch_shard_rounds(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out,
-                                   step, s, packed ? kRowsPacked : kRowsInt32);
-    return launch_prefix_commit_shard(ctx, d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta),
-                                      d_table_out, flags, step, s, packed ? kRowsPacked : kRowsInt32);
+    long long* delta = reinterpret_cast<long long*>(d_delta);
+    if (release) return launch_release(ctx, d_req_core, d_req_mem, R, d_out_idx, delta, d_table_out, flags, s, fmt, step + 1);
+    if (rounds) return launch_shard_rounds(ctx, egpu_batch{d_req_core, d_req_mem, R, d_out_idx, d_delta, d_table_out}, step, s, fmt);
+    return launch_prefix_commit_shard(ctx, d_req_core, d_req_mem, R, d_out_idx, delta, d_table_out, flags, step, s, fmt);
 }
 
 int egpu_bestfit_batch_shard_lag_dev(egpu_ctx* ctx, const int32_t* d_req_core, const int32_t* d_req_mem, int64_t R,
@@ -1847,9 +1722,9 @@ int egpu_bestfit_batch_shard_lag_dev(egpu_ctx* ctx, const int32_t* d_req_core, c
                                      int32_t* d_table_out_lagged, void* stream) {
     // This entry point never checked flags other than EGPU_F_COMMIT, so a call with EGPU_F_PACKED and
     // two int32 arrays has always run as int32 and still does: packed needs the flag AND a NULL d_req_mem.
-    const bool packed = (flags & EGPU_F_PACKED) && !d_req_mem;
+    const RowFormat fmt = (flags & EGPU_F_PACKED) && !d_req_mem ? kRowsPacked : kRowsInt32;
     if (!ctx || R < 0 || (flags & EGPU_F_COMMIT) || lag < 1 || lag > 16 || step >= (1ull << 47)) return EGPU_ERR_INVALID;
-    if (packed ? !rows_ok(R, {d_req_core, d_out_idx}) : !rows_ok(R, {d_req_core, d_req_mem, d_out_idx})) return EGPU_ERR_INVALID;
+    if (!arrays_ok(fmt, R, d_req_core, d_req_mem, d_out_idx)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsPeers, stream, &s);
@@ -1857,7 +1732,7 @@ int egpu_bestfit_batch_shard_lag_dev(egpu_ctx* ctx, const int32_t* d_req_core, c
     Snapshot a{d_req_core, d_req_mem, R, d_out_idx, reinterpret_cast<long long*>(d_delta), d_table_out_lagged, flags};
     a.push_step_plus1 = step + 1;
     a.lag = lag;
-    a.packed = packed;
+    a.packed = fmt == kRowsPacked;
     return launch_snapshot(ctx, a, s);
 }
 
@@ -1897,7 +1772,7 @@ int64_t egpu_peer_last_timeout(egpu_ctx* ctx) {
 
 int egpu_bestfit_batch_packed_dev(egpu_ctx* ctx, const uint32_t* d_req_packed, int64_t R, int8_t* d_out_idx8,
                                   int64_t* d_delta, int32_t* d_table_out, int flags, void* stream) {
-    if (!ctx || R < 0 || !rows_ok(R, {d_req_packed, d_out_idx8})) return EGPU_ERR_INVALID;
+    if (!ctx || R < 0 || !arrays_ok(kRowsPacked, R, d_req_packed, nullptr, d_out_idx8)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     const int rc = enter(ctx, kNeedsTable, stream, &s);
@@ -1918,13 +1793,11 @@ int egpu_bestfit_batch_packed_dev(egpu_ctx* ctx, const uint32_t* d_req_packed, i
 
 int egpu_bestfit_batch_packed(egpu_ctx* ctx, const uint32_t* req_packed, int64_t R, int8_t* out_idx8,
                               int64_t* out_delta_core, int64_t* out_delta_mem, int commit) {
-    if (!ctx || R < 0) return EGPU_ERR_INVALID;
-    if (R > 0 && (!req_packed || !out_idx8)) return EGPU_ERR_INVALID;
+    if (!ctx || R < 0 || !arrays_ok(kRowsPacked, R, req_packed, nullptr, out_idx8, false)) return EGPU_ERR_INVALID;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaStream_t s;
     int rc = enter(ctx, kNeedsTable, nullptr, &s);
     if (rc != EGPU_OK) return rc;
-    const int D = ctx->D;
     const uint32_t* zr = R > 0 ? static_cast<const uint32_t*>(mapped_alias(req_packed)) : nullptr;
     signed char* zi = R > 0 ? static_cast<signed char*>(mapped_alias(out_idx8)) : nullptr;
     if (zr && zi && aligned16(zr) && aligned16(zi) && !ctx->no_zero_copy) {  // zero-copy across PCIe, see egpu_bestfit_batch
@@ -1932,18 +1805,16 @@ int egpu_bestfit_batch_packed(egpu_ctx* ctx, const uint32_t* req_packed, int64_t
         if (rc != EGPU_OK) return rc;
         EGPU_CUDA(ctx, cudaStreamSynchronize(s));
     } else {
-        rc = ensure_staging(ctx, R > 0 ? R : 1);  // d_req_core holds the packed words, d_idx the bytes
+        rc = stage_in(ctx, s, R, req_packed, nullptr, nullptr, 0);  // d_req_core holds the packed words, d_idx the bytes
         if (rc != EGPU_OK) return rc;
-        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->d_req_core, req_packed, sizeof(uint32_t) * R, cudaMemcpyHostToDevice, s));
         rc = launch_packed(ctx, reinterpret_cast<const uint32_t*>(ctx->d_req_core), R, reinterpret_cast<signed char*>(ctx->d_idx),
                            ctx->d_delta, nullptr, commit ? EGPU_F_COMMIT : 0, s, 16);
         if (rc != EGPU_OK) return rc;
-        if (R > 0) EGPU_CUDA(ctx, cudaMemcpyAsync(out_idx8, ctx->d_idx, static_cast<size_t>(R), cudaMemcpyDeviceToHost, s));
-        EGPU_CUDA(ctx, cudaMemcpyAsync(ctx->h_delta, ctx->d_delta, sizeof(long long) * 2 * D, cudaMemcpyDeviceToHost, s));
+        rc = stage_out(ctx, s, R, out_idx8, sizeof(int8_t), true);
+        if (rc != EGPU_OK) return rc;
         EGPU_CUDA(ctx, cudaStreamSynchronize(s));
     }
-    if (out_delta_core) std::memcpy(out_delta_core, ctx->h_delta, sizeof(int64_t) * D);
-    if (out_delta_mem) std::memcpy(out_delta_mem, ctx->h_delta + D, sizeof(int64_t) * D);
+    sums_out(ctx, ctx->h_delta, out_delta_core, out_delta_mem);
     return EGPU_OK;
 }
 

@@ -13,32 +13,25 @@
 
 using namespace egpu;  // internal header: the context is made of the kernels' types
 
-// The scan kernels the launchers of egpu_alloc.cu choose from, one per D bucket (D <= 8, 16, 32, 64)
+// The scan kernels the launchers of egpu_alloc.cu choose from, one per D bucket (D <= 8, 16, 32, 64) ...
 enum ScanFamily {
     kScanSorted, kScanSortedContig, kScanGrid, kScanLut, kScanLutContig, kScanSortedMulti, kScanLutMulti, kScanPacked,
     kScanFamilies
 };
-// The packed multi-batch kernels (egpu_bestfit_batches_dev with EGPU_F_PACKED), one per D bucket as well
-enum PackedFamily { kPackedSortedMulti, kPackedLutMulti, kPackedFamilies };
-// The packed prefix-commit scans (CONTIG tiles; egpu_bestfit_batch[_dev] with EGPU_F_PACKED), per D bucket
-enum PackedContigFamily { kPackedSortedContig, kPackedLutContig, kPackedContigFamilies };
-// The packed sharded scans (round-robin tiles; egpu_bestfit_batch_shard[_lag]_dev with EGPU_F_PACKED), per D bucket
-enum PackedSnapFamily { kPackedSortedSnap, kPackedLutSnap, kPackedSnapFamilies };
-// The one-launch rounds (EGPU_F_DEVICE_ROUNDS), per row format and D bucket
-enum DeviceRoundsFamily { kRoundsSorted, kRoundsLut, kRoundsFamilies };
+// ... and the kernels of the other launches, numbered on from them.  A family has a table per row format
+// (RowFormat), one kernel per D bucket, and every such kernel its own entry in egpu_ctx::ctas_per_sm.
+enum LaunchFamily {
+    kRoundsSorted = kScanFamilies, kRoundsLut,  // EGPU_F_DEVICE_ROUNDS, one batch
+    kRoundsMultiSorted, kRoundsMultiLut,         // ... K batches (egpu_bestfit_batches_dev)
+    kShardPrefixSorted, kShardPrefixLut,         // EGPU_F_PREFIX_COMMIT on egpu_bestfit_batches_shard_dev
+    kShardRoundsSorted, kShardRoundsLut,         // EGPU_F_DEVICE_ROUNDS on egpu_bestfit_batch_shard_prefix_dev
+    kRelease, kReleaseShard,                     // EGPU_F_RELEASE, one GPU and over row shards
+    kKernelFamilies
+};
 
 struct egpu_ctx {
     std::mutex mu;
-    int scan_ctas_per_sm[kScanFamilies][4] = {};  // resident CTAs per SM of each scan kernel, 0 = not asked yet
-    int packed_ctas_per_sm[kPackedFamilies][4] = {};  // ... and of each packed multi-batch kernel
-    int packed_contig_ctas_per_sm[kPackedContigFamilies][4] = {};  // ... and of each packed prefix-commit scan
-    int packed_snap_ctas_per_sm[kPackedSnapFamilies][4] = {};  // ... and of each packed sharded scan
-    int rounds_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each one-launch rounds kernel ([family][packed][bucket])
-    int rounds_multi_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each multi-batch one-launch rounds kernel
-    int shard_prefix_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each multi-batch sharded prefix-commit kernel
-    int shard_rounds_ctas_per_sm[kRoundsFamilies][2][4] = {};  // ... and of each sharded one-launch rounds kernel
-    int release_ctas_per_sm[2][4] = {};  // ... and of each release kernel ([packed][bucket])
-    int release_shard_ctas_per_sm[2][4] = {};  // ... and of each sharded release kernel ([packed][bucket])
+    int ctas_per_sm[kKernelFamilies * 2 * 4] = {};  // resident CTAs per SM of each kernel (Kernel::slot), 0 = not asked yet
     void* h_qtable = nullptr;        // pinned host image of that table (the part of DevState before `peer`)
     DevState* d_qstate = nullptr;     // scratch table of egpu_bestfit_query (the context's own table is not touched)
     unsigned long long* h_gate = nullptr;      // pinned: start gates the host has opened (egpu_peer_gate_open)

@@ -1,7 +1,7 @@
 """Every scan kernel the launch table can select, against a plain reference of the same operation.
 
-The snapshot scans are one kernel per (family, D bucket): `kKernels<family>[d_bucket(D)]` in
-csrc/egpu_alloc.cu, 8 families x 4 buckets (D <= 8, 16, 32, 64).  This file drives each cell through the
+The snapshot scans are one kernel per (family, D bucket): `kKernels<family, format>[d_bucket(D)]` in
+csrc/egpu_alloc.cu (this file: the int32 tables, and kScanPacked's), 8 families x 4 buckets (D <= 8, 16, 32, 64).  This file drives each cell through the
 entry point that selects it, at the D values on both sides of every bucket edge, and the grid-sizing
 rules of the launchers at their thresholds:
 

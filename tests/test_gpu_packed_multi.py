@@ -2,8 +2,8 @@
 
 Every batch's d_req_core holds packed words (EGPU_PACK_REQUEST: core << 18 | mem; a word >= 2^25 is
 not a request), d_req_mem is NULL and d_out_idx receives int8 indices.  The launch runs the packed
-twins of the multi-batch kernels (csrc/egpu_alloc.cu: kPackedKernels<family>[d_bucket(D)], the
-register scan and the lookup scan).  Each GPU case compares every batch exactly with
+twins of the multi-batch kernels (csrc/egpu_alloc.cu: kKernels<kScanSortedMulti or kScanLutMulti,
+kRowsPacked>[d_bucket(D)], the register scan and the lookup scan).  Each GPU case compares every batch exactly with
 oracle/bestfit_np.py or the C oracle on the requests the words stand for, and, where it says so, with a
 non-committing egpu_bestfit_batch_packed_dev call on the same words:
 
@@ -40,7 +40,14 @@ GUARD = 16  # guard bytes after every int8 index array
 
 # ---- the packed kernel table -------------------------------------------------------------------------
 PACKED_FAMILIES = ("sorted", "lut")
-PACKED_ENUM = ("kPackedSortedMulti", "kPackedLutMulti")
+PACKED_TWINS = {"kScanSortedMulti": "bestfit_sorted_packed_multi_kernel", "kScanLutMulti": "bestfit_lut_packed_multi_kernel"}
+
+
+def packed_twins(kind):
+    """{scan family: its packed twin kernel} of family_kernel() (csrc/egpu_alloc.cu), for the twins named *_packed_<kind>_kernel"""
+    src = open(os.path.join(CSRC, "egpu_alloc.cu")).read()
+    twins = dict(re.findall(r"F == (kScan\w+)\) return kernel\(P \? (\w+)<", src))
+    return {f: k for f, k in twins.items() if k.endswith(f"_packed_{kind}_kernel")}
 
 
 def family(variant, D):
@@ -51,11 +58,10 @@ def family(variant, D):
 CELLS = [(v, D) for v in (AUTO, SORTED, LUT) for D in km.D_ALL]
 
 
-def test_matrix_covers_every_packed_cell():
-    src = open(os.path.join(CSRC, "egpu_ctx.h")).read()
-    enum = re.search(r"enum PackedFamily \{(.*?)\};", src, re.S).group(1)
-    names = [n.strip() for n in enum.split(",") if n.strip()]
-    assert names[-1] == "kPackedFamilies" and tuple(names[:-1]) == PACKED_ENUM
+def test_packed_multi_twins_cover_every_cell():
+    """the packed twins of the multi-batch scans in the kernel table, and a matrix cell for each of their buckets"""
+    twins = packed_twins("multi")
+    assert twins == PACKED_TWINS and tuple(k.split("_")[1] for k in twins.values()) == PACKED_FAMILIES
     want = {(f, b) for f in PACKED_FAMILIES for b in range(len(km.BUCKET_TOPS))}
     assert {(family(v, D), km.d_bucket(D)) for v, D in CELLS} == want
     for v in (SORTED, LUT):  # every variant reaches every bucket

@@ -2,7 +2,7 @@
 
 The request array holds packed words (EGPU_PACK_REQUEST: core << 18 | mem; a word >= 2^25 is not a
 request), req_mem is NULL and the indices are int8.  The call runs the packed twins of the CONTIG scans
-(csrc/egpu_alloc.cu: kPackedContigKernels<family>[d_bucket(D)]), then prefix_cut_packed_kernel,
+(csrc/egpu_alloc.cu: kKernels<kScanSortedContig or kScanLutContig, kRowsPacked>[d_bucket(D)]), then prefix_cut_packed_kernel,
 prefix_apply_packed_kernel and prefix_finalize_kernel.  Every case compares exactly with
 oracle/bestfit_np.py or the C oracle on the requests the words stand for (not a request: (-1, -1)), and
 most also with the int32 prefix-commit of egpu_bestfit_batch_dev on the same requests:
@@ -20,7 +20,6 @@ most also with the int32 prefix-commit of egpu_bestfit_batch_dev on the same req
 """
 import ctypes as C
 import os
-import re
 import sys
 import zlib
 
@@ -36,15 +35,14 @@ MEM_MAX = (1 << 18) - 1
 ERR_INVALID, ERR_STATE = -1, -6
 AUTO, GRID, SORTED, LUT = 0, 1, 2, 3
 F_COMMIT, F_INPUTS_READY, F_PREFIX, F_PACKED = 1, 2, 4, 16
-PACKED_CONTIG_ENUM = ("kPackedSortedContig", "kPackedLutContig")
+PACKED_CONTIG_TWINS = {"kScanSortedContig": "bestfit_sorted_packed_contig_kernel", "kScanLutContig": "bestfit_lut_packed_contig_kernel"}
 CELLS = pm.CELLS
 
 
-def test_matrix_covers_every_packed_contig_cell():
-    src = open(os.path.join(pm.CSRC, "egpu_ctx.h")).read()
-    enum = re.search(r"enum PackedContigFamily \{(.*?)\};", src, re.S).group(1)
-    names = [n.strip() for n in enum.split(",") if n.strip()]
-    assert names[-1] == "kPackedContigFamilies" and tuple(names[:-1]) == PACKED_CONTIG_ENUM
+def test_packed_contig_twins_cover_every_cell():
+    """the packed twins of the CONTIG scans in the kernel table, and a matrix cell for each of their buckets"""
+    twins = pm.packed_twins("contig")
+    assert twins == PACKED_CONTIG_TWINS and tuple(k.split("_")[1] for k in twins.values()) == pm.PACKED_FAMILIES
     want = {(f, b) for f in pm.PACKED_FAMILIES for b in range(len(km.BUCKET_TOPS))}
     assert {(pm.family(v, D), km.d_bucket(D)) for v, D in CELLS} == want
 

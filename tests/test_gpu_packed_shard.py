@@ -2,8 +2,8 @@
 and egpu_bestfit_batch_shard_prefix_dev.
 
 d_req_core holds packed words (EGPU_PACK_REQUEST: core << 18 | mem; a word >= 2^25 is not a request), d_req_mem is
-NULL and the indices are int8.  The sharded scans run kPackedSnapKernels<family>[d_bucket(D)] (csrc/egpu_alloc.cu),
-the round-robin packed twins of the single-batch scans with the push and lag epilogue; the sharded prefix-commit
+NULL and the indices are int8.  The sharded scans run kKernels<kScanSorted or kScanLut, kRowsPacked>[d_bucket(D)]
+(csrc/egpu_alloc.cu), the round-robin packed twins of the single-batch scans with the push and lag epilogue; the sharded prefix-commit
 runs the packed CONTIG scans, prefix_cut_packed_shard_kernel and prefix_apply_packed_kernel.  The exchange is the
 int32 one.  Every case compares exactly with oracle/bestfit_np.py or the C oracle on the requests the words stand for
 (not a request: (-1, -1)), and where it says so with the int32 call on the same requests:
@@ -23,7 +23,6 @@ int32 one.  Every case compares exactly with oracle/bestfit_np.py or the C oracl
 """
 import ctypes as C
 import os
-import re
 import sys
 
 import numpy as np
@@ -45,10 +44,11 @@ SHARD_ROWS = (0, 1, 3, 5, 511, 513, 4099)
 CELLS = pm.CELLS
 
 
-def test_packed_snap_enum():
-    src = open(os.path.join(pm.CSRC, "egpu_ctx.h")).read()
-    enum = re.search(r"enum PackedSnapFamily \{(.*?)\};", src, re.S).group(1)
-    assert [n.strip() for n in enum.split(",") if n.strip()] == ["kPackedSortedSnap", "kPackedLutSnap", "kPackedSnapFamilies"]
+def test_packed_snap_twins():
+    """the packed twins of the round-robin scans in the kernel table, and a cell for each of their families"""
+    twins = pm.packed_twins("snap")
+    assert twins == {"kScanSorted": "bestfit_sorted_packed_snap_kernel", "kScanLut": "bestfit_lut_packed_snap_kernel"}
+    assert tuple(k.split("_")[1] for k in twins.values()) == pm.PACKED_FAMILIES
     assert {pm.family(v, D) for v, D in CELLS} == {"sorted", "lut"}
 
 

@@ -1,8 +1,8 @@
 """egpu_bestfit_batch_packed_dev on the snapshot launch path.
 
 The call scores R packed words (EGPU_PACK_REQUEST: core << 18 | mem; a word >= 2^25 is not a request) into R int8
-indices.  Outside the grid variant it runs kPackedSnapKernels<family>[d_bucket(D)] (csrc/egpu_alloc.cu), the
-round-robin packed scans of the sharded calls, in the scan the context's variant selects, and pipelines under
+indices.  Outside the grid variant it runs kKernels<kScanSorted or kScanLut, kRowsPacked>[d_bucket(D)]
+(csrc/egpu_alloc.cu), the round-robin packed scans of the sharded calls, in the scan the context's variant selects, and pipelines under
 EGPU_F_INPUTS_READY with the other scans of the context; under EGPU_VARIANT_GRID it keeps the warp-chunk scan of
 egpu_bestfit_batch_packed.  Every case compares exactly with the C oracle on the requests the words stand for (not a
 request: (-1, -1)), and where it says so with the int32 egpu_bestfit_batch_dev on the same requests:
