@@ -236,4 +236,76 @@ __device__ __forceinline__ int32_t sat_i32(long long v) {
     return v > 2147483647LL ? 2147483647 : (v < -2147483648LL ? static_cast<int32_t>(-2147483648LL) : static_cast<int32_t>(v));
 }
 
+// --- grid barrier of the one-launch rounds (cooperative launches) ----------------------------------------------
+constexpr unsigned long long kRoundsBarrierTimeoutNs = 2000000000ull;  // the ~2 s bound of every device wait
+
+// Grid-barrier words of a rounds launch: the context's rounds scratch (zero when allocated, and every launch
+// leaves them zero except gen, which only counts up), or the scratch of egpu::place_tables (zeroed before
+// every launch).
+struct RoundsCtl {
+    unsigned int arrive;  // CTAs at the current barrier
+    unsigned int gen;     // barriers completed: the word a waiting CTA watches
+    unsigned int abort;   // a CTA gave up waiting: every CTA leaves at its next barrier
+    unsigned int exited;  // CTAs that have left the launch; the last one re-zeroes arrive, abort and exited
+};
+
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+// Grid-wide barrier.  Thread 0 of each CTA releases the CTA's writes and arrives; the last to arrive
+// re-arms the counter and publishes the next generation, the others spin on it with acquire loads.
+// A spin gives up after ~2 s: the first CTA to give up counts the timeout in *timeouts (a context's
+// DevState::rounds_timeouts) and raises ctl->abort, and from then on every barrier returns false (the
+// caller leaves).  `gen` is thread 0's copy of the generation.
+__device__ __forceinline__ bool grid_barrier(RoundsCtl* ctl, unsigned long long* timeouts, unsigned int& gen, int* sOk) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        bool ok = true;
+        fence_acq_rel_gpu();  // release: this CTA's writes, ordered before thread 0 by the CTA barrier
+        if (atomicAdd(&ctl->arrive, 1u) == gridDim.x - 1) {
+            atomicExch(&ctl->arrive, 0u);
+            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(&ctl->gen), "r"(gen + 1) : "memory");
+        } else {
+            const unsigned long long t0 = globaltimer_ns();
+            for (;;) {
+                unsigned int g;
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(g) : "l"(&ctl->gen) : "memory");
+                if (g != gen) break;
+                if (*reinterpret_cast<volatile unsigned int*>(&ctl->abort)) {
+                    ok = false;
+                    break;
+                }
+                if (globaltimer_ns() - t0 > kRoundsBarrierTimeoutNs) {
+                    if (atomicExch(&ctl->abort, 1u) == 0u) atomicAdd(timeouts, 1ull);
+                    ok = false;
+                    break;
+                }
+                __nanosleep(32);
+            }
+        }
+        gen += 1;
+        fence_acq_rel_gpu();  // acquire: the other CTAs' writes before their arrivals
+        if (*reinterpret_cast<volatile unsigned int*>(&ctl->abort)) ok = false;
+        *sOk = ok;
+    }
+    __syncthreads();
+    return *sOk != 0;
+}
+
+// A CTA leaves the launch; the last one re-arms the barrier words for the next launch.
+__device__ __forceinline__ void rounds_exit(RoundsCtl* ctl) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        fence_acq_rel_gpu();
+        if (atomicAdd(&ctl->exited, 1u) == gridDim.x - 1) {
+            *reinterpret_cast<volatile unsigned int*>(&ctl->arrive) = 0u;
+            *reinterpret_cast<volatile unsigned int*>(&ctl->abort) = 0u;
+            *reinterpret_cast<volatile unsigned int*>(&ctl->exited) = 0u;
+        }
+    }
+}
+
 }  // namespace egpu

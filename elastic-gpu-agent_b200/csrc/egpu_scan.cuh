@@ -1932,16 +1932,6 @@ round_writeback_packed_kernel(const signed char* __restrict__ idx_k, const int32
 // Everything a phase reads that another CTA wrote in this launch is read with coherent loads
 // (kLoadCoherent scans, plain or .cg loads elsewhere; never the non-coherent path).
 constexpr int kRoundsThreads = 256;
-constexpr unsigned long long kRoundsBarrierTimeoutNs = 2000000000ull;  // the ~2 s bound of every device wait
-
-// Grid-barrier words of a rounds launch, in the context's rounds scratch.  Zero when allocated, and
-// every launch leaves them zero (except gen, which only counts up).
-struct RoundsCtl {
-    unsigned int arrive;  // CTAs at the current barrier
-    unsigned int gen;     // barriers completed: the word a waiting CTA watches
-    unsigned int abort;   // a CTA gave up waiting: every CTA leaves at its next barrier
-    unsigned int exited;  // CTAs that have left the launch; the last one re-zeroes arrive, abort and exited
-};
 
 struct RoundsArgs {
     const int32_t* rc;             // round 1: the caller's rows (packed: the words)
@@ -1959,65 +1949,6 @@ struct RoundsArgs {
     RoundsCtl* ctl;
     DevLut* lut;                   // lookup kernels: rebuilt at the start and after every commit
 };
-
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
-// Grid-wide barrier.  Thread 0 of each CTA releases the CTA's writes and arrives; the last to arrive
-// re-arms the counter and publishes the next generation, the others spin on it with acquire loads.
-// A spin gives up after ~2 s: the first CTA to give up counts the timeout in DevState::rounds_timeouts
-// and raises ctl->abort, and from then on every barrier returns false (the caller leaves).  `gen` is
-// thread 0's copy of the generation.
-__device__ __forceinline__ bool grid_barrier(RoundsCtl* ctl, DevState* st, unsigned int& gen, int* sOk) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        bool ok = true;
-        fence_acq_rel_gpu();  // release: this CTA's writes, ordered before thread 0 by the CTA barrier
-        if (atomicAdd(&ctl->arrive, 1u) == gridDim.x - 1) {
-            atomicExch(&ctl->arrive, 0u);
-            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(&ctl->gen), "r"(gen + 1) : "memory");
-        } else {
-            const unsigned long long t0 = globaltimer_ns();
-            for (;;) {
-                unsigned int g;
-                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(g) : "l"(&ctl->gen) : "memory");
-                if (g != gen) break;
-                if (*reinterpret_cast<volatile unsigned int*>(&ctl->abort)) {
-                    ok = false;
-                    break;
-                }
-                if (globaltimer_ns() - t0 > kRoundsBarrierTimeoutNs) {
-                    if (atomicExch(&ctl->abort, 1u) == 0u) atomicAdd(&st->rounds_timeouts, 1ull);
-                    ok = false;
-                    break;
-                }
-                __nanosleep(32);
-            }
-        }
-        gen += 1;
-        fence_acq_rel_gpu();  // acquire: the other CTAs' writes before their arrivals
-        if (*reinterpret_cast<volatile unsigned int*>(&ctl->abort)) ok = false;
-        *sOk = ok;
-    }
-    __syncthreads();
-    return *sOk != 0;
-}
-
-// A CTA leaves the launch; the last one re-arms the barrier words for the next launch.
-__device__ __forceinline__ void rounds_exit(RoundsCtl* ctl) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        fence_acq_rel_gpu();
-        if (atomicAdd(&ctl->exited, 1u) == gridDim.x - 1) {
-            *reinterpret_cast<volatile unsigned int*>(&ctl->arrive) = 0u;
-            *reinterpret_cast<volatile unsigned int*>(&ctl->abort) = 0u;
-            *reinterpret_cast<volatile unsigned int*>(&ctl->exited) = 0u;
-        }
-    }
-}
 
 // Per-device sums of tile `tile` from the per-warp sums in shared memory (the layout of
 // epilogue_publish), for the cut.  Called by all threads after a __syncthreads().
@@ -2107,7 +2038,7 @@ __device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Sc
         // see the host's bookkeeping): build it from the table as it is now
         if constexpr (LUT) lut_build_cta(st, a.lut);
     }
-    if constexpr (LUT) ok = grid_barrier(a.ctl, st, gen, &sOk);
+    if constexpr (LUT) ok = grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk);
     const int32_t* rc = a.rc;
     const int32_t* rm = a.rm;
     const int32_t* map = nullptr;
@@ -2117,10 +2048,10 @@ __device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Sc
     [[maybe_unused]] int k = 0;  // MULTI: the batch these rounds place
     while (ok) {
         scan(rc, rm, n, idx, b, G);  // 1
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         if (static_cast<int>(b) < D)  // 2
             prefix_cut_cta<FMT>(st, idx, rc, rm, n, static_cast<int>(G), a.tile_sums, a.pf, nullptr);
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         if constexpr (FMT == kRowsPacked)  // 3
             prefix_apply_packed_rows(a.pf, D, n, reinterpret_cast<signed char*>(idx));
         else
@@ -2136,16 +2067,16 @@ __device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Sc
                 lut_build_cta(st, a.lut);
             }
         }
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         if (map) round_writeback_rows<FMT>(idx, map, n, MULTI ? list[k].idx : a.idx);  // 4
         const long long tiles = (n + kCompactTile - 1) / kCompactTile;
         for (long long t = b; t < tiles; t += G) {
             deferred_count_cta<FMT>(idx, n, a.tile_count, static_cast<unsigned int>(t));
             __syncthreads();
         }
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         if (b == 0) tile_offsets_cta(a.tile_count, tiles, a.deferred);  // 5
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         const unsigned long long left = __ldcg(a.deferred);
         if (left == 0) {
             if constexpr (MULTI) {
@@ -2176,7 +2107,7 @@ __device__ __forceinline__ void rounds_cta(DevState* st, const RoundsArgs& a, Sc
             deferred_scatter_cta<FMT>(idx, rc, rm, map, n, a.tile_count, n_rc, n_rm, n_map, static_cast<unsigned int>(t));
             __syncthreads();
         }
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         rc = n_rc;
         rm = n_rm;
         map = n_map;
@@ -2337,12 +2268,12 @@ __device__ __forceinline__ void shard_prefix_cta(DevState* st, const ShardPrefix
         }
     };
     bool ok = true;
-    if constexpr (LUT) ok = grid_barrier(a.ctl, st, gen, &sOk);
+    if constexpr (LUT) ok = grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk);
     for (int k = 0; ok && k < a.K; ++k) {
         const RoundsBatch& in = a.b[k];
         const unsigned long long push = a.first_step_plus1 + 2ull * static_cast<unsigned long long>(k);
         scan(in.rc, in.rm, in.R, in.idx, b, G);  // 1
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) {
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) {
             defer_tile(in);
             break;
         }
@@ -2372,7 +2303,7 @@ __device__ __forceinline__ void shard_prefix_cta(DevState* st, const ShardPrefix
             prefix_cut_cta<FMT>(st, in.idx, in.rc, in.rm, in.R, static_cast<int>(G), a.tile_sums, a.pf, sBase);
         }
         // a base pull that gave up raised the stop word before its CTA arrived: every CTA that passes sees it
-        if (!grid_barrier(a.ctl, st, gen, &sOk) || *reinterpret_cast<volatile unsigned int*>(a.stop)) {
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk) || *reinterpret_cast<volatile unsigned int*>(a.stop)) {
             defer_tile(in);
             break;
         }
@@ -2393,7 +2324,7 @@ __device__ __forceinline__ void shard_prefix_cta(DevState* st, const ShardPrefix
                 atomicExch(a.stop, 1u);
             }
         }
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         if (*reinterpret_cast<volatile unsigned int*>(a.stop)) break;
     }
     rounds_exit(a.ctl);
@@ -2526,7 +2457,7 @@ __device__ __forceinline__ void shard_rounds_cta(DevState* st, const ShardRounds
         }
     };
     bool ok = true;
-    if constexpr (LUT) ok = grid_barrier(a.ctl, st, gen, &sOk);
+    if constexpr (LUT) ok = grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk);
     const int32_t* rc = a.rc;
     const int32_t* rm = a.rm;
     const int32_t* map = nullptr;  // nullptr in round 1: the rows are the caller's own
@@ -2536,7 +2467,7 @@ __device__ __forceinline__ void shard_rounds_cta(DevState* st, const ShardRounds
     while (ok) {
         if (b == 0 && tid == 0) *again = 0u;
         scan(rc, rm, n, idx, b, G);  // 1
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) {
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) {
             if (!map) defer_tile();
             break;
         }
@@ -2568,7 +2499,7 @@ __device__ __forceinline__ void shard_rounds_cta(DevState* st, const ShardRounds
             __syncthreads();
             prefix_cut_cta<FMT>(st, idx, rc, rm, n, static_cast<int>(G), a.tile_sums, a.pf, sBase);
         }
-        if (!grid_barrier(a.ctl, st, gen, &sOk) || *stop) {
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk) || *stop) {
             if (!map) defer_tile();
             break;
         }
@@ -2592,7 +2523,7 @@ __device__ __forceinline__ void shard_rounds_cta(DevState* st, const ShardRounds
                 atomicExch(s.stop, 1u);
             }
         }
-        if (!grid_barrier(a.ctl, st, gen, &sOk) || *stop) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk) || *stop) break;
         if (map) round_writeback_rows<FMT>(idx, map, n, a.idx);  // 4
         if (last) {
             if (b == 0 && a.delta_out && tid < 2 * D) a.delta_out[tid] = a.total[tid];
@@ -2603,9 +2534,9 @@ __device__ __forceinline__ void shard_rounds_cta(DevState* st, const ShardRounds
             deferred_count_cta<FMT>(idx, n, a.tile_count, static_cast<unsigned int>(t));
             __syncthreads();
         }
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         if (b == 0) tile_offsets_cta(a.tile_count, tiles, a.deferred);  // 5
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         const unsigned long long left = __ldcg(a.deferred);
         int32_t* const n_rc = which ? a.set[1][0] : a.set[0][0];  // 6
         int32_t* const n_rm = which ? a.set[1][1] : a.set[0][1];
@@ -2615,7 +2546,7 @@ __device__ __forceinline__ void shard_rounds_cta(DevState* st, const ShardRounds
             deferred_scatter_cta<FMT>(idx, rc, rm, map, n, a.tile_count, n_rc, n_rm, n_map, static_cast<unsigned int>(t));
             __syncthreads();
         }
-        if (!grid_barrier(a.ctl, st, gen, &sOk)) break;
+        if (!grid_barrier(a.ctl, &st->rounds_timeouts, gen, &sOk)) break;
         rc = n_rc;
         rm = n_rm;
         map = n_map;

@@ -12,12 +12,50 @@
 #include "egpu_kernels.cuh"
 #include "egpu_tables.h"
 
+#include <algorithm>
+#include <atomic>
+
 namespace egpu {
 
 constexpr int kTabWarps = 8;  // tables per CTA
 constexpr int kTabThreads = kTabWarps * 32;
 constexpr int kTabStep = 4 * 32;       // requests one warp scores per step
 constexpr uint32_t kNoKey = 0x7fffffffu;  // the key of "no feasible device"
+
+// Warp-level rank sort of one table's first dv rows by (fc, fm, d), as resort_table_cta sorts a context's table.
+// sK[pos] = the packed compare word (kPadWord past the rows); sBase[pos] = fc << 24 | fm << 6 | d, and kNoKey at
+// every position that is no row, including "none" (32 for DT <= 32, 64 for DT = 64).  A table outside §2.1's
+// domain (dv not in [1, D], or a row value out of range) gets no rows; dv is not read past D.  COHERENT: the table
+// may have been written earlier in the same launch by another CTA, so it is read from L2.  Returns the rows.
+template <int DT, bool COHERENT>
+__device__ __forceinline__ int sort_table_warp(const int32_t* fc_row, const int32_t* fm_row, int dv, int D, uint32_t* sK,
+                                               uint32_t* sBase, uint32_t* sRank) {
+    const int lane = threadIdx.x & 31;
+    bool ok = dv >= 1 && dv <= D;
+    for (int j = lane; j < DT; j += 32) {
+        uint32_t rank = 0xffffffffu;
+        if (ok && j < dv) {
+            const int32_t c = COHERENT ? __ldcg(fc_row + j) : fc_row[j], m = COHERENT ? __ldcg(fm_row + j) : fm_row[j];
+            if (c < 0 || c > kCoreMax || m < 0 || m > kMemMax) ok = false;
+            rank = (static_cast<uint32_t>(c) << 24) | (static_cast<uint32_t>(m) << 6) | static_cast<uint32_t>(j);
+        }
+        sRank[j] = rank;
+        sK[j] = kPadWord;
+    }
+    for (int j = lane; j <= kMaxD; j += 32) sBase[j] = kNoKey;
+    const int rows = __all_sync(0xffffffffu, ok) ? dv : 0;
+    __syncwarp();
+    for (int j = lane; j < rows; j += 32) {
+        const uint32_t mine = sRank[j];
+        int pos = 0;
+        for (int k = 0; k < rows; ++k) pos += sRank[k] < mine;
+        sK[pos] = pack_table_word(static_cast<int32_t>(mine >> 24), static_cast<int32_t>((mine >> 6) & 0x3FFFFu)) |
+                  (static_cast<uint32_t>(pos) & 31u);
+        sBase[pos] = mine;
+    }
+    __syncwarp();
+    return rows;
+}
 
 template <int DT, bool VEC>
 __global__ void __launch_bounds__(kTabThreads)
@@ -39,32 +77,8 @@ bestfit_tables_kernel(const int32_t* __restrict__ free_core, const int32_t* __re
     // A table outside §2.1's domain (d_valid not in [1, D], or a row value out of range) answers -1 everywhere.
     // The operator's Python interface refuses such tables before the launch; this keeps the kernel defined
     // for callers of the raw operator, whose checks cannot read device data.
-    const int dv = d_valid[n];
-    bool ok = dv >= 1 && dv <= D;
-    const int32_t* fc_row = free_core + static_cast<size_t>(n) * D;
-    const int32_t* fm_row = free_mem + static_cast<size_t>(n) * D;
-    for (int j = lane; j < DT; j += 32) {
-        uint32_t rank = 0xffffffffu;
-        if (ok && j < dv) {
-            const int32_t c = fc_row[j], m = fm_row[j];
-            if (c < 0 || c > kCoreMax || m < 0 || m > kMemMax) ok = false;
-            rank = (static_cast<uint32_t>(c) << 24) | (static_cast<uint32_t>(m) << 6) | static_cast<uint32_t>(j);
-        }
-        sRank[warp][j] = rank;
-        sK[warp][j] = kPadWord;
-    }
-    for (int j = lane; j <= kMaxD; j += 32) sBase[warp][j] = kNoKey;
-    const int rows = __all_sync(0xffffffffu, ok) ? dv : 0;
-    __syncwarp();
-    for (int j = lane; j < rows; j += 32) {
-        const uint32_t mine = sRank[warp][j];
-        int pos = 0;
-        for (int k = 0; k < rows; ++k) pos += sRank[warp][k] < mine;
-        sK[warp][pos] = pack_table_word(static_cast<int32_t>(mine >> 24), static_cast<int32_t>((mine >> 6) & 0x3FFFFu)) |
-                        (static_cast<uint32_t>(pos) & 31u);
-        sBase[warp][pos] = mine;
-    }
-    __syncwarp();
+    sort_table_warp<DT, false>(free_core + static_cast<size_t>(n) * D, free_mem + static_cast<size_t>(n) * D, d_valid[n], D,
+                               sK[warp], sBase[warp], sRank[warp]);
     uint32_t K[DT];
 #pragma unroll
     for (int j = 0; j < DT; j += 4) {
@@ -142,6 +156,418 @@ cudaError_t tables_launch(const int32_t* free_core, const int32_t* free_mem, con
     if (D <= 16) return launch_bucket<16>(vec, grid, stream, free_core, free_mem, d_valid, N, D, req_core, req_mem, P, chunk, out_idx, out_key);
     if (D <= 32) return launch_bucket<32>(vec, grid, stream, free_core, free_mem, d_valid, N, D, req_core, req_mem, P, chunk, out_idx, out_key);
     return launch_bucket<64>(vec, grid, stream, free_core, free_mem, d_valid, N, D, req_core, req_mem, P, chunk, out_idx, out_key);
+}
+
+// ---- egpu::place_tables (DESIGN.md §2.11, §4.6): best-fit rounds to the fixed point over N tables ---------------
+//
+// One cooperative launch of resident CTAs (256 threads, 8 warps, a warp per table as above) runs every round.
+// A round is three phases separated by grid barriers:
+//   1. choose: work items are (row chunk of kPlaceChunk pending rows, tile of 8 tables), cut into contiguous
+//      ranges per CTA.  Each warp sorts its table from the current free_*_out and scores the chunk; the CTA
+//      keeps each row's best word over its warps and over every tile it scores for that chunk in registers,
+//      then does one atomicMax per row (the words are stored inverted, so 0 is "no choice yet");
+//   2. commit: the CTA of a table tile streams the pending rows' words in row order, once, for its 8 warps (up to
+//      kPlaceStage rows are staged in shared memory once per round for every tile the CTA takes); the warp of
+//      table n walks the rows that chose n and commits each row while the running demand of the rows that chose
+//      its device fits (§2.5 per device; rows of one 32-row step that share a device are summed in order with
+//      __match_any_sync), then writes its table's new values;
+//   3. compact: deferred rows go, in row order, into the other pending set (per-tile counts from phase 2,
+//      exclusive offsets summed by every CTA), and their words are reset; rows that chose nothing become -1.
+// Round 1 reads the caller's tables and requests directly and copies every table to free_*_out.  Everything a
+// phase reads that another CTA wrote in this launch is read from L2 (__ldcg).
+constexpr int kPlaceChunk = 1024;           // pending rows per choose work item
+constexpr int kPlaceBlock = kTabThreads;    // rows per compaction tile
+constexpr int kPlaceStage = kTabWarps * kPlaceBlock;  // pending rows the commit phase stages at once
+constexpr int kPlaceDevices = 64;           // CUDA devices whose occupancy answer is cached
+
+struct PlaceCtl {
+    RoundsCtl bar;                // grid-barrier words
+    unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
+    unsigned int in_domain;       // some request is in the domain
+    unsigned int pad_[3];
+};
+
+struct PlaceArgs {
+    const int32_t* fc;               // the caller's tables [N][D], d_valid [N] and requests [P]
+    const int32_t* fm;
+    const int32_t* dv;
+    const int32_t* rc;
+    const int32_t* rm;
+    int N, D;
+    long long P;
+    int32_t* node;                   // outputs: placement [P], tables after every commit [N][D], info [2]
+    int8_t* dev;
+    int32_t* fc_out;
+    int32_t* fm_out;
+    int32_t* info;
+    unsigned long long* best;        // [P]: each pending row's choice, inverted (0 = none yet)
+    int32_t* set[2];                 // [P] each: the pending rows of a round, in row order
+    unsigned int* count[2];          // [P / 256] each, by round parity: deferred rows per compaction tile
+    PlaceCtl* ctl;
+    uint32_t gx, gm;                 // kGuards, kCandMask (in registers: see DevState::cand_xor)
+};
+
+template <int DT, bool VEC>
+__global__ void __launch_bounds__(kTabThreads, 2)
+place_tables_kernel(const __grid_constant__ PlaceArgs a) {
+    __shared__ __align__(16) uint32_t sK[kTabWarps][DT];
+    __shared__ uint32_t sBase[kTabWarps][kMaxD + 1];
+    __shared__ uint32_t sRank[kTabWarps][kMaxD];
+    __shared__ unsigned long long sW[kTabWarps][kPlaceBlock];  // choose: each warp's (inverted) words for a block of rows
+    __shared__ int32_t sFc[kTabWarps][kMaxD], sFm[kTabWarps][kMaxD];    // commit: the table as the round found it
+    __shared__ int32_t sAccC[kTabWarps][kMaxD], sAccM[kTabWarps][kMaxD];  // ... demand committed per device
+    __shared__ int32_t sClosed[kTabWarps][kMaxD];                          // ... a row did not fit: later rows cannot
+    __shared__ int32_t sRow[kPlaceStage];  // commit: the staged rows (their words are staged in sW)
+    __shared__ unsigned int sRed[2][kTabWarps];
+    __shared__ int sOk;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int N = a.N, D = a.D, T = (N + kTabWarps - 1) / kTabWarps;
+    unsigned int gen = 0;
+
+    // every row undecided; note whether any row is in the domain (info[0] counts rounds only then)
+    bool in_domain = false;
+    for (long long p = static_cast<long long>(b) * kTabThreads + tid; p < a.P; p += static_cast<long long>(G) * kTabThreads) {
+        const int32_t c = __ldg(a.rc + p), m = __ldg(a.rm + p);
+        in_domain |= c >= 0 && c <= kCoreMax && m >= 0 && m <= kMemMax;
+        a.node[p] = -2;
+        a.dev[p] = -2;
+    }
+    if (__syncthreads_or(in_domain) && tid == 0) a.ctl->in_domain = 1u;
+
+    const int32_t* cur = nullptr;  // pending rows in row order; round 1: every row (position = row)
+    long long n = a.P;
+    int which = 0, round = 0;
+    bool done = false;
+    while (!done) {
+        ++round;
+        const int32_t* tab_c = round == 1 ? a.fc : a.fc_out;
+        const int32_t* tab_m = round == 1 ? a.fm : a.fm_out;
+
+        // ---- 1. choose
+        {
+            const long long chunks = (n + kPlaceChunk - 1) / kPlaceChunk, items = chunks * T;
+            const long long lo = items * b / G, hi = items * (b + 1) / G;
+            unsigned long long mine[kPlaceChunk / kPlaceBlock];
+            long long held = -1;  // the chunk `mine` belongs to
+            for (long long it = lo; it <= hi; ++it) {
+                const long long chunk = it < hi ? it / T : -1;
+                if (held >= 0 && chunk != held) {  // the CTA's last tile of a chunk: one atomic per row
+#pragma unroll
+                    for (int s = 0; s < kPlaceChunk / kPlaceBlock; ++s) {
+                        const long long i = held * kPlaceChunk + s * kPlaceBlock + tid;
+                        if (i < n && mine[s]) atomicMax(a.best + (cur ? __ldcg(cur + i) : i), mine[s]);
+                    }
+                }
+                if (it == hi) break;
+                if (chunk != held) {
+                    held = chunk;
+#pragma unroll
+                    for (int s = 0; s < kPlaceChunk / kPlaceBlock; ++s) mine[s] = 0;
+                }
+                const int tile = static_cast<int>(it - chunk * T);
+                const int tn = tile * kTabWarps + warp;
+                const size_t off = static_cast<size_t>(tn) * D;
+                sort_table_warp<DT, true>(tab_c + off, tab_m + off, tn < N ? __ldg(a.dv + tn) : 0, D, sK[warp], sBase[warp],
+                                          sRank[warp]);
+                if (round == 1 && chunk == 0 && tn < N)
+                    for (int j = lane; j < D; j += 32) {
+                        a.fc_out[off + j] = a.fc[off + j];
+                        a.fm_out[off + j] = a.fm[off + j];
+                    }
+                uint32_t K[DT];
+#pragma unroll
+                for (int j = 0; j < DT; j += 4) {
+                    const uint4 k4 = *reinterpret_cast<const uint4*>(&sK[warp][j]);
+                    K[j] = k4.x; K[j + 1] = k4.y; K[j + 2] = k4.z; K[j + 3] = k4.w;
+                }
+                const uint32_t* base_of = sBase[warp];
+                // ~((lc << 18 | lm) << 38 | n << 6 | d): the unsigned order of the word is (lc, lm, n, d)
+                auto choose = [&](int32_t core, int32_t mem) -> unsigned long long {
+                    const uint32_t base = base_of[first_feasible<DT>(K, pack_request_word(core, mem), a.gx, a.gm)];
+                    if (base == kNoKey) return 0ull;
+                    const uint32_t key = base - ((static_cast<uint32_t>(core) << 24) | (static_cast<uint32_t>(mem) << 6));
+                    return ~((static_cast<unsigned long long>(key >> 6) << 38) | (static_cast<unsigned long long>(tn) << 6) |
+                             (key & 63u));
+                };
+#pragma unroll
+                for (int s = 0; s < kPlaceChunk / kPlaceBlock; ++s) {
+                    const long long i0 = chunk * kPlaceChunk + s * kPlaceBlock;
+                    if (i0 >= n) break;
+                    if (VEC && round == 1) {  // P % 4 == 0 and 16-byte aligned requests: 4 consecutive rows per lane
+#pragma unroll
+                        for (int h = 0; h < kPlaceBlock / 128; ++h) {
+                            const int j = h * 128 + 4 * lane;
+                            unsigned long long w0 = 0, w1 = 0, w2 = 0, w3 = 0;
+                            if (i0 + j < n) {
+                                const int4 c = __ldg(reinterpret_cast<const int4*>(a.rc + i0 + j));
+                                const int4 m = __ldg(reinterpret_cast<const int4*>(a.rm + i0 + j));
+                                w0 = choose(c.x, m.x); w1 = choose(c.y, m.y); w2 = choose(c.z, m.z); w3 = choose(c.w, m.w);
+                            }
+                            sW[warp][j] = w0; sW[warp][j + 1] = w1; sW[warp][j + 2] = w2; sW[warp][j + 3] = w3;
+                        }
+                    } else {
+#pragma unroll 4
+                        for (int j = lane; j < kPlaceBlock; j += 32) {
+                            const long long i = i0 + j;
+                            unsigned long long w = 0;
+                            if (i < n) {
+                                const long long row = cur ? __ldcg(cur + i) : i;
+                                w = choose(__ldg(a.rc + row), __ldg(a.rm + row));
+                            }
+                            sW[warp][j] = w;
+                        }
+                    }
+                    __syncthreads();
+                    unsigned long long m = sW[0][tid];
+#pragma unroll
+                    for (int w = 1; w < kTabWarps; ++w) m = max(m, sW[w][tid]);
+                    mine[s] = max(mine[s], m);
+                    __syncthreads();
+                }
+            }
+        }
+        if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) break;
+
+        // ---- 2. commit
+        unsigned int* const count = a.count[(round - 1) & 1];
+        unsigned long long* const sStage = &sW[0][0];  // kPlaceStage words: the choose phase is over
+        long long staged = -1;                         // the first pending row staged in sStage / sRow
+        for (int tile = static_cast<int>(b); tile < T; tile += static_cast<int>(G)) {
+            const int tn = tile * kTabWarps + warp;
+            const int dv = tn < N ? __ldg(a.dv + tn) : 0;
+            const bool live = dv >= 1 && dv <= D;  // a table outside the domain is never chosen: it keeps its copy
+            const size_t off = static_cast<size_t>(tn) * D;
+            for (int j = lane; j < kMaxD; j += 32) {
+                sAccC[warp][j] = 0;
+                sAccM[warp][j] = 0;
+                sClosed[warp][j] = 0;
+                if (live && j < dv) {
+                    sFc[warp][j] = __ldcg(tab_c + off + j);
+                    sFm[warp][j] = __ldcg(tab_m + off + j);
+                }
+            }
+            __syncwarp();
+            bool dirty = false;
+            for (long long i0 = 0; i0 < n; i0 += kPlaceStage) {
+                if (i0 != staged) {  // at most kPlaceStage pending rows are staged once per round for every tile
+                    __syncthreads();  // every warp is done with the rows staged before
+#pragma unroll
+                    for (int k = tid; k < kPlaceStage; k += kTabThreads) {
+                        const long long i = i0 + k;
+                        unsigned long long w = ~0ull;  // names no table
+                        if (i < n) {
+                            const int32_t row = cur ? __ldcg(cur + i) : static_cast<int32_t>(i);
+                            sRow[k] = row;
+                            w = ~__ldcg(a.best + row);
+                        }
+                        sStage[k] = w;
+                    }
+                    __syncthreads();
+                    staged = i0;
+                }
+                if (!live) continue;
+                const int len = static_cast<int>(min(static_cast<long long>(kPlaceStage), n - i0));
+                for (int j0 = 0; j0 < len; j0 += kPlaceBlock) {  // one compaction tile
+                    unsigned int deferred = 0;
+                    for (int j = j0 + lane; j < j0 + kPlaceBlock; j += 32) {
+                        const unsigned long long w = sStage[j];
+                        const bool matched = static_cast<int>((w >> 6) & 0x7fffffffu) == tn;
+                        const unsigned int mb = __ballot_sync(0xffffffffu, matched);
+                        if (mb == 0u) continue;
+                        const int d = static_cast<int>(w & 63u);
+                        const int32_t row = sRow[j];
+                        const int32_t core = matched ? __ldg(a.rc + row) : 0, mem = matched ? __ldg(a.rm + row) : 0;
+                        // in-order demand of the rows of this step that chose the same device, up to and including this one
+                        const unsigned int peers = __match_any_sync(0xffffffffu, matched ? d : kMaxD);
+                        int32_t pc = 0, pm = 0;
+                        for (unsigned int r = mb; r; r &= r - 1u) {
+                            const int src = __ffs(r) - 1;
+                            const int32_t vc = __shfl_sync(0xffffffffu, core, src), vm = __shfl_sync(0xffffffffu, mem, src);
+                            if (((peers >> src) & 1u) && src <= lane) {
+                                pc += vc;
+                                pm += vm;
+                            }
+                        }
+                        int32_t acc_c = 0, acc_m = 0;
+                        bool fits = false;
+                        if (matched) {
+                            acc_c = sAccC[warp][d] + pc;
+                            acc_m = sAccM[warp][d] + pm;
+                            fits = !sClosed[warp][d] && acc_c <= sFc[warp][d] && acc_m <= sFm[warp][d];
+                        }
+                        const unsigned int fb = __ballot_sync(0xffffffffu, fits);
+                        __syncwarp();
+                        if (fits) {
+                            a.node[row] = tn;
+                            a.dev[row] = static_cast<int8_t>(d);
+                            if (lane == 31 - __clz(peers & fb)) {  // the last row of the device that fits
+                                sAccC[warp][d] = acc_c;
+                                sAccM[warp][d] = acc_m;
+                            }
+                        } else if (matched && lane == 31 - __clz(peers & ~fb)) {
+                            sClosed[warp][d] = 1;  // demand only grows: every later row of this device is deferred
+                        }
+                        __syncwarp();
+                        dirty |= fb != 0u;
+                        deferred += __popc(mb & ~fb);
+                    }
+                    if (lane == 0 && deferred) atomicAdd(count + (i0 + j0) / kPlaceBlock, deferred);
+                }
+            }
+            __syncwarp();
+            if (dirty)
+                for (int j = lane; j < dv; j += 32) {
+                    a.fc_out[off + j] = sFc[warp][j] - sAccC[warp][j];
+                    a.fm_out[off + j] = sFm[warp][j] - sAccM[warp][j];
+                }
+        }
+        if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) break;
+
+        // ---- 3. compact
+        {
+            const long long tiles = (n + kPlaceBlock - 1) / kPlaceBlock;
+            unsigned int* const next_count = a.count[round & 1];  // last read in the previous round's phase 3
+            for (long long t = static_cast<long long>(b) * kTabThreads + tid; t < tiles; t += static_cast<long long>(G) * kTabThreads)
+                next_count[t] = 0u;
+            const long long lo = tiles * b / G, hi = tiles * (b + 1) / G;
+            unsigned int before = 0, total = 0;
+            for (long long t = tid; t < tiles; t += kTabThreads) {
+                const unsigned int c = __ldcg(count + t);
+                total += c;
+                before += t < lo ? c : 0u;
+            }
+#pragma unroll
+            for (int o = 16; o; o >>= 1) {
+                before += __shfl_xor_sync(0xffffffffu, before, o);
+                total += __shfl_xor_sync(0xffffffffu, total, o);
+            }
+            if (lane == 0) {
+                sRed[0][warp] = before;
+                sRed[1][warp] = total;
+            }
+            __syncthreads();
+            before = 0;
+            total = 0;
+#pragma unroll
+            for (int w = 0; w < kTabWarps; ++w) {
+                before += sRed[0][w];
+                total += sRed[1][w];
+            }
+            __syncthreads();
+            int32_t* const next = a.set[which];
+            for (long long t = lo; t < hi; ++t) {
+                const long long i = t * kPlaceBlock + tid;
+                bool defer = false;
+                int32_t row = 0;
+                if (i < n) {
+                    row = cur ? __ldcg(cur + i) : static_cast<int32_t>(i);
+                    if (__ldcg(a.best + row) == 0ull) {
+                        a.node[row] = -1;
+                        a.dev[row] = -1;
+                    } else if (__ldcg(a.node + row) == -2) {
+                        defer = true;
+                        a.best[row] = 0ull;
+                    }
+                }
+                const unsigned int bal = __ballot_sync(0xffffffffu, defer);
+                if (lane == 0) sRed[0][warp] = __popc(bal);
+                __syncthreads();
+                unsigned int at = before, in_tile = 0;
+#pragma unroll
+                for (int w = 0; w < kTabWarps; ++w) {
+                    at += w < warp ? sRed[0][w] : 0u;
+                    in_tile += sRed[0][w];
+                }
+                if (defer) next[at + __popc(bal & ((1u << lane) - 1u))] = row;
+                before += in_tile;
+                __syncthreads();
+            }
+            if (total == 0u) {
+                done = true;
+            } else {
+                cur = next;
+                n = total;
+                which ^= 1;
+            }
+        }
+        if (!done && !grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) break;
+    }
+    if (b == 0 && tid == 0) {
+        a.info[0] = *reinterpret_cast<volatile unsigned int*>(&a.ctl->in_domain) ? round : 0;
+        a.info[1] = done ? 0 : 1;
+    }
+}
+
+template <int DT>
+cudaError_t place_bucket(bool vec, int device, cudaStream_t stream, const PlaceArgs& a) {
+    auto fn = vec ? place_tables_kernel<DT, true> : place_tables_kernel<DT, false>;
+    // resident CTAs per SM of this kernel on each device, asked once
+    static std::atomic<int> per_sm_cache[kPlaceDevices][2];
+    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device][vec].load(std::memory_order_relaxed) : 0;
+    if (per_sm == 0) {
+        cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kTabThreads, 0);
+        if (err != cudaSuccess) return err;
+        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
+        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device][vec].store(per_sm, std::memory_order_relaxed);
+    }
+    int sms = 0;
+    cudaError_t err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err != cudaSuccess) return err;
+    // Grid: one resident wave, no more CTAs than round 1 has work items of any phase (the barriers cost per CTA).
+    const long long tiles = (a.N + kTabWarps - 1) / kTabWarps;
+    const long long items = tiles * ((a.P + kPlaceChunk - 1) / kPlaceChunk);
+    const long long blocks = (a.P + kPlaceBlock - 1) / kPlaceBlock;
+    long long grid = static_cast<long long>(sms) * per_sm;
+    grid = std::min(grid, std::max(items, blocks));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.blockDim = dim3(kTabThreads);
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, fn, a);
+}
+
+size_t place_scratch_bytes(int P) {
+    const size_t blocks = (static_cast<size_t>(P) + kPlaceBlock - 1) / kPlaceBlock;
+    const size_t zeroed = 8 * static_cast<size_t>(P) + sizeof(PlaceCtl) + 2 * 4 * blocks;
+    return ((zeroed + 15) & ~size_t(15)) + 2 * 4 * static_cast<size_t>(P);
+}
+
+cudaError_t place_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
+                         const int32_t* req_core, const int32_t* req_mem, int P, int32_t* out_node, int8_t* out_dev,
+                         int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch, int device,
+                         cudaStream_t stream) {
+    // scratch: best uint64[P] | barrier words | deferred counts 2 x uint32[P / 256] | (16-aligned) two pending sets
+    // int32[P]; everything before the pending sets starts at zero
+    const size_t blocks = (static_cast<size_t>(P) + kPlaceBlock - 1) / kPlaceBlock;
+    char* s = static_cast<char*>(scratch);
+    PlaceArgs a{};
+    a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem;
+    a.N = N; a.D = D; a.P = P;
+    a.node = out_node; a.dev = out_dev; a.fc_out = free_core_out; a.fm_out = free_mem_out; a.info = info;
+    a.best = reinterpret_cast<unsigned long long*>(s);
+    a.ctl = reinterpret_cast<PlaceCtl*>(s + 8 * static_cast<size_t>(P));
+    a.count[0] = reinterpret_cast<unsigned int*>(s + 8 * static_cast<size_t>(P) + sizeof(PlaceCtl));
+    a.count[1] = a.count[0] + blocks;
+    const size_t zeroed = 8 * static_cast<size_t>(P) + sizeof(PlaceCtl) + 2 * 4 * blocks;
+    a.set[0] = reinterpret_cast<int32_t*>(s + ((zeroed + 15) & ~size_t(15)));
+    a.set[1] = a.set[0] + P;
+    a.gx = kGuards;
+    a.gm = kCandMask;
+    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    if (err != cudaSuccess) return err;
+    const bool vec = (P % 4) == 0 && (reinterpret_cast<uintptr_t>(req_core) % 16) == 0 &&
+                     (reinterpret_cast<uintptr_t>(req_mem) % 16) == 0;
+    if (D <= 8) return place_bucket<8>(vec, device, stream, a);
+    if (D <= 16) return place_bucket<16>(vec, device, stream, a);
+    if (D <= 32) return place_bucket<32>(vec, device, stream, a);
+    return place_bucket<64>(vec, device, stream, a);
 }
 
 }  // namespace egpu

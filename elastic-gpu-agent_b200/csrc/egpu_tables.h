@@ -1,6 +1,8 @@
-// egpu_tables.h — launcher of the multi-table best-fit scan (egpu_tables.cu), called by the
-// PyTorch operator egpu::bestfit_tables (egpu_tables_op.cc).  Not part of the C ABI of include/.
+// egpu_tables.h — launchers of the multi-table best-fit scan and placement (egpu_tables.cu), called by the
+// PyTorch operators egpu::bestfit_tables and egpu::place_tables (egpu_tables_op.cc).  Not part of the C ABI of
+// include/.
 #pragma once
+#include <cstddef>
 #include <cstdint>
 #include <cuda_runtime.h>
 
@@ -13,5 +15,17 @@ namespace egpu {
 cudaError_t tables_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
                           const int32_t* req_core, const int32_t* req_mem, int P, int8_t* out_idx, int32_t* out_key,
                           int device, cudaStream_t stream);
+
+// Bytes of device scratch place_launch needs for P requests (16-byte aligned, from the caller's allocator).
+size_t place_scratch_bytes(int P);
+
+// Places P requests on N tables by best-fit rounds to the fixed point (DESIGN.md §2.11) in one cooperative
+// launch.  Inputs as tables_launch; out_node: int32[P]; out_dev: int8[P]; free_core_out / free_mem_out:
+// int32[N][D]; info: int32[2].  scratch: place_scratch_bytes(P) bytes; its head is zeroed here on `stream`.
+// N >= 1, P >= 1.  Asynchronous on `stream`; returns the first error of the memset or the launch.
+cudaError_t place_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
+                         const int32_t* req_core, const int32_t* req_mem, int P, int32_t* out_node, int8_t* out_dev,
+                         int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch, int device,
+                         cudaStream_t stream);
 
 }  // namespace egpu

@@ -1,12 +1,13 @@
-"""Best fit of many pending requests against many capacity tables in one launch: the PyTorch operator
-`egpu::bestfit_tables` (DESIGN.md §2.10).
+"""Best fit of many pending requests against many capacity tables in one launch: the PyTorch operators
+`egpu::bestfit_tables` (DESIGN.md §2.10) and `egpu::place_tables` (§2.11).
 
-A scheduler scores every pending pod against every node's device table; this does all N x P pairs in
-one CUDA launch on the current stream instead of N `egpu_bestfit_query` calls.  The kernel lives in
-csrc/egpu_tables.cu and is built by __graft_entry__.build() as lib/libegpu_tables.so; it is separate
-from libegpu_alloc.so and its C ABI, reads no context and writes no table.  Importing this module does
-not load the library; the first call (or `load()`) does, and a missing library raises: there is no
-fallback.
+A scheduler scores every pending pod against every node's device table; `bestfit_tables` does all N x P
+pairs in one CUDA launch on the current stream instead of N `egpu_bestfit_query` calls.  `place_tables`
+places the pods: best-fit rounds of prefix-commit to the fixed point over every node's devices, in one
+launch, so that no device is oversubscribed.  The kernels live in csrc/egpu_tables.cu and are built by
+__graft_entry__.build() as lib/libegpu_tables.so; it is separate from libegpu_alloc.so and its C ABI,
+reads no context and writes no table of a context.  Importing this module does not load the library; the
+first call (or `load()`) does, and a missing library raises: there is no fallback.
 """
 from __future__ import annotations
 
@@ -26,7 +27,8 @@ _loaded = False
 
 
 def load() -> None:
-    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables) and the operator's fake implementation."""
+    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables and egpu::place_tables) and the operators'
+    fake implementations."""
     global _loaded
     if _loaded:
         return
@@ -36,39 +38,40 @@ def load() -> None:
             "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.")
     torch.ops.load_library(LIB_PATH)
     torch.library.register_fake("egpu::bestfit_tables")(_fake)
+    torch.library.register_fake("egpu::place_tables")(_fake_place)
     _loaded = True
 
 
-def check_args(free_core, free_mem, d_valid, req_core, req_mem) -> None:
-    """The operator's checks on dtypes, contiguity, shapes and device (no data is read), in the operator's order:
-    RuntimeError for a dtype, layout or device, ValueError for a shape."""
+def check_args(free_core, free_mem, d_valid, req_core, req_mem, op: str = "bestfit_tables") -> None:
+    """The operators' checks on dtypes, contiguity, shapes and device (no data is read), in the operators' order:
+    RuntimeError for a dtype, layout or device, ValueError for a shape.  `op` names the operator in the messages."""
     names = ("free_core", "free_mem", "d_valid", "req_core", "req_mem")
     ts = (free_core, free_mem, d_valid, req_core, req_mem)
     for name, t in zip(names, ts):
         if t.dtype != torch.int32:
-            raise RuntimeError(f"bestfit_tables: {name} must be int32, got {t.dtype}")
+            raise RuntimeError(f"{op}: {name} must be int32, got {t.dtype}")
         if not t.is_contiguous():
-            raise RuntimeError(f"bestfit_tables: {name} must be contiguous")
+            raise RuntimeError(f"{op}: {name} must be contiguous")
     if free_core.dim() != 2 or free_mem.shape != free_core.shape:
-        raise ValueError(f"bestfit_tables: free_core and free_mem must both be [N, D], got {tuple(free_core.shape)} "
+        raise ValueError(f"{op}: free_core and free_mem must both be [N, D], got {tuple(free_core.shape)} "
                          f"and {tuple(free_mem.shape)}")
     N, D = free_core.shape
     if not 1 <= D <= MAX_DEVICES:
-        raise ValueError(f"bestfit_tables: D must be in [1, 64], got {D}")
+        raise ValueError(f"{op}: D must be in [1, 64], got {D}")
     if d_valid.dim() != 1 or d_valid.shape[0] != N:
-        raise ValueError(f"bestfit_tables: d_valid must be [N] = [{N}], got {tuple(d_valid.shape)}")
+        raise ValueError(f"{op}: d_valid must be [N] = [{N}], got {tuple(d_valid.shape)}")
     if req_core.dim() != 1 or req_mem.shape != req_core.shape:
-        raise ValueError(f"bestfit_tables: req_core and req_mem must both be [P], got {tuple(req_core.shape)} "
+        raise ValueError(f"{op}: req_core and req_mem must both be [P], got {tuple(req_core.shape)} "
                          f"and {tuple(req_mem.shape)}")
     if N >= 2**31 or req_core.shape[0] >= 2**31:
-        raise ValueError(f"bestfit_tables: N and P must be below 2^31, got {N} and {req_core.shape[0]}")
+        raise ValueError(f"{op}: N and P must be below 2^31, got {N} and {req_core.shape[0]}")
     dev = free_core.device
     for t in ts:
         if t.device.type != "cuda" or t.device != dev:
-            raise RuntimeError(f"bestfit_tables: every tensor must be on one CUDA device, got {t.device} and {dev}")
+            raise RuntimeError(f"{op}: every tensor must be on one CUDA device, got {t.device} and {dev}")
 
 
-def check_tables(free_core, free_mem, d_valid) -> None:
+def check_tables(free_core, free_mem, d_valid, op: str = "bestfit_tables") -> None:
     """ValueError unless every table is in §2.1's domain: 1 <= d_valid[n] <= D, and the first d_valid[n] devices of
     table n have free_core in [0, 100] and free_mem in [0, 2^18 - 1].  Reads the data: one host round trip."""
     D = free_core.shape[1]
@@ -78,9 +81,9 @@ def check_tables(free_core, free_mem, d_valid) -> None:
     bad_dv = int(((dv < 1) | (dv > D)).sum())
     bad_rows = int((live & out).any(dim=1).sum())
     if bad_dv:
-        raise ValueError(f"bestfit_tables: {bad_dv} table(s) with d_valid outside [1, {D}]")
+        raise ValueError(f"{op}: {bad_dv} table(s) with d_valid outside [1, {D}]")
     if bad_rows:
-        raise ValueError(f"bestfit_tables: {bad_rows} table(s) outside the domain (free_core in [0, 100], "
+        raise ValueError(f"{op}: {bad_rows} table(s) outside the domain (free_core in [0, 100], "
                          f"free_mem in [0, 2^18 - 1] on the first d_valid devices)")
 
 
@@ -116,3 +119,37 @@ def bestfit_tables(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: tor
     if not torch.compiler.is_compiling() and not torch.cuda.is_current_stream_capturing():
         check_tables(free_core, free_mem, d_valid)
     return torch.ops.egpu.bestfit_tables(free_core, free_mem, d_valid, req_core, req_mem)
+
+
+def _fake_place(free_core, free_mem, d_valid, req_core, req_mem):
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op="place_tables")
+    P = req_core.shape[0]
+    return (req_core.new_empty((P,), dtype=torch.int32), req_core.new_empty((P,), dtype=torch.int8),
+            torch.empty_like(free_core), torch.empty_like(free_mem), free_core.new_empty((2,), dtype=torch.int32))
+
+
+def place_tables(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.Tensor,
+                 req_core: torch.Tensor, req_mem: torch.Tensor):
+    """Place P requests on N capacity tables in one launch, without oversubscribing a device (DESIGN.md §2.11).
+
+    Inputs as bestfit_tables.  A request takes the feasible device (n, d), d < d_valid[n], with the smallest
+    (free_core - core, free_mem - mem, n, d): best fit over every table's valid devices, node-major.  Rounds of
+    prefix-commit run to the fixed point: per device, in request order, a request commits while the running demand
+    of the requests that chose the device fits; the deferred ones are scored again against the tables the round
+    left, until a round defers nothing.  A request that fits nowhere when scored is -1.
+
+    Returns (node int32[P], dev int8[P], free_core_out int32[N, D], free_mem_out int32[N, D], info int32[2]):
+    the placement (-1, -1 when none), the tables after every commit (columns at or past d_valid copied unchanged),
+    and info = [rounds run (0 when no request is in the domain), 1 if a grid wait gave up after ~2 s, else 0].
+    When a wait gives up, unfinished requests stay -2 and the tables are those of the last committed round.
+    The inputs are not written.  N = 0 or P = 0 gives -1 placements, copied tables and info [0, 0].
+
+    Stateless and asynchronous on the current stream; it captures into a CUDA graph and traces under
+    torch.compile(fullgraph=True).  Refusals are those of bestfit_tables, with "place_tables" in the messages;
+    during capture or tracing a table outside the domain offers no device and is copied unchanged.
+    """
+    load()
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op="place_tables")
+    if not torch.compiler.is_compiling() and not torch.cuda.is_current_stream_capturing():
+        check_tables(free_core, free_mem, d_valid, op="place_tables")
+    return torch.ops.egpu.place_tables(free_core, free_mem, d_valid, req_core, req_mem)
