@@ -570,4 +570,488 @@ cudaError_t place_launch(const int32_t* free_core, const int32_t* free_mem, cons
     return place_bucket<64>(vec, device, stream, a);
 }
 
+// ---- egpu::place_pods (DESIGN.md §2.12, §4.7): whole pods, best-fit rounds to the fixed point over N tables -------
+//
+// One cooperative launch, the round structure of place_tables_kernel with a pod in place of a row:
+//   0. the grid checks pod_offsets (first 0, last P, every step in [1, kMaxPod]) before any container is read
+//      through them; if one is bad nothing is placed, the tables are copied and info[2] = 1;
+//   1. choose: work items are (block of 256 pending pods, tile of 8 tables).  A warp stages its table's
+//      valid devices in shared memory and each lane replays one pod on it (pod_replay); the CTA keeps each pod's
+//      best word over warps and tiles and does one atomicMax per pod (words inverted, 0 = no node yet);
+//   2. commit: the warp of table n walks the pending pods that chose n in pod order.  The lanes replay their pods
+//      again against the round's table to recover the containers' devices, then, one pod after another, a pod
+//      commits when none of its devices is closed and the demand committed so far on each of them, plus its own,
+//      fits; otherwise it closes all of them;
+//   3. compact: deferred pods go, in pod order, into the other pending set; pods that chose nothing become -1.
+// The pods' devices are not kept between phases: the replay is deterministic, so commit recomputes them.
+constexpr int kMaxPod = 8;                 // containers per pod
+constexpr int kPodBlock = kTabThreads;     // pods per choose work item and per compaction tile
+constexpr int kPodStage = kTabWarps * kPodBlock;  // pending pods the commit phase stages at once
+
+struct PodsCtl {
+    RoundsCtl bar;                // grid-barrier words
+    unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
+    unsigned int in_domain;       // some pod is in the domain
+    unsigned int bad_offsets;     // pod_offsets failed the check (info[2])
+    unsigned int pad_[2];
+};
+
+struct PodsArgs {
+    const int32_t* fc;               // the caller's tables [N][D], d_valid [N], containers [P], pod_offsets [G + 1]
+    const int32_t* fm;
+    const int32_t* dv;
+    const int32_t* rc;
+    const int32_t* rm;
+    const int32_t* off;
+    int N, D;
+    long long P, G;
+    int32_t* node;                   // outputs: node per pod [G], device per container [P], tables [N][D], info [3]
+    int8_t* dev;
+    int32_t* fc_out;
+    int32_t* fm_out;
+    int32_t* info;
+    unsigned long long* best;        // [G]: each pending pod's choice, inverted (0 = none yet)
+    int32_t* set[2];                 // [G] each: the pending pods of a round, in pod order
+    unsigned int* count[2];          // [G / 256] each, by round parity: deferred pods per compaction tile
+    PodsCtl* ctl;
+};
+
+// What a pod's in-node replay leaves: the devices its containers touched (at most one per container), with the
+// free values the pod left on them, and each container's device in 6 bits.
+struct PodFit {
+    int nt;                  // devices touched
+    int td[kMaxPod];         // ... their indices
+    int32_t tc[kMaxPod];     // ... free core and memory after the pod
+    int32_t tm[kMaxPod];
+    unsigned long long cdev; // container k's device in bits 6k .. 6k + 5
+    uint32_t slc, slm;       // sums of the containers' leftovers at the moment each was placed
+};
+
+// §2.12's in-node replay: containers [c0, c0 + len) placed one after another on a table whose first `rows`
+// devices are sc / sm (shared memory), each by §2.3's best fit, the smallest (lc, lm, d), against what the earlier
+// containers left.  Untouched devices are read at the table's values; the touched ones are kept in registers (the
+// slots are indexed by compile-time constants only).  Returns false when a container is outside §2.1's domain or
+// finds no device.
+__device__ __forceinline__ bool pod_replay(const int32_t* sc, const int32_t* sm, int rows, const int32_t* __restrict__ rc,
+                                           const int32_t* __restrict__ rm, long long c0, int len, PodFit& f) {
+    f.nt = 0;
+    f.cdev = 0;
+    f.slc = 0;
+    f.slm = 0;
+    unsigned long long touched = 0;
+#pragma unroll
+    for (int s = 0; s < kMaxPod; ++s) {
+        f.td[s] = 0;
+        f.tc[s] = 0;
+        f.tm[s] = 0;
+    }
+    for (int k = 0; k < len; ++k) {
+        const int32_t core = __ldg(rc + c0 + k), mem = __ldg(rm + c0 + k);
+        if (core < 0 || core > kCoreMax || mem < 0 || mem > kMemMax) return false;
+        uint32_t key = kNoKey;  // (lc << 24 | lm << 6 | d): its unsigned order is best fit's
+#pragma unroll 4
+        for (int d = 0; d < rows; ++d) {
+            if ((touched >> d) & 1ull) continue;
+            const int32_t lc = sc[d] - core, lm = sm[d] - mem;
+            if ((lc | lm) >= 0)
+                key = min(key, (static_cast<uint32_t>(lc) << 24) | (static_cast<uint32_t>(lm) << 6) | static_cast<uint32_t>(d));
+        }
+#pragma unroll
+        for (int s = 0; s < kMaxPod; ++s) {
+            const int32_t lc = f.tc[s] - core, lm = f.tm[s] - mem;
+            if (s < f.nt && (lc | lm) >= 0)
+                key = min(key, (static_cast<uint32_t>(lc) << 24) | (static_cast<uint32_t>(lm) << 6) |
+                                   static_cast<uint32_t>(f.td[s]));
+        }
+        if (key == kNoKey) return false;
+        const int d = static_cast<int>(key & 63u);
+        f.slc += key >> 24;
+        f.slm += (key >> 6) & 0x3FFFFu;
+        f.cdev |= static_cast<unsigned long long>(d) << (6 * k);
+        if ((touched >> d) & 1ull) {
+#pragma unroll
+            for (int s = 0; s < kMaxPod; ++s)
+                if (s < f.nt && f.td[s] == d) {
+                    f.tc[s] -= core;
+                    f.tm[s] -= mem;
+                }
+        } else {
+#pragma unroll
+            for (int s = 0; s < kMaxPod; ++s)
+                if (s == f.nt) {
+                    f.td[s] = d;
+                    f.tc[s] = sc[d] - core;
+                    f.tm[s] = sm[d] - mem;
+                }
+            ++f.nt;
+            touched |= 1ull << d;
+        }
+    }
+    return true;
+}
+
+// Stages table tn's first D devices into sc / sm (the warp's rows of shared memory) and returns the number of
+// devices it offers: d_valid, or 0 for a table outside §2.1's domain or past N.  COHERENT: read from L2.
+__device__ __forceinline__ int stage_table_warp(const int32_t* fc_row, const int32_t* fm_row, int dv, int D, int32_t* sc,
+                                                int32_t* sm) {
+    const int lane = threadIdx.x & 31;
+    bool ok = dv >= 1 && dv <= D;
+    for (int j = lane; ok && j < dv; j += 32) {
+        const int32_t c = __ldcg(fc_row + j), m = __ldcg(fm_row + j);
+        ok = c >= 0 && c <= kCoreMax && m >= 0 && m <= kMemMax;
+        sc[j] = c;
+        sm[j] = m;
+    }
+    const int rows = __all_sync(0xffffffffu, ok) ? dv : 0;
+    __syncwarp();
+    return rows;
+}
+
+__global__ void __launch_bounds__(kTabThreads, 2)
+place_pods_kernel(const __grid_constant__ PodsArgs a) {
+    __shared__ unsigned long long sW[kTabWarps][kPodBlock];  // choose: each warp's (inverted) words for a block of pods
+    __shared__ int32_t sFc[kTabWarps][kMaxD], sFm[kTabWarps][kMaxD];      // the table as the round found it
+    __shared__ int32_t sAccC[kTabWarps][kMaxD], sAccM[kTabWarps][kMaxD];  // commit: demand committed per device
+    __shared__ int32_t sClosed[kTabWarps][kMaxD];                          // ... a pod did not commit: later pods cannot
+    __shared__ int32_t sPod[kPodStage];  // commit: the staged pods (their words are staged in sW)
+    __shared__ unsigned int sRed[2][kTabWarps];
+    __shared__ int sOk;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int N = a.N, D = a.D, T = (N + kTabWarps - 1) / kTabWarps;
+    const long long stride = static_cast<long long>(G) * kTabThreads, first = static_cast<long long>(b) * kTabThreads + tid;
+    unsigned int gen = 0;
+    int round = 0;
+    bool done = false;
+
+    // ---- 0. every pod and container undecided; the offsets checked before a container is read through them
+    {
+        bool bad = false;
+        for (long long g = first; g <= a.G; g += stride) {
+            const int32_t o = __ldg(a.off + g);
+            if (g == 0) bad |= o != 0;
+            if (g == a.G) bad |= o != a.P;
+            if (g < a.G) {
+                const long long step = static_cast<long long>(__ldg(a.off + g + 1)) - o;
+                bad |= step < 1 || step > kMaxPod;
+                a.node[g] = -2;
+            }
+        }
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -2;
+        if (__syncthreads_or(bad) && tid == 0) atomicExch(&a.ctl->bad_offsets, 1u);
+    }
+    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+    if (*reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_offsets)) {  // nothing is placed
+        for (long long g = first; g < a.G; g += stride) a.node[g] = -1;
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -1;
+        for (long long j = first; j < static_cast<long long>(N) * D; j += stride) {
+            a.fc_out[j] = a.fc[j];
+            a.fm_out[j] = a.fm[j];
+        }
+        done = true;
+        goto finish;
+    }
+    {  // note whether any pod is in the domain (info[0] counts rounds only then)
+        bool in_domain = false;
+        for (long long g = first; g < a.G; g += stride) {
+            const int32_t c0 = __ldg(a.off + g), c1 = __ldg(a.off + g + 1);
+            bool ok = true;
+            for (int32_t c = c0; c < c1; ++c) {
+                const int32_t core = __ldg(a.rc + c), mem = __ldg(a.rm + c);
+                ok &= core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
+            }
+            in_domain |= ok;
+        }
+        if (__syncthreads_or(in_domain) && tid == 0) a.ctl->in_domain = 1u;
+    }
+
+    {
+        const int32_t* cur = nullptr;  // pending pods in pod order; round 1: every pod (position = pod)
+        long long n = a.G;
+        int which = 0;
+        while (!done) {
+            ++round;
+            const int32_t* tab_c = round == 1 ? a.fc : a.fc_out;
+            const int32_t* tab_m = round == 1 ? a.fm : a.fm_out;
+
+            // ---- 1. choose
+            {
+                const long long blocks = (n + kPodBlock - 1) / kPodBlock, items = blocks * T;
+                const long long lo = items * b / G, hi = items * (b + 1) / G;
+                unsigned long long mine = 0;
+                long long held = -1;  // the block of pods `mine` belongs to
+                for (long long it = lo; it <= hi; ++it) {
+                    const long long blk = it < hi ? it / T : -1;
+                    if (held >= 0 && blk != held) {  // the CTA's last tile of a block: one atomic per pod
+                        const long long i = held * kPodBlock + tid;
+                        if (i < n && mine) atomicMax(a.best + (cur ? __ldcg(cur + i) : i), mine);
+                        mine = 0;
+                    }
+                    if (it == hi) break;
+                    held = blk;
+                    const int tn = static_cast<int>(it - blk * T) * kTabWarps + warp;
+                    const size_t off = static_cast<size_t>(tn) * D;
+                    const int rows = stage_table_warp(tab_c + off, tab_m + off, tn < N ? __ldg(a.dv + tn) : 0, D, sFc[warp],
+                                                      sFm[warp]);
+                    if (round == 1 && blk == 0 && tn < N)
+                        for (int j = lane; j < D; j += 32) {
+                            a.fc_out[off + j] = a.fc[off + j];
+                            a.fm_out[off + j] = a.fm[off + j];
+                        }
+                    for (int j = lane; j < kPodBlock; j += 32) {
+                        const long long i = blk * kPodBlock + j;
+                        unsigned long long w = 0;
+                        if (i < n && rows) {
+                            const long long g = cur ? __ldcg(cur + i) : i;
+                            const int32_t c0 = __ldg(a.off + g);
+                            PodFit f;
+                            // ~(sum lc << 52 | sum lm << 31 | n): the unsigned order of the word is (sum lc, sum lm, n)
+                            if (pod_replay(sFc[warp], sFm[warp], rows, a.rc, a.rm, c0, __ldg(a.off + g + 1) - c0, f))
+                                w = ~((static_cast<unsigned long long>(f.slc) << 52) |
+                                      (static_cast<unsigned long long>(f.slm) << 31) | static_cast<unsigned long long>(tn));
+                        }
+                        sW[warp][j] = w;
+                    }
+                    __syncthreads();
+#pragma unroll
+                    for (int w = 0; w < kTabWarps; ++w) mine = max(mine, sW[w][tid]);
+                    __syncthreads();
+                }
+            }
+            if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) break;
+
+            // ---- 2. commit
+            unsigned int* const count = a.count[(round - 1) & 1];
+            unsigned long long* const sStage = &sW[0][0];  // kPodStage words: the choose phase is over
+            long long staged = -1;                         // the first pending pod staged in sStage / sPod
+            for (int tile = static_cast<int>(b); tile < T; tile += static_cast<int>(G)) {
+                const int tn = tile * kTabWarps + warp;
+                const size_t off = static_cast<size_t>(tn) * D;
+                // a table outside the domain offers no device, so no pod chose it: it keeps its copy
+                const int rows = stage_table_warp(tab_c + off, tab_m + off, tn < N ? __ldg(a.dv + tn) : 0, D, sFc[warp],
+                                                  sFm[warp]);
+                for (int j = lane; j < kMaxD; j += 32) {
+                    sAccC[warp][j] = 0;
+                    sAccM[warp][j] = 0;
+                    sClosed[warp][j] = 0;
+                }
+                __syncwarp();
+                bool dirty = false;
+                for (long long i0 = 0; i0 < n; i0 += kPodStage) {
+                    if (i0 != staged) {  // at most kPodStage pending pods are staged once per round for every tile
+                        __syncthreads();  // every warp is done with the pods staged before
+                        for (int k = tid; k < kPodStage; k += kTabThreads) {
+                            const long long i = i0 + k;
+                            unsigned long long w = ~0ull;  // names no table
+                            if (i < n) {
+                                const int32_t g = cur ? __ldcg(cur + i) : static_cast<int32_t>(i);
+                                sPod[k] = g;
+                                w = ~__ldcg(a.best + g);
+                            }
+                            sStage[k] = w;
+                        }
+                        __syncthreads();
+                        staged = i0;
+                    }
+                    if (!rows) continue;
+                    const int len = static_cast<int>(min(static_cast<long long>(kPodStage), n - i0));
+                    for (int j0 = 0; j0 < len; j0 += kPodBlock) {  // one compaction tile
+                        unsigned int deferred = 0;
+                        for (int j = j0 + lane; j < j0 + kPodBlock; j += 32) {
+                            const unsigned long long w = sStage[j];
+                            const bool matched = static_cast<int>(w & 0x7fffffffu) == tn;
+                            const unsigned int mb = __ballot_sync(0xffffffffu, matched);
+                            if (mb == 0u) continue;
+                            PodFit f;
+                            int32_t g = 0, c0 = 0, c1 = 0;
+                            if (matched) {  // the choose phase's replay, again: it fitted then, so it fits now
+                                g = sPod[j];
+                                c0 = __ldg(a.off + g);
+                                c1 = __ldg(a.off + g + 1);
+                                pod_replay(sFc[warp], sFm[warp], rows, a.rc, a.rm, c0, c1 - c0, f);
+                            }
+                            // one pod after another, in pod order (lane order)
+                            bool fits = false;
+                            for (unsigned int r = mb; r; r &= r - 1u) {
+                                if (lane == __ffs(r) - 1) {
+                                    bool ok = true;
+#pragma unroll
+                                    for (int s = 0; s < kMaxPod; ++s)
+                                        if (s < f.nt) {  // committed + the pod's demand <= free  <=>  committed <= what the pod leaves
+                                            const int d = f.td[s];
+                                            ok &= !sClosed[warp][d] && sAccC[warp][d] <= f.tc[s] && sAccM[warp][d] <= f.tm[s];
+                                        }
+#pragma unroll
+                                    for (int s = 0; s < kMaxPod; ++s)
+                                        if (s < f.nt) {
+                                            const int d = f.td[s];
+                                            if (ok) {
+                                                sAccC[warp][d] += sFc[warp][d] - f.tc[s];
+                                                sAccM[warp][d] += sFm[warp][d] - f.tm[s];
+                                            } else {
+                                                sClosed[warp][d] = 1;
+                                            }
+                                        }
+                                    fits = ok;
+                                }
+                                __syncwarp();
+                            }
+                            if (fits) {
+                                a.node[g] = tn;
+                                for (int32_t c = c0; c < c1; ++c)
+                                    a.dev[c] = static_cast<int8_t>((f.cdev >> (6 * (c - c0))) & 63u);
+                            }
+                            const unsigned int fb = __ballot_sync(0xffffffffu, fits);
+                            dirty |= fb != 0u;
+                            deferred += __popc(mb & ~fb);
+                        }
+                        if (lane == 0 && deferred) atomicAdd(count + (i0 + j0) / kPodBlock, deferred);
+                    }
+                }
+                __syncwarp();
+                if (dirty)
+                    for (int j = lane; j < rows; j += 32) {
+                        a.fc_out[off + j] = sFc[warp][j] - sAccC[warp][j];
+                        a.fm_out[off + j] = sFm[warp][j] - sAccM[warp][j];
+                    }
+            }
+            if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) break;
+
+            // ---- 3. compact
+            {
+                const long long tiles = (n + kPodBlock - 1) / kPodBlock;
+                unsigned int* const next_count = a.count[round & 1];  // last read in the previous round's phase 3
+                for (long long t = first; t < tiles; t += stride) next_count[t] = 0u;
+                const long long lo = tiles * b / G, hi = tiles * (b + 1) / G;
+                unsigned int before = 0, total = 0;
+                for (long long t = tid; t < tiles; t += kTabThreads) {
+                    const unsigned int c = __ldcg(count + t);
+                    total += c;
+                    before += t < lo ? c : 0u;
+                }
+#pragma unroll
+                for (int o = 16; o; o >>= 1) {
+                    before += __shfl_xor_sync(0xffffffffu, before, o);
+                    total += __shfl_xor_sync(0xffffffffu, total, o);
+                }
+                if (lane == 0) {
+                    sRed[0][warp] = before;
+                    sRed[1][warp] = total;
+                }
+                __syncthreads();
+                before = 0;
+                total = 0;
+#pragma unroll
+                for (int w = 0; w < kTabWarps; ++w) {
+                    before += sRed[0][w];
+                    total += sRed[1][w];
+                }
+                __syncthreads();
+                int32_t* const next = a.set[which];
+                for (long long t = lo; t < hi; ++t) {
+                    const long long i = t * kPodBlock + tid;
+                    bool defer = false;
+                    int32_t g = 0;
+                    if (i < n) {
+                        g = cur ? __ldcg(cur + i) : static_cast<int32_t>(i);
+                        if (__ldcg(a.best + g) == 0ull) {
+                            a.node[g] = -1;
+                            for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
+                        } else if (__ldcg(a.node + g) == -2) {
+                            defer = true;
+                            a.best[g] = 0ull;
+                        }
+                    }
+                    const unsigned int bal = __ballot_sync(0xffffffffu, defer);
+                    if (lane == 0) sRed[0][warp] = __popc(bal);
+                    __syncthreads();
+                    unsigned int at = before, in_tile = 0;
+#pragma unroll
+                    for (int w = 0; w < kTabWarps; ++w) {
+                        at += w < warp ? sRed[0][w] : 0u;
+                        in_tile += sRed[0][w];
+                    }
+                    if (defer) next[at + __popc(bal & ((1u << lane) - 1u))] = g;
+                    before += in_tile;
+                    __syncthreads();
+                }
+                if (total == 0u) {
+                    done = true;
+                } else {
+                    cur = next;
+                    n = total;
+                    which ^= 1;
+                }
+            }
+            if (!done && !grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) break;
+        }
+    }
+finish:
+    if (b == 0 && tid == 0) {
+        const bool bad = *reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_offsets) != 0u;
+        a.info[0] = !bad && *reinterpret_cast<volatile unsigned int*>(&a.ctl->in_domain) ? round : 0;
+        a.info[1] = done ? 0 : 1;
+        a.info[2] = bad ? 1 : 0;
+    }
+}
+
+size_t pods_scratch_bytes(int G) {
+    const size_t blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
+    const size_t zeroed = 8 * static_cast<size_t>(G) + sizeof(PodsCtl) + 2 * 4 * blocks;
+    return ((zeroed + 15) & ~size_t(15)) + 2 * 4 * static_cast<size_t>(G);
+}
+
+cudaError_t pods_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
+                        const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets, int G,
+                        int32_t* out_node, int8_t* out_dev, int32_t* free_core_out, int32_t* free_mem_out, int32_t* info,
+                        void* scratch, int device, cudaStream_t stream) {
+    // scratch: best uint64[G] | barrier words | deferred counts 2 x uint32[G / 256] | (16-aligned) two pending sets
+    // int32[G]; everything before the pending sets starts at zero
+    const size_t blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
+    char* s = static_cast<char*>(scratch);
+    PodsArgs a{};
+    a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem; a.off = pod_offsets;
+    a.N = N; a.D = D; a.P = P; a.G = G;
+    a.node = out_node; a.dev = out_dev; a.fc_out = free_core_out; a.fm_out = free_mem_out; a.info = info;
+    a.best = reinterpret_cast<unsigned long long*>(s);
+    a.ctl = reinterpret_cast<PodsCtl*>(s + 8 * static_cast<size_t>(G));
+    a.count[0] = reinterpret_cast<unsigned int*>(s + 8 * static_cast<size_t>(G) + sizeof(PodsCtl));
+    a.count[1] = a.count[0] + blocks;
+    const size_t zeroed = 8 * static_cast<size_t>(G) + sizeof(PodsCtl) + 2 * 4 * blocks;
+    a.set[0] = reinterpret_cast<int32_t*>(s + ((zeroed + 15) & ~size_t(15)));
+    a.set[1] = a.set[0] + G;
+    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    if (err != cudaSuccess) return err;
+
+    // resident CTAs per SM on each device, asked once
+    static std::atomic<int> per_sm_cache[kPlaceDevices];
+    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
+    if (per_sm == 0) {
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, place_pods_kernel, kTabThreads, 0);
+        if (err != cudaSuccess) return err;
+        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
+        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
+    }
+    int sms = 0;
+    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err != cudaSuccess) return err;
+    // Grid: one resident wave, no more CTAs than round 1 has choose work items (the barriers cost per CTA); at
+    // least one, which finds G = 0's offsets bad.
+    const long long tiles = (static_cast<long long>(N) + kTabWarps - 1) / kTabWarps;
+    const long long items = tiles * static_cast<long long>(blocks);
+    long long grid = static_cast<long long>(sms) * per_sm;
+    grid = std::max(1ll, std::min(grid, items));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.blockDim = dim3(kTabThreads);
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, place_pods_kernel, a);
+}
+
 }  // namespace egpu

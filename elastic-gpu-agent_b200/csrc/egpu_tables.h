@@ -1,6 +1,6 @@
-// egpu_tables.h — launchers of the multi-table best-fit scan and placement (egpu_tables.cu), called by the
-// PyTorch operators egpu::bestfit_tables and egpu::place_tables (egpu_tables_op.cc).  Not part of the C ABI of
-// include/.
+// egpu_tables.h — launchers of the multi-table best-fit scan and placements (egpu_tables.cu), called by the
+// PyTorch operators egpu::bestfit_tables, egpu::place_tables and egpu::place_pods (egpu_tables_op.cc).  Not part
+// of the C ABI of include/.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -27,5 +27,19 @@ cudaError_t place_launch(const int32_t* free_core, const int32_t* free_mem, cons
                          const int32_t* req_core, const int32_t* req_mem, int P, int32_t* out_node, int8_t* out_dev,
                          int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch, int device,
                          cudaStream_t stream);
+
+// Bytes of device scratch pods_launch needs for G pods (16-byte aligned, from the caller's allocator).
+size_t pods_scratch_bytes(int G);
+
+// Places G pods of P containers on N tables, every container of a pod on one node, by best-fit rounds to the fixed
+// point (DESIGN.md §2.12) in one cooperative launch.  Tables and containers as place_launch; pod_offsets:
+// int32[G + 1], checked by the kernel before any container is read through it; out_node: int32[G]; out_dev:
+// int8[P]; free_core_out / free_mem_out: int32[N][D]; info: int32[3].  scratch: pods_scratch_bytes(G) bytes; its
+// head is zeroed here on `stream`.  N >= 1, P >= 1, G >= 0.  Asynchronous on `stream`; returns the first error of
+// the memset or the launch.
+cudaError_t pods_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
+                        const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets, int G,
+                        int32_t* out_node, int8_t* out_dev, int32_t* free_core_out, int32_t* free_mem_out, int32_t* info,
+                        void* scratch, int device, cudaStream_t stream);
 
 }  // namespace egpu

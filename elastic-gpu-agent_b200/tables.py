@@ -1,10 +1,11 @@
 """Best fit of many pending requests against many capacity tables in one launch: the PyTorch operators
-`egpu::bestfit_tables` (DESIGN.md §2.10) and `egpu::place_tables` (§2.11).
+`egpu::bestfit_tables` (DESIGN.md §2.10), `egpu::place_tables` (§2.11) and `egpu::place_pods` (§2.12).
 
 A scheduler scores every pending pod against every node's device table; `bestfit_tables` does all N x P
 pairs in one CUDA launch on the current stream instead of N `egpu_bestfit_query` calls.  `place_tables`
 places the pods: best-fit rounds of prefix-commit to the fixed point over every node's devices, in one
-launch, so that no device is oversubscribed.  The kernels live in csrc/egpu_tables.cu and are built by
+launch, so that no device is oversubscribed.  `place_pods` does the same for pods of several containers, every
+container of a pod on one node.  The kernels live in csrc/egpu_tables.cu and are built by
 __graft_entry__.build() as lib/libegpu_tables.so; it is separate from libegpu_alloc.so and its C ABI,
 reads no context and writes no table of a context.  Importing this module does not load the library; the
 first call (or `load()`) does, and a missing library raises: there is no fallback.
@@ -19,6 +20,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libegpu_tables.so")
 
 MAX_DEVICES = 64
+MAX_POD = 8  # containers per pod (place_pods)
 CORE_MAX = 100
 MEM_MAX = (1 << 18) - 1
 NO_KEY = 0x7FFFFFFF  # key of a pair with no feasible device
@@ -27,8 +29,8 @@ _loaded = False
 
 
 def load() -> None:
-    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables and egpu::place_tables) and the operators'
-    fake implementations."""
+    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables, egpu::place_tables and egpu::place_pods) and
+    the operators' fake implementations."""
     global _loaded
     if _loaded:
         return
@@ -39,6 +41,7 @@ def load() -> None:
     torch.ops.load_library(LIB_PATH)
     torch.library.register_fake("egpu::bestfit_tables")(_fake)
     torch.library.register_fake("egpu::place_tables")(_fake_place)
+    torch.library.register_fake("egpu::place_pods")(_fake_pods)
     _loaded = True
 
 
@@ -153,3 +156,82 @@ def place_tables(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch
     if not torch.compiler.is_compiling() and not torch.cuda.is_current_stream_capturing():
         check_tables(free_core, free_mem, d_valid, op="place_tables")
     return torch.ops.egpu.place_tables(free_core, free_mem, d_valid, req_core, req_mem)
+
+
+def check_pod_args(free_core, pod_offsets) -> None:
+    """place_pods' checks on pod_offsets' dtype, layout, shape and device (no data is read), after check_args and in
+    the operator's order: RuntimeError for a dtype, layout or device, ValueError for a shape."""
+    if pod_offsets.dtype != torch.int32:
+        raise RuntimeError(f"place_pods: pod_offsets must be int32, got {pod_offsets.dtype}")
+    if not pod_offsets.is_contiguous():
+        raise RuntimeError("place_pods: pod_offsets must be contiguous")
+    if pod_offsets.dim() != 1 or pod_offsets.shape[0] < 1:
+        raise ValueError(f"place_pods: pod_offsets must be [G + 1], got {tuple(pod_offsets.shape)}")
+    if pod_offsets.shape[0] >= 2**31:
+        raise ValueError(f"place_pods: G + 1 must be below 2^31, got {pod_offsets.shape[0]}")
+    if pod_offsets.device.type != "cuda" or pod_offsets.device != free_core.device:
+        raise RuntimeError(f"place_pods: every tensor must be on one CUDA device, got {pod_offsets.device} and "
+                           f"{free_core.device}")
+
+
+def check_pods(pod_offsets, P: int) -> None:
+    """ValueError unless pod_offsets lists pods of 1 to MAX_POD containers each, covering all P containers: first 0,
+    last P, every step in [1, MAX_POD].  Reads the data: one host round trip."""
+    o = pod_offsets.to(torch.int64)
+    if int(o[0]) != 0:
+        raise ValueError(f"place_pods: pod_offsets must start at 0, got {int(o[0])}")
+    if int(o[-1]) != P:
+        raise ValueError(f"place_pods: pod_offsets must end at P = {P}, got {int(o[-1])}")
+    step = o[1:] - o[:-1]
+    bad = int(((step < 1) | (step > MAX_POD)).sum())
+    if bad:
+        raise ValueError(f"place_pods: {bad} pod(s) with a container count outside [1, {MAX_POD}]")
+
+
+def _fake_pods(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets):
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op="place_pods")
+    check_pod_args(free_core, pod_offsets)
+    G, P = pod_offsets.shape[0] - 1, req_core.shape[0]
+    return (pod_offsets.new_empty((G,), dtype=torch.int32), req_core.new_empty((P,), dtype=torch.int8),
+            torch.empty_like(free_core), torch.empty_like(free_mem), free_core.new_empty((3,), dtype=torch.int32))
+
+
+def place_pods(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.Tensor, req_core: torch.Tensor,
+               req_mem: torch.Tensor, pod_offsets: torch.Tensor):
+    """Place G pods on N capacity tables in one launch, every container of a pod on one node, without
+    oversubscribing a device (DESIGN.md §2.12).
+
+    Tables as bestfit_tables.  req_core, req_mem: int32[P], the containers listed pod by pod; pod g holds
+    containers pod_offsets[g] .. pod_offsets[g + 1] - 1 (pod_offsets int32[G + 1], first 0, last P, 1 to MAX_POD
+    containers per pod).  A pod with a container outside the domain is -1.
+
+    A pod's fit on node n is the in-node replay: its containers placed in order on table n, each by best fit
+    (smallest (free_core - core, free_mem - mem, d), d < d_valid[n]) against the table as the pod's earlier
+    containers left it.  The pod fits n when every container finds a device, and scores (sum of core leftovers,
+    sum of memory leftovers, n); it takes the node with the smallest score.  Per node, in pod order, a pod commits
+    when none of the devices it chose is closed and, on each of them, the demand committed so far plus its own fits;
+    a pod that does not commit is deferred and closes every device it chose.  Deferred pods are scored again against
+    the tables the round left, until a round defers nothing.  A pod that fits no node when scored is -1.  A pod's
+    fit is not monotone in the table (a container can take the device a later one needed), so -1 means "fit no node
+    when last scored", not "fits no output table".
+
+    Returns (node int32[G], dev int8[P], free_core_out int32[N, D], free_mem_out int32[N, D], info int32[3]): each
+    pod's node and each container's device on it (all of a pod's containers are placed or none is; -1 when none),
+    the tables after every commit (columns at or past d_valid, and tables outside the domain, copied unchanged), and
+    info = [rounds run (0 when no pod is in the domain), 1 if a grid wait gave up after ~2 s else 0, 1 if the kernel
+    refused pod_offsets else 0].  When a wait gives up, unfinished pods stay -2.  The inputs are not written.  N = 0
+    or P = 0 gives -1 placements, copied tables and info [0, 0, 0].
+
+    Stateless and asynchronous on the current stream; it captures into a CUDA graph and traces under
+    torch.compile(fullgraph=True).  Refusals are those of bestfit_tables with "place_pods" in the messages, then
+    pod_offsets' dtype, layout, shape and device.  Eagerly this function also checks the tables and the offsets'
+    values (ValueError), which reads them back; during capture or tracing the kernel checks the offsets itself and,
+    if one is bad, places nothing: all -1, tables copied, info[2] = 1.
+    """
+    load()
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op="place_pods")
+    check_pod_args(free_core, pod_offsets)
+    if not torch.compiler.is_compiling() and not torch.cuda.is_current_stream_capturing():
+        check_tables(free_core, free_mem, d_valid, op="place_pods")
+        check_pods(pod_offsets, req_core.shape[0])
+    return torch.ops.egpu.place_pods(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets)
