@@ -1054,4 +1054,451 @@ cudaError_t pods_launch(const int32_t* free_core, const int32_t* free_mem, const
     return cudaLaunchKernelEx(&cfg, place_pods_kernel, a);
 }
 
+// ---- egpu::place_gangs (DESIGN.md §2.13, §4.8): gangs of pods, each kept or given back, in order, in one launch ---
+//
+// One cooperative launch with an outer loop over gangs; inside it, place_pods_kernel's rounds over the current gang's
+// pending pods only:
+//   0. the grid checks pod_offsets, gang_offsets and gang_min, marks every pod and container -2, every gang's placed
+//      count 0, and copies the tables to free_*_out (every round reads them there).  After a barrier: if an index is
+//      bad nothing is placed and info[2] = 1; otherwise each pod in the domain is counted into its gang (binary search
+//      of gang_offsets), and a second barrier follows;
+//   per gang j, while it has pending pods and placed + pending >= gang_min[j] (round 1's pending pods are the gang's
+//   pods in the domain, its contiguous range holds them):
+//   1. choose and 2. commit as §4.7; the commit also counts the gang's committed pods;
+//   3. compact: every CTA first reads the round's committed and deferred counts.  If nothing is deferred, or
+//      committed + deferred < gang_min, the gang ends with this round.  A gang that ends with fewer than gang_min pods
+//      committed is rolled back instead of compacted: its committed containers' demand goes back to free_*_out by
+//      integer atomics and all its pods become -1; one barrier follows before the next gang's choose reads the tables.
+//      A kept gang ends without a barrier: the next gang's choose reads nothing this phase writes.
+// Deferred counts are indexed by the launch's round number over all gangs, so their zeroing follows §4.7's parity.
+struct GangsCtl {
+    RoundsCtl bar;                // grid-barrier words
+    unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
+    unsigned int bad_index;       // pod_offsets, gang_offsets or gang_min failed the check (info[2])
+    unsigned int pad_[3];
+};
+
+struct GangsArgs {
+    const int32_t* fc;               // the caller's tables [N][D], d_valid [N], containers [P], pod_offsets [G + 1],
+    const int32_t* fm;               // gang_offsets [J + 1], gang_min [J]
+    const int32_t* dv;
+    const int32_t* rc;
+    const int32_t* rm;
+    const int32_t* off;
+    const int32_t* goff;
+    const int32_t* gmin;
+    int N, D;
+    long long P, G, J;
+    int32_t* node;                   // outputs: node per pod [G], device per container [P], placed per gang [J],
+    int8_t* dev;                     // tables [N][D], info [3]
+    int32_t* placed;
+    int32_t* fc_out;
+    int32_t* fm_out;
+    int32_t* info;
+    unsigned long long* best;        // [G]: each pending pod's choice, inverted (0 = none yet)
+    int32_t* set[2];                 // [G] each: the pending pods of a round, in pod order
+    unsigned int* count[2];          // [G / 256] each, by round parity: deferred pods per compaction tile
+    unsigned int* in_domain;         // [J]: each gang's pods in the domain
+    unsigned int* committed;         // [J]: each gang's committed pods
+    GangsCtl* ctl;
+};
+
+__global__ void __launch_bounds__(kTabThreads, 2)
+place_gangs_kernel(const __grid_constant__ GangsArgs a) {
+    __shared__ unsigned long long sW[kTabWarps][kPodBlock];  // choose: each warp's (inverted) words for a block of pods
+    __shared__ int32_t sFc[kTabWarps][kMaxD], sFm[kTabWarps][kMaxD];      // the table as the round found it
+    __shared__ int32_t sAccC[kTabWarps][kMaxD], sAccM[kTabWarps][kMaxD];  // commit: demand committed per device
+    __shared__ int32_t sClosed[kTabWarps][kMaxD];                          // ... a pod did not commit: later pods cannot
+    __shared__ int32_t sPod[kPodStage];  // commit: the staged pods (their words are staged in sW)
+    __shared__ unsigned int sRed[2][kTabWarps];
+    __shared__ int sOk;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int N = a.N, D = a.D, T = (N + kTabWarps - 1) / kTabWarps;
+    const long long stride = static_cast<long long>(G) * kTabThreads, first = static_cast<long long>(b) * kTabThreads + tid;
+    unsigned int gen = 0;
+    int round = 0;  // rounds run by every gang so far: info[0], and the parity of the deferred counts
+    bool done = false;
+
+    // ---- 0. the three index tensors checked before anything is read through them; outputs marked, tables copied
+    {
+        bool bad = false;
+        for (long long g = first; g <= a.G; g += stride) {
+            const int32_t o = __ldg(a.off + g);
+            if (g == 0) bad |= o != 0;
+            if (g == a.G) bad |= o != a.P;
+            if (g < a.G) {
+                const long long step = static_cast<long long>(__ldg(a.off + g + 1)) - o;
+                bad |= step < 1 || step > kMaxPod;
+                a.node[g] = -2;
+            }
+        }
+        for (long long j = first; j <= a.J; j += stride) {
+            const int32_t o = __ldg(a.goff + j);
+            if (j == 0) bad |= o != 0;
+            if (j == a.J) bad |= o != a.G;
+            if (j < a.J) {
+                const long long size = static_cast<long long>(__ldg(a.goff + j + 1)) - o;
+                const int32_t m = __ldg(a.gmin + j);
+                bad |= size < 1 || m < 1 || m > size;
+                a.placed[j] = 0;
+            }
+        }
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -2;
+        for (long long j = first; j < static_cast<long long>(N) * D; j += stride) {
+            a.fc_out[j] = a.fc[j];
+            a.fm_out[j] = a.fm[j];
+        }
+        if (__syncthreads_or(bad) && tid == 0) atomicExch(&a.ctl->bad_index, 1u);
+    }
+    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+    if (*reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_index)) {  // nothing is placed
+        for (long long g = first; g < a.G; g += stride) a.node[g] = -1;
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -1;
+        done = true;
+        goto finish;
+    }
+    // each gang's pods in the domain: round 1's pending pods
+    for (long long g0 = static_cast<long long>(b) * kTabThreads; g0 < a.G; g0 += stride) {
+        const long long g = g0 + tid;
+        bool ok = g < a.G;
+        long long j = 0;
+        if (ok) {
+            for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) {
+                const int32_t core = __ldg(a.rc + c), mem = __ldg(a.rm + c);
+                ok &= core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
+            }
+            long long lo = 0, hi = a.J - 1;  // the last gang whose first pod is at or before g
+            while (lo < hi) {
+                const long long mid = (lo + hi + 1) >> 1;
+                if (__ldg(a.goff + mid) <= g) lo = mid;
+                else hi = mid - 1;
+            }
+            j = lo;
+        }
+        // the pods of a warp are consecutive, so most share a gang: one atomic per gang and warp
+        const unsigned int peers = __match_any_sync(0xffffffffu, ok ? j : -1ll);
+        if (ok && lane == __ffs(peers) - 1) atomicAdd(a.in_domain + j, static_cast<unsigned int>(__popc(peers)));
+    }
+    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+
+    for (long long gang = 0; gang < a.J; ++gang) {
+        const int32_t g_lo = __ldg(a.goff + gang), g_hi = __ldg(a.goff + gang + 1), need = __ldg(a.gmin + gang);
+        const int32_t* cur = nullptr;  // pending pods in pod order; round 1: the gang's range (position = pod - g_lo)
+        long long n = __ldcg(a.in_domain + gang);  // pending pods
+        long long m = g_hi - g_lo;                  // positions of the pending set
+        int which = 0;
+        bool gang_done = n < need;  // also n == 0: never rounds, nothing committed
+        if (gang_done)
+            for (long long g = g_lo + first; g < g_hi; g += stride) {
+                a.node[g] = -1;
+                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
+            }
+        while (!gang_done) {
+            ++round;
+
+            // ---- 1. choose
+            {
+                const long long blocks = (m + kPodBlock - 1) / kPodBlock, items = blocks * T;
+                const long long lo = items * b / G, hi = items * (b + 1) / G;
+                unsigned long long mine = 0;
+                long long held = -1;  // the block of pods `mine` belongs to
+                for (long long it = lo; it <= hi; ++it) {
+                    const long long blk = it < hi ? it / T : -1;
+                    if (held >= 0 && blk != held) {  // the CTA's last tile of a block: one atomic per pod
+                        const long long i = held * kPodBlock + tid;
+                        if (i < m && mine) atomicMax(a.best + (cur ? __ldcg(cur + i) : g_lo + i), mine);
+                        mine = 0;
+                    }
+                    if (it == hi) break;
+                    held = blk;
+                    const int tn = static_cast<int>(it - blk * T) * kTabWarps + warp;
+                    const size_t off = static_cast<size_t>(tn) * D;
+                    const int rows = stage_table_warp(a.fc_out + off, a.fm_out + off, tn < N ? __ldg(a.dv + tn) : 0, D,
+                                                      sFc[warp], sFm[warp]);
+                    for (int j = lane; j < kPodBlock; j += 32) {
+                        const long long i = blk * kPodBlock + j;
+                        unsigned long long w = 0;
+                        if (i < m && rows) {
+                            const long long g = cur ? __ldcg(cur + i) : g_lo + i;
+                            const int32_t c0 = __ldg(a.off + g);
+                            PodFit f;
+                            // ~(sum lc << 52 | sum lm << 31 | n): the unsigned order of the word is (sum lc, sum lm, n)
+                            if (pod_replay(sFc[warp], sFm[warp], rows, a.rc, a.rm, c0, __ldg(a.off + g + 1) - c0, f))
+                                w = ~((static_cast<unsigned long long>(f.slc) << 52) |
+                                      (static_cast<unsigned long long>(f.slm) << 31) | static_cast<unsigned long long>(tn));
+                        }
+                        sW[warp][j] = w;
+                    }
+                    __syncthreads();
+#pragma unroll
+                    for (int w = 0; w < kTabWarps; ++w) mine = max(mine, sW[w][tid]);
+                    __syncthreads();
+                }
+            }
+            if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+
+            // ---- 2. commit
+            unsigned int* const count = a.count[(round - 1) & 1];
+            {
+                unsigned long long* const sStage = &sW[0][0];  // kPodStage words: the choose phase is over
+                long long staged = -1;                         // the first pending position staged in sStage / sPod
+                unsigned int committed = 0;                    // this warp's committed pods (lane 0's count)
+                for (int tile = static_cast<int>(b); tile < T; tile += static_cast<int>(G)) {
+                    const int tn = tile * kTabWarps + warp;
+                    const size_t off = static_cast<size_t>(tn) * D;
+                    // a table outside the domain offers no device, so no pod chose it: it keeps its copy
+                    const int rows = stage_table_warp(a.fc_out + off, a.fm_out + off, tn < N ? __ldg(a.dv + tn) : 0, D,
+                                                      sFc[warp], sFm[warp]);
+                    for (int j = lane; j < kMaxD; j += 32) {
+                        sAccC[warp][j] = 0;
+                        sAccM[warp][j] = 0;
+                        sClosed[warp][j] = 0;
+                    }
+                    __syncwarp();
+                    bool dirty = false;
+                    for (long long i0 = 0; i0 < m; i0 += kPodStage) {
+                        if (i0 != staged) {  // at most kPodStage pending pods are staged once per round for every tile
+                            __syncthreads();  // every warp is done with the pods staged before
+                            for (int k = tid; k < kPodStage; k += kTabThreads) {
+                                const long long i = i0 + k;
+                                unsigned long long w = ~0ull;  // names no table
+                                if (i < m) {
+                                    const int32_t g = cur ? __ldcg(cur + i) : static_cast<int32_t>(g_lo + i);
+                                    sPod[k] = g;
+                                    w = ~__ldcg(a.best + g);
+                                }
+                                sStage[k] = w;
+                            }
+                            __syncthreads();
+                            staged = i0;
+                        }
+                        if (!rows) continue;
+                        const int len = static_cast<int>(min(static_cast<long long>(kPodStage), m - i0));
+                        for (int j0 = 0; j0 < len; j0 += kPodBlock) {  // one compaction tile
+                            unsigned int deferred = 0;
+                            for (int j = j0 + lane; j < j0 + kPodBlock; j += 32) {
+                                const unsigned long long w = sStage[j];
+                                const bool matched = static_cast<int>(w & 0x7fffffffu) == tn;
+                                const unsigned int mb = __ballot_sync(0xffffffffu, matched);
+                                if (mb == 0u) continue;
+                                PodFit f;
+                                int32_t g = 0, c0 = 0, c1 = 0;
+                                if (matched) {  // the choose phase's replay, again: it fitted then, so it fits now
+                                    g = sPod[j];
+                                    c0 = __ldg(a.off + g);
+                                    c1 = __ldg(a.off + g + 1);
+                                    pod_replay(sFc[warp], sFm[warp], rows, a.rc, a.rm, c0, c1 - c0, f);
+                                }
+                                // one pod after another, in pod order (lane order)
+                                bool fits = false;
+                                for (unsigned int r = mb; r; r &= r - 1u) {
+                                    if (lane == __ffs(r) - 1) {
+                                        bool ok = true;
+#pragma unroll
+                                        for (int s = 0; s < kMaxPod; ++s)
+                                            if (s < f.nt) {  // committed + the pod's demand <= free  <=>  committed <= what the pod leaves
+                                                const int d = f.td[s];
+                                                ok &= !sClosed[warp][d] && sAccC[warp][d] <= f.tc[s] && sAccM[warp][d] <= f.tm[s];
+                                            }
+#pragma unroll
+                                        for (int s = 0; s < kMaxPod; ++s)
+                                            if (s < f.nt) {
+                                                const int d = f.td[s];
+                                                if (ok) {
+                                                    sAccC[warp][d] += sFc[warp][d] - f.tc[s];
+                                                    sAccM[warp][d] += sFm[warp][d] - f.tm[s];
+                                                } else {
+                                                    sClosed[warp][d] = 1;
+                                                }
+                                            }
+                                        fits = ok;
+                                    }
+                                    __syncwarp();
+                                }
+                                if (fits) {
+                                    a.node[g] = tn;
+                                    for (int32_t c = c0; c < c1; ++c)
+                                        a.dev[c] = static_cast<int8_t>((f.cdev >> (6 * (c - c0))) & 63u);
+                                }
+                                const unsigned int fb = __ballot_sync(0xffffffffu, fits);
+                                dirty |= fb != 0u;
+                                committed += __popc(fb);
+                                deferred += __popc(mb & ~fb);
+                            }
+                            if (lane == 0 && deferred) atomicAdd(count + (i0 + j0) / kPodBlock, deferred);
+                        }
+                    }
+                    __syncwarp();
+                    if (dirty)
+                        for (int j = lane; j < rows; j += 32) {
+                            a.fc_out[off + j] = sFc[warp][j] - sAccC[warp][j];
+                            a.fm_out[off + j] = sFm[warp][j] - sAccM[warp][j];
+                        }
+                }
+                if (lane == 0 && committed) atomicAdd(a.committed + gang, committed);
+            }
+            if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+
+            // ---- 3. compact, or end the gang: keep it, or give it back
+            {
+                const long long tiles = (m + kPodBlock - 1) / kPodBlock;
+                unsigned int* const next_count = a.count[round & 1];  // last read in the previous round's phase 3
+                // the next round may be the next gang's first, over up to G positions
+                for (long long t = first; t < (a.G + kPodBlock - 1) / kPodBlock; t += stride) next_count[t] = 0u;
+                const long long lo = tiles * b / G, hi = tiles * (b + 1) / G;
+                unsigned int before = 0, total = 0;
+                for (long long t = tid; t < tiles; t += kTabThreads) {
+                    const unsigned int c = __ldcg(count + t);
+                    total += c;
+                    before += t < lo ? c : 0u;
+                }
+#pragma unroll
+                for (int o = 16; o; o >>= 1) {
+                    before += __shfl_xor_sync(0xffffffffu, before, o);
+                    total += __shfl_xor_sync(0xffffffffu, total, o);
+                }
+                if (lane == 0) {
+                    sRed[0][warp] = before;
+                    sRed[1][warp] = total;
+                }
+                __syncthreads();
+                before = 0;
+                total = 0;
+#pragma unroll
+                for (int w = 0; w < kTabWarps; ++w) {
+                    before += sRed[0][w];
+                    total += sRed[1][w];
+                }
+                __syncthreads();
+                const long long placed = __ldcg(a.committed + gang);
+                gang_done = total == 0u || placed + total < need;
+                if (gang_done && placed < need) {  // roll back: every pod of the gang -1, its demand given back
+                    for (long long g = g_lo + first; g < g_hi; g += stride) {
+                        const int32_t nd = __ldcg(a.node + g);
+                        for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) {
+                            if (nd >= 0) {
+                                const size_t at = static_cast<size_t>(nd) * D + __ldcg(a.dev + c);
+                                atomicAdd(a.fc_out + at, __ldg(a.rc + c));
+                                atomicAdd(a.fm_out + at, __ldg(a.rm + c));
+                            }
+                            a.dev[c] = -1;
+                        }
+                        a.node[g] = -1;
+                    }
+                    if (gang + 1 < a.J && !grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+                } else {
+                    if (gang_done && b == 0 && tid == 0) a.placed[gang] = static_cast<int32_t>(placed);
+                    int32_t* const next = a.set[which];
+                    for (long long t = lo; t < hi; ++t) {
+                        const long long i = t * kPodBlock + tid;
+                        bool defer = false;
+                        int32_t g = 0;
+                        if (i < m) {
+                            g = cur ? __ldcg(cur + i) : static_cast<int32_t>(g_lo + i);
+                            if (__ldcg(a.best + g) == 0ull) {
+                                a.node[g] = -1;
+                                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
+                            } else if (__ldcg(a.node + g) == -2) {
+                                defer = true;
+                                a.best[g] = 0ull;
+                            }
+                        }
+                        const unsigned int bal = __ballot_sync(0xffffffffu, defer);
+                        if (lane == 0) sRed[0][warp] = __popc(bal);
+                        __syncthreads();
+                        unsigned int at = before, in_tile = 0;
+#pragma unroll
+                        for (int w = 0; w < kTabWarps; ++w) {
+                            at += w < warp ? sRed[0][w] : 0u;
+                            in_tile += sRed[0][w];
+                        }
+                        if (defer) next[at + __popc(bal & ((1u << lane) - 1u))] = g;
+                        before += in_tile;
+                        __syncthreads();
+                    }
+                    if (!gang_done) {
+                        cur = next;
+                        m = n = total;
+                        which ^= 1;
+                        if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+                    }
+                }
+            }
+        }
+    }
+    done = true;
+finish:
+    if (b == 0 && tid == 0) {
+        const bool bad = *reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_index) != 0u;
+        a.info[0] = bad ? 0 : round;
+        a.info[1] = done ? 0 : 1;
+        a.info[2] = bad ? 1 : 0;
+    }
+}
+
+size_t gangs_scratch_bytes(int G, int J) {
+    const size_t blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
+    const size_t zeroed = 8 * static_cast<size_t>(G) + sizeof(GangsCtl) + 2 * 4 * blocks + 2 * 4 * static_cast<size_t>(J);
+    return ((zeroed + 15) & ~size_t(15)) + 2 * 4 * static_cast<size_t>(G);
+}
+
+cudaError_t gangs_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
+                         const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets, int G,
+                         const int32_t* gang_offsets, const int32_t* gang_min, int J, int32_t* out_node, int8_t* out_dev,
+                         int32_t* out_placed, int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch,
+                         int device, cudaStream_t stream) {
+    // scratch: best uint64[G] | barrier words | deferred counts 2 x uint32[G / 256] | pods in the domain uint32[J] |
+    // committed pods uint32[J] | (16-aligned) two pending sets int32[G]; everything before the pending sets starts at 0
+    const size_t blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
+    char* s = static_cast<char*>(scratch);
+    GangsArgs a{};
+    a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem; a.off = pod_offsets;
+    a.goff = gang_offsets; a.gmin = gang_min;
+    a.N = N; a.D = D; a.P = P; a.G = G; a.J = J;
+    a.node = out_node; a.dev = out_dev; a.placed = out_placed; a.fc_out = free_core_out; a.fm_out = free_mem_out;
+    a.info = info;
+    a.best = reinterpret_cast<unsigned long long*>(s);
+    a.ctl = reinterpret_cast<GangsCtl*>(s + 8 * static_cast<size_t>(G));
+    a.count[0] = reinterpret_cast<unsigned int*>(s + 8 * static_cast<size_t>(G) + sizeof(GangsCtl));
+    a.count[1] = a.count[0] + blocks;
+    a.in_domain = a.count[1] + blocks;
+    a.committed = a.in_domain + J;
+    const size_t zeroed = 8 * static_cast<size_t>(G) + sizeof(GangsCtl) + 2 * 4 * blocks + 2 * 4 * static_cast<size_t>(J);
+    a.set[0] = reinterpret_cast<int32_t*>(s + ((zeroed + 15) & ~size_t(15)));
+    a.set[1] = a.set[0] + G;
+    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    if (err != cudaSuccess) return err;
+
+    // resident CTAs per SM on each device, asked once
+    static std::atomic<int> per_sm_cache[kPlaceDevices];
+    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
+    if (per_sm == 0) {
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, place_gangs_kernel, kTabThreads, 0);
+        if (err != cudaSuccess) return err;
+        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
+        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
+    }
+    int sms = 0;
+    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err != cudaSuccess) return err;
+    // Grid: as pods_launch, from N and G alone (the gang sizes are device data): one resident wave, no more CTAs
+    // than a round over all G pods has choose work items; at least one, which finds G = 0's offsets bad.
+    const long long tiles = (static_cast<long long>(N) + kTabWarps - 1) / kTabWarps;
+    const long long items = tiles * static_cast<long long>(blocks);
+    long long grid = static_cast<long long>(sms) * per_sm;
+    grid = std::max(1ll, std::min(grid, items));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.blockDim = dim3(kTabThreads);
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, place_gangs_kernel, a);
+}
+
 }  // namespace egpu

@@ -1,6 +1,6 @@
 // egpu_tables.h — launchers of the multi-table best-fit scan and placements (egpu_tables.cu), called by the
-// PyTorch operators egpu::bestfit_tables, egpu::place_tables and egpu::place_pods (egpu_tables_op.cc).  Not part
-// of the C ABI of include/.
+// PyTorch operators egpu::bestfit_tables, egpu::place_tables, egpu::place_pods and egpu::place_gangs
+// (egpu_tables_op.cc).  Not part of the C ABI of include/.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -41,5 +41,21 @@ cudaError_t pods_launch(const int32_t* free_core, const int32_t* free_mem, const
                         const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets, int G,
                         int32_t* out_node, int8_t* out_dev, int32_t* free_core_out, int32_t* free_mem_out, int32_t* info,
                         void* scratch, int device, cudaStream_t stream);
+
+// Bytes of device scratch gangs_launch needs for G pods in J gangs (16-byte aligned, from the caller's allocator).
+size_t gangs_scratch_bytes(int G, int J);
+
+// Places J gangs of G pods of P containers on N tables, in gang order, each gang kept when at least gang_min of its pods
+// are placed and rolled back otherwise (DESIGN.md §2.13), in one cooperative launch.  Tables, containers and
+// pod_offsets as pods_launch; gang_offsets: int32[J + 1]; gang_min: int32[J]; the kernel checks all three index
+// tensors before it reads anything through them.  out_node: int32[G]; out_dev: int8[P]; out_placed: int32[J];
+// free_core_out / free_mem_out: int32[N][D]; info: int32[3].  scratch: gangs_scratch_bytes(G, J) bytes; its head is
+// zeroed here on `stream`.  N >= 1, P >= 1, G >= 0, J >= 0.  Asynchronous on `stream`; returns the first error of the
+// memset or the launch.
+cudaError_t gangs_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
+                         const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets, int G,
+                         const int32_t* gang_offsets, const int32_t* gang_min, int J, int32_t* out_node, int8_t* out_dev,
+                         int32_t* out_placed, int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch,
+                         int device, cudaStream_t stream);
 
 }  // namespace egpu

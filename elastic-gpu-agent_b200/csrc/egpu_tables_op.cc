@@ -1,8 +1,8 @@
-// egpu_tables_op.cc — the PyTorch operators egpu::bestfit_tables (DESIGN.md §2.10), egpu::place_tables (§2.11)
-// and egpu::place_pods (§2.12): argument checks on the host, outputs and scratch from the caching allocator, one
-// launch of bestfit_tables_kernel, place_tables_kernel or place_pods_kernel on the current stream.  No
-// synchronisation and no host copy, so every operator can be captured into a CUDA graph.  The fake (shape)
-// implementations are registered from Python (tables.py).
+// egpu_tables_op.cc — the PyTorch operators egpu::bestfit_tables (DESIGN.md §2.10), egpu::place_tables (§2.11),
+// egpu::place_pods (§2.12) and egpu::place_gangs (§2.13): argument checks on the host, outputs and scratch from the
+// caching allocator, one launch of bestfit_tables_kernel, place_tables_kernel, place_pods_kernel or
+// place_gangs_kernel on the current stream.  No synchronisation and no host copy, so every operator can be captured
+// into a CUDA graph.  The fake (shape) implementations are registered from Python (tables.py).
 #include <ATen/core/Tensor.h>
 #include <ATen/ops/empty.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -100,15 +100,14 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> place_tab
 
 // DESIGN.md §2.12.  The checks of check_inputs, then pod_offsets' dtype, layout, shape and device; its values are
 // the kernel's to check (they are device data).  Returns G.
-int64_t check_pod_offsets(const at::Tensor& free_core, const at::Tensor& pod_offsets) {
-    check_int32_contiguous("place_pods", pod_offsets, "pod_offsets");
-    TORCH_CHECK_VALUE(pod_offsets.dim() == 1 && pod_offsets.size(0) >= 1, "place_pods: pod_offsets must be [G + 1], got ",
+int64_t check_pod_offsets(const char* op, const at::Tensor& free_core, const at::Tensor& pod_offsets) {
+    check_int32_contiguous(op, pod_offsets, "pod_offsets");
+    TORCH_CHECK_VALUE(pod_offsets.dim() == 1 && pod_offsets.size(0) >= 1, op, ": pod_offsets must be [G + 1], got ",
                       pod_offsets.sizes());
-    TORCH_CHECK_VALUE(pod_offsets.size(0) <= std::numeric_limits<int32_t>::max(),
-                      "place_pods: G + 1 must be below 2^31, got ", pod_offsets.size(0));
-    TORCH_CHECK(pod_offsets.is_cuda() && pod_offsets.device() == free_core.device(),
-                "place_pods: every tensor must be on one CUDA device, got ", pod_offsets.device(), " and ",
-                free_core.device());
+    TORCH_CHECK_VALUE(pod_offsets.size(0) <= std::numeric_limits<int32_t>::max(), op,
+                      ": G + 1 must be below 2^31, got ", pod_offsets.size(0));
+    TORCH_CHECK(pod_offsets.is_cuda() && pod_offsets.device() == free_core.device(), op,
+                ": every tensor must be on one CUDA device, got ", pod_offsets.device(), " and ", free_core.device());
     return pod_offsets.size(0) - 1;
 }
 
@@ -116,7 +115,7 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> place_pod
     const at::Tensor& free_core, const at::Tensor& free_mem, const at::Tensor& d_valid, const at::Tensor& req_core,
     const at::Tensor& req_mem, const at::Tensor& pod_offsets) {
     const auto [N, D, P] = check_inputs("place_pods", free_core, free_mem, d_valid, req_core, req_mem);
-    const int64_t G = check_pod_offsets(free_core, pod_offsets);
+    const int64_t G = check_pod_offsets("place_pods", free_core, pod_offsets);
     const at::Device dev = free_core.device();
     const c10::cuda::CUDAGuard guard(dev);
     at::Tensor node = at::empty({G}, free_core.options());
@@ -144,6 +143,62 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> place_pod
     return {node, dv_out, fc_out, fm_out, info};
 }
 
+// DESIGN.md §2.13.  place_pods' checks naming place_gangs, then gang_offsets' and gang_min's dtype and layout, shapes
+// and device; their values are the kernel's to check (they are device data).  Returns J.
+int64_t check_gangs(const at::Tensor& free_core, const at::Tensor& gang_offsets, const at::Tensor& gang_min) {
+    check_int32_contiguous("place_gangs", gang_offsets, "gang_offsets");
+    check_int32_contiguous("place_gangs", gang_min, "gang_min");
+    TORCH_CHECK_VALUE(gang_offsets.dim() == 1 && gang_offsets.size(0) >= 1,
+                      "place_gangs: gang_offsets must be [J + 1], got ", gang_offsets.sizes());
+    TORCH_CHECK_VALUE(gang_offsets.size(0) <= std::numeric_limits<int32_t>::max(),
+                      "place_gangs: J + 1 must be below 2^31, got ", gang_offsets.size(0));
+    const int64_t J = gang_offsets.size(0) - 1;
+    TORCH_CHECK_VALUE(gang_min.dim() == 1 && gang_min.size(0) == J, "place_gangs: gang_min must be [J] = [", J,
+                      "], got ", gang_min.sizes());
+    for (const at::Tensor* t : {&gang_offsets, &gang_min})
+        TORCH_CHECK(t->is_cuda() && t->device() == free_core.device(),
+                    "place_gangs: every tensor must be on one CUDA device, got ", t->device(), " and ", free_core.device());
+    return J;
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> place_gangs(
+    const at::Tensor& free_core, const at::Tensor& free_mem, const at::Tensor& d_valid, const at::Tensor& req_core,
+    const at::Tensor& req_mem, const at::Tensor& pod_offsets, const at::Tensor& gang_offsets,
+    const at::Tensor& gang_min) {
+    const auto [N, D, P] = check_inputs("place_gangs", free_core, free_mem, d_valid, req_core, req_mem);
+    const int64_t G = check_pod_offsets("place_gangs", free_core, pod_offsets);
+    const int64_t J = check_gangs(free_core, gang_offsets, gang_min);
+    const at::Device dev = free_core.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    at::Tensor node = at::empty({G}, free_core.options());
+    at::Tensor dv_out = at::empty({P}, free_core.options().dtype(at::kChar));
+    at::Tensor placed = at::empty({J}, free_core.options());
+    at::Tensor fc_out = at::empty({N, D}, free_core.options());
+    at::Tensor fm_out = at::empty({N, D}, free_core.options());
+    at::Tensor info = at::empty({3}, free_core.options());
+    if (N == 0 || P == 0) {  // nothing to place, or nowhere to place it
+        node.fill_(-1);
+        dv_out.fill_(-1);
+        placed.zero_();
+        fc_out.copy_(free_core);
+        fm_out.copy_(free_mem);
+        info.zero_();
+        return {node, dv_out, placed, fc_out, fm_out, info};
+    }
+    at::Tensor scratch =
+        at::empty({static_cast<int64_t>(egpu::gangs_scratch_bytes(static_cast<int>(G), static_cast<int>(J)))},
+                  free_core.options().dtype(at::kByte));
+    const cudaError_t err = egpu::gangs_launch(
+        free_core.data_ptr<int32_t>(), free_mem.data_ptr<int32_t>(), d_valid.data_ptr<int32_t>(), static_cast<int>(N),
+        static_cast<int>(D), req_core.data_ptr<int32_t>(), req_mem.data_ptr<int32_t>(), static_cast<int>(P),
+        pod_offsets.data_ptr<int32_t>(), static_cast<int>(G), gang_offsets.data_ptr<int32_t>(),
+        gang_min.data_ptr<int32_t>(), static_cast<int>(J), node.data_ptr<int32_t>(), dv_out.data_ptr<int8_t>(),
+        placed.data_ptr<int32_t>(), fc_out.data_ptr<int32_t>(), fm_out.data_ptr<int32_t>(), info.data_ptr<int32_t>(),
+        scratch.data_ptr(), dev.index(), c10::cuda::getCurrentCUDAStream(dev.index()).stream());
+    TORCH_CHECK(err == cudaSuccess, "place_gangs: launch failed: ", cudaGetErrorString(err));
+    return {node, dv_out, placed, fc_out, fm_out, info};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(egpu, m) {
@@ -153,6 +208,8 @@ TORCH_LIBRARY(egpu, m) {
           "(Tensor, Tensor, Tensor, Tensor, Tensor)");
     m.def("place_pods(Tensor free_core, Tensor free_mem, Tensor d_valid, Tensor req_core, Tensor req_mem, "
           "Tensor pod_offsets) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
+    m.def("place_gangs(Tensor free_core, Tensor free_mem, Tensor d_valid, Tensor req_core, Tensor req_mem, "
+          "Tensor pod_offsets, Tensor gang_offsets, Tensor gang_min) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)");
 }
 
 // The CPU registration only refuses (the device check above): a CPU caller gets the same messages as a CUDA one.
@@ -160,9 +217,11 @@ TORCH_LIBRARY_IMPL(egpu, CUDA, m) {
     m.impl("bestfit_tables", &bestfit_tables);
     m.impl("place_tables", &place_tables);
     m.impl("place_pods", &place_pods);
+    m.impl("place_gangs", &place_gangs);
 }
 TORCH_LIBRARY_IMPL(egpu, CPU, m) {
     m.impl("bestfit_tables", &bestfit_tables);
     m.impl("place_tables", &place_tables);
     m.impl("place_pods", &place_pods);
+    m.impl("place_gangs", &place_gangs);
 }

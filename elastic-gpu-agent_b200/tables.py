@@ -1,11 +1,14 @@
 """Best fit of many pending requests against many capacity tables in one launch: the PyTorch operators
-`egpu::bestfit_tables` (DESIGN.md §2.10), `egpu::place_tables` (§2.11) and `egpu::place_pods` (§2.12).
+`egpu::bestfit_tables` (DESIGN.md §2.10), `egpu::place_tables` (§2.11), `egpu::place_pods` (§2.12) and
+`egpu::place_gangs` (§2.13).
 
 A scheduler scores every pending pod against every node's device table; `bestfit_tables` does all N x P
 pairs in one CUDA launch on the current stream instead of N `egpu_bestfit_query` calls.  `place_tables`
 places the pods: best-fit rounds of prefix-commit to the fixed point over every node's devices, in one
 launch, so that no device is oversubscribed.  `place_pods` does the same for pods of several containers, every
-container of a pod on one node.  The kernels live in csrc/egpu_tables.cu and are built by
+container of a pod on one node.  `place_gangs` places jobs (gangs of pods) in queue order, each kept only when at
+least its `minAvailable` pods are placed and given back otherwise, so that no job holds capacity it cannot start
+with.  The kernels live in csrc/egpu_tables.cu and are built by
 __graft_entry__.build() as lib/libegpu_tables.so; it is separate from libegpu_alloc.so and its C ABI,
 reads no context and writes no table of a context.  Importing this module does not load the library; the
 first call (or `load()`) does, and a missing library raises: there is no fallback.
@@ -29,8 +32,8 @@ _loaded = False
 
 
 def load() -> None:
-    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables, egpu::place_tables and egpu::place_pods) and
-    the operators' fake implementations."""
+    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables, egpu::place_tables, egpu::place_pods and
+    egpu::place_gangs) and the operators' fake implementations."""
     global _loaded
     if _loaded:
         return
@@ -42,6 +45,7 @@ def load() -> None:
     torch.library.register_fake("egpu::bestfit_tables")(_fake)
     torch.library.register_fake("egpu::place_tables")(_fake_place)
     torch.library.register_fake("egpu::place_pods")(_fake_pods)
+    torch.library.register_fake("egpu::place_gangs")(_fake_gangs)
     _loaded = True
 
 
@@ -158,34 +162,35 @@ def place_tables(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch
     return torch.ops.egpu.place_tables(free_core, free_mem, d_valid, req_core, req_mem)
 
 
-def check_pod_args(free_core, pod_offsets) -> None:
+def check_pod_args(free_core, pod_offsets, op: str = "place_pods") -> None:
     """place_pods' checks on pod_offsets' dtype, layout, shape and device (no data is read), after check_args and in
-    the operator's order: RuntimeError for a dtype, layout or device, ValueError for a shape."""
+    the operator's order: RuntimeError for a dtype, layout or device, ValueError for a shape.  `op` names the
+    operator in the messages."""
     if pod_offsets.dtype != torch.int32:
-        raise RuntimeError(f"place_pods: pod_offsets must be int32, got {pod_offsets.dtype}")
+        raise RuntimeError(f"{op}: pod_offsets must be int32, got {pod_offsets.dtype}")
     if not pod_offsets.is_contiguous():
-        raise RuntimeError("place_pods: pod_offsets must be contiguous")
+        raise RuntimeError(f"{op}: pod_offsets must be contiguous")
     if pod_offsets.dim() != 1 or pod_offsets.shape[0] < 1:
-        raise ValueError(f"place_pods: pod_offsets must be [G + 1], got {tuple(pod_offsets.shape)}")
+        raise ValueError(f"{op}: pod_offsets must be [G + 1], got {tuple(pod_offsets.shape)}")
     if pod_offsets.shape[0] >= 2**31:
-        raise ValueError(f"place_pods: G + 1 must be below 2^31, got {pod_offsets.shape[0]}")
+        raise ValueError(f"{op}: G + 1 must be below 2^31, got {pod_offsets.shape[0]}")
     if pod_offsets.device.type != "cuda" or pod_offsets.device != free_core.device:
-        raise RuntimeError(f"place_pods: every tensor must be on one CUDA device, got {pod_offsets.device} and "
+        raise RuntimeError(f"{op}: every tensor must be on one CUDA device, got {pod_offsets.device} and "
                            f"{free_core.device}")
 
 
-def check_pods(pod_offsets, P: int) -> None:
+def check_pods(pod_offsets, P: int, op: str = "place_pods") -> None:
     """ValueError unless pod_offsets lists pods of 1 to MAX_POD containers each, covering all P containers: first 0,
     last P, every step in [1, MAX_POD].  Reads the data: one host round trip."""
     o = pod_offsets.to(torch.int64)
     if int(o[0]) != 0:
-        raise ValueError(f"place_pods: pod_offsets must start at 0, got {int(o[0])}")
+        raise ValueError(f"{op}: pod_offsets must start at 0, got {int(o[0])}")
     if int(o[-1]) != P:
-        raise ValueError(f"place_pods: pod_offsets must end at P = {P}, got {int(o[-1])}")
+        raise ValueError(f"{op}: pod_offsets must end at P = {P}, got {int(o[-1])}")
     step = o[1:] - o[:-1]
     bad = int(((step < 1) | (step > MAX_POD)).sum())
     if bad:
-        raise ValueError(f"place_pods: {bad} pod(s) with a container count outside [1, {MAX_POD}]")
+        raise ValueError(f"{op}: {bad} pod(s) with a container count outside [1, {MAX_POD}]")
 
 
 def _fake_pods(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets):
@@ -235,3 +240,95 @@ def place_pods(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.T
         check_tables(free_core, free_mem, d_valid, op="place_pods")
         check_pods(pod_offsets, req_core.shape[0])
     return torch.ops.egpu.place_pods(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets)
+
+
+def check_gang_args(free_core, gang_offsets, gang_min) -> None:
+    """place_gangs' checks on gang_offsets' and gang_min's dtype, layout, shapes and device (no data is read), after
+    check_args and check_pod_args and in the operator's order: RuntimeError for a dtype, layout or device,
+    ValueError for a shape."""
+    for name, t in (("gang_offsets", gang_offsets), ("gang_min", gang_min)):
+        if t.dtype != torch.int32:
+            raise RuntimeError(f"place_gangs: {name} must be int32, got {t.dtype}")
+        if not t.is_contiguous():
+            raise RuntimeError(f"place_gangs: {name} must be contiguous")
+    if gang_offsets.dim() != 1 or gang_offsets.shape[0] < 1:
+        raise ValueError(f"place_gangs: gang_offsets must be [J + 1], got {tuple(gang_offsets.shape)}")
+    if gang_offsets.shape[0] >= 2**31:
+        raise ValueError(f"place_gangs: J + 1 must be below 2^31, got {gang_offsets.shape[0]}")
+    J = gang_offsets.shape[0] - 1
+    if gang_min.dim() != 1 or gang_min.shape[0] != J:
+        raise ValueError(f"place_gangs: gang_min must be [J] = [{J}], got {tuple(gang_min.shape)}")
+    for t in (gang_offsets, gang_min):
+        if t.device.type != "cuda" or t.device != free_core.device:
+            raise RuntimeError(f"place_gangs: every tensor must be on one CUDA device, got {t.device} and "
+                               f"{free_core.device}")
+
+
+def check_gangs(gang_offsets, gang_min, G: int) -> None:
+    """ValueError unless gang_offsets lists gangs of at least one pod each, covering all G pods (first 0, last G,
+    every step >= 1), and every gang_min[j] is in [1, size of gang j].  Reads the data: one host round trip."""
+    o, m = torch.cat([gang_offsets.to(torch.int64), gang_min.to(torch.int64)]).cpu().split(
+        [gang_offsets.shape[0], gang_min.shape[0]])
+    if int(o[0]) != 0:
+        raise ValueError(f"place_gangs: gang_offsets must start at 0, got {int(o[0])}")
+    if int(o[-1]) != G:
+        raise ValueError(f"place_gangs: gang_offsets must end at G = {G}, got {int(o[-1])}")
+    size = o[1:] - o[:-1]
+    bad = int((size < 1).sum())
+    if bad:
+        raise ValueError(f"place_gangs: {bad} gang(s) with no pod")
+    bad = int(((m < 1) | (m > size)).sum())
+    if bad:
+        raise ValueError(f"place_gangs: {bad} gang(s) with gang_min outside [1, gang size]")
+
+
+def _fake_gangs(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_offsets, gang_min):
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op="place_gangs")
+    check_pod_args(free_core, pod_offsets, op="place_gangs")
+    check_gang_args(free_core, gang_offsets, gang_min)
+    G, P, J = pod_offsets.shape[0] - 1, req_core.shape[0], gang_offsets.shape[0] - 1
+    return (pod_offsets.new_empty((G,), dtype=torch.int32), req_core.new_empty((P,), dtype=torch.int8),
+            gang_offsets.new_empty((J,), dtype=torch.int32), torch.empty_like(free_core), torch.empty_like(free_mem),
+            free_core.new_empty((3,), dtype=torch.int32))
+
+
+def place_gangs(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.Tensor, req_core: torch.Tensor,
+                req_mem: torch.Tensor, pod_offsets: torch.Tensor, gang_offsets: torch.Tensor, gang_min: torch.Tensor):
+    """Place J gangs (jobs) of pods on N capacity tables in one launch, in gang order, each gang kept only when at
+    least gang_min of its pods are placed, and given back otherwise (DESIGN.md §2.13).
+
+    Tables, containers and pod_offsets as place_pods.  The pods are listed gang by gang: gang j holds pods
+    gang_offsets[j] .. gang_offsets[j + 1] - 1 (gang_offsets int32[J + 1], first 0, last G, at least one pod per
+    gang).  gang_min int32[J] is each gang's minAvailable, in [1, size of the gang]; gang_min = size is all or nothing.
+
+    The rule is a loop over place_pods: for j = 0 .. J - 1, gang j's pods are placed by place_pods against the tables
+    the gangs before it left; if at least gang_min[j] of them are placed, their placement and tables are kept, and
+    otherwise every pod of the gang is -1 and the tables are as before it, so later gangs see the capacity it gave
+    back.  A gang's rounds stop as soon as its placed plus pending pods fall below gang_min[j] (before round 1, its
+    pods in the domain are pending): it can no longer be kept.
+
+    Returns (node int32[G], dev int8[P], placed int32[J], free_core_out int32[N, D], free_mem_out int32[N, D],
+    info int32[3]): node and dev as place_pods; placed[j] is 0 for a gang given back and its placed pods (in
+    [gang_min[j], size]) for a gang kept; the tables after every kept gang (columns at or past d_valid, and tables
+    outside the domain, copied unchanged); info = [rounds run, summed over gangs, 1 if a grid wait gave up after ~2 s
+    else 0, 1 if the kernel refused pod_offsets, gang_offsets or gang_min else 0].  When a wait gives up the outputs
+    are not a placement and the caller must discard them.  The inputs are not written.  N = 0 or P = 0 gives -1
+    placements, placed all 0, copied tables and info [0, 0, 0].
+
+    Stateless and asynchronous on the current stream; it captures into a CUDA graph and traces under
+    torch.compile(fullgraph=True).  Refusals are place_pods' with "place_gangs" in the messages, then gang_offsets'
+    and gang_min's dtype, layout, shapes and device.  Eagerly this function also checks the tables and the values of
+    pod_offsets, gang_offsets and gang_min (ValueError), which reads them back; during capture or tracing the kernel
+    checks the three index tensors itself and, if one is bad, places nothing: all -1, placed all 0, tables copied,
+    info = [0, 0, 1].
+    """
+    load()
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op="place_gangs")
+    check_pod_args(free_core, pod_offsets, op="place_gangs")
+    check_gang_args(free_core, gang_offsets, gang_min)
+    if not torch.compiler.is_compiling() and not torch.cuda.is_current_stream_capturing():
+        check_tables(free_core, free_mem, d_valid, op="place_gangs")
+        check_pods(pod_offsets, req_core.shape[0], op="place_gangs")
+        check_gangs(gang_offsets, gang_min, pod_offsets.shape[0] - 1)
+    return torch.ops.egpu.place_gangs(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_offsets,
+                                      gang_min)
