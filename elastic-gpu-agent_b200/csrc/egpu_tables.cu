@@ -1501,4 +1501,563 @@ cudaError_t gangs_launch(const int32_t* free_core, const int32_t* free_mem, cons
     return cudaLaunchKernelEx(&cfg, place_gangs_kernel, a);
 }
 
+// ---- egpu::preempt_pods (DESIGN.md §2.14, §4.9): whole pods with priority preemption, rounds to the fixed point ----
+//
+// One cooperative launch.  Every (pod, node) question is answered by one warp holding the node's table in registers
+// (lane l owns devices l and l + 32), so the in-node replay of a container is one __reduce_min_sync, and the reprieve
+// chain of §2.14 step 3, serial per pair, runs a replay per step without touching shared memory:
+//   0. the grid checks pod_offsets, run_offsets and node_offsets before anything is read through them, marks every
+//      pod and container -2 and every running pod -1 (alive), and copies the tables to free_*_out (every round reads
+//      them there).  After a barrier: if an index is bad nothing is placed and info[2] = 1; otherwise pods outside
+//      the domain become -1, and each node is marked usable when its table is in §2.1's domain and its running data
+//      is consistent (an unusable node offers no candidate and is never written);
+//   per round, over the pending pods (node = -2):
+//   1a. choose, empty victim set: work items are (pod, chunk of nodes), chunk-major so that one pod's chunks spread
+//       over CTAs.  Each warp replays the pod on its nodes of the chunk; the CTA reduces the warps' best keys and
+//       writes one record per item.  A pod that fits some node as it is is flagged;
+//   1b. choose, with victims: the same items, for the pods no node took as it is: steps 2 and 3 of §2.14 per node
+//       where the pod outranks an alive running pod; the records are overwritten;
+//   2.  reduce: one thread per pending pod takes the smallest of its K records (§2.14's key is 142 bits, so the
+//       records are three 64-bit words compared in order, not an atomic); a pod with none becomes -1;
+//   3.  commit: the warp of node n walks the pending pods that chose n in pod order, §2.14's commit rule.  The replay
+//       and the chain are deterministic and nothing changed node n since the choose phases, so the warp recomputes a
+//       pod's devices, and a committing preemptor's victims, instead of storing them;
+//   then every CTA reads the round's deferred count: zero ends the launch.
+constexpr int kMaxRun = 128;     // running pods per node
+constexpr int kPreChunks = 32;   // node chunks per pending pod in the choose phases
+
+struct PreemptCtl {
+    RoundsCtl bar;                // grid-barrier words
+    unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
+    unsigned int bad_index;       // pod_offsets, run_offsets or node_offsets failed the check (info[2])
+    unsigned int in_domain;       // some pod is in the domain
+    unsigned int deferred[2];     // pods deferred by a round's commit, by round parity
+};
+
+struct PreemptArgs {
+    const int32_t* fc;     // the caller's tables [N][D], d_valid [N], containers [P], pod_offsets [G + 1], pod_prio [G]
+    const int32_t* fm;
+    const int32_t* dv;
+    const int32_t* rc;
+    const int32_t* rm;
+    const int32_t* off;
+    const int32_t* prio;
+    const int32_t* qc;     // running containers [Q], run_offsets [H + 1], run_prio [H], node_offsets [N + 1]
+    const int32_t* qm;
+    const int8_t* qd;
+    const int32_t* roff;
+    const int32_t* rprio;
+    const int32_t* noff;
+    int N, D, K;           // K: node chunks per pod in the choose phases
+    long long P, G, Q, H;
+    int32_t* node;         // outputs: node per pod [G], device per container [P], evictor per running pod [H],
+    int8_t* dev;           // tables [N][D], info [3]
+    int32_t* evicted;
+    int32_t* fc_out;
+    int32_t* fm_out;
+    int32_t* info;
+    unsigned long long* rec;     // [G][K][3]: each (pod, chunk)'s smallest key
+    unsigned long long* choice;  // [G]: the chosen node, bit 32 set when the victim set is not empty; ~0 = none
+    unsigned int* has_empty;     // [G]: some node takes the pod as it is (phase 1a -> 1b)
+    unsigned int* usable;        // [N]: table in the domain and running data consistent
+    PreemptCtl* ctl;
+};
+
+// A node's table as one warp holds it: lane l's devices l and l + 32.
+struct WarpTab {
+    int32_t c[2], m[2];
+};
+
+// §2.14's choice key (highest victim priority, sum of victim priorities, victims, sum lc, sum lm, n) as three
+// words compared in order: a = 0 for no victim, else (highest prio + 2^31) + 1; b = sum (prio + 2^31) << 8 | |V|;
+// c = (sum lc << 21 | sum lm) << 31 | n.  All ones: no candidate.
+struct PreKey {
+    unsigned long long a, b, c;
+};
+
+__device__ __forceinline__ bool pre_less(const PreKey& x, const PreKey& y) {
+    return x.a != y.a ? x.a < y.a : x.b != y.b ? x.b < y.b : x.c < y.c;
+}
+
+// §2.12's in-node replay by one warp on the table t (its first `rows` devices), updated to what the pod leaves.
+// Each container takes the device with the smallest (lc, lm, d), one __reduce_min_sync over the lanes' keys.
+// used: the lane's devices some container chose (bit 0: lane, bit 1: lane + 32).  Returns false when a container is
+// outside §2.1's domain or finds no device.
+__device__ __forceinline__ bool warp_replay(WarpTab& t, int rows, const int32_t* __restrict__ rc,
+                                            const int32_t* __restrict__ rm, long long c0, int len, uint32_t& slc,
+                                            uint32_t& slm, unsigned long long& cdev, unsigned int& used) {
+    const int lane = threadIdx.x & 31;
+    slc = 0;
+    slm = 0;
+    cdev = 0;
+    used = 0;
+    for (int k = 0; k < len; ++k) {
+        const int32_t core = __ldg(rc + c0 + k), mem = __ldg(rm + c0 + k);
+        if (core < 0 || core > kCoreMax || mem < 0 || mem > kMemMax) return false;
+        uint32_t key = kNoKey;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int d = lane + 32 * i;
+            const int32_t lc = t.c[i] - core, lm = t.m[i] - mem;
+            if (d < rows && (lc | lm) >= 0)
+                key = min(key, (static_cast<uint32_t>(lc) << 24) | (static_cast<uint32_t>(lm) << 6) | static_cast<uint32_t>(d));
+        }
+        key = __reduce_min_sync(0xffffffffu, key);
+        if (key == kNoKey) return false;
+        const int d = static_cast<int>(key & 63u);
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+            if (d == lane + 32 * i) {
+                t.c[i] -= core;
+                t.m[i] -= mem;
+                used |= 1u << i;
+            }
+        slc += key >> 24;
+        slm += (key >> 6) & 0x3FFFFu;
+        cdev |= static_cast<unsigned long long>(d) << (6 * k);
+    }
+    return true;
+}
+
+// t += sign x the demand of running pod h (its containers' devices are in range: the node is usable).
+__device__ __forceinline__ void add_running(const PreemptArgs& a, WarpTab& t, long long h, int sign) {
+    const int lane = threadIdx.x & 31;
+    for (int32_t c = __ldg(a.roff + h), c1 = __ldg(a.roff + h + 1); c < c1; ++c) {
+        const int d = __ldg(a.qd + c);
+        const int32_t core = sign * __ldg(a.qc + c), mem = sign * __ldg(a.qm + c);
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+            if (d == lane + 32 * i) {
+                t.c[i] += core;
+                t.m[i] += mem;
+            }
+    }
+}
+
+// §2.14 steps 2 and 3 for the pod of priority p and containers [c0, c0 + len) on node n, whose table as the round
+// found it is t and whose running pods are [h0, h1) (at most kMaxRun: running pod h0 + lane + 32 i is slot i of the
+// lane).  The caller knows step 1 failed.  Returns false when n is not a candidate; otherwise t becomes the table plus
+// the demand of V minus the pod's (what committing leaves), in_v holds V by slot, cdev the pod's devices and k the
+// key.
+__device__ __forceinline__ bool pre_victims(const PreemptArgs& a, WarpTab& t, int rows, int32_t p, long long c0, int len,
+                                            long long h0, long long h1, int n, unsigned int& in_v, PreKey& k,
+                                            unsigned long long& cdev) {
+    const int lane = threadIdx.x & 31;
+    unsigned int cand = 0;  // C: alive running pods of lower priority
+    uint32_t q[4];          // priority + 2^31: its unsigned order is the priority's
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const long long h = h0 + lane + 32 * i;
+        q[i] = 0;
+        if (h < h1) {
+            const int32_t r = __ldg(a.rprio + h);
+            q[i] = static_cast<uint32_t>(r) ^ 0x80000000u;
+            if (r < p && __ldcg(a.evicted + h) == -1) cand |= 1u << i;
+        }
+    }
+    if (!__any_sync(0xffffffffu, cand != 0u)) return false;
+    WarpTab base = t;  // the table plus the demand of V
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+        for (unsigned int m = __ballot_sync(0xffffffffu, (cand >> i) & 1u); m; m &= m - 1u)
+            add_running(a, base, h0 + (__ffs(m) - 1) + 32 * i, 1);
+    WarpTab w = base;
+    uint32_t slc, slm;
+    unsigned int used;
+    if (!warp_replay(w, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used)) return false;
+    // walk C by (priority descending, h ascending): h is reprieved when the pod fits without evicting it
+    in_v = cand;
+    unsigned int left = cand;
+    while (__any_sync(0xffffffffu, left != 0u)) {
+        uint32_t bq = 0;
+        int bi = 4;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+            if (((left >> i) & 1u) && (bi == 4 || q[i] > bq)) {
+                bq = q[i];
+                bi = i;
+            }
+        const uint32_t top = __reduce_max_sync(0xffffffffu, bi < 4 ? bq : 0u);
+        const uint32_t at = __reduce_min_sync(0xffffffffu, bi < 4 && bq == top ? static_cast<uint32_t>(lane + 32 * bi) : ~0u);
+        const int slot = static_cast<int>(at >> 5), owner = static_cast<int>(at & 31u);
+        if (lane == owner) left &= ~(1u << slot);
+        WarpTab trial = base;
+        add_running(a, trial, h0 + at, -1);
+        WarpTab tw = trial;
+        uint32_t tlc, tlm;
+        unsigned long long tdev;
+        if (warp_replay(tw, rows, a.rc, a.rm, c0, len, tlc, tlm, tdev, used)) {
+            base = trial;
+            w = tw;
+            slc = tlc;
+            slm = tlm;
+            cdev = tdev;
+            if (lane == owner) in_v &= ~(1u << slot);
+        }
+    }
+    uint32_t top = 0;
+    unsigned long long sum = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+        if ((in_v >> i) & 1u) {
+            top = max(top, q[i]);
+            sum += q[i];
+        }
+    top = __reduce_max_sync(0xffffffffu, top);
+    const unsigned int count = __reduce_add_sync(0xffffffffu, static_cast<unsigned int>(__popc(in_v)));
+#pragma unroll
+    for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    k.a = static_cast<unsigned long long>(top) + 1ull;
+    k.b = (sum << 8) | count;
+    k.c = (((static_cast<unsigned long long>(slc) << 21) | slm) << 31) | static_cast<unsigned long long>(n);
+    t = w;
+    return true;
+}
+
+// Node n's table from free_*_out into the warp's registers (the values past `rows` are not read).
+__device__ __forceinline__ WarpTab load_tab(const PreemptArgs& a, int n, int rows) {
+    const int lane = threadIdx.x & 31;
+    WarpTab t;
+    const size_t off = static_cast<size_t>(n) * a.D;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int d = lane + 32 * i;
+        t.c[i] = d < rows ? __ldcg(a.fc_out + off + d) : 0;
+        t.m[i] = d < rows ? __ldcg(a.fm_out + off + d) : 0;
+    }
+    return t;
+}
+
+__global__ void __launch_bounds__(kTabThreads, 2)
+preempt_pods_kernel(const __grid_constant__ PreemptArgs a) {
+    __shared__ int32_t sSumC[kTabWarps][kMaxD], sSumM[kTabWarps][kMaxD];  // phase 0: free + running demand per device
+    __shared__ PreKey sKey[kTabWarps];
+    __shared__ int sOk;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int N = a.N, D = a.D, K = a.K;
+    const long long stride = static_cast<long long>(G) * kTabThreads, first = static_cast<long long>(b) * kTabThreads + tid;
+    const long long wstride = static_cast<long long>(G) * kTabWarps, wfirst = static_cast<long long>(b) * kTabWarps + warp;
+    const PreKey none{~0ull, ~0ull, ~0ull};
+    unsigned int gen = 0;
+    int round = 0;
+    bool done = false;
+
+    // ---- 0. the three index tensors checked before anything is read through them; outputs marked, tables copied
+    {
+        bool bad = false;
+        for (long long g = first; g <= a.G; g += stride) {
+            const int32_t o = __ldg(a.off + g);
+            if (g == 0) bad |= o != 0;
+            if (g == a.G) bad |= o != a.P;
+            if (g < a.G) {
+                const long long step = static_cast<long long>(__ldg(a.off + g + 1)) - o;
+                bad |= step < 1 || step > kMaxPod;
+                a.node[g] = -2;
+            }
+        }
+        for (long long h = first; h <= a.H; h += stride) {
+            const int32_t o = __ldg(a.roff + h);
+            if (h == 0) bad |= o != 0;
+            if (h == a.H) bad |= o != a.Q;
+            if (h < a.H) {
+                const long long step = static_cast<long long>(__ldg(a.roff + h + 1)) - o;
+                bad |= step < 1 || step > kMaxPod;
+                a.evicted[h] = -1;
+            }
+        }
+        for (long long n = first; n <= N; n += stride) {
+            const int32_t o = __ldg(a.noff + n);
+            if (n == 0) bad |= o != 0;
+            if (n == N) bad |= o != a.H;
+            if (n < N) {
+                const long long step = static_cast<long long>(__ldg(a.noff + n + 1)) - o;
+                bad |= step < 0 || step > kMaxRun;
+            }
+        }
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -2;
+        for (long long j = first; j < static_cast<long long>(N) * D; j += stride) {
+            a.fc_out[j] = a.fc[j];
+            a.fm_out[j] = a.fm[j];
+        }
+        if (__syncthreads_or(bad) && tid == 0) atomicExch(&a.ctl->bad_index, 1u);
+    }
+    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+    if (*reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_index)) {  // nothing is placed or evicted
+        for (long long g = first; g < a.G; g += stride) a.node[g] = -1;
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -1;
+        done = true;
+        goto finish;
+    }
+    {  // pods outside the domain are -1; the nodes a pod may use
+        bool in_domain = false;
+        for (long long g = first; g < a.G; g += stride) {
+            const int32_t c0 = __ldg(a.off + g), c1 = __ldg(a.off + g + 1);
+            bool ok = true;
+            for (int32_t c = c0; c < c1; ++c) {
+                const int32_t core = __ldg(a.rc + c), mem = __ldg(a.rm + c);
+                ok &= core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
+            }
+            if (!ok) {
+                a.node[g] = -1;
+                for (int32_t c = c0; c < c1; ++c) a.dev[c] = -1;
+            }
+            in_domain |= ok;
+        }
+        if (__syncthreads_or(in_domain) && tid == 0) a.ctl->in_domain = 1u;
+        for (long long n = wfirst; n < N; n += wstride) {
+            const int dv = __ldg(a.dv + n);
+            bool ok = dv >= 1 && dv <= D;
+            const size_t off = static_cast<size_t>(n) * D;
+            for (int j = lane; j < kMaxD; j += 32) {
+                const int32_t c = ok && j < dv ? __ldg(a.fc + off + j) : 0, m = ok && j < dv ? __ldg(a.fm + off + j) : 0;
+                ok &= c >= 0 && c <= kCoreMax && m >= 0 && m <= kMemMax;
+                sSumC[warp][j] = c;
+                sSumM[warp][j] = m;
+            }
+            __syncwarp();
+            const int32_t q0 = __ldg(a.roff + __ldg(a.noff + n)), q1 = __ldg(a.roff + __ldg(a.noff + n + 1));
+            for (int32_t c = q0 + lane; ok && c < q1; c += 32) {
+                const int d = __ldg(a.qd + c);
+                const int32_t core = __ldg(a.qc + c), mem = __ldg(a.qm + c);
+                ok = d >= 0 && d < dv && core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
+                if (ok) {
+                    atomicAdd(&sSumC[warp][d], core);
+                    atomicAdd(&sSumM[warp][d], mem);
+                }
+            }
+            __syncwarp();
+            for (int j = lane; ok && j < dv; j += 32) ok = sSumC[warp][j] <= kCoreMax && sSumM[warp][j] <= kMemMax;
+            ok = __all_sync(0xffffffffu, ok);
+            if (lane == 0) a.usable[n] = ok ? 1u : 0u;
+            __syncwarp();
+        }
+    }
+    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+    done = *reinterpret_cast<volatile unsigned int*>(&a.ctl->in_domain) == 0u;
+
+    while (!done) {
+        ++round;
+        // ---- 1a. / 1b. choose: (pod, chunk) items, chunk-major
+        for (int pass = 0; pass < 2; ++pass) {
+            // this round's count was round - 2's, which every CTA read before the barriers of round - 1
+            if (pass == 1 && b == 0 && tid == 0) a.ctl->deferred[round & 1] = 0u;
+            const long long items = static_cast<long long>(K) * a.G;
+            for (long long it = items * b / G, hi = items * (b + 1) / G; it < hi; ++it) {
+                const long long g = it % a.G, k = it / a.G;
+                if (__ldcg(a.node + g) != -2) continue;
+                if (pass == 1 && __ldcg(a.has_empty + g)) continue;
+                const int32_t c0 = __ldg(a.off + g), len = __ldg(a.off + g + 1) - c0, p = __ldg(a.prio + g);
+                PreKey best = none;
+                for (long long n = N * k / K + warp, n1 = N * (k + 1) / K; n < n1; n += kTabWarps) {
+                    const int rows = __ldcg(a.usable + n) ? __ldg(a.dv + n) : 0;
+                    if (!rows) continue;
+                    WarpTab t = load_tab(a, static_cast<int>(n), rows);
+                    uint32_t slc, slm;
+                    unsigned long long cdev;
+                    unsigned int used;
+                    PreKey key = none;
+                    if (pass == 0) {
+                        if (warp_replay(t, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used))
+                            key = PreKey{0ull, 0ull,
+                                         (((static_cast<unsigned long long>(slc) << 21) | slm) << 31) |
+                                             static_cast<unsigned long long>(n)};
+                    } else {
+                        unsigned int in_v;
+                        pre_victims(a, t, rows, p, c0, len, __ldg(a.noff + n), __ldg(a.noff + n + 1),
+                                    static_cast<int>(n), in_v, key, cdev);
+                    }
+                    if (pre_less(key, best)) best = key;
+                }
+                if (lane == 0) sKey[warp] = best;
+                __syncthreads();
+                if (tid == 0) {
+                    for (int w = 1; w < kTabWarps; ++w)
+                        if (pre_less(sKey[w], best)) best = sKey[w];
+                    unsigned long long* r = a.rec + 3 * (g * K + k);
+                    r[0] = best.a;
+                    r[1] = best.b;
+                    r[2] = best.c;
+                    if (pass == 0 && best.a == 0ull) a.has_empty[g] = 1u;
+                }
+                __syncthreads();
+            }
+            if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+        }
+
+        // ---- 2. reduce: each pending pod's smallest record
+        for (long long g = first; g < a.G; g += stride) {
+            if (__ldcg(a.node + g) != -2) continue;
+            PreKey best = none;
+            for (int k = 0; k < K; ++k) {
+                const unsigned long long* r = a.rec + 3 * (g * K + k);
+                const PreKey key{__ldcg(r), __ldcg(r + 1), __ldcg(r + 2)};
+                if (pre_less(key, best)) best = key;
+            }
+            a.has_empty[g] = 0u;
+            if (best.a == ~0ull) {  // fits no node when scored: -1 for good
+                a.choice[g] = ~0ull;
+                a.node[g] = -1;
+                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
+            } else {
+                a.choice[g] = (best.a != 0ull ? 1ull << 32 : 0ull) | (best.c & 0x7fffffffull);
+            }
+        }
+        if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+
+        // ---- 3. commit: per node, the pods that chose it in pod order
+        for (long long n = wfirst; n < N; n += wstride) {
+            const int rows = __ldcg(a.usable + n) ? __ldg(a.dv + n) : 0;
+            if (!rows) continue;  // no pod chose it: it keeps its copy
+            WarpTab t = load_tab(a, static_cast<int>(n), rows);
+            int32_t acc_c[2] = {0, 0}, acc_m[2] = {0, 0};
+            unsigned int closed = 0;  // the lane's devices a pod that did not commit chose
+            bool node_closed = false, chosen = false, dirty = false;
+            unsigned int deferred = 0;
+            const long long h0 = __ldg(a.noff + n), h1 = __ldg(a.noff + n + 1);
+            for (long long g0 = 0; g0 < a.G; g0 += 32) {
+                const long long gl = g0 + lane;
+                unsigned long long ch = ~0ull;
+                if (gl < a.G && __ldcg(a.node + gl) == -2) ch = __ldcg(a.choice + gl);
+                for (unsigned int mb = __ballot_sync(0xffffffffu, (ch & 0xffffffffull) == static_cast<unsigned long long>(n));
+                     mb; mb &= mb - 1u) {
+                    const int j = __ffs(mb) - 1;
+                    const long long g = g0 + j;
+                    const bool evicts = (__shfl_sync(0xffffffffu, ch, j) >> 32) != 0ull;
+                    if (node_closed || (evicts && chosen)) {
+                        chosen = true;
+                        node_closed |= evicts;
+                        ++deferred;
+                        continue;
+                    }
+                    chosen = true;
+                    const int32_t c0 = __ldg(a.off + g), len = __ldg(a.off + g + 1) - c0;
+                    WarpTab w = t;
+                    unsigned long long cdev;
+                    bool commit = true;
+                    if (!evicts) {  // §2.12: no closed device, and the demand fits on top of what committed before
+                        uint32_t slc, slm;
+                        unsigned int used;
+                        warp_replay(w, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used);
+                        bool ok = true;
+#pragma unroll
+                        for (int i = 0; i < 2; ++i)
+                            if ((used >> i) & 1u)
+                                ok &= !((closed >> i) & 1u) && acc_c[i] <= w.c[i] && acc_m[i] <= w.m[i];
+                        commit = __all_sync(0xffffffffu, ok);
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            if (commit) {
+                                acc_c[i] += t.c[i] - w.c[i];
+                                acc_m[i] += t.m[i] - w.m[i];
+                            } else {
+                                closed |= used;
+                            }
+                        }
+                    } else {  // the first pod of the round on n: evict V, then take the pod's demand
+                        unsigned int in_v;
+                        PreKey key;
+                        pre_victims(a, w, rows, __ldg(a.prio + g), c0, len, h0, h1, static_cast<int>(n), in_v, key, cdev);
+#pragma unroll
+                        for (int i = 0; i < 4; ++i)
+                            if ((in_v >> i) & 1u) a.evicted[h0 + lane + 32 * i] = static_cast<int32_t>(g);
+                        t = w;
+                        node_closed = true;
+                    }
+                    if (commit) {
+                        if (lane == 0) a.node[g] = static_cast<int32_t>(n);
+                        if (lane < len) a.dev[c0 + lane] = static_cast<int8_t>((cdev >> (6 * lane)) & 63u);
+                        dirty = true;
+                    } else {
+                        ++deferred;
+                    }
+                }
+            }
+            if (dirty) {
+                const size_t off = static_cast<size_t>(n) * D;
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (lane + 32 * i < rows) {
+                        a.fc_out[off + lane + 32 * i] = t.c[i] - acc_c[i];
+                        a.fm_out[off + lane + 32 * i] = t.m[i] - acc_m[i];
+                    }
+            }
+            if (lane == 0 && deferred) atomicAdd(&a.ctl->deferred[round & 1], deferred);
+        }
+        if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+        done = *reinterpret_cast<volatile unsigned int*>(&a.ctl->deferred[round & 1]) == 0u;
+    }
+finish:
+    if (b == 0 && tid == 0) {
+        const bool bad = *reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_index) != 0u;
+        a.info[0] = !bad && *reinterpret_cast<volatile unsigned int*>(&a.ctl->in_domain) ? round : 0;
+        a.info[1] = done ? 0 : 1;
+        a.info[2] = bad ? 1 : 0;
+    }
+}
+
+static int preempt_chunks(int N) { return std::max(1, std::min(kPreChunks, (N + kTabWarps - 1) / kTabWarps)); }
+
+size_t preempt_scratch_bytes(int N, int G) {
+    const size_t zeroed = sizeof(PreemptCtl) + 4 * static_cast<size_t>(G);
+    return ((zeroed + 15) & ~size_t(15)) + 24 * static_cast<size_t>(G) * preempt_chunks(N) + 8 * static_cast<size_t>(G) +
+           4 * static_cast<size_t>(N);
+}
+
+cudaError_t preempt_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
+                           const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets,
+                           const int32_t* pod_prio, int G, const int32_t* run_core, const int32_t* run_mem,
+                           const int8_t* run_dev, int Q, const int32_t* run_offsets, const int32_t* run_prio, int H,
+                           const int32_t* node_offsets, int32_t* out_node, int8_t* out_dev, int32_t* out_evicted,
+                           int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch, int device,
+                           cudaStream_t stream) {
+    // scratch: barrier words | has_empty uint32[G] | (16-aligned) records uint64[G][K][3] | choice uint64[G] |
+    // usable uint32[N]; everything before the records starts at zero
+    const int K = preempt_chunks(N);
+    char* s = static_cast<char*>(scratch);
+    PreemptArgs a{};
+    a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem; a.off = pod_offsets;
+    a.prio = pod_prio; a.qc = run_core; a.qm = run_mem; a.qd = run_dev; a.roff = run_offsets; a.rprio = run_prio;
+    a.noff = node_offsets;
+    a.N = N; a.D = D; a.K = K; a.P = P; a.G = G; a.Q = Q; a.H = H;
+    a.node = out_node; a.dev = out_dev; a.evicted = out_evicted; a.fc_out = free_core_out; a.fm_out = free_mem_out;
+    a.info = info;
+    a.ctl = reinterpret_cast<PreemptCtl*>(s);
+    a.has_empty = reinterpret_cast<unsigned int*>(s + sizeof(PreemptCtl));
+    const size_t zeroed = sizeof(PreemptCtl) + 4 * static_cast<size_t>(G);
+    a.rec = reinterpret_cast<unsigned long long*>(s + ((zeroed + 15) & ~size_t(15)));
+    a.choice = a.rec + 3 * static_cast<size_t>(G) * K;
+    a.usable = reinterpret_cast<unsigned int*>(a.choice + G);
+    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    if (err != cudaSuccess) return err;
+
+    // resident CTAs per SM on each device, asked once
+    static std::atomic<int> per_sm_cache[kPlaceDevices];
+    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
+    if (per_sm == 0) {
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, preempt_pods_kernel, kTabThreads, 0);
+        if (err != cudaSuccess) return err;
+        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
+        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
+    }
+    int sms = 0;
+    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err != cudaSuccess) return err;
+    // Grid: one resident wave, no more CTAs than round 1 has choose items; at least one, which finds G = 0's offsets
+    // bad.
+    long long grid = static_cast<long long>(sms) * per_sm;
+    grid = std::max(1ll, std::min(grid, static_cast<long long>(K) * G));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.blockDim = dim3(kTabThreads);
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, preempt_pods_kernel, a);
+}
+
 }  // namespace egpu

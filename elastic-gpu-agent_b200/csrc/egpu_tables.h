@@ -1,6 +1,6 @@
 // egpu_tables.h — launchers of the multi-table best-fit scan and placements (egpu_tables.cu), called by the
-// PyTorch operators egpu::bestfit_tables, egpu::place_tables, egpu::place_pods and egpu::place_gangs
-// (egpu_tables_op.cc).  Not part of the C ABI of include/.
+// PyTorch operators egpu::bestfit_tables, egpu::place_tables, egpu::place_pods, egpu::place_gangs and
+// egpu::preempt_pods (egpu_tables_op.cc).  Not part of the C ABI of include/.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -57,5 +57,24 @@ cudaError_t gangs_launch(const int32_t* free_core, const int32_t* free_mem, cons
                          const int32_t* gang_offsets, const int32_t* gang_min, int J, int32_t* out_node, int8_t* out_dev,
                          int32_t* out_placed, int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch,
                          int device, cudaStream_t stream);
+
+// Bytes of device scratch preempt_launch needs for G pods on N tables (16-byte aligned, from the caller's allocator).
+size_t preempt_scratch_bytes(int N, int G);
+
+// Places G pods of P containers on N tables as pods_launch, evicting lower-priority running pods where a pod fits no
+// table as it is (DESIGN.md §2.14), in one cooperative launch.  Tables, containers and pod_offsets as pods_launch;
+// pod_prio: int32[G]; running containers run_core / run_mem: int32[Q], run_dev: int8[Q]; run_offsets: int32[H + 1];
+// run_prio: int32[H]; node_offsets: int32[N + 1].  The kernel checks the three offset tensors before it reads anything
+// through them.  out_node: int32[G]; out_dev: int8[P]; out_evicted: int32[H]; free_core_out / free_mem_out:
+// int32[N][D]; info: int32[3].  scratch: preempt_scratch_bytes(N, G) bytes; its head is zeroed here on `stream`.
+// N >= 1, P >= 1, G >= 0, Q >= 0, H >= 0.  Asynchronous on `stream`; returns the first error of the memset or the
+// launch.
+cudaError_t preempt_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
+                           const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets,
+                           const int32_t* pod_prio, int G, const int32_t* run_core, const int32_t* run_mem,
+                           const int8_t* run_dev, int Q, const int32_t* run_offsets, const int32_t* run_prio, int H,
+                           const int32_t* node_offsets, int32_t* out_node, int8_t* out_dev, int32_t* out_evicted,
+                           int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch, int device,
+                           cudaStream_t stream);
 
 }  // namespace egpu

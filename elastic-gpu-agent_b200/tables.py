@@ -1,6 +1,6 @@
 """Best fit of many pending requests against many capacity tables in one launch: the PyTorch operators
 `egpu::bestfit_tables` (DESIGN.md §2.10), `egpu::place_tables` (§2.11), `egpu::place_pods` (§2.12) and
-`egpu::place_gangs` (§2.13).
+`egpu::place_gangs` (§2.13) and `egpu::preempt_pods` (§2.14).
 
 A scheduler scores every pending pod against every node's device table; `bestfit_tables` does all N x P
 pairs in one CUDA launch on the current stream instead of N `egpu_bestfit_query` calls.  `place_tables`
@@ -8,7 +8,8 @@ places the pods: best-fit rounds of prefix-commit to the fixed point over every 
 launch, so that no device is oversubscribed.  `place_pods` does the same for pods of several containers, every
 container of a pod on one node.  `place_gangs` places jobs (gangs of pods) in queue order, each kept only when at
 least its `minAvailable` pods are placed and given back otherwise, so that no job holds capacity it cannot start
-with.  The kernels live in csrc/egpu_tables.cu and are built by
+with.  `preempt_pods` places pods as `place_pods` does, and where a pod fits no node as it is, evicts the fewest,
+lowest-priority running pods of one node that make it fit.  The kernels live in csrc/egpu_tables.cu and are built by
 __graft_entry__.build() as lib/libegpu_tables.so; it is separate from libegpu_alloc.so and its C ABI,
 reads no context and writes no table of a context.  Importing this module does not load the library; the
 first call (or `load()`) does, and a missing library raises: there is no fallback.
@@ -24,6 +25,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libegpu_tables.so")
 
 MAX_DEVICES = 64
 MAX_POD = 8  # containers per pod (place_pods)
+MAX_RUN = 128  # running pods per node (preempt_pods)
 CORE_MAX = 100
 MEM_MAX = (1 << 18) - 1
 NO_KEY = 0x7FFFFFFF  # key of a pair with no feasible device
@@ -32,8 +34,8 @@ _loaded = False
 
 
 def load() -> None:
-    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables, egpu::place_tables, egpu::place_pods and
-    egpu::place_gangs) and the operators' fake implementations."""
+    """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables, egpu::place_tables, egpu::place_pods,
+    egpu::place_gangs and egpu::preempt_pods) and the operators' fake implementations."""
     global _loaded
     if _loaded:
         return
@@ -46,6 +48,7 @@ def load() -> None:
     torch.library.register_fake("egpu::place_tables")(_fake_place)
     torch.library.register_fake("egpu::place_pods")(_fake_pods)
     torch.library.register_fake("egpu::place_gangs")(_fake_gangs)
+    torch.library.register_fake("egpu::preempt_pods")(_fake_preempt)
     _loaded = True
 
 
@@ -332,3 +335,144 @@ def place_gangs(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.
         check_gangs(gang_offsets, gang_min, pod_offsets.shape[0] - 1)
     return torch.ops.egpu.place_gangs(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_offsets,
                                       gang_min)
+
+
+def check_preempt_args(free_core, pod_offsets, pod_prio, run_core, run_mem, run_dev, run_offsets, run_prio,
+                       node_offsets) -> None:
+    """preempt_pods' checks on the six new tensors' dtype, layout, shapes and device (no data is read), after
+    check_args and check_pod_args and in the operator's order: RuntimeError for a dtype, layout or device,
+    ValueError for a shape."""
+    op = "preempt_pods"
+    for name, t, dt in (("pod_prio", pod_prio, torch.int32), ("run_core", run_core, torch.int32),
+                        ("run_mem", run_mem, torch.int32), ("run_dev", run_dev, torch.int8),
+                        ("run_offsets", run_offsets, torch.int32), ("run_prio", run_prio, torch.int32),
+                        ("node_offsets", node_offsets, torch.int32)):
+        if t.dtype != dt:
+            raise RuntimeError(f"{op}: {name} must be {str(dt).replace('torch.', '')}, got {t.dtype}")
+        if not t.is_contiguous():
+            raise RuntimeError(f"{op}: {name} must be contiguous")
+    N, G = free_core.shape[0], pod_offsets.shape[0] - 1
+    if pod_prio.dim() != 1 or pod_prio.shape[0] != G:
+        raise ValueError(f"{op}: pod_prio must be [G] = [{G}], got {tuple(pod_prio.shape)}")
+    if run_core.dim() != 1 or run_mem.shape != run_core.shape or run_dev.shape != run_core.shape:
+        raise ValueError(f"{op}: run_core, run_mem and run_dev must all be [Q], got {tuple(run_core.shape)}, "
+                         f"{tuple(run_mem.shape)} and {tuple(run_dev.shape)}")
+    if run_offsets.dim() != 1 or run_offsets.shape[0] < 1:
+        raise ValueError(f"{op}: run_offsets must be [H + 1], got {tuple(run_offsets.shape)}")
+    Q, H = run_core.shape[0], run_offsets.shape[0] - 1
+    if Q >= 2**31 - 1 or H >= 2**31 - 1:
+        raise ValueError(f"{op}: Q and H + 1 must be below 2^31, got {Q} and {H + 1}")
+    if run_prio.dim() != 1 or run_prio.shape[0] != H:
+        raise ValueError(f"{op}: run_prio must be [H] = [{H}], got {tuple(run_prio.shape)}")
+    if node_offsets.dim() != 1 or node_offsets.shape[0] != N + 1:
+        raise ValueError(f"{op}: node_offsets must be [N + 1] = [{N + 1}], got {tuple(node_offsets.shape)}")
+    for t in (pod_prio, run_core, run_mem, run_dev, run_offsets, run_prio, node_offsets):
+        if t.device.type != "cuda" or t.device != free_core.device:
+            raise RuntimeError(f"{op}: every tensor must be on one CUDA device, got {t.device} and {free_core.device}")
+
+
+def check_running(free_core, free_mem, d_valid, run_core, run_mem, run_dev, run_offsets, node_offsets) -> None:
+    """ValueError unless run_offsets lists running pods of 1 to MAX_POD containers covering all Q containers (first
+    0, last Q, every step in [1, MAX_POD]), node_offsets lists 0 to MAX_RUN running pods per node covering all H
+    (first 0, last H, every step in [0, MAX_RUN]), and every node's running data is consistent: each run_dev in
+    [0, d_valid[n]), each running container in the request domain, and on each device free plus the demand of its
+    running containers within the table domain.  Reads the data: one host round trip."""
+    op = "preempt_pods"
+    ro, no = run_offsets.to(torch.int64).cpu(), node_offsets.to(torch.int64).cpu()
+    Q, H = run_core.shape[0], ro.shape[0] - 1
+    if int(ro[0]) != 0:
+        raise ValueError(f"{op}: run_offsets must start at 0, got {int(ro[0])}")
+    if int(ro[-1]) != Q:
+        raise ValueError(f"{op}: run_offsets must end at Q = {Q}, got {int(ro[-1])}")
+    step = ro[1:] - ro[:-1]
+    bad = int(((step < 1) | (step > MAX_POD)).sum())
+    if bad:
+        raise ValueError(f"{op}: {bad} running pod(s) with a container count outside [1, {MAX_POD}]")
+    if int(no[0]) != 0:
+        raise ValueError(f"{op}: node_offsets must start at 0, got {int(no[0])}")
+    if int(no[-1]) != H:
+        raise ValueError(f"{op}: node_offsets must end at H = {H}, got {int(no[-1])}")
+    step = no[1:] - no[:-1]
+    bad = int(((step < 0) | (step > MAX_RUN)).sum())
+    if bad:
+        raise ValueError(f"{op}: {bad} node(s) with a running pod count outside [0, {MAX_RUN}]")
+    if Q == 0:
+        return
+    N, D = free_core.shape
+    dev = free_core.device
+    pod_of = torch.repeat_interleave(torch.arange(H), ro[1:] - ro[:-1])
+    node_of = torch.repeat_interleave(torch.arange(N), no[1:] - no[:-1])[pod_of].to(dev)
+    d = run_dev.to(torch.int64)
+    bad_c = (d < 0) | (d >= d_valid.to(torch.int64)[node_of]) | (run_core < 0) | (run_core > CORE_MAX) | \
+        (run_mem < 0) | (run_mem > MEM_MAX)
+    flat = node_of * D + d.clamp(0, D - 1)
+    tot_c = free_core.to(torch.int64).flatten().index_add(0, flat, run_core.to(torch.int64))
+    tot_m = free_mem.to(torch.int64).flatten().index_add(0, flat, run_mem.to(torch.int64))
+    over = ((tot_c > CORE_MAX) | (tot_m > MEM_MAX)).view(N, D)
+    live = torch.arange(D, device=dev)[None, :] < d_valid.to(torch.int64)[:, None]
+    bad_n = torch.zeros(N, dtype=torch.int64, device=dev).index_add(0, node_of, bad_c.to(torch.int64)) > 0
+    bad = int((bad_n | (over & live).any(dim=1)).sum())
+    if bad:
+        raise ValueError(f"{op}: {bad} node(s) with inconsistent running data (run_dev outside [0, d_valid), a "
+                         f"running container outside the domain, or free plus running demand outside the domain)")
+
+
+def _fake_preempt(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, pod_prio, run_core, run_mem, run_dev,
+                  run_offsets, run_prio, node_offsets):
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op="preempt_pods")
+    check_pod_args(free_core, pod_offsets, op="preempt_pods")
+    check_preempt_args(free_core, pod_offsets, pod_prio, run_core, run_mem, run_dev, run_offsets, run_prio,
+                       node_offsets)
+    G, P, H = pod_offsets.shape[0] - 1, req_core.shape[0], run_offsets.shape[0] - 1
+    return (pod_offsets.new_empty((G,), dtype=torch.int32), req_core.new_empty((P,), dtype=torch.int8),
+            run_offsets.new_empty((H,), dtype=torch.int32), torch.empty_like(free_core), torch.empty_like(free_mem),
+            free_core.new_empty((3,), dtype=torch.int32))
+
+
+def preempt_pods(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.Tensor, req_core: torch.Tensor,
+                 req_mem: torch.Tensor, pod_offsets: torch.Tensor, pod_prio: torch.Tensor, run_core: torch.Tensor,
+                 run_mem: torch.Tensor, run_dev: torch.Tensor, run_offsets: torch.Tensor, run_prio: torch.Tensor,
+                 node_offsets: torch.Tensor):
+    """Place G pods on N capacity tables in one launch as place_pods does, evicting the fewest, lowest-priority
+    running pods of one node where a pod fits no node as it is (DESIGN.md §2.14).
+
+    Tables, containers and pod_offsets as place_pods; pod_prio int32[G] is each pod's priority.  The running pods:
+    running pod h holds containers run_offsets[h] .. run_offsets[h + 1] - 1 (run_core, run_mem int32[Q], run_dev
+    int8[Q] the device on its node; 1 to MAX_POD containers per pod) and has priority run_prio[h]; node n holds
+    running pods node_offsets[n] .. node_offsets[n + 1] - 1 (0 to MAX_RUN), oldest first.  The tables are what is
+    free with the running pods in place.
+
+    Pod g's victims on node n: none when its in-node replay fits table n as it is; otherwise C, the alive running
+    pods of n below pod_prio[g], if the replay fits table n plus C's demand (else n is no candidate), less each member
+    of C, walked by (priority descending, h ascending), without which the replay still fits.  The pod takes the
+    candidate with the smallest (highest victim priority, sum of (priority + 2^31), victims, sum lc, sum lm, n); no
+    victim ranks below every victim.  Per node, in pod order: a pod without victims commits as in place_pods; a pod
+    with victims commits only when it is the first of the round to choose the node, evicts them and takes its demand,
+    and closes the node for the round either way.  Deferred pods are scored again against the tables and running pods
+    the round left, until a round defers nothing.  With no pod above any running pod the outputs are place_pods'.
+
+    Returns (node int32[G], dev int8[P], evicted int32[H], free_core_out int32[N, D], free_mem_out int32[N, D],
+    info int32[3]): node and dev as place_pods; evicted[h] the pod that evicted running pod h, or -1; the tables
+    after every eviction and placement, assuming the evicted pods are gone; info = [rounds run (0 when no pod is in
+    the domain), 1 if a grid wait gave up after ~2 s else 0, 1 if the kernel refused an index tensor else 0].  When a
+    wait gives up the outputs are not a placement and the caller must discard them.  The inputs are not written.
+    N = 0 or P = 0 gives -1 placements, evicted all -1, copied tables and info [0, 0, 0].
+
+    Stateless and asynchronous on the current stream; it captures into a CUDA graph and traces under
+    torch.compile(fullgraph=True).  Refusals are place_pods' with "preempt_pods" in the messages, then the six new
+    tensors' dtype, layout, shapes and device.  Eagerly this function also checks the tables, pod_offsets, and the
+    running pods (check_running; ValueError), which reads them back; during capture or tracing the kernel checks the
+    three offset tensors itself and, if one is bad, places and evicts nothing: all -1, tables copied, info = [0, 0, 1];
+    a node whose table is outside the domain or whose running data is inconsistent offers no candidate and is copied.
+    """
+    load()
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op="preempt_pods")
+    check_pod_args(free_core, pod_offsets, op="preempt_pods")
+    check_preempt_args(free_core, pod_offsets, pod_prio, run_core, run_mem, run_dev, run_offsets, run_prio,
+                       node_offsets)
+    if not torch.compiler.is_compiling() and not torch.cuda.is_current_stream_capturing():
+        check_tables(free_core, free_mem, d_valid, op="preempt_pods")
+        check_pods(pod_offsets, req_core.shape[0], op="preempt_pods")
+        check_running(free_core, free_mem, d_valid, run_core, run_mem, run_dev, run_offsets, node_offsets)
+    return torch.ops.egpu.preempt_pods(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, pod_prio, run_core,
+                                       run_mem, run_dev, run_offsets, run_prio, node_offsets)
