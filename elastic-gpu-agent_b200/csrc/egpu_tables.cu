@@ -2060,4 +2060,691 @@ cudaError_t preempt_launch(const int32_t* free_core, const int32_t* free_mem, co
     return cudaLaunchKernelEx(&cfg, preempt_pods_kernel, a);
 }
 
+// ---- egpu::preempt_gangs (DESIGN.md §2.15, §4.10): gangs with priority preemption, in gang order ----
+//
+// One cooperative launch.  The outer loop over gangs is place_gangs_kernel's; a gang's rounds are preempt_pods_kernel's
+// phases over the gang's pending pods (node = -2 inside [gang_offsets[j], gang_offsets[j + 1])), with two changes:
+//   0. as preempt_pods, plus gang_offsets, gang_min, run_gang and run_gang_min checked before anything is read through
+//      them.  After the check's barrier, each gang's pods in the domain and each running job's alive pods are counted;
+//      a job's slack is max(0, alive - run_gang_min) wherever it is read, so evictions and their undoing only move
+//      the alive count;
+//   1a. before the choose items, one warp per usable node writes the capped C (§2.15 rule 1) as a 128-bit slot mask
+//       from the round-start slacks; 1b's reprieve walk starts from that mask (pre_victims_capped);
+//   3.  commit: as preempt_pods, except that a first-on-node preemptor with a victim in a running job only records
+//       its victims and devices and flags the round.  In a flagged round one warp then walks the gang's recorded
+//       preemptors in pod order and counts their victims per job (§2.15 rule 2; a pod passes when no atomicAdd of its
+//       own victims finds the count at the job's slack), and after another barrier the passing ones are applied, one
+//       warp per pod.  Unflagged rounds (every round when no running pod is in a job) skip both barriers;
+//   end of a gang: placed + deferred < gang_min or nothing deferred ends it.  A gang given back is rolled back by
+//   integer atomics: its pods' demand returns to the tables, and every running pod it evicted is alive again, its
+//   demand taken from the tables and its job's count restored; one barrier follows before the next gang reads them.
+struct PreGangsCtl {
+    RoundsCtl bar;                // grid-barrier words
+    unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
+    unsigned int bad_index;       // an index tensor or run_gang_min failed the check (info[2])
+    unsigned int deferred[2];     // pods deferred by a round's commit, by round parity
+    unsigned int budget[2];       // a round recorded a preemptor with a victim in a running job, by round parity
+    unsigned int pad_[3];
+};
+
+struct PreGangsArgs {
+    PreemptArgs p;               // tables, containers, pod_offsets, running pods, the outputs node, dev, evicted,
+                                 // tables and info, and the scratch rec, choice, has_empty, usable (p.prio, p.ctl unused)
+    const int32_t* goff;         // gang_offsets [J + 1], gang_min [J], gang_prio [J], run_gang [H], run_gang_min [R]
+    const int32_t* gmin;
+    const int32_t* gprio;
+    const int32_t* rgang;
+    const int32_t* rgmin;
+    long long J, R;
+    int32_t* placed;             // output: placed pods per gang [J]
+    unsigned int* in_domain;     // [J]: each gang's pods in the domain
+    unsigned int* committed;     // [J]: each gang's committed pods
+    int32_t* alive;              // [R]: each running job's pods not evicted
+    int32_t* used;               // [R]: the budget pass's victims per job, zeroed again by the apply phase
+    unsigned int* pre;           // [G]: 1 a preemptor waiting for the budget, 2 it passed, 0 otherwise
+    unsigned int* vmask;         // [G][4]: a waiting preemptor's victims by slot (bit lane of word i: slot lane + 32 i)
+    unsigned long long* vdev;    // [G]: a waiting preemptor's devices
+    unsigned int* cap;           // [N][4]: the round's capped C per node, by slot
+    PreGangsCtl* ctl;
+};
+
+// pre_victims with C given: cand holds the lane's slots of C (bit i: slot lane + 32 i).  The same walk, key and
+// result.
+__device__ __forceinline__ bool pre_victims_capped(const PreemptArgs& a, WarpTab& t, int rows, unsigned int cand,
+                                                   long long c0, int len, long long h0, long long h1, int n,
+                                                   unsigned int& in_v, PreKey& k, unsigned long long& cdev) {
+    const int lane = threadIdx.x & 31;
+    if (!__any_sync(0xffffffffu, cand != 0u)) return false;
+    uint32_t q[4];  // priority + 2^31: its unsigned order is the priority's
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const long long h = h0 + lane + 32 * i;
+        q[i] = h < h1 ? static_cast<uint32_t>(__ldg(a.rprio + h)) ^ 0x80000000u : 0u;
+    }
+    WarpTab base = t;  // the table plus the demand of V
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+        for (unsigned int m = __ballot_sync(0xffffffffu, (cand >> i) & 1u); m; m &= m - 1u)
+            add_running(a, base, h0 + (__ffs(m) - 1) + 32 * i, 1);
+    WarpTab w = base;
+    uint32_t slc, slm;
+    unsigned int used;
+    if (!warp_replay(w, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used)) return false;
+    in_v = cand;
+    unsigned int left = cand;
+    while (__any_sync(0xffffffffu, left != 0u)) {
+        uint32_t bq = 0;
+        int bi = 4;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+            if (((left >> i) & 1u) && (bi == 4 || q[i] > bq)) {
+                bq = q[i];
+                bi = i;
+            }
+        const uint32_t top = __reduce_max_sync(0xffffffffu, bi < 4 ? bq : 0u);
+        const uint32_t at = __reduce_min_sync(0xffffffffu, bi < 4 && bq == top ? static_cast<uint32_t>(lane + 32 * bi) : ~0u);
+        const int slot = static_cast<int>(at >> 5), owner = static_cast<int>(at & 31u);
+        if (lane == owner) left &= ~(1u << slot);
+        WarpTab trial = base;
+        add_running(a, trial, h0 + at, -1);
+        WarpTab tw = trial;
+        uint32_t tlc, tlm;
+        unsigned long long tdev;
+        if (warp_replay(tw, rows, a.rc, a.rm, c0, len, tlc, tlm, tdev, used)) {
+            base = trial;
+            w = tw;
+            slc = tlc;
+            slm = tlm;
+            cdev = tdev;
+            if (lane == owner) in_v &= ~(1u << slot);
+        }
+    }
+    uint32_t top = 0;
+    unsigned long long sum = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+        if ((in_v >> i) & 1u) {
+            top = max(top, q[i]);
+            sum += q[i];
+        }
+    top = __reduce_max_sync(0xffffffffu, top);
+    const unsigned int count = __reduce_add_sync(0xffffffffu, static_cast<unsigned int>(__popc(in_v)));
+#pragma unroll
+    for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    k.a = static_cast<unsigned long long>(top) + 1ull;
+    k.b = (sum << 8) | count;
+    k.c = (((static_cast<unsigned long long>(slc) << 21) | slm) << 31) | static_cast<unsigned long long>(n);
+    t = w;
+    return true;
+}
+
+__global__ void __launch_bounds__(kTabThreads, 2)
+preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
+    __shared__ int32_t sSumC[kTabWarps][kMaxD], sSumM[kTabWarps][kMaxD];  // phase 0: free + running demand per device
+    __shared__ PreKey sKey[kTabWarps];
+    __shared__ int sOk;
+    const PreemptArgs& a = ga.p;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int N = a.N, D = a.D, K = a.K;
+    const long long stride = static_cast<long long>(G) * kTabThreads, first = static_cast<long long>(b) * kTabThreads + tid;
+    const long long wstride = static_cast<long long>(G) * kTabWarps, wfirst = static_cast<long long>(b) * kTabWarps + warp;
+    const PreKey none{~0ull, ~0ull, ~0ull};
+    unsigned int gen = 0;
+    int round = 0;  // rounds run by every gang so far: info[0], and the parity of the round counters
+    bool done = false;
+
+    // ---- 0. the five index tensors and run_gang_min checked before anything is read through them
+    {
+        bool bad = false;
+        for (long long g = first; g <= a.G; g += stride) {
+            const int32_t o = __ldg(a.off + g);
+            if (g == 0) bad |= o != 0;
+            if (g == a.G) bad |= o != a.P;
+            if (g < a.G) {
+                const long long step = static_cast<long long>(__ldg(a.off + g + 1)) - o;
+                bad |= step < 1 || step > kMaxPod;
+                a.node[g] = -2;
+            }
+        }
+        for (long long j = first; j <= ga.J; j += stride) {
+            const int32_t o = __ldg(ga.goff + j);
+            if (j == 0) bad |= o != 0;
+            if (j == ga.J) bad |= o != a.G;
+            if (j < ga.J) {
+                const long long size = static_cast<long long>(__ldg(ga.goff + j + 1)) - o;
+                const int32_t m = __ldg(ga.gmin + j);
+                bad |= size < 1 || m < 1 || m > size;
+                ga.placed[j] = 0;
+            }
+        }
+        for (long long h = first; h <= a.H; h += stride) {
+            const int32_t o = __ldg(a.roff + h);
+            if (h == 0) bad |= o != 0;
+            if (h == a.H) bad |= o != a.Q;
+            if (h < a.H) {
+                const long long step = static_cast<long long>(__ldg(a.roff + h + 1)) - o;
+                const int32_t r = __ldg(ga.rgang + h);
+                bad |= step < 1 || step > kMaxPod || r < -1 || r >= ga.R;
+                a.evicted[h] = -1;
+            }
+        }
+        for (long long n = first; n <= N; n += stride) {
+            const int32_t o = __ldg(a.noff + n);
+            if (n == 0) bad |= o != 0;
+            if (n == N) bad |= o != a.H;
+            if (n < N) {
+                const long long step = static_cast<long long>(__ldg(a.noff + n + 1)) - o;
+                bad |= step < 0 || step > kMaxRun;
+            }
+        }
+        for (long long r = first; r < ga.R; r += stride) bad |= __ldg(ga.rgmin + r) < 0;
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -2;
+        for (long long j = first; j < static_cast<long long>(N) * D; j += stride) {
+            a.fc_out[j] = a.fc[j];
+            a.fm_out[j] = a.fm[j];
+        }
+        if (__syncthreads_or(bad) && tid == 0) atomicExch(&ga.ctl->bad_index, 1u);
+    }
+    if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+    if (*reinterpret_cast<volatile unsigned int*>(&ga.ctl->bad_index)) {  // nothing is placed or evicted
+        for (long long g = first; g < a.G; g += stride) a.node[g] = -1;
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -1;
+        done = true;
+        goto finish;
+    }
+    {  // pods outside the domain are -1, the others counted into their gang; the usable nodes; the jobs' alive pods
+        for (long long g0 = static_cast<long long>(b) * kTabThreads; g0 < a.G; g0 += stride) {
+            const long long g = g0 + tid;
+            bool ok = g < a.G;
+            long long j = 0;
+            if (ok) {
+                const int32_t c0 = __ldg(a.off + g), c1 = __ldg(a.off + g + 1);
+                for (int32_t c = c0; c < c1; ++c) {
+                    const int32_t core = __ldg(a.rc + c), mem = __ldg(a.rm + c);
+                    ok &= core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
+                }
+                if (!ok) {
+                    a.node[g] = -1;
+                    for (int32_t c = c0; c < c1; ++c) a.dev[c] = -1;
+                }
+                long long lo = 0, hi = ga.J - 1;  // the last gang whose first pod is at or before g
+                while (lo < hi) {
+                    const long long mid = (lo + hi + 1) >> 1;
+                    if (__ldg(ga.goff + mid) <= g) lo = mid;
+                    else hi = mid - 1;
+                }
+                j = lo;
+            }
+            const unsigned int peers = __match_any_sync(0xffffffffu, ok ? j : -1ll);
+            if (ok && lane == __ffs(peers) - 1) atomicAdd(ga.in_domain + j, static_cast<unsigned int>(__popc(peers)));
+        }
+        for (long long h = first; h < a.H; h += stride) {
+            const int32_t r = __ldg(ga.rgang + h);
+            if (r >= 0) atomicAdd(ga.alive + r, 1);
+        }
+        for (long long n = wfirst; n < N; n += wstride) {
+            const int dv = __ldg(a.dv + n);
+            bool ok = dv >= 1 && dv <= D;
+            const size_t off = static_cast<size_t>(n) * D;
+            for (int j = lane; j < kMaxD; j += 32) {
+                const int32_t c = ok && j < dv ? __ldg(a.fc + off + j) : 0, m = ok && j < dv ? __ldg(a.fm + off + j) : 0;
+                ok &= c >= 0 && c <= kCoreMax && m >= 0 && m <= kMemMax;
+                sSumC[warp][j] = c;
+                sSumM[warp][j] = m;
+            }
+            __syncwarp();
+            const int32_t q0 = __ldg(a.roff + __ldg(a.noff + n)), q1 = __ldg(a.roff + __ldg(a.noff + n + 1));
+            for (int32_t c = q0 + lane; ok && c < q1; c += 32) {
+                const int d = __ldg(a.qd + c);
+                const int32_t core = __ldg(a.qc + c), mem = __ldg(a.qm + c);
+                ok = d >= 0 && d < dv && core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
+                if (ok) {
+                    atomicAdd(&sSumC[warp][d], core);
+                    atomicAdd(&sSumM[warp][d], mem);
+                }
+            }
+            __syncwarp();
+            for (int j = lane; ok && j < dv; j += 32) ok = sSumC[warp][j] <= kCoreMax && sSumM[warp][j] <= kMemMax;
+            ok = __all_sync(0xffffffffu, ok);
+            if (lane == 0) a.usable[n] = ok ? 1u : 0u;
+            __syncwarp();
+        }
+    }
+    if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+
+    for (long long gang = 0; gang < ga.J; ++gang) {
+        const int32_t g_lo = __ldg(ga.goff + gang), g_hi = __ldg(ga.goff + gang + 1), need = __ldg(ga.gmin + gang);
+        const int32_t p = __ldg(ga.gprio + gang);
+        const long long size = g_hi - g_lo;
+        bool gang_done = static_cast<long long>(__ldcg(ga.in_domain + gang)) < need;  // never rounds, nothing changes
+        if (gang_done)
+            for (long long g = g_lo + first; g < g_hi; g += stride) {
+                a.node[g] = -1;
+                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
+            }
+        while (!gang_done) {
+            ++round;
+            // ---- 1a. / 1b. choose: (pod, chunk) items over the gang's pods, chunk-major
+            for (int pass = 0; pass < 2; ++pass) {
+                if (pass == 0)  // the capped C of every usable node, from the round-start slacks
+                    for (long long n = wfirst; n < N; n += wstride) {
+                        if (!__ldcg(a.usable + n)) continue;
+                        const long long h0 = __ldg(a.noff + n), h1 = __ldg(a.noff + n + 1);
+                        bool in_c[4];
+                        int32_t job[4];
+                        uint32_t q[4];
+                        int later[4];
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const long long h = h0 + lane + 32 * i;
+                            in_c[i] = false;
+                            job[i] = -1;
+                            q[i] = 0;
+                            later[i] = 0;
+                            if (h < h1) {
+                                const int32_t r = __ldg(a.rprio + h);
+                                q[i] = static_cast<uint32_t>(r) ^ 0x80000000u;
+                                in_c[i] = r < p && __ldcg(a.evicted + h) == -1;
+                                job[i] = in_c[i] ? __ldg(ga.rgang + h) : -1;
+                            }
+                        }
+                        if (__any_sync(0xffffffffu, job[0] >= 0 || job[1] >= 0 || job[2] >= 0 || job[3] >= 0))
+                            // later[i]: the pods of C in slot i's job after it in the walk order (priority
+                            // descending, h ascending)
+                            for (int s = 0; s < static_cast<int>(h1 - h0); ++s) {
+                                const int si = s >> 5, src = s & 31;
+                                const int32_t js = __shfl_sync(0xffffffffu, si == 0 ? job[0] : si == 1 ? job[1] : si == 2 ? job[2] : job[3], src);
+                                const uint32_t qs = __shfl_sync(0xffffffffu, si == 0 ? q[0] : si == 1 ? q[1] : si == 2 ? q[2] : q[3], src);
+                                if (js < 0) continue;
+#pragma unroll
+                                for (int i = 0; i < 4; ++i)
+                                    later[i] += job[i] == js && (qs < q[i] || (qs == q[i] && s > lane + 32 * i));
+                            }
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            bool keep = in_c[i];
+                            if (keep && job[i] >= 0)
+                                keep = later[i] < __ldcg(ga.alive + job[i]) - __ldg(ga.rgmin + job[i]);
+                            const unsigned int m = __ballot_sync(0xffffffffu, keep);
+                            if (lane == 0) ga.cap[4 * n + i] = m;
+                        }
+                    }
+                if (pass == 1 && b == 0 && tid == 0) {  // round - 2's counters, read before round - 1's barriers
+                    ga.ctl->deferred[round & 1] = 0u;
+                    ga.ctl->budget[round & 1] = 0u;
+                }
+                const long long items = static_cast<long long>(K) * size;
+                for (long long it = items * b / G, hi = items * (b + 1) / G; it < hi; ++it) {
+                    const long long g = g_lo + it % size, k = it / size;
+                    if (__ldcg(a.node + g) != -2) continue;
+                    if (pass == 1 && __ldcg(a.has_empty + g)) continue;
+                    const int32_t c0 = __ldg(a.off + g), len = __ldg(a.off + g + 1) - c0;
+                    PreKey best = none;
+                    for (long long n = N * k / K + warp, n1 = N * (k + 1) / K; n < n1; n += kTabWarps) {
+                        const int rows = __ldcg(a.usable + n) ? __ldg(a.dv + n) : 0;
+                        if (!rows) continue;
+                        WarpTab t = load_tab(a, static_cast<int>(n), rows);
+                        uint32_t slc, slm;
+                        unsigned long long cdev;
+                        unsigned int used;
+                        PreKey key = none;
+                        if (pass == 0) {
+                            if (warp_replay(t, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used))
+                                key = PreKey{0ull, 0ull,
+                                             (((static_cast<unsigned long long>(slc) << 21) | slm) << 31) |
+                                                 static_cast<unsigned long long>(n)};
+                        } else {
+                            unsigned int cand = 0, in_v;
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) cand |= ((__ldcg(ga.cap + 4 * n + i) >> lane) & 1u) << i;
+                            pre_victims_capped(a, t, rows, cand, c0, len, __ldg(a.noff + n), __ldg(a.noff + n + 1),
+                                               static_cast<int>(n), in_v, key, cdev);
+                        }
+                        if (pre_less(key, best)) best = key;
+                    }
+                    if (lane == 0) sKey[warp] = best;
+                    __syncthreads();
+                    if (tid == 0) {
+                        for (int w = 1; w < kTabWarps; ++w)
+                            if (pre_less(sKey[w], best)) best = sKey[w];
+                        unsigned long long* r = a.rec + 3 * (g * K + k);
+                        r[0] = best.a;
+                        r[1] = best.b;
+                        r[2] = best.c;
+                        if (pass == 0 && best.a == 0ull) a.has_empty[g] = 1u;
+                    }
+                    __syncthreads();
+                }
+                if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+            }
+
+            // ---- 2. reduce: each pending pod's smallest record
+            for (long long g = g_lo + first; g < g_hi; g += stride) {
+                if (__ldcg(a.node + g) != -2) continue;
+                PreKey best = none;
+                for (int k = 0; k < K; ++k) {
+                    const unsigned long long* r = a.rec + 3 * (g * K + k);
+                    const PreKey key{__ldcg(r), __ldcg(r + 1), __ldcg(r + 2)};
+                    if (pre_less(key, best)) best = key;
+                }
+                a.has_empty[g] = 0u;
+                if (best.a == ~0ull) {  // fits no node when scored: -1 for good
+                    a.choice[g] = ~0ull;
+                    a.node[g] = -1;
+                    for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
+                } else {
+                    a.choice[g] = (best.a != 0ull ? 1ull << 32 : 0ull) | (best.c & 0x7fffffffull);
+                }
+            }
+            if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+
+            // ---- 3. commit: per node, the gang's pods that chose it in pod order
+            for (long long n = wfirst; n < N; n += wstride) {
+                const int rows = __ldcg(a.usable + n) ? __ldg(a.dv + n) : 0;
+                if (!rows) continue;  // no pod chose it: it keeps its copy
+                WarpTab t = load_tab(a, static_cast<int>(n), rows);
+                int32_t acc_c[2] = {0, 0}, acc_m[2] = {0, 0};
+                unsigned int closed = 0;  // the lane's devices a pod that did not commit chose
+                bool node_closed = false, chosen = false, dirty = false;
+                unsigned int deferred = 0, committed = 0;
+                const long long h0 = __ldg(a.noff + n), h1 = __ldg(a.noff + n + 1);
+                for (long long g0 = g_lo; g0 < g_hi; g0 += 32) {
+                    const long long gl = g0 + lane;
+                    unsigned long long ch = ~0ull;
+                    if (gl < g_hi && __ldcg(a.node + gl) == -2) ch = __ldcg(a.choice + gl);
+                    for (unsigned int mb = __ballot_sync(0xffffffffu, (ch & 0xffffffffull) == static_cast<unsigned long long>(n));
+                         mb; mb &= mb - 1u) {
+                        const int j = __ffs(mb) - 1;
+                        const long long g = g0 + j;
+                        const bool evicts = (__shfl_sync(0xffffffffu, ch, j) >> 32) != 0ull;
+                        if (node_closed || (evicts && chosen)) {
+                            chosen = true;
+                            node_closed |= evicts;
+                            ++deferred;
+                            continue;
+                        }
+                        chosen = true;
+                        const int32_t c0 = __ldg(a.off + g), len = __ldg(a.off + g + 1) - c0;
+                        WarpTab w = t;
+                        unsigned long long cdev;
+                        bool commit = true;
+                        if (!evicts) {  // §2.12: no closed device, and the demand fits on top of what committed before
+                            uint32_t slc, slm;
+                            unsigned int used;
+                            warp_replay(w, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used);
+                            bool ok = true;
+#pragma unroll
+                            for (int i = 0; i < 2; ++i)
+                                if ((used >> i) & 1u)
+                                    ok &= !((closed >> i) & 1u) && acc_c[i] <= w.c[i] && acc_m[i] <= w.m[i];
+                            commit = __all_sync(0xffffffffu, ok);
+#pragma unroll
+                            for (int i = 0; i < 2; ++i) {
+                                if (commit) {
+                                    acc_c[i] += t.c[i] - w.c[i];
+                                    acc_m[i] += t.m[i] - w.m[i];
+                                } else {
+                                    closed |= used;
+                                }
+                            }
+                            if (!commit) ++deferred;
+                        } else {  // the first pod of the round on n: its victims from the same capped C
+                            unsigned int cand = 0, in_v;
+                            PreKey key;
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) cand |= ((__ldcg(ga.cap + 4 * n + i) >> lane) & 1u) << i;
+                            pre_victims_capped(a, w, rows, cand, c0, len, h0, h1, static_cast<int>(n), in_v, key, cdev);
+                            bool in_job = false;
+#pragma unroll
+                            for (int i = 0; i < 4; ++i)
+                                if ((in_v >> i) & 1u) in_job |= __ldg(ga.rgang + h0 + lane + 32 * i) >= 0;
+                            node_closed = true;
+                            if (__any_sync(0xffffffffu, in_job)) {  // the budget pass decides
+#pragma unroll
+                                for (int i = 0; i < 4; ++i) {
+                                    const unsigned int m = __ballot_sync(0xffffffffu, (in_v >> i) & 1u);
+                                    if (lane == 0) ga.vmask[4 * g + i] = m;
+                                }
+                                if (lane == 0) {
+                                    ga.vdev[g] = cdev;
+                                    ga.pre[g] = 1u;
+                                    ga.ctl->budget[round & 1] = 1u;
+                                }
+                                continue;
+                            }
+#pragma unroll
+                            for (int i = 0; i < 4; ++i)
+                                if ((in_v >> i) & 1u) a.evicted[h0 + lane + 32 * i] = static_cast<int32_t>(g);
+                            t = w;
+                        }
+                        if (commit) {
+                            if (lane == 0) a.node[g] = static_cast<int32_t>(n);
+                            if (lane < len) a.dev[c0 + lane] = static_cast<int8_t>((cdev >> (6 * lane)) & 63u);
+                            dirty = true;
+                            ++committed;
+                        }
+                    }
+                }
+                if (dirty) {
+                    const size_t off = static_cast<size_t>(n) * D;
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+                        if (lane + 32 * i < rows) {
+                            a.fc_out[off + lane + 32 * i] = t.c[i] - acc_c[i];
+                            a.fm_out[off + lane + 32 * i] = t.m[i] - acc_m[i];
+                        }
+                }
+                if (lane == 0 && deferred) atomicAdd(&ga.ctl->deferred[round & 1], deferred);
+                if (lane == 0 && committed) atomicAdd(ga.committed + gang, committed);
+            }
+            if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+
+            if (*reinterpret_cast<volatile unsigned int*>(&ga.ctl->budget[round & 1])) {
+                // ---- 3b. the round budget: the recorded preemptors in pod order, their victims counted per job
+                if (b == 0 && warp == 0)
+                    for (long long g0 = g_lo; g0 < g_hi; g0 += 32) {
+                        const long long gl = g0 + lane;
+                        const bool waiting = gl < g_hi && __ldcg(ga.pre + gl) == 1u;
+                        for (unsigned int mb = __ballot_sync(0xffffffffu, waiting); mb; mb &= mb - 1u) {
+                            const long long g = g0 + __ffs(mb) - 1;
+                            const long long h0 = __ldg(a.noff + (__ldcg(a.choice + g) & 0x7fffffffull));
+                            bool over = false;
+#pragma unroll
+                            for (int i = 0; i < 4; ++i)
+                                if ((__ldcg(ga.vmask + 4 * g + i) >> lane) & 1u) {
+                                    const int32_t r = __ldg(ga.rgang + h0 + lane + 32 * i);
+                                    if (r >= 0)
+                                        over |= atomicAdd(ga.used + r, 1) >= __ldcg(ga.alive + r) - __ldg(ga.rgmin + r);
+                                }
+                            if (!__any_sync(0xffffffffu, over) && lane == 0) ga.pre[g] = 2u;
+                        }
+                    }
+                if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+
+                // ---- 3c. apply the preemptors that passed, one warp per pod; the others are deferred
+                unsigned int deferred = 0, committed = 0;
+                for (long long g = g_lo + wfirst; g < g_hi; g += wstride) {
+                    const unsigned int st = __ldcg(ga.pre + g);
+                    if (st == 0u) continue;
+                    const int n = static_cast<int>(__ldcg(a.choice + g) & 0x7fffffffull);
+                    const long long h0 = __ldg(a.noff + n);
+                    unsigned int in_v = 0;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) in_v |= ((__ldcg(ga.vmask + 4 * g + i) >> lane) & 1u) << i;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+                        if ((in_v >> i) & 1u) {
+                            const int32_t r = __ldg(ga.rgang + h0 + lane + 32 * i);
+                            if (r >= 0) {
+                                ga.used[r] = 0;
+                                if (st == 2u) atomicSub(ga.alive + r, 1);
+                            }
+                            if (st == 2u) a.evicted[h0 + lane + 32 * i] = static_cast<int32_t>(g);
+                        }
+                    if (lane == 0) ga.pre[g] = 0u;
+                    if (st != 2u) {
+                        deferred += lane == 0;
+                        continue;
+                    }
+                    const int rows = __ldg(a.dv + n);
+                    WarpTab t = load_tab(a, n, rows);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+                        for (unsigned int m = __ballot_sync(0xffffffffu, (in_v >> i) & 1u); m; m &= m - 1u)
+                            add_running(a, t, h0 + (__ffs(m) - 1) + 32 * i, 1);
+                    const int32_t c0 = __ldg(a.off + g), len = __ldg(a.off + g + 1) - c0;
+                    const unsigned long long cdev = __ldcg(ga.vdev + g);
+                    for (int k = 0; k < len; ++k) {
+                        const int d = static_cast<int>((cdev >> (6 * k)) & 63u);
+#pragma unroll
+                        for (int i = 0; i < 2; ++i)
+                            if (d == lane + 32 * i) {
+                                t.c[i] -= __ldg(a.rc + c0 + k);
+                                t.m[i] -= __ldg(a.rm + c0 + k);
+                            }
+                    }
+                    const size_t off = static_cast<size_t>(n) * D;
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+                        if (lane + 32 * i < rows) {
+                            a.fc_out[off + lane + 32 * i] = t.c[i];
+                            a.fm_out[off + lane + 32 * i] = t.m[i];
+                        }
+                    if (lane == 0) a.node[g] = n;
+                    if (lane < len) a.dev[c0 + lane] = static_cast<int8_t>((cdev >> (6 * lane)) & 63u);
+                    committed += lane == 0;
+                }
+                if (deferred) atomicAdd(&ga.ctl->deferred[round & 1], deferred);
+                if (committed) atomicAdd(ga.committed + gang, committed);
+                if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+            }
+
+            // ---- 4. end the gang, or run another round
+            const unsigned int pending = *reinterpret_cast<volatile unsigned int*>(&ga.ctl->deferred[round & 1]);
+            const long long placed = __ldcg(ga.committed + gang);
+            gang_done = pending == 0u || placed + pending < need;
+            if (!gang_done) continue;
+            if (placed >= need) {
+                if (b == 0 && tid == 0) ga.placed[gang] = static_cast<int32_t>(placed);
+                break;  // nothing is pending: the next gang reads only what the barriers before published
+            }
+            // give the gang back: its pods' demand, and every running pod it evicted
+            for (long long g = g_lo + first; g < g_hi; g += stride) {
+                const int32_t nd = __ldcg(a.node + g);
+                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) {
+                    if (nd >= 0) {
+                        const size_t at = static_cast<size_t>(nd) * D + __ldcg(a.dev + c);
+                        atomicAdd(a.fc_out + at, __ldg(a.rc + c));
+                        atomicAdd(a.fm_out + at, __ldg(a.rm + c));
+                    }
+                    a.dev[c] = -1;
+                }
+                a.node[g] = -1;
+            }
+            for (long long n = wfirst; n < N; n += wstride)
+                for (long long h = __ldg(a.noff + n) + lane, h1 = __ldg(a.noff + n + 1); h < h1; h += 32) {
+                    const int32_t e = __ldcg(a.evicted + h);
+                    if (e < g_lo || e >= g_hi) continue;
+                    a.evicted[h] = -1;
+                    for (int32_t c = __ldg(a.roff + h), c1 = __ldg(a.roff + h + 1); c < c1; ++c) {
+                        const size_t at = static_cast<size_t>(n) * D + __ldg(a.qd + c);
+                        atomicSub(a.fc_out + at, __ldg(a.qc + c));
+                        atomicSub(a.fm_out + at, __ldg(a.qm + c));
+                    }
+                    const int32_t r = __ldg(ga.rgang + h);
+                    if (r >= 0) atomicAdd(ga.alive + r, 1);
+                }
+            if (gang + 1 < ga.J && !grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+        }
+    }
+    done = true;
+finish:
+    if (b == 0 && tid == 0) {
+        const bool bad = *reinterpret_cast<volatile unsigned int*>(&ga.ctl->bad_index) != 0u;
+        a.info[0] = bad ? 0 : round;
+        a.info[1] = done ? 0 : 1;
+        a.info[2] = bad ? 1 : 0;
+    }
+}
+
+size_t preempt_gangs_scratch_bytes(int N, int G, int J, int R) {
+    const size_t zeroed = sizeof(PreGangsCtl) + 4 * (2 * static_cast<size_t>(G) + 2 * static_cast<size_t>(J) +
+                                                     2 * static_cast<size_t>(R));
+    return ((zeroed + 15) & ~size_t(15)) + 24 * static_cast<size_t>(G) * preempt_chunks(N) +
+           16 * static_cast<size_t>(G) + 16 * static_cast<size_t>(G) + 16 * static_cast<size_t>(N) +
+           4 * static_cast<size_t>(N);
+}
+
+cudaError_t preempt_gangs_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N,
+                                 int D, const int32_t* req_core, const int32_t* req_mem, int P,
+                                 const int32_t* pod_offsets, int G, const int32_t* gang_offsets, const int32_t* gang_min,
+                                 const int32_t* gang_prio, int J, const int32_t* run_core, const int32_t* run_mem,
+                                 const int8_t* run_dev, int Q, const int32_t* run_offsets, const int32_t* run_prio,
+                                 int H, const int32_t* node_offsets, const int32_t* run_gang,
+                                 const int32_t* run_gang_min, int R, int32_t* out_node, int8_t* out_dev,
+                                 int32_t* out_placed, int32_t* out_evicted, int32_t* free_core_out,
+                                 int32_t* free_mem_out, int32_t* info, void* scratch, int device, cudaStream_t stream) {
+    // scratch: barrier words | has_empty uint32[G] | pre uint32[G] | in_domain uint32[J] | committed uint32[J] |
+    // alive int32[R] | used int32[R] | (16-aligned) records uint64[G][K][3] | choice uint64[G] | vdev uint64[G] |
+    // vmask uint32[G][4] | cap uint32[N][4] | usable uint32[N]; everything before the records starts at zero
+    const int K = preempt_chunks(N);
+    char* s = static_cast<char*>(scratch);
+    PreGangsArgs ga{};
+    PreemptArgs& a = ga.p;
+    a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem; a.off = pod_offsets;
+    a.qc = run_core; a.qm = run_mem; a.qd = run_dev; a.roff = run_offsets; a.rprio = run_prio; a.noff = node_offsets;
+    a.N = N; a.D = D; a.K = K; a.P = P; a.G = G; a.Q = Q; a.H = H;
+    a.node = out_node; a.dev = out_dev; a.evicted = out_evicted; a.fc_out = free_core_out; a.fm_out = free_mem_out;
+    a.info = info;
+    ga.goff = gang_offsets; ga.gmin = gang_min; ga.gprio = gang_prio; ga.rgang = run_gang; ga.rgmin = run_gang_min;
+    ga.J = J; ga.R = R;
+    ga.placed = out_placed;
+    ga.ctl = reinterpret_cast<PreGangsCtl*>(s);
+    a.has_empty = reinterpret_cast<unsigned int*>(s + sizeof(PreGangsCtl));
+    ga.pre = a.has_empty + G;
+    ga.in_domain = ga.pre + G;
+    ga.committed = ga.in_domain + J;
+    ga.alive = reinterpret_cast<int32_t*>(ga.committed + J);
+    ga.used = ga.alive + R;
+    const size_t zeroed = sizeof(PreGangsCtl) + 4 * (2 * static_cast<size_t>(G) + 2 * static_cast<size_t>(J) +
+                                                     2 * static_cast<size_t>(R));
+    a.rec = reinterpret_cast<unsigned long long*>(s + ((zeroed + 15) & ~size_t(15)));
+    a.choice = a.rec + 3 * static_cast<size_t>(G) * K;
+    ga.vdev = a.choice + G;
+    ga.vmask = reinterpret_cast<unsigned int*>(ga.vdev + G);
+    ga.cap = ga.vmask + 4 * static_cast<size_t>(G);
+    a.usable = ga.cap + 4 * static_cast<size_t>(N);
+    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    if (err != cudaSuccess) return err;
+
+    // resident CTAs per SM on each device, asked once
+    static std::atomic<int> per_sm_cache[kPlaceDevices];
+    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
+    if (per_sm == 0) {
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, preempt_gangs_kernel, kTabThreads, 0);
+        if (err != cudaSuccess) return err;
+        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
+        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
+    }
+    int sms = 0;
+    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err != cudaSuccess) return err;
+    // Grid: as preempt_launch, from N and G alone (the gang sizes are device data): one resident wave, no more CTAs
+    // than a round over all G pods has choose items; at least one, which finds G = 0's offsets bad.
+    long long grid = static_cast<long long>(sms) * per_sm;
+    grid = std::max(1ll, std::min(grid, static_cast<long long>(K) * G));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.blockDim = dim3(kTabThreads);
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, preempt_gangs_kernel, ga);
+}
+
 }  // namespace egpu

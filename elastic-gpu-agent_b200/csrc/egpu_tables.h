@@ -1,6 +1,6 @@
 // egpu_tables.h — launchers of the multi-table best-fit scan and placements (egpu_tables.cu), called by the
-// PyTorch operators egpu::bestfit_tables, egpu::place_tables, egpu::place_pods, egpu::place_gangs and
-// egpu::preempt_pods (egpu_tables_op.cc).  Not part of the C ABI of include/.
+// PyTorch operators egpu::bestfit_tables, egpu::place_tables, egpu::place_pods, egpu::place_gangs,
+// egpu::preempt_pods and egpu::preempt_gangs (egpu_tables_op.cc).  Not part of the C ABI of include/.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -76,5 +76,27 @@ cudaError_t preempt_launch(const int32_t* free_core, const int32_t* free_mem, co
                            const int32_t* node_offsets, int32_t* out_node, int8_t* out_dev, int32_t* out_evicted,
                            int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch, int device,
                            cudaStream_t stream);
+
+// Bytes of device scratch preempt_gangs_launch needs for G pods in J gangs on N tables with R running jobs (16-byte
+// aligned, from the caller's allocator).
+size_t preempt_gangs_scratch_bytes(int N, int G, int J, int R);
+
+// Places J gangs of G pods of P containers on N tables in gang order as gangs_launch, each gang's pods by
+// preempt_launch's rounds at the gang's priority, never evicting a running job below its minAvailable (DESIGN.md
+// §2.15), in one cooperative launch.  Tables, containers, pod_offsets, gang_offsets and gang_min as gangs_launch;
+// gang_prio: int32[J]; running pods as preempt_launch; run_gang: int32[H] in [-1, R); run_gang_min: int32[R] >= 0.
+// The kernel checks the five index tensors and run_gang_min before it reads anything through them.  out_node:
+// int32[G]; out_dev: int8[P]; out_placed: int32[J]; out_evicted: int32[H]; free_core_out / free_mem_out: int32[N][D];
+// info: int32[3].  scratch: preempt_gangs_scratch_bytes(N, G, J, R) bytes; its head is zeroed here on `stream`.
+// N >= 1, P >= 1, G, J, Q, H, R >= 0.  Asynchronous on `stream`; returns the first error of the memset or the launch.
+cudaError_t preempt_gangs_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N,
+                                 int D, const int32_t* req_core, const int32_t* req_mem, int P,
+                                 const int32_t* pod_offsets, int G, const int32_t* gang_offsets, const int32_t* gang_min,
+                                 const int32_t* gang_prio, int J, const int32_t* run_core, const int32_t* run_mem,
+                                 const int8_t* run_dev, int Q, const int32_t* run_offsets, const int32_t* run_prio,
+                                 int H, const int32_t* node_offsets, const int32_t* run_gang,
+                                 const int32_t* run_gang_min, int R, int32_t* out_node, int8_t* out_dev,
+                                 int32_t* out_placed, int32_t* out_evicted, int32_t* free_core_out,
+                                 int32_t* free_mem_out, int32_t* info, void* scratch, int device, cudaStream_t stream);
 
 }  // namespace egpu

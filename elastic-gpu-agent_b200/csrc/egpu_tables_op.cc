@@ -1,7 +1,8 @@
 // egpu_tables_op.cc — the PyTorch operators egpu::bestfit_tables (DESIGN.md §2.10), egpu::place_tables (§2.11),
-// egpu::place_pods (§2.12), egpu::place_gangs (§2.13) and egpu::preempt_pods (§2.14): argument checks on the host,
-// outputs and scratch from the caching allocator, one launch of bestfit_tables_kernel, place_tables_kernel,
-// place_pods_kernel, place_gangs_kernel or preempt_pods_kernel on the current stream.  No synchronisation and no host copy, so every operator can be captured
+// egpu::place_pods (§2.12), egpu::place_gangs (§2.13), egpu::preempt_pods (§2.14) and egpu::preempt_gangs (§2.15):
+// argument checks on the host, outputs and scratch from the caching allocator, one launch of bestfit_tables_kernel,
+// place_tables_kernel, place_pods_kernel, place_gangs_kernel, preempt_pods_kernel or preempt_gangs_kernel on the
+// current stream.  No synchronisation and no host copy, so every operator can be captured
 // into a CUDA graph.  The fake (shape) implementations are registered from Python (tables.py).
 #include <ATen/core/Tensor.h>
 #include <ATen/ops/empty.h>
@@ -145,19 +146,20 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> place_pod
 
 // DESIGN.md §2.13.  place_pods' checks naming place_gangs, then gang_offsets' and gang_min's dtype and layout, shapes
 // and device; their values are the kernel's to check (they are device data).  Returns J.
-int64_t check_gangs(const at::Tensor& free_core, const at::Tensor& gang_offsets, const at::Tensor& gang_min) {
-    check_int32_contiguous("place_gangs", gang_offsets, "gang_offsets");
-    check_int32_contiguous("place_gangs", gang_min, "gang_min");
-    TORCH_CHECK_VALUE(gang_offsets.dim() == 1 && gang_offsets.size(0) >= 1,
-                      "place_gangs: gang_offsets must be [J + 1], got ", gang_offsets.sizes());
-    TORCH_CHECK_VALUE(gang_offsets.size(0) <= std::numeric_limits<int32_t>::max(),
-                      "place_gangs: J + 1 must be below 2^31, got ", gang_offsets.size(0));
+int64_t check_gangs(const char* op, const at::Tensor& free_core, const at::Tensor& gang_offsets,
+                    const at::Tensor& gang_min) {
+    check_int32_contiguous(op, gang_offsets, "gang_offsets");
+    check_int32_contiguous(op, gang_min, "gang_min");
+    TORCH_CHECK_VALUE(gang_offsets.dim() == 1 && gang_offsets.size(0) >= 1, op,
+                      ": gang_offsets must be [J + 1], got ", gang_offsets.sizes());
+    TORCH_CHECK_VALUE(gang_offsets.size(0) <= std::numeric_limits<int32_t>::max(), op,
+                      ": J + 1 must be below 2^31, got ", gang_offsets.size(0));
     const int64_t J = gang_offsets.size(0) - 1;
-    TORCH_CHECK_VALUE(gang_min.dim() == 1 && gang_min.size(0) == J, "place_gangs: gang_min must be [J] = [", J,
+    TORCH_CHECK_VALUE(gang_min.dim() == 1 && gang_min.size(0) == J, op, ": gang_min must be [J] = [", J,
                       "], got ", gang_min.sizes());
     for (const at::Tensor* t : {&gang_offsets, &gang_min})
-        TORCH_CHECK(t->is_cuda() && t->device() == free_core.device(),
-                    "place_gangs: every tensor must be on one CUDA device, got ", t->device(), " and ", free_core.device());
+        TORCH_CHECK(t->is_cuda() && t->device() == free_core.device(), op,
+                    ": every tensor must be on one CUDA device, got ", t->device(), " and ", free_core.device());
     return J;
 }
 
@@ -167,7 +169,7 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tenso
     const at::Tensor& gang_min) {
     const auto [N, D, P] = check_inputs("place_gangs", free_core, free_mem, d_valid, req_core, req_mem);
     const int64_t G = check_pod_offsets("place_gangs", free_core, pod_offsets);
-    const int64_t J = check_gangs(free_core, gang_offsets, gang_min);
+    const int64_t J = check_gangs("place_gangs", free_core, gang_offsets, gang_min);
     const at::Device dev = free_core.device();
     const c10::cuda::CUDAGuard guard(dev);
     at::Tensor node = at::empty({G}, free_core.options());
@@ -200,13 +202,14 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tenso
 }
 
 // DESIGN.md §2.14.  place_pods' checks naming preempt_pods, then the dtype and layout of the six new tensors, their
-// shapes, and their device; their values are the kernel's to check (they are device data).  Returns (Q, H).
-std::tuple<int64_t, int64_t> check_running(const at::Tensor& free_core, int64_t G, const at::Tensor& pod_prio,
-                                           const at::Tensor& run_core, const at::Tensor& run_mem,
-                                           const at::Tensor& run_dev, const at::Tensor& run_offsets,
-                                           const at::Tensor& run_prio, const at::Tensor& node_offsets) {
-    constexpr const char* op = "preempt_pods";
-    check_int32_contiguous(op, pod_prio, "pod_prio");
+// shapes, and their device; their values are the kernel's to check (they are device data).  preempt_gangs (§2.15)
+// has no pod_prio (its priority is per gang) and passes nullptr.  Returns (Q, H).
+std::tuple<int64_t, int64_t> check_running(const char* op, const at::Tensor& free_core, int64_t G,
+                                           const at::Tensor* pod_prio, const at::Tensor& run_core,
+                                           const at::Tensor& run_mem, const at::Tensor& run_dev,
+                                           const at::Tensor& run_offsets, const at::Tensor& run_prio,
+                                           const at::Tensor& node_offsets) {
+    if (pod_prio) check_int32_contiguous(op, *pod_prio, "pod_prio");
     check_int32_contiguous(op, run_core, "run_core");
     check_int32_contiguous(op, run_mem, "run_mem");
     TORCH_CHECK(run_dev.scalar_type() == at::kChar, op, ": run_dev must be int8, got ", run_dev.scalar_type());
@@ -215,8 +218,9 @@ std::tuple<int64_t, int64_t> check_running(const at::Tensor& free_core, int64_t 
     check_int32_contiguous(op, run_prio, "run_prio");
     check_int32_contiguous(op, node_offsets, "node_offsets");
     const int64_t N = free_core.size(0);
-    TORCH_CHECK_VALUE(pod_prio.dim() == 1 && pod_prio.size(0) == G, op, ": pod_prio must be [G] = [", G, "], got ",
-                      pod_prio.sizes());
+    if (pod_prio)
+        TORCH_CHECK_VALUE(pod_prio->dim() == 1 && pod_prio->size(0) == G, op, ": pod_prio must be [G] = [", G,
+                          "], got ", pod_prio->sizes());
     TORCH_CHECK_VALUE(run_core.dim() == 1 && run_mem.sizes() == run_core.sizes() && run_dev.sizes() == run_core.sizes(),
                       op, ": run_core, run_mem and run_dev must all be [Q], got ", run_core.sizes(), ", ",
                       run_mem.sizes(), " and ", run_dev.sizes());
@@ -229,8 +233,8 @@ std::tuple<int64_t, int64_t> check_running(const at::Tensor& free_core, int64_t 
                       run_prio.sizes());
     TORCH_CHECK_VALUE(node_offsets.dim() == 1 && node_offsets.size(0) == N + 1, op, ": node_offsets must be [N + 1] = [",
                       N + 1, "], got ", node_offsets.sizes());
-    for (const at::Tensor* t : {&pod_prio, &run_core, &run_mem, &run_dev, &run_offsets, &run_prio, &node_offsets})
-        TORCH_CHECK(t->is_cuda() && t->device() == free_core.device(), op,
+    for (const at::Tensor* t : {pod_prio, &run_core, &run_mem, &run_dev, &run_offsets, &run_prio, &node_offsets})
+        TORCH_CHECK(!t || t->is_cuda() && t->device() == free_core.device(), op,
                     ": every tensor must be on one CUDA device, got ", t->device(), " and ", free_core.device());
     return {Q, H};
 }
@@ -242,8 +246,8 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tenso
     const at::Tensor& node_offsets) {
     const auto [N, D, P] = check_inputs("preempt_pods", free_core, free_mem, d_valid, req_core, req_mem);
     const int64_t G = check_pod_offsets("preempt_pods", free_core, pod_offsets);
-    const auto [Q, H] = check_running(free_core, G, pod_prio, run_core, run_mem, run_dev, run_offsets, run_prio,
-                                      node_offsets);
+    const auto [Q, H] = check_running("preempt_pods", free_core, G, &pod_prio, run_core, run_mem, run_dev, run_offsets,
+                                      run_prio, node_offsets);
     const at::Device dev = free_core.device();
     const c10::cuda::CUDAGuard guard(dev);
     at::Tensor node = at::empty({G}, free_core.options());
@@ -276,6 +280,77 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tenso
     return {node, dv_out, evicted, fc_out, fm_out, info};
 }
 
+// DESIGN.md §2.15.  place_gangs' and preempt_pods' checks naming preempt_gangs, then the dtype and layout of
+// gang_prio, run_gang and run_gang_min, their shapes, and their device; their values are the kernel's to check.
+// Returns R.
+int64_t check_running_gangs(const at::Tensor& free_core, int64_t J, int64_t H, const at::Tensor& gang_prio,
+                            const at::Tensor& run_gang, const at::Tensor& run_gang_min) {
+    constexpr const char* op = "preempt_gangs";
+    check_int32_contiguous(op, gang_prio, "gang_prio");
+    check_int32_contiguous(op, run_gang, "run_gang");
+    check_int32_contiguous(op, run_gang_min, "run_gang_min");
+    TORCH_CHECK_VALUE(gang_prio.dim() == 1 && gang_prio.size(0) == J, op, ": gang_prio must be [J] = [", J, "], got ",
+                      gang_prio.sizes());
+    TORCH_CHECK_VALUE(run_gang.dim() == 1 && run_gang.size(0) == H, op, ": run_gang must be [H] = [", H, "], got ",
+                      run_gang.sizes());
+    TORCH_CHECK_VALUE(run_gang_min.dim() == 1, op, ": run_gang_min must be [R], got ", run_gang_min.sizes());
+    const int64_t R = run_gang_min.size(0);
+    TORCH_CHECK_VALUE(R < std::numeric_limits<int32_t>::max(), op, ": R must be below 2^31 - 1, got ", R);
+    for (const at::Tensor* t : {&gang_prio, &run_gang, &run_gang_min})
+        TORCH_CHECK(t->is_cuda() && t->device() == free_core.device(), op,
+                    ": every tensor must be on one CUDA device, got ", t->device(), " and ", free_core.device());
+    return R;
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> preempt_gangs(
+    const at::Tensor& free_core, const at::Tensor& free_mem, const at::Tensor& d_valid, const at::Tensor& req_core,
+    const at::Tensor& req_mem, const at::Tensor& pod_offsets, const at::Tensor& gang_offsets,
+    const at::Tensor& gang_min, const at::Tensor& gang_prio, const at::Tensor& run_core, const at::Tensor& run_mem,
+    const at::Tensor& run_dev, const at::Tensor& run_offsets, const at::Tensor& run_prio,
+    const at::Tensor& node_offsets, const at::Tensor& run_gang, const at::Tensor& run_gang_min) {
+    constexpr const char* op = "preempt_gangs";
+    const auto [N, D, P] = check_inputs(op, free_core, free_mem, d_valid, req_core, req_mem);
+    const int64_t G = check_pod_offsets(op, free_core, pod_offsets);
+    const int64_t J = check_gangs(op, free_core, gang_offsets, gang_min);
+    const auto [Q, H] = check_running(op, free_core, G, nullptr, run_core, run_mem, run_dev, run_offsets, run_prio,
+                                      node_offsets);
+    const int64_t R = check_running_gangs(free_core, J, H, gang_prio, run_gang, run_gang_min);
+    const at::Device dev = free_core.device();
+    const c10::cuda::CUDAGuard guard(dev);
+    at::Tensor node = at::empty({G}, free_core.options());
+    at::Tensor dv_out = at::empty({P}, free_core.options().dtype(at::kChar));
+    at::Tensor placed = at::empty({J}, free_core.options());
+    at::Tensor evicted = at::empty({H}, free_core.options());
+    at::Tensor fc_out = at::empty({N, D}, free_core.options());
+    at::Tensor fm_out = at::empty({N, D}, free_core.options());
+    at::Tensor info = at::empty({3}, free_core.options());
+    if (N == 0 || P == 0) {  // nothing to place, or nowhere to place it
+        node.fill_(-1);
+        dv_out.fill_(-1);
+        placed.zero_();
+        evicted.fill_(-1);
+        fc_out.copy_(free_core);
+        fm_out.copy_(free_mem);
+        info.zero_();
+        return {node, dv_out, placed, evicted, fc_out, fm_out, info};
+    }
+    at::Tensor scratch = at::empty({static_cast<int64_t>(egpu::preempt_gangs_scratch_bytes(
+                                       static_cast<int>(N), static_cast<int>(G), static_cast<int>(J), static_cast<int>(R)))},
+                                   free_core.options().dtype(at::kByte));
+    const cudaError_t err = egpu::preempt_gangs_launch(
+        free_core.data_ptr<int32_t>(), free_mem.data_ptr<int32_t>(), d_valid.data_ptr<int32_t>(), static_cast<int>(N),
+        static_cast<int>(D), req_core.data_ptr<int32_t>(), req_mem.data_ptr<int32_t>(), static_cast<int>(P),
+        pod_offsets.data_ptr<int32_t>(), static_cast<int>(G), gang_offsets.data_ptr<int32_t>(),
+        gang_min.data_ptr<int32_t>(), gang_prio.data_ptr<int32_t>(), static_cast<int>(J), run_core.data_ptr<int32_t>(),
+        run_mem.data_ptr<int32_t>(), run_dev.data_ptr<int8_t>(), static_cast<int>(Q), run_offsets.data_ptr<int32_t>(),
+        run_prio.data_ptr<int32_t>(), static_cast<int>(H), node_offsets.data_ptr<int32_t>(), run_gang.data_ptr<int32_t>(),
+        run_gang_min.data_ptr<int32_t>(), static_cast<int>(R), node.data_ptr<int32_t>(), dv_out.data_ptr<int8_t>(),
+        placed.data_ptr<int32_t>(), evicted.data_ptr<int32_t>(), fc_out.data_ptr<int32_t>(), fm_out.data_ptr<int32_t>(),
+        info.data_ptr<int32_t>(), scratch.data_ptr(), dev.index(), c10::cuda::getCurrentCUDAStream(dev.index()).stream());
+    TORCH_CHECK(err == cudaSuccess, "preempt_gangs: launch failed: ", cudaGetErrorString(err));
+    return {node, dv_out, placed, evicted, fc_out, fm_out, info};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(egpu, m) {
@@ -290,6 +365,10 @@ TORCH_LIBRARY(egpu, m) {
     m.def("preempt_pods(Tensor free_core, Tensor free_mem, Tensor d_valid, Tensor req_core, Tensor req_mem, "
           "Tensor pod_offsets, Tensor pod_prio, Tensor run_core, Tensor run_mem, Tensor run_dev, Tensor run_offsets, "
           "Tensor run_prio, Tensor node_offsets) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)");
+    m.def("preempt_gangs(Tensor free_core, Tensor free_mem, Tensor d_valid, Tensor req_core, Tensor req_mem, "
+          "Tensor pod_offsets, Tensor gang_offsets, Tensor gang_min, Tensor gang_prio, Tensor run_core, Tensor run_mem, "
+          "Tensor run_dev, Tensor run_offsets, Tensor run_prio, Tensor node_offsets, Tensor run_gang, "
+          "Tensor run_gang_min) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)");
 }
 
 // The CPU registration only refuses (the device check above): a CPU caller gets the same messages as a CUDA one.
@@ -299,6 +378,7 @@ TORCH_LIBRARY_IMPL(egpu, CUDA, m) {
     m.impl("place_pods", &place_pods);
     m.impl("place_gangs", &place_gangs);
     m.impl("preempt_pods", &preempt_pods);
+    m.impl("preempt_gangs", &preempt_gangs);
 }
 TORCH_LIBRARY_IMPL(egpu, CPU, m) {
     m.impl("bestfit_tables", &bestfit_tables);
@@ -306,4 +386,5 @@ TORCH_LIBRARY_IMPL(egpu, CPU, m) {
     m.impl("place_pods", &place_pods);
     m.impl("place_gangs", &place_gangs);
     m.impl("preempt_pods", &preempt_pods);
+    m.impl("preempt_gangs", &preempt_gangs);
 }

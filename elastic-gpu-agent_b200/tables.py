@@ -1,6 +1,6 @@
 """Best fit of many pending requests against many capacity tables in one launch: the PyTorch operators
-`egpu::bestfit_tables` (DESIGN.md §2.10), `egpu::place_tables` (§2.11), `egpu::place_pods` (§2.12) and
-`egpu::place_gangs` (§2.13) and `egpu::preempt_pods` (§2.14).
+`egpu::bestfit_tables` (DESIGN.md §2.10), `egpu::place_tables` (§2.11), `egpu::place_pods` (§2.12),
+`egpu::place_gangs` (§2.13), `egpu::preempt_pods` (§2.14) and `egpu::preempt_gangs` (§2.15).
 
 A scheduler scores every pending pod against every node's device table; `bestfit_tables` does all N x P
 pairs in one CUDA launch on the current stream instead of N `egpu_bestfit_query` calls.  `place_tables`
@@ -9,7 +9,9 @@ launch, so that no device is oversubscribed.  `place_pods` does the same for pod
 container of a pod on one node.  `place_gangs` places jobs (gangs of pods) in queue order, each kept only when at
 least its `minAvailable` pods are placed and given back otherwise, so that no job holds capacity it cannot start
 with.  `preempt_pods` places pods as `place_pods` does, and where a pod fits no node as it is, evicts the fewest,
-lowest-priority running pods of one node that make it fit.  The kernels live in csrc/egpu_tables.cu and are built by
+lowest-priority running pods of one node that make it fit.  `preempt_gangs` places gangs as `place_gangs` does,
+each at its priority with `preempt_pods`' evictions, keeps a gang's evictions only when the gang is kept, and never
+evicts a running job below its `minAvailable`.  The kernels live in csrc/egpu_tables.cu and are built by
 __graft_entry__.build() as lib/libegpu_tables.so; it is separate from libegpu_alloc.so and its C ABI,
 reads no context and writes no table of a context.  Importing this module does not load the library; the
 first call (or `load()`) does, and a missing library raises: there is no fallback.
@@ -35,7 +37,7 @@ _loaded = False
 
 def load() -> None:
     """Load lib/libegpu_tables.so (it registers egpu::bestfit_tables, egpu::place_tables, egpu::place_pods,
-    egpu::place_gangs and egpu::preempt_pods) and the operators' fake implementations."""
+    egpu::place_gangs, egpu::preempt_pods and egpu::preempt_gangs) and the operators' fake implementations."""
     global _loaded
     if _loaded:
         return
@@ -49,6 +51,7 @@ def load() -> None:
     torch.library.register_fake("egpu::place_pods")(_fake_pods)
     torch.library.register_fake("egpu::place_gangs")(_fake_gangs)
     torch.library.register_fake("egpu::preempt_pods")(_fake_preempt)
+    torch.library.register_fake("egpu::preempt_gangs")(_fake_preempt_gangs)
     _loaded = True
 
 
@@ -245,44 +248,44 @@ def place_pods(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.T
     return torch.ops.egpu.place_pods(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets)
 
 
-def check_gang_args(free_core, gang_offsets, gang_min) -> None:
+def check_gang_args(free_core, gang_offsets, gang_min, op: str = "place_gangs") -> None:
     """place_gangs' checks on gang_offsets' and gang_min's dtype, layout, shapes and device (no data is read), after
     check_args and check_pod_args and in the operator's order: RuntimeError for a dtype, layout or device,
-    ValueError for a shape."""
+    ValueError for a shape.  `op` names the operator in the messages."""
     for name, t in (("gang_offsets", gang_offsets), ("gang_min", gang_min)):
         if t.dtype != torch.int32:
-            raise RuntimeError(f"place_gangs: {name} must be int32, got {t.dtype}")
+            raise RuntimeError(f"{op}: {name} must be int32, got {t.dtype}")
         if not t.is_contiguous():
-            raise RuntimeError(f"place_gangs: {name} must be contiguous")
+            raise RuntimeError(f"{op}: {name} must be contiguous")
     if gang_offsets.dim() != 1 or gang_offsets.shape[0] < 1:
-        raise ValueError(f"place_gangs: gang_offsets must be [J + 1], got {tuple(gang_offsets.shape)}")
+        raise ValueError(f"{op}: gang_offsets must be [J + 1], got {tuple(gang_offsets.shape)}")
     if gang_offsets.shape[0] >= 2**31:
-        raise ValueError(f"place_gangs: J + 1 must be below 2^31, got {gang_offsets.shape[0]}")
+        raise ValueError(f"{op}: J + 1 must be below 2^31, got {gang_offsets.shape[0]}")
     J = gang_offsets.shape[0] - 1
     if gang_min.dim() != 1 or gang_min.shape[0] != J:
-        raise ValueError(f"place_gangs: gang_min must be [J] = [{J}], got {tuple(gang_min.shape)}")
+        raise ValueError(f"{op}: gang_min must be [J] = [{J}], got {tuple(gang_min.shape)}")
     for t in (gang_offsets, gang_min):
         if t.device.type != "cuda" or t.device != free_core.device:
-            raise RuntimeError(f"place_gangs: every tensor must be on one CUDA device, got {t.device} and "
+            raise RuntimeError(f"{op}: every tensor must be on one CUDA device, got {t.device} and "
                                f"{free_core.device}")
 
 
-def check_gangs(gang_offsets, gang_min, G: int) -> None:
+def check_gangs(gang_offsets, gang_min, G: int, op: str = "place_gangs") -> None:
     """ValueError unless gang_offsets lists gangs of at least one pod each, covering all G pods (first 0, last G,
     every step >= 1), and every gang_min[j] is in [1, size of gang j].  Reads the data: one host round trip."""
     o, m = torch.cat([gang_offsets.to(torch.int64), gang_min.to(torch.int64)]).cpu().split(
         [gang_offsets.shape[0], gang_min.shape[0]])
     if int(o[0]) != 0:
-        raise ValueError(f"place_gangs: gang_offsets must start at 0, got {int(o[0])}")
+        raise ValueError(f"{op}: gang_offsets must start at 0, got {int(o[0])}")
     if int(o[-1]) != G:
-        raise ValueError(f"place_gangs: gang_offsets must end at G = {G}, got {int(o[-1])}")
+        raise ValueError(f"{op}: gang_offsets must end at G = {G}, got {int(o[-1])}")
     size = o[1:] - o[:-1]
     bad = int((size < 1).sum())
     if bad:
-        raise ValueError(f"place_gangs: {bad} gang(s) with no pod")
+        raise ValueError(f"{op}: {bad} gang(s) with no pod")
     bad = int(((m < 1) | (m > size)).sum())
     if bad:
-        raise ValueError(f"place_gangs: {bad} gang(s) with gang_min outside [1, gang size]")
+        raise ValueError(f"{op}: {bad} gang(s) with gang_min outside [1, gang size]")
 
 
 def _fake_gangs(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_offsets, gang_min):
@@ -338,21 +341,23 @@ def place_gangs(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.
 
 
 def check_preempt_args(free_core, pod_offsets, pod_prio, run_core, run_mem, run_dev, run_offsets, run_prio,
-                       node_offsets) -> None:
+                       node_offsets, op: str = "preempt_pods") -> None:
     """preempt_pods' checks on the six new tensors' dtype, layout, shapes and device (no data is read), after
     check_args and check_pod_args and in the operator's order: RuntimeError for a dtype, layout or device,
-    ValueError for a shape."""
-    op = "preempt_pods"
+    ValueError for a shape.  `op` names the operator in the messages; preempt_gangs, whose priority is per gang,
+    passes pod_prio=None and its checks are skipped."""
     for name, t, dt in (("pod_prio", pod_prio, torch.int32), ("run_core", run_core, torch.int32),
                         ("run_mem", run_mem, torch.int32), ("run_dev", run_dev, torch.int8),
                         ("run_offsets", run_offsets, torch.int32), ("run_prio", run_prio, torch.int32),
                         ("node_offsets", node_offsets, torch.int32)):
+        if t is None:
+            continue
         if t.dtype != dt:
             raise RuntimeError(f"{op}: {name} must be {str(dt).replace('torch.', '')}, got {t.dtype}")
         if not t.is_contiguous():
             raise RuntimeError(f"{op}: {name} must be contiguous")
     N, G = free_core.shape[0], pod_offsets.shape[0] - 1
-    if pod_prio.dim() != 1 or pod_prio.shape[0] != G:
+    if pod_prio is not None and (pod_prio.dim() != 1 or pod_prio.shape[0] != G):
         raise ValueError(f"{op}: pod_prio must be [G] = [{G}], got {tuple(pod_prio.shape)}")
     if run_core.dim() != 1 or run_mem.shape != run_core.shape or run_dev.shape != run_core.shape:
         raise ValueError(f"{op}: run_core, run_mem and run_dev must all be [Q], got {tuple(run_core.shape)}, "
@@ -367,17 +372,17 @@ def check_preempt_args(free_core, pod_offsets, pod_prio, run_core, run_mem, run_
     if node_offsets.dim() != 1 or node_offsets.shape[0] != N + 1:
         raise ValueError(f"{op}: node_offsets must be [N + 1] = [{N + 1}], got {tuple(node_offsets.shape)}")
     for t in (pod_prio, run_core, run_mem, run_dev, run_offsets, run_prio, node_offsets):
-        if t.device.type != "cuda" or t.device != free_core.device:
+        if t is not None and (t.device.type != "cuda" or t.device != free_core.device):
             raise RuntimeError(f"{op}: every tensor must be on one CUDA device, got {t.device} and {free_core.device}")
 
 
-def check_running(free_core, free_mem, d_valid, run_core, run_mem, run_dev, run_offsets, node_offsets) -> None:
+def check_running(free_core, free_mem, d_valid, run_core, run_mem, run_dev, run_offsets, node_offsets,
+                  op: str = "preempt_pods") -> None:
     """ValueError unless run_offsets lists running pods of 1 to MAX_POD containers covering all Q containers (first
     0, last Q, every step in [1, MAX_POD]), node_offsets lists 0 to MAX_RUN running pods per node covering all H
     (first 0, last H, every step in [0, MAX_RUN]), and every node's running data is consistent: each run_dev in
     [0, d_valid[n]), each running container in the request domain, and on each device free plus the demand of its
     running containers within the table domain.  Reads the data: one host round trip."""
-    op = "preempt_pods"
     ro, no = run_offsets.to(torch.int64).cpu(), node_offsets.to(torch.int64).cpu()
     Q, H = run_core.shape[0], ro.shape[0] - 1
     if int(ro[0]) != 0:
@@ -476,3 +481,115 @@ def preempt_pods(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch
         check_running(free_core, free_mem, d_valid, run_core, run_mem, run_dev, run_offsets, node_offsets)
     return torch.ops.egpu.preempt_pods(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, pod_prio, run_core,
                                        run_mem, run_dev, run_offsets, run_prio, node_offsets)
+
+
+def check_preempt_gang_args(free_core, gang_offsets, run_offsets, gang_prio, run_gang, run_gang_min) -> None:
+    """preempt_gangs' checks on gang_prio's, run_gang's and run_gang_min's dtype, layout, shapes and device (no data is
+    read), after those of place_gangs and preempt_pods and in the operator's order: RuntimeError for a dtype, layout
+    or device, ValueError for a shape."""
+    op = "preempt_gangs"
+    for name, t in (("gang_prio", gang_prio), ("run_gang", run_gang), ("run_gang_min", run_gang_min)):
+        if t.dtype != torch.int32:
+            raise RuntimeError(f"{op}: {name} must be int32, got {t.dtype}")
+        if not t.is_contiguous():
+            raise RuntimeError(f"{op}: {name} must be contiguous")
+    J, H = gang_offsets.shape[0] - 1, run_offsets.shape[0] - 1
+    if gang_prio.dim() != 1 or gang_prio.shape[0] != J:
+        raise ValueError(f"{op}: gang_prio must be [J] = [{J}], got {tuple(gang_prio.shape)}")
+    if run_gang.dim() != 1 or run_gang.shape[0] != H:
+        raise ValueError(f"{op}: run_gang must be [H] = [{H}], got {tuple(run_gang.shape)}")
+    if run_gang_min.dim() != 1:
+        raise ValueError(f"{op}: run_gang_min must be [R], got {tuple(run_gang_min.shape)}")
+    if run_gang_min.shape[0] >= 2**31 - 1:
+        raise ValueError(f"{op}: R must be below 2^31 - 1, got {run_gang_min.shape[0]}")
+    for t in (gang_prio, run_gang, run_gang_min):
+        if t.device.type != "cuda" or t.device != free_core.device:
+            raise RuntimeError(f"{op}: every tensor must be on one CUDA device, got {t.device} and {free_core.device}")
+
+
+def check_running_gangs(run_gang, run_gang_min) -> None:
+    """ValueError unless every run_gang[h] is in [-1, R) (R = run_gang_min's length) and every run_gang_min[r] is at
+    least 0.  Reads the data: one host round trip."""
+    op = "preempt_gangs"
+    R = run_gang_min.shape[0]
+    bad = int(((run_gang < -1) | (run_gang >= R)).sum())
+    if bad:
+        raise ValueError(f"{op}: {bad} running pod(s) with run_gang outside [-1, {R})")
+    bad = int((run_gang_min < 0).sum())
+    if bad:
+        raise ValueError(f"{op}: {bad} running job(s) with run_gang_min below 0")
+
+
+def _fake_preempt_gangs(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_offsets, gang_min,
+                        gang_prio, run_core, run_mem, run_dev, run_offsets, run_prio, node_offsets, run_gang,
+                        run_gang_min):
+    op = "preempt_gangs"
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op=op)
+    check_pod_args(free_core, pod_offsets, op=op)
+    check_gang_args(free_core, gang_offsets, gang_min, op=op)
+    check_preempt_args(free_core, pod_offsets, None, run_core, run_mem, run_dev, run_offsets, run_prio, node_offsets,
+                       op=op)
+    check_preempt_gang_args(free_core, gang_offsets, run_offsets, gang_prio, run_gang, run_gang_min)
+    G, P, J, H = pod_offsets.shape[0] - 1, req_core.shape[0], gang_offsets.shape[0] - 1, run_offsets.shape[0] - 1
+    return (pod_offsets.new_empty((G,), dtype=torch.int32), req_core.new_empty((P,), dtype=torch.int8),
+            gang_offsets.new_empty((J,), dtype=torch.int32), run_offsets.new_empty((H,), dtype=torch.int32),
+            torch.empty_like(free_core), torch.empty_like(free_mem), free_core.new_empty((3,), dtype=torch.int32))
+
+
+def preempt_gangs(free_core: torch.Tensor, free_mem: torch.Tensor, d_valid: torch.Tensor, req_core: torch.Tensor,
+                  req_mem: torch.Tensor, pod_offsets: torch.Tensor, gang_offsets: torch.Tensor, gang_min: torch.Tensor,
+                  gang_prio: torch.Tensor, run_core: torch.Tensor, run_mem: torch.Tensor, run_dev: torch.Tensor,
+                  run_offsets: torch.Tensor, run_prio: torch.Tensor, node_offsets: torch.Tensor,
+                  run_gang: torch.Tensor, run_gang_min: torch.Tensor):
+    """Place J gangs (jobs) of pods on N capacity tables in one launch, in gang order, each gang's pods placed as
+    preempt_pods places them at the gang's priority, kept only when at least gang_min of them are placed, and never
+    evicting a running job below its minAvailable (DESIGN.md §2.15).
+
+    Tables, containers, pod_offsets, gang_offsets and gang_min as place_gangs; gang_prio int32[J] is each gang's
+    priority (one PodGroup, one priority class).  The running pods as preempt_pods; run_gang int32[H] in [-1, R) names
+    the running job (gang) each running pod belongs to (-1: none), and run_gang_min int32[R] >= 0 is each running
+    job's minAvailable.  A running job's slack is its listed running pods not evicted, on any node, less its
+    minAvailable (0 when that is negative).
+
+    The rule is place_gangs' loop over gangs, each gang's pods placed by preempt_pods' rounds, with two changes.  On
+    each node, C keeps of each running job only the slack pods of that job that come last in the walk order (priority
+    descending, h ascending), the slack read at the start of the round.  And a round's first-on-node preemptors with
+    a victim in a running job commit, in pod order, only while every such job's victims of this pod and of the
+    preemptors before it stay within the job's slack; the others are deferred.  A gang that ends with fewer than
+    gang_min pods placed is given back: placements and evictions are undone, and later gangs see the tables, the
+    running pods and the slacks as they were before it.
+
+    Returns (node int32[G], dev int8[P], placed int32[J], evicted int32[H], free_core_out int32[N, D], free_mem_out
+    int32[N, D], info int32[3]): node and dev as place_pods; placed as place_gangs; evicted[h] the pod that evicted
+    running pod h, or -1 (only pods of kept gangs evict); the tables after every kept gang, assuming the evicted pods
+    are gone; info = [rounds run, summed over gangs, 1 if a grid wait gave up after ~2 s else 0, 1 if the kernel
+    refused an index tensor or run_gang_min else 0].  When a wait gives up the outputs are not a placement and the
+    caller must discard them.  The inputs are not written.  N = 0 or P = 0 gives -1 placements, placed all 0, evicted
+    all -1, copied tables and info [0, 0, 0].
+
+    Stateless and asynchronous on the current stream; it captures into a CUDA graph and traces under
+    torch.compile(fullgraph=True).  Refusals are place_gangs' and preempt_pods' (without pod_prio) with
+    "preempt_gangs" in the messages, then gang_prio's, run_gang's and run_gang_min's dtype, layout, shapes and device.
+    Eagerly this function also checks the tables, the index tensors, the running pods and the running jobs
+    (ValueError), which reads them back; during capture or tracing the kernel checks the five index tensors and
+    run_gang_min itself and, if one is bad, places and evicts nothing: all -1, placed all 0, tables copied,
+    info = [0, 0, 1]; a node whose table is outside the domain or whose running data is inconsistent offers no
+    candidate and is copied.
+    """
+    load()
+    op = "preempt_gangs"
+    check_args(free_core, free_mem, d_valid, req_core, req_mem, op=op)
+    check_pod_args(free_core, pod_offsets, op=op)
+    check_gang_args(free_core, gang_offsets, gang_min, op=op)
+    check_preempt_args(free_core, pod_offsets, None, run_core, run_mem, run_dev, run_offsets, run_prio, node_offsets,
+                       op=op)
+    check_preempt_gang_args(free_core, gang_offsets, run_offsets, gang_prio, run_gang, run_gang_min)
+    if not torch.compiler.is_compiling() and not torch.cuda.is_current_stream_capturing():
+        check_tables(free_core, free_mem, d_valid, op=op)
+        check_pods(pod_offsets, req_core.shape[0], op=op)
+        check_gangs(gang_offsets, gang_min, pod_offsets.shape[0] - 1, op=op)
+        check_running(free_core, free_mem, d_valid, run_core, run_mem, run_dev, run_offsets, node_offsets, op=op)
+        check_running_gangs(run_gang, run_gang_min)
+    return torch.ops.egpu.preempt_gangs(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_offsets,
+                                        gang_min, gang_prio, run_core, run_mem, run_dev, run_offsets, run_prio,
+                                        node_offsets, run_gang, run_gang_min)
