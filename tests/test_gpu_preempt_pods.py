@@ -45,8 +45,9 @@ def run(tables, a, raw=False):
     return [t.cpu().numpy() for t in out]
 
 
-def check(a, out):
-    exp = ref.place(*a)
+def check(a, out, exp=None):
+    """out equals the restatement's outputs exp (computed here when not given), info included."""
+    exp = ref.place(*a) if exp is None else exp
     assert out[0].dtype == np.int32 and out[1].dtype == np.int8 and out[2].dtype == np.int32
     for x, y in zip(out[:5], exp[:5]):
         np.testing.assert_array_equal(x, y)
@@ -145,12 +146,19 @@ def test_contended_and_ragged(N, D, G, tables):
     assert out[5][0] >= 3 and (out[2] >= 0).any()
 
 
+# running pods per node at every slot edge (a node's running pod h0 + lane + 32 i is slot i of the lane)
+SLOT_EDGES = [1, 31, 32, 33, 63, 64, 65, 95, 96, 97, 127, 128]
+
+
 @pytest.mark.gpu
+@pytest.mark.parametrize("counts", [[0, 128, 128, 0, 5, 128], SLOT_EDGES], ids=["0_5_128", "slot_edges"])
 @pytest.mark.parametrize("D", [8, 64])
-def test_nodes_at_0_and_128_running_pods(D, tables):
-    g = np.random.default_rng(77 + D)
-    N, G = 6, 120
-    counts = [0, 128, 128, 0, 5, 128]
+def test_nodes_at_0_and_128_running_pods(D, counts, tables):
+    """With SLOT_EDGES node n's running priorities are constant over h0 + [0, 16), [16, 48), [48, 80), [80, 112) and
+    [112, 128), at (-2, 1, -1, 2, 0) rotated by n: the walk (priority descending, h ascending) jumps between slots,
+    and each run of equal priorities but the first and last spans two slots."""
+    g = np.random.default_rng(77 + D + (0 if counts[0] == 0 else 1000))
+    N, G = len(counts), 120
     fc = np.zeros((N, D), np.int32)
     fm = np.zeros((N, D), np.int32)
     qc, qm, qd, roff, rprio = [], [], [], [0], []
@@ -164,7 +172,7 @@ def test_nodes_at_0_and_128_running_pods(D, tables):
             qm.append(0)
             qd.append(d)
             roff.append(roff[-1] + 1)
-            rprio.append(int(g.integers(-3, 4)))
+            rprio.append(int(g.integers(-3, 4)) if counts[0] == 0 else ((h + 16) // 32 * 3 + n) % 5 - 2)
         fc[n] = left // 4  # most of what the running pods leave is held by pods the caller does not list
         fm[n] = 1000
     noff = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
@@ -178,7 +186,11 @@ def test_nodes_at_0_and_128_running_pods(D, tables):
     check(a, out)
     invariants(a, out)
     run_node = np.repeat(np.arange(N), counts)
-    assert (out[2][np.isin(run_node, [1, 2, 5])] >= 0).any() and (out[2] >= 0).sum() >= 5
+    if counts[0] == 0:
+        assert (out[2][np.isin(run_node, [1, 2, 5])] >= 0).any() and (out[2] >= 0).sum() >= 5
+    else:  # victims in every slot
+        slot = (np.arange(run_node.size) - noff[run_node]) >> 5
+        assert set(slot[out[2] >= 0].tolist()) == {0, 1, 2, 3}
 
 
 # ---- 6. empty calls, inputs unchanged, repeat calls ------------------------------------------------------------
