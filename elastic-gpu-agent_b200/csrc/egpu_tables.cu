@@ -14,6 +14,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <climits>
 
 namespace egpu {
 
@@ -206,6 +207,58 @@ struct PlaceArgs {
     PlaceCtl* ctl;
     uint32_t gx, gm;                 // kGuards, kCandMask (in registers: see DevState::cand_xor)
 };
+
+// The compaction's offsets, summed by the whole CTA from the per-tile deferred counts (read from L2: every CTA's
+// commit wrote them): `before`, the rows deferred in the tiles before `lo`, and `total`, those of all `tiles`.
+__device__ __forceinline__ void deferred_prefix(const unsigned int* count, long long tiles, long long lo,
+                                                unsigned int& before, unsigned int& total,
+                                                unsigned int (*red)[kTabWarps]) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    before = 0;
+    total = 0;
+    for (long long t = tid; t < tiles; t += kTabThreads) {
+        const unsigned int c = __ldcg(count + t);
+        total += c;
+        before += t < lo ? c : 0u;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        before += __shfl_xor_sync(0xffffffffu, before, o);
+        total += __shfl_xor_sync(0xffffffffu, total, o);
+    }
+    if (lane == 0) {
+        red[0][warp] = before;
+        red[1][warp] = total;
+    }
+    __syncthreads();
+    before = 0;
+    total = 0;
+#pragma unroll
+    for (int w = 0; w < kTabWarps; ++w) {
+        before += red[0][w];
+        total += red[1][w];
+    }
+    __syncthreads();
+}
+
+// One compaction tile, every thread of the CTA with its row: the rows that defer go to next[before ...] in row order,
+// and `before` moves past them.
+__device__ __forceinline__ void append_deferred(bool defer, int32_t row, int32_t* next, unsigned int& before,
+                                                unsigned int* red) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned int bal = __ballot_sync(0xffffffffu, defer);
+    if (lane == 0) red[warp] = __popc(bal);
+    __syncthreads();
+    unsigned int at = before, in_tile = 0;
+#pragma unroll
+    for (int w = 0; w < kTabWarps; ++w) {
+        at += w < warp ? red[w] : 0u;
+        in_tile += red[w];
+    }
+    if (defer) next[at + __popc(bal & ((1u << lane) - 1u))] = row;
+    before += in_tile;
+    __syncthreads();
+}
 
 template <int DT, bool VEC>
 __global__ void __launch_bounds__(kTabThreads, 2)
@@ -431,30 +484,8 @@ place_tables_kernel(const __grid_constant__ PlaceArgs a) {
             for (long long t = static_cast<long long>(b) * kTabThreads + tid; t < tiles; t += static_cast<long long>(G) * kTabThreads)
                 next_count[t] = 0u;
             const long long lo = tiles * b / G, hi = tiles * (b + 1) / G;
-            unsigned int before = 0, total = 0;
-            for (long long t = tid; t < tiles; t += kTabThreads) {
-                const unsigned int c = __ldcg(count + t);
-                total += c;
-                before += t < lo ? c : 0u;
-            }
-#pragma unroll
-            for (int o = 16; o; o >>= 1) {
-                before += __shfl_xor_sync(0xffffffffu, before, o);
-                total += __shfl_xor_sync(0xffffffffu, total, o);
-            }
-            if (lane == 0) {
-                sRed[0][warp] = before;
-                sRed[1][warp] = total;
-            }
-            __syncthreads();
-            before = 0;
-            total = 0;
-#pragma unroll
-            for (int w = 0; w < kTabWarps; ++w) {
-                before += sRed[0][w];
-                total += sRed[1][w];
-            }
-            __syncthreads();
+            unsigned int before, total;
+            deferred_prefix(count, tiles, lo, before, total, sRed);
             int32_t* const next = a.set[which];
             for (long long t = lo; t < hi; ++t) {
                 const long long i = t * kPlaceBlock + tid;
@@ -470,18 +501,7 @@ place_tables_kernel(const __grid_constant__ PlaceArgs a) {
                         a.best[row] = 0ull;
                     }
                 }
-                const unsigned int bal = __ballot_sync(0xffffffffu, defer);
-                if (lane == 0) sRed[0][warp] = __popc(bal);
-                __syncthreads();
-                unsigned int at = before, in_tile = 0;
-#pragma unroll
-                for (int w = 0; w < kTabWarps; ++w) {
-                    at += w < warp ? sRed[0][w] : 0u;
-                    in_tile += sRed[0][w];
-                }
-                if (defer) next[at + __popc(bal & ((1u << lane) - 1u))] = row;
-                before += in_tile;
-                __syncthreads();
+                append_deferred(defer, row, next, before, sRed[0]);
             }
             if (total == 0u) {
                 done = true;
@@ -499,29 +519,24 @@ place_tables_kernel(const __grid_constant__ PlaceArgs a) {
     }
 }
 
-template <int DT>
-cudaError_t place_bucket(bool vec, int device, cudaStream_t stream, const PlaceArgs& a) {
-    auto fn = vec ? place_tables_kernel<DT, true> : place_tables_kernel<DT, false>;
-    // resident CTAs per SM of this kernel on each device, asked once
-    static std::atomic<int> per_sm_cache[kPlaceDevices][2];
-    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device][vec].load(std::memory_order_relaxed) : 0;
+// The cooperative launch of every round kernel: one resident wave of kTabThreads-thread CTAs on `device`, at most
+// `cap` of them (the caller's count of work items: the barriers cost per CTA) and at least one.  The resident CTAs
+// per SM are asked once per kernel and device: each instantiation has its own cache.
+template <auto kernel, class Args>
+cudaError_t coop_launch(const Args& a, long long cap, int device, cudaStream_t stream) {
+    static std::atomic<int> per_sm_cache[kPlaceDevices];
+    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
     if (per_sm == 0) {
-        cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kTabThreads, 0);
+        cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kTabThreads, 0);
         if (err != cudaSuccess) return err;
         if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
-        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device][vec].store(per_sm, std::memory_order_relaxed);
+        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
     }
     int sms = 0;
     cudaError_t err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     if (err != cudaSuccess) return err;
-    // Grid: one resident wave, no more CTAs than round 1 has work items of any phase (the barriers cost per CTA).
-    const long long tiles = (a.N + kTabWarps - 1) / kTabWarps;
-    const long long items = tiles * ((a.P + kPlaceChunk - 1) / kPlaceChunk);
-    const long long blocks = (a.P + kPlaceBlock - 1) / kPlaceBlock;
-    long long grid = static_cast<long long>(sms) * per_sm;
-    grid = std::min(grid, std::max(items, blocks));
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(grid));
+    cfg.gridDim = dim3(static_cast<unsigned>(std::max(1ll, std::min(static_cast<long long>(sms) * per_sm, cap))));
     cfg.blockDim = dim3(kTabThreads);
     cfg.dynamicSmemBytes = 0;
     cfg.stream = stream;
@@ -530,37 +545,54 @@ cudaError_t place_bucket(bool vec, int device, cudaStream_t stream, const PlaceA
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, fn, a);
+    return cudaLaunchKernelEx(&cfg, kernel, a);
 }
 
-size_t place_scratch_bytes(int P) {
-    const size_t blocks = (static_cast<size_t>(P) + kPlaceBlock - 1) / kPlaceBlock;
-    const size_t zeroed = 8 * static_cast<size_t>(P) + sizeof(PlaceCtl) + 2 * 4 * blocks;
-    return ((zeroed + 15) & ~size_t(15)) + 2 * 4 * static_cast<size_t>(P);
+template <int DT>
+cudaError_t place_bucket(bool vec, int device, cudaStream_t stream, const PlaceArgs& a) {
+    // Grid: no more CTAs than round 1 has work items of any phase.
+    const long long tiles = (a.N + kTabWarps - 1) / kTabWarps;
+    const long long items = tiles * ((a.P + kPlaceChunk - 1) / kPlaceChunk);
+    const long long blocks = (a.P + kPlaceBlock - 1) / kPlaceBlock;
+    return vec ? coop_launch<place_tables_kernel<DT, true>>(a, std::max(items, blocks), device, stream)
+               : coop_launch<place_tables_kernel<DT, false>>(a, std::max(items, blocks), device, stream);
 }
+
+// place_tables' scratch, byte offsets: best uint64[P] | barrier words | deferred counts 2 x uint32[P / 256] |
+// (16-aligned) two pending sets int32[P]; everything before the pending sets (`zeroed` bytes) starts at zero.
+struct PlaceScratch {
+    size_t blocks, ctl, count, zeroed, set, total;
+    explicit PlaceScratch(int P) {
+        blocks = (static_cast<size_t>(P) + kPlaceBlock - 1) / kPlaceBlock;
+        ctl = 8 * static_cast<size_t>(P);
+        count = ctl + sizeof(PlaceCtl);
+        zeroed = count + 2 * 4 * blocks;
+        set = (zeroed + 15) & ~size_t(15);
+        total = set + 2 * 4 * static_cast<size_t>(P);
+    }
+};
+
+size_t place_scratch_bytes(int P) { return PlaceScratch(P).total; }
 
 cudaError_t place_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
                          const int32_t* req_core, const int32_t* req_mem, int P, int32_t* out_node, int8_t* out_dev,
                          int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch, int device,
                          cudaStream_t stream) {
-    // scratch: best uint64[P] | barrier words | deferred counts 2 x uint32[P / 256] | (16-aligned) two pending sets
-    // int32[P]; everything before the pending sets starts at zero
-    const size_t blocks = (static_cast<size_t>(P) + kPlaceBlock - 1) / kPlaceBlock;
+    const PlaceScratch L(P);
     char* s = static_cast<char*>(scratch);
     PlaceArgs a{};
     a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem;
     a.N = N; a.D = D; a.P = P;
     a.node = out_node; a.dev = out_dev; a.fc_out = free_core_out; a.fm_out = free_mem_out; a.info = info;
     a.best = reinterpret_cast<unsigned long long*>(s);
-    a.ctl = reinterpret_cast<PlaceCtl*>(s + 8 * static_cast<size_t>(P));
-    a.count[0] = reinterpret_cast<unsigned int*>(s + 8 * static_cast<size_t>(P) + sizeof(PlaceCtl));
-    a.count[1] = a.count[0] + blocks;
-    const size_t zeroed = 8 * static_cast<size_t>(P) + sizeof(PlaceCtl) + 2 * 4 * blocks;
-    a.set[0] = reinterpret_cast<int32_t*>(s + ((zeroed + 15) & ~size_t(15)));
+    a.ctl = reinterpret_cast<PlaceCtl*>(s + L.ctl);
+    a.count[0] = reinterpret_cast<unsigned int*>(s + L.count);
+    a.count[1] = a.count[0] + L.blocks;
+    a.set[0] = reinterpret_cast<int32_t*>(s + L.set);
     a.set[1] = a.set[0] + P;
     a.gx = kGuards;
     a.gm = kCandMask;
-    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    cudaError_t err = cudaMemsetAsync(scratch, 0, L.zeroed, stream);
     if (err != cudaSuccess) return err;
     const bool vec = (P % 4) == 0 && (reinterpret_cast<uintptr_t>(req_core) % 16) == 0 &&
                      (reinterpret_cast<uintptr_t>(req_mem) % 16) == 0;
@@ -574,15 +606,17 @@ cudaError_t place_launch(const int32_t* free_core, const int32_t* free_mem, cons
 //
 // One cooperative launch, the round structure of place_tables_kernel with a pod in place of a row:
 //   0. the grid checks pod_offsets (first 0, last P, every step in [1, kMaxPod]) before any container is read
-//      through them; if one is bad nothing is placed, the tables are copied and info[2] = 1;
-//   1. choose: work items are (block of 256 pending pods, tile of 8 tables).  A warp stages its table's
+//      through them and copies the tables to free_*_out (every round reads them there); if an offset is bad
+//      nothing is placed and info[2] = 1;
+//   1. choose (pods_choose): work items are (block of 256 pending pods, tile of 8 tables).  A warp stages its table's
 //      valid devices in shared memory and each lane replays one pod on it (pod_replay); the CTA keeps each pod's
 //      best word over warps and tiles and does one atomicMax per pod (words inverted, 0 = no node yet);
-//   2. commit: the warp of table n walks the pending pods that chose n in pod order.  The lanes replay their pods
-//      again against the round's table to recover the containers' devices, then, one pod after another, a pod
-//      commits when none of its devices is closed and the demand committed so far on each of them, plus its own,
-//      fits; otherwise it closes all of them;
-//   3. compact: deferred pods go, in pod order, into the other pending set; pods that chose nothing become -1.
+//   2. commit (pods_commit): the warp of table n walks the pending pods that chose n in pod order.  The lanes replay
+//      their pods again against the round's table to recover the containers' devices, then, one pod after another,
+//      a pod commits when none of its devices is closed and the demand committed so far on each of them, plus its
+//      own, fits; otherwise it closes all of them;
+//   3. compact (deferred_prefix, pods_compact): deferred pods go, in pod order, into the other pending set; pods that
+//      chose nothing become -1.
 // The pods' devices are not kept between phases: the replay is deterministic, so commit recomputes them.
 constexpr int kMaxPod = 8;                 // containers per pod
 constexpr int kPodBlock = kTabThreads;     // pods per choose work item and per compaction tile
@@ -591,8 +625,8 @@ constexpr int kPodStage = kTabWarps * kPodBlock;  // pending pods the commit pha
 struct PodsCtl {
     RoundsCtl bar;                // grid-barrier words
     unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
-    unsigned int in_domain;       // some pod is in the domain
-    unsigned int bad_offsets;     // pod_offsets failed the check (info[2])
+    unsigned int in_domain;       // some pod is in the domain (place_pods)
+    unsigned int bad_index;       // an index tensor failed the check (info[2])
     unsigned int pad_[2];
 };
 
@@ -707,47 +741,233 @@ __device__ __forceinline__ int stage_table_warp(const int32_t* fc_row, const int
     return rows;
 }
 
-__global__ void __launch_bounds__(kTabThreads, 2)
-place_pods_kernel(const __grid_constant__ PodsArgs a) {
-    __shared__ unsigned long long sW[kTabWarps][kPodBlock];  // choose: each warp's (inverted) words for a block of pods
-    __shared__ int32_t sFc[kTabWarps][kMaxD], sFm[kTabWarps][kMaxD];      // the table as the round found it
-    __shared__ int32_t sAccC[kTabWarps][kMaxD], sAccM[kTabWarps][kMaxD];  // commit: demand committed per device
-    __shared__ int32_t sClosed[kTabWarps][kMaxD];                          // ... a pod did not commit: later pods cannot
-    __shared__ int32_t sPod[kPodStage];  // commit: the staged pods (their words are staged in sW)
-    __shared__ unsigned int sRed[2][kTabWarps];
-    __shared__ int sOk;
+// One position of the check of a CSR offset array off [n + 1] over `total` entries: the first offset is 0, the last
+// is total, and every step off[i + 1] - off[i] is in [lo, hi].  True when position i (0 <= i <= n) fails it.
+__device__ __forceinline__ bool csr_bad(const int32_t* off, long long i, long long n, long long total, long long lo,
+                                        long long hi) {
+    const int32_t o = __ldg(off + i);
+    const bool bad = i == 0 && o != 0;
+    if (i == n) return bad || o != total;
+    const long long step = static_cast<long long>(__ldg(off + i + 1)) - o;
+    return bad || step < lo || step > hi;
+}
+
+// The shared memory of place_pods_kernel and place_gangs_kernel, the grid barrier's word apart.
+struct PodsSmem {
+    unsigned long long W[kTabWarps][kPodBlock];  // choose: each warp's (inverted) words for a block of pods
+    int32_t Fc[kTabWarps][kMaxD], Fm[kTabWarps][kMaxD];      // the table as the round found it
+    int32_t AccC[kTabWarps][kMaxD], AccM[kTabWarps][kMaxD];  // commit: demand committed per device
+    int32_t Closed[kTabWarps][kMaxD];                        // ... a pod did not commit: later pods cannot
+    int32_t Pod[kPodStage];  // commit: the staged pods (their words are staged in W)
+    unsigned int Red[2][kTabWarps];
+};
+
+// The phases of place_pods_kernel and place_gangs_kernel.  The pending set of a round is positions [0, m): position i
+// is pod cur[i], or pod pos0 + i when cur is null (round 1 of place_pods, pos0 = 0, and of a gang, pos0 = its first
+// pod).  Every thread of the CTA calls them.
+
+// ---- 1. choose
+__device__ __forceinline__ void pods_choose(const PodsArgs& a, const int32_t* cur, long long pos0, long long m,
+                                            PodsSmem& s) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const unsigned int b = blockIdx.x, G = gridDim.x;
     const int N = a.N, D = a.D, T = (N + kTabWarps - 1) / kTabWarps;
+    const long long blocks = (m + kPodBlock - 1) / kPodBlock, items = blocks * T;
+    const long long lo = items * b / G, hi = items * (b + 1) / G;
+    unsigned long long mine = 0;
+    long long held = -1;  // the block of pods `mine` belongs to
+    for (long long it = lo; it <= hi; ++it) {
+        const long long blk = it < hi ? it / T : -1;
+        if (held >= 0 && blk != held) {  // the CTA's last tile of a block: one atomic per pod
+            const long long i = held * kPodBlock + tid;
+            if (i < m && mine) atomicMax(a.best + (cur ? __ldcg(cur + i) : pos0 + i), mine);
+            mine = 0;
+        }
+        if (it == hi) break;
+        held = blk;
+        const int tn = static_cast<int>(it - blk * T) * kTabWarps + warp;
+        const size_t off = static_cast<size_t>(tn) * D;
+        const int rows = stage_table_warp(a.fc_out + off, a.fm_out + off, tn < N ? __ldg(a.dv + tn) : 0, D, s.Fc[warp],
+                                          s.Fm[warp]);
+        for (int j = lane; j < kPodBlock; j += 32) {
+            const long long i = blk * kPodBlock + j;
+            unsigned long long w = 0;
+            if (i < m && rows) {
+                const long long g = cur ? __ldcg(cur + i) : pos0 + i;
+                const int32_t c0 = __ldg(a.off + g);
+                PodFit f;
+                // ~(sum lc << 52 | sum lm << 31 | n): the unsigned order of the word is (sum lc, sum lm, n)
+                if (pod_replay(s.Fc[warp], s.Fm[warp], rows, a.rc, a.rm, c0, __ldg(a.off + g + 1) - c0, f))
+                    w = ~((static_cast<unsigned long long>(f.slc) << 52) |
+                          (static_cast<unsigned long long>(f.slm) << 31) | static_cast<unsigned long long>(tn));
+            }
+            s.W[warp][j] = w;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int w = 0; w < kTabWarps; ++w) mine = max(mine, s.W[w][tid]);
+        __syncthreads();
+    }
+}
+
+// ---- 2. commit: adds each compaction tile's deferred pods to count[tile]; returns the warp's committed pods.
+__device__ __forceinline__ unsigned int pods_commit(const PodsArgs& a, unsigned int* count, const int32_t* cur,
+                                                    long long pos0, long long m, PodsSmem& s) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int N = a.N, D = a.D, T = (N + kTabWarps - 1) / kTabWarps;
+    unsigned long long* const sStage = &s.W[0][0];  // kPodStage words: the choose phase is over
+    long long staged = -1;                          // the first pending position staged in sStage / s.Pod
+    unsigned int committed = 0;                     // this warp's committed pods
+    for (int tile = static_cast<int>(b); tile < T; tile += static_cast<int>(G)) {
+        const int tn = tile * kTabWarps + warp;
+        const size_t off = static_cast<size_t>(tn) * D;
+        // a table outside the domain offers no device, so no pod chose it: it keeps its copy
+        const int rows = stage_table_warp(a.fc_out + off, a.fm_out + off, tn < N ? __ldg(a.dv + tn) : 0, D, s.Fc[warp],
+                                          s.Fm[warp]);
+        for (int j = lane; j < kMaxD; j += 32) {
+            s.AccC[warp][j] = 0;
+            s.AccM[warp][j] = 0;
+            s.Closed[warp][j] = 0;
+        }
+        __syncwarp();
+        bool dirty = false;
+        for (long long i0 = 0; i0 < m; i0 += kPodStage) {
+            if (i0 != staged) {  // at most kPodStage pending pods are staged once per round for every tile
+                __syncthreads();  // every warp is done with the pods staged before
+                for (int k = tid; k < kPodStage; k += kTabThreads) {
+                    const long long i = i0 + k;
+                    unsigned long long w = ~0ull;  // names no table
+                    if (i < m) {
+                        const int32_t g = cur ? __ldcg(cur + i) : static_cast<int32_t>(pos0 + i);
+                        s.Pod[k] = g;
+                        w = ~__ldcg(a.best + g);
+                    }
+                    sStage[k] = w;
+                }
+                __syncthreads();
+                staged = i0;
+            }
+            if (!rows) continue;
+            const int len = static_cast<int>(min(static_cast<long long>(kPodStage), m - i0));
+            for (int j0 = 0; j0 < len; j0 += kPodBlock) {  // one compaction tile
+                unsigned int deferred = 0;
+                for (int j = j0 + lane; j < j0 + kPodBlock; j += 32) {
+                    const unsigned long long w = sStage[j];
+                    const bool matched = static_cast<int>(w & 0x7fffffffu) == tn;
+                    const unsigned int mb = __ballot_sync(0xffffffffu, matched);
+                    if (mb == 0u) continue;
+                    PodFit f;
+                    int32_t g = 0, c0 = 0, c1 = 0;
+                    if (matched) {  // the choose phase's replay, again: it fitted then, so it fits now
+                        g = s.Pod[j];
+                        c0 = __ldg(a.off + g);
+                        c1 = __ldg(a.off + g + 1);
+                        pod_replay(s.Fc[warp], s.Fm[warp], rows, a.rc, a.rm, c0, c1 - c0, f);
+                    }
+                    // one pod after another, in pod order (lane order)
+                    bool fits = false;
+                    for (unsigned int r = mb; r; r &= r - 1u) {
+                        if (lane == __ffs(r) - 1) {
+                            bool ok = true;
+#pragma unroll
+                            for (int k = 0; k < kMaxPod; ++k)
+                                if (k < f.nt) {  // committed + the pod's demand <= free  <=>  committed <= what the pod leaves
+                                    const int d = f.td[k];
+                                    ok &= !s.Closed[warp][d] && s.AccC[warp][d] <= f.tc[k] && s.AccM[warp][d] <= f.tm[k];
+                                }
+#pragma unroll
+                            for (int k = 0; k < kMaxPod; ++k)
+                                if (k < f.nt) {
+                                    const int d = f.td[k];
+                                    if (ok) {
+                                        s.AccC[warp][d] += s.Fc[warp][d] - f.tc[k];
+                                        s.AccM[warp][d] += s.Fm[warp][d] - f.tm[k];
+                                    } else {
+                                        s.Closed[warp][d] = 1;
+                                    }
+                                }
+                            fits = ok;
+                        }
+                        __syncwarp();
+                    }
+                    if (fits) {
+                        a.node[g] = tn;
+                        for (int32_t c = c0; c < c1; ++c)
+                            a.dev[c] = static_cast<int8_t>((f.cdev >> (6 * (c - c0))) & 63u);
+                    }
+                    const unsigned int fb = __ballot_sync(0xffffffffu, fits);
+                    dirty |= fb != 0u;
+                    committed += __popc(fb);
+                    deferred += __popc(mb & ~fb);
+                }
+                if (lane == 0 && deferred) atomicAdd(count + (i0 + j0) / kPodBlock, deferred);
+            }
+        }
+        __syncwarp();
+        if (dirty)
+            for (int j = lane; j < rows; j += 32) {
+                a.fc_out[off + j] = s.Fc[warp][j] - s.AccC[warp][j];
+                a.fm_out[off + j] = s.Fm[warp][j] - s.AccM[warp][j];
+            }
+    }
+    return committed;
+}
+
+// ---- 3. compact the CTA's compaction tiles [lo, hi), `before` the deferred pods of the tiles before lo
+__device__ __forceinline__ void pods_compact(const PodsArgs& a, const int32_t* cur, long long pos0, long long m,
+                                             long long lo, long long hi, int32_t* next, unsigned int before,
+                                             PodsSmem& s) {
+    const int tid = threadIdx.x;
+    for (long long t = lo; t < hi; ++t) {
+        const long long i = t * kPodBlock + tid;
+        bool defer = false;
+        int32_t g = 0;
+        if (i < m) {
+            g = cur ? __ldcg(cur + i) : static_cast<int32_t>(pos0 + i);
+            if (__ldcg(a.best + g) == 0ull) {
+                a.node[g] = -1;
+                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
+            } else if (__ldcg(a.node + g) == -2) {
+                defer = true;
+                a.best[g] = 0ull;
+            }
+        }
+        append_deferred(defer, g, next, before, s.Red[0]);
+    }
+}
+
+__global__ void __launch_bounds__(kTabThreads, 2)
+place_pods_kernel(const __grid_constant__ PodsArgs a) {
+    __shared__ PodsSmem s;
+    __shared__ int sOk;
+    const int tid = threadIdx.x;
+    const unsigned int b = blockIdx.x, G = gridDim.x;
+    const int N = a.N, D = a.D;
     const long long stride = static_cast<long long>(G) * kTabThreads, first = static_cast<long long>(b) * kTabThreads + tid;
     unsigned int gen = 0;
     int round = 0;
     bool done = false;
 
-    // ---- 0. every pod and container undecided; the offsets checked before a container is read through them
+    // ---- 0. every pod and container undecided, the tables copied; the offsets checked before a container is read
+    // through them
     {
         bool bad = false;
         for (long long g = first; g <= a.G; g += stride) {
-            const int32_t o = __ldg(a.off + g);
-            if (g == 0) bad |= o != 0;
-            if (g == a.G) bad |= o != a.P;
-            if (g < a.G) {
-                const long long step = static_cast<long long>(__ldg(a.off + g + 1)) - o;
-                bad |= step < 1 || step > kMaxPod;
-                a.node[g] = -2;
-            }
+            bad |= csr_bad(a.off, g, a.G, a.P, 1, kMaxPod);
+            if (g < a.G) a.node[g] = -2;
         }
         for (long long c = first; c < a.P; c += stride) a.dev[c] = -2;
-        if (__syncthreads_or(bad) && tid == 0) atomicExch(&a.ctl->bad_offsets, 1u);
-    }
-    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
-    if (*reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_offsets)) {  // nothing is placed
-        for (long long g = first; g < a.G; g += stride) a.node[g] = -1;
-        for (long long c = first; c < a.P; c += stride) a.dev[c] = -1;
         for (long long j = first; j < static_cast<long long>(N) * D; j += stride) {
             a.fc_out[j] = a.fc[j];
             a.fm_out[j] = a.fm[j];
         }
+        if (__syncthreads_or(bad) && tid == 0) atomicExch(&a.ctl->bad_index, 1u);
+    }
+    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+    if (*reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_index)) {  // nothing is placed
+        for (long long g = first; g < a.G; g += stride) a.node[g] = -1;
+        for (long long c = first; c < a.P; c += stride) a.dev[c] = -1;
         done = true;
         goto finish;
     }
@@ -771,150 +991,10 @@ place_pods_kernel(const __grid_constant__ PodsArgs a) {
         int which = 0;
         while (!done) {
             ++round;
-            const int32_t* tab_c = round == 1 ? a.fc : a.fc_out;
-            const int32_t* tab_m = round == 1 ? a.fm : a.fm_out;
-
-            // ---- 1. choose
-            {
-                const long long blocks = (n + kPodBlock - 1) / kPodBlock, items = blocks * T;
-                const long long lo = items * b / G, hi = items * (b + 1) / G;
-                unsigned long long mine = 0;
-                long long held = -1;  // the block of pods `mine` belongs to
-                for (long long it = lo; it <= hi; ++it) {
-                    const long long blk = it < hi ? it / T : -1;
-                    if (held >= 0 && blk != held) {  // the CTA's last tile of a block: one atomic per pod
-                        const long long i = held * kPodBlock + tid;
-                        if (i < n && mine) atomicMax(a.best + (cur ? __ldcg(cur + i) : i), mine);
-                        mine = 0;
-                    }
-                    if (it == hi) break;
-                    held = blk;
-                    const int tn = static_cast<int>(it - blk * T) * kTabWarps + warp;
-                    const size_t off = static_cast<size_t>(tn) * D;
-                    const int rows = stage_table_warp(tab_c + off, tab_m + off, tn < N ? __ldg(a.dv + tn) : 0, D, sFc[warp],
-                                                      sFm[warp]);
-                    if (round == 1 && blk == 0 && tn < N)
-                        for (int j = lane; j < D; j += 32) {
-                            a.fc_out[off + j] = a.fc[off + j];
-                            a.fm_out[off + j] = a.fm[off + j];
-                        }
-                    for (int j = lane; j < kPodBlock; j += 32) {
-                        const long long i = blk * kPodBlock + j;
-                        unsigned long long w = 0;
-                        if (i < n && rows) {
-                            const long long g = cur ? __ldcg(cur + i) : i;
-                            const int32_t c0 = __ldg(a.off + g);
-                            PodFit f;
-                            // ~(sum lc << 52 | sum lm << 31 | n): the unsigned order of the word is (sum lc, sum lm, n)
-                            if (pod_replay(sFc[warp], sFm[warp], rows, a.rc, a.rm, c0, __ldg(a.off + g + 1) - c0, f))
-                                w = ~((static_cast<unsigned long long>(f.slc) << 52) |
-                                      (static_cast<unsigned long long>(f.slm) << 31) | static_cast<unsigned long long>(tn));
-                        }
-                        sW[warp][j] = w;
-                    }
-                    __syncthreads();
-#pragma unroll
-                    for (int w = 0; w < kTabWarps; ++w) mine = max(mine, sW[w][tid]);
-                    __syncthreads();
-                }
-            }
+            pods_choose(a, cur, 0, n, s);
             if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) break;
-
-            // ---- 2. commit
             unsigned int* const count = a.count[(round - 1) & 1];
-            unsigned long long* const sStage = &sW[0][0];  // kPodStage words: the choose phase is over
-            long long staged = -1;                         // the first pending pod staged in sStage / sPod
-            for (int tile = static_cast<int>(b); tile < T; tile += static_cast<int>(G)) {
-                const int tn = tile * kTabWarps + warp;
-                const size_t off = static_cast<size_t>(tn) * D;
-                // a table outside the domain offers no device, so no pod chose it: it keeps its copy
-                const int rows = stage_table_warp(tab_c + off, tab_m + off, tn < N ? __ldg(a.dv + tn) : 0, D, sFc[warp],
-                                                  sFm[warp]);
-                for (int j = lane; j < kMaxD; j += 32) {
-                    sAccC[warp][j] = 0;
-                    sAccM[warp][j] = 0;
-                    sClosed[warp][j] = 0;
-                }
-                __syncwarp();
-                bool dirty = false;
-                for (long long i0 = 0; i0 < n; i0 += kPodStage) {
-                    if (i0 != staged) {  // at most kPodStage pending pods are staged once per round for every tile
-                        __syncthreads();  // every warp is done with the pods staged before
-                        for (int k = tid; k < kPodStage; k += kTabThreads) {
-                            const long long i = i0 + k;
-                            unsigned long long w = ~0ull;  // names no table
-                            if (i < n) {
-                                const int32_t g = cur ? __ldcg(cur + i) : static_cast<int32_t>(i);
-                                sPod[k] = g;
-                                w = ~__ldcg(a.best + g);
-                            }
-                            sStage[k] = w;
-                        }
-                        __syncthreads();
-                        staged = i0;
-                    }
-                    if (!rows) continue;
-                    const int len = static_cast<int>(min(static_cast<long long>(kPodStage), n - i0));
-                    for (int j0 = 0; j0 < len; j0 += kPodBlock) {  // one compaction tile
-                        unsigned int deferred = 0;
-                        for (int j = j0 + lane; j < j0 + kPodBlock; j += 32) {
-                            const unsigned long long w = sStage[j];
-                            const bool matched = static_cast<int>(w & 0x7fffffffu) == tn;
-                            const unsigned int mb = __ballot_sync(0xffffffffu, matched);
-                            if (mb == 0u) continue;
-                            PodFit f;
-                            int32_t g = 0, c0 = 0, c1 = 0;
-                            if (matched) {  // the choose phase's replay, again: it fitted then, so it fits now
-                                g = sPod[j];
-                                c0 = __ldg(a.off + g);
-                                c1 = __ldg(a.off + g + 1);
-                                pod_replay(sFc[warp], sFm[warp], rows, a.rc, a.rm, c0, c1 - c0, f);
-                            }
-                            // one pod after another, in pod order (lane order)
-                            bool fits = false;
-                            for (unsigned int r = mb; r; r &= r - 1u) {
-                                if (lane == __ffs(r) - 1) {
-                                    bool ok = true;
-#pragma unroll
-                                    for (int s = 0; s < kMaxPod; ++s)
-                                        if (s < f.nt) {  // committed + the pod's demand <= free  <=>  committed <= what the pod leaves
-                                            const int d = f.td[s];
-                                            ok &= !sClosed[warp][d] && sAccC[warp][d] <= f.tc[s] && sAccM[warp][d] <= f.tm[s];
-                                        }
-#pragma unroll
-                                    for (int s = 0; s < kMaxPod; ++s)
-                                        if (s < f.nt) {
-                                            const int d = f.td[s];
-                                            if (ok) {
-                                                sAccC[warp][d] += sFc[warp][d] - f.tc[s];
-                                                sAccM[warp][d] += sFm[warp][d] - f.tm[s];
-                                            } else {
-                                                sClosed[warp][d] = 1;
-                                            }
-                                        }
-                                    fits = ok;
-                                }
-                                __syncwarp();
-                            }
-                            if (fits) {
-                                a.node[g] = tn;
-                                for (int32_t c = c0; c < c1; ++c)
-                                    a.dev[c] = static_cast<int8_t>((f.cdev >> (6 * (c - c0))) & 63u);
-                            }
-                            const unsigned int fb = __ballot_sync(0xffffffffu, fits);
-                            dirty |= fb != 0u;
-                            deferred += __popc(mb & ~fb);
-                        }
-                        if (lane == 0 && deferred) atomicAdd(count + (i0 + j0) / kPodBlock, deferred);
-                    }
-                }
-                __syncwarp();
-                if (dirty)
-                    for (int j = lane; j < rows; j += 32) {
-                        a.fc_out[off + j] = sFc[warp][j] - sAccC[warp][j];
-                        a.fm_out[off + j] = sFm[warp][j] - sAccM[warp][j];
-                    }
-            }
+            pods_commit(a, count, cur, 0, n, s);
             if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) break;
 
             // ---- 3. compact
@@ -923,62 +1003,13 @@ place_pods_kernel(const __grid_constant__ PodsArgs a) {
                 unsigned int* const next_count = a.count[round & 1];  // last read in the previous round's phase 3
                 for (long long t = first; t < tiles; t += stride) next_count[t] = 0u;
                 const long long lo = tiles * b / G, hi = tiles * (b + 1) / G;
-                unsigned int before = 0, total = 0;
-                for (long long t = tid; t < tiles; t += kTabThreads) {
-                    const unsigned int c = __ldcg(count + t);
-                    total += c;
-                    before += t < lo ? c : 0u;
-                }
-#pragma unroll
-                for (int o = 16; o; o >>= 1) {
-                    before += __shfl_xor_sync(0xffffffffu, before, o);
-                    total += __shfl_xor_sync(0xffffffffu, total, o);
-                }
-                if (lane == 0) {
-                    sRed[0][warp] = before;
-                    sRed[1][warp] = total;
-                }
-                __syncthreads();
-                before = 0;
-                total = 0;
-#pragma unroll
-                for (int w = 0; w < kTabWarps; ++w) {
-                    before += sRed[0][w];
-                    total += sRed[1][w];
-                }
-                __syncthreads();
-                int32_t* const next = a.set[which];
-                for (long long t = lo; t < hi; ++t) {
-                    const long long i = t * kPodBlock + tid;
-                    bool defer = false;
-                    int32_t g = 0;
-                    if (i < n) {
-                        g = cur ? __ldcg(cur + i) : static_cast<int32_t>(i);
-                        if (__ldcg(a.best + g) == 0ull) {
-                            a.node[g] = -1;
-                            for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
-                        } else if (__ldcg(a.node + g) == -2) {
-                            defer = true;
-                            a.best[g] = 0ull;
-                        }
-                    }
-                    const unsigned int bal = __ballot_sync(0xffffffffu, defer);
-                    if (lane == 0) sRed[0][warp] = __popc(bal);
-                    __syncthreads();
-                    unsigned int at = before, in_tile = 0;
-#pragma unroll
-                    for (int w = 0; w < kTabWarps; ++w) {
-                        at += w < warp ? sRed[0][w] : 0u;
-                        in_tile += sRed[0][w];
-                    }
-                    if (defer) next[at + __popc(bal & ((1u << lane) - 1u))] = g;
-                    before += in_tile;
-                    __syncthreads();
-                }
+                unsigned int before, total;
+                deferred_prefix(count, tiles, lo, before, total, s.Red);
+                pods_compact(a, cur, 0, n, lo, hi, a.set[which], before, s);
                 if (total == 0u) {
                     done = true;
                 } else {
-                    cur = next;
+                    cur = a.set[which];
                     n = total;
                     which ^= 1;
                 }
@@ -988,70 +1019,58 @@ place_pods_kernel(const __grid_constant__ PodsArgs a) {
     }
 finish:
     if (b == 0 && tid == 0) {
-        const bool bad = *reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_offsets) != 0u;
+        const bool bad = *reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_index) != 0u;
         a.info[0] = !bad && *reinterpret_cast<volatile unsigned int*>(&a.ctl->in_domain) ? round : 0;
         a.info[1] = done ? 0 : 1;
         a.info[2] = bad ? 1 : 0;
     }
 }
 
-size_t pods_scratch_bytes(int G) {
-    const size_t blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
-    const size_t zeroed = 8 * static_cast<size_t>(G) + sizeof(PodsCtl) + 2 * 4 * blocks;
-    return ((zeroed + 15) & ~size_t(15)) + 2 * 4 * static_cast<size_t>(G);
+// place_pods' and place_gangs' scratch (place_pods: J = 0), byte offsets: best uint64[G] | barrier words | deferred
+// counts 2 x uint32[G / 256] | pods in the domain uint32[J] | committed pods uint32[J] | (16-aligned) two pending
+// sets int32[G]; everything before the pending sets (`zeroed` bytes) starts at zero.
+struct PodsScratch {
+    size_t blocks, ctl, count, in_domain, committed, zeroed, set, total;
+    PodsScratch(int G, int J) {
+        blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
+        ctl = 8 * static_cast<size_t>(G);
+        count = ctl + sizeof(PodsCtl);
+        in_domain = count + 2 * 4 * blocks;
+        committed = in_domain + 4 * static_cast<size_t>(J);
+        zeroed = committed + 4 * static_cast<size_t>(J);
+        set = (zeroed + 15) & ~size_t(15);
+        total = set + 2 * 4 * static_cast<size_t>(G);
+    }
+};
+
+// Points a's scratch arrays into `scratch` as L lays them out (a.G set) and zeroes its head on `stream`.
+static cudaError_t pods_scratch(PodsArgs& a, void* scratch, const PodsScratch& L, cudaStream_t stream) {
+    char* s = static_cast<char*>(scratch);
+    a.best = reinterpret_cast<unsigned long long*>(s);
+    a.ctl = reinterpret_cast<PodsCtl*>(s + L.ctl);
+    a.count[0] = reinterpret_cast<unsigned int*>(s + L.count);
+    a.count[1] = a.count[0] + L.blocks;
+    a.set[0] = reinterpret_cast<int32_t*>(s + L.set);
+    a.set[1] = a.set[0] + a.G;
+    return cudaMemsetAsync(scratch, 0, L.zeroed, stream);
 }
+
+size_t pods_scratch_bytes(int G) { return PodsScratch(G, 0).total; }
 
 cudaError_t pods_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
                         const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets, int G,
                         int32_t* out_node, int8_t* out_dev, int32_t* free_core_out, int32_t* free_mem_out, int32_t* info,
                         void* scratch, int device, cudaStream_t stream) {
-    // scratch: best uint64[G] | barrier words | deferred counts 2 x uint32[G / 256] | (16-aligned) two pending sets
-    // int32[G]; everything before the pending sets starts at zero
-    const size_t blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
-    char* s = static_cast<char*>(scratch);
+    const PodsScratch L(G, 0);
     PodsArgs a{};
     a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem; a.off = pod_offsets;
     a.N = N; a.D = D; a.P = P; a.G = G;
     a.node = out_node; a.dev = out_dev; a.fc_out = free_core_out; a.fm_out = free_mem_out; a.info = info;
-    a.best = reinterpret_cast<unsigned long long*>(s);
-    a.ctl = reinterpret_cast<PodsCtl*>(s + 8 * static_cast<size_t>(G));
-    a.count[0] = reinterpret_cast<unsigned int*>(s + 8 * static_cast<size_t>(G) + sizeof(PodsCtl));
-    a.count[1] = a.count[0] + blocks;
-    const size_t zeroed = 8 * static_cast<size_t>(G) + sizeof(PodsCtl) + 2 * 4 * blocks;
-    a.set[0] = reinterpret_cast<int32_t*>(s + ((zeroed + 15) & ~size_t(15)));
-    a.set[1] = a.set[0] + G;
-    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    const cudaError_t err = pods_scratch(a, scratch, L, stream);
     if (err != cudaSuccess) return err;
-
-    // resident CTAs per SM on each device, asked once
-    static std::atomic<int> per_sm_cache[kPlaceDevices];
-    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
-    if (per_sm == 0) {
-        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, place_pods_kernel, kTabThreads, 0);
-        if (err != cudaSuccess) return err;
-        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
-        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
-    }
-    int sms = 0;
-    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    if (err != cudaSuccess) return err;
-    // Grid: one resident wave, no more CTAs than round 1 has choose work items (the barriers cost per CTA); at
-    // least one, which finds G = 0's offsets bad.
+    // Grid: no more CTAs than round 1 has choose work items; at least one, which finds G = 0's offsets bad.
     const long long tiles = (static_cast<long long>(N) + kTabWarps - 1) / kTabWarps;
-    const long long items = tiles * static_cast<long long>(blocks);
-    long long grid = static_cast<long long>(sms) * per_sm;
-    grid = std::max(1ll, std::min(grid, items));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(grid));
-    cfg.blockDim = dim3(kTabThreads);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, place_pods_kernel, a);
+    return coop_launch<place_pods_kernel>(a, tiles * static_cast<long long>(L.blocks), device, stream);
 }
 
 // ---- egpu::place_gangs (DESIGN.md §2.13, §4.8): gangs of pods, each kept or given back, in order, in one launch ---
@@ -1060,61 +1079,74 @@ cudaError_t pods_launch(const int32_t* free_core, const int32_t* free_mem, const
 // pending pods only:
 //   0. the grid checks pod_offsets, gang_offsets and gang_min, marks every pod and container -2, every gang's placed
 //      count 0, and copies the tables to free_*_out (every round reads them there).  After a barrier: if an index is
-//      bad nothing is placed and info[2] = 1; otherwise each pod in the domain is counted into its gang (binary search
-//      of gang_offsets), and a second barrier follows;
+//      bad nothing is placed and info[2] = 1; otherwise each pod in the domain is counted into its gang
+//      (count_into_gang), and a second barrier follows;
 //   per gang j, while it has pending pods and placed + pending >= gang_min[j] (round 1's pending pods are the gang's
 //   pods in the domain, its contiguous range holds them):
-//   1. choose and 2. commit as §4.7; the commit also counts the gang's committed pods;
+//   1. choose and 2. commit as §4.7 (pods_choose, pods_commit); the commit also counts the gang's committed pods;
 //   3. compact: every CTA first reads the round's committed and deferred counts.  If nothing is deferred, or
 //      committed + deferred < gang_min, the gang ends with this round.  A gang that ends with fewer than gang_min pods
-//      committed is rolled back instead of compacted: its committed containers' demand goes back to free_*_out by
-//      integer atomics and all its pods become -1; one barrier follows before the next gang's choose reads the tables.
-//      A kept gang ends without a barrier: the next gang's choose reads nothing this phase writes.
+//      committed is rolled back instead of compacted (give_back_pods): its committed containers' demand goes back to
+//      free_*_out by integer atomics and all its pods become -1; one barrier follows before the next gang's choose
+//      reads the tables.  A kept gang ends without a barrier: the next gang's choose reads nothing this phase writes.
 // Deferred counts are indexed by the launch's round number over all gangs, so their zeroing follows §4.7's parity.
-struct GangsCtl {
-    RoundsCtl bar;                // grid-barrier words
-    unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
-    unsigned int bad_index;       // pod_offsets, gang_offsets or gang_min failed the check (info[2])
-    unsigned int pad_[3];
-};
-
 struct GangsArgs {
-    const int32_t* fc;               // the caller's tables [N][D], d_valid [N], containers [P], pod_offsets [G + 1],
-    const int32_t* fm;               // gang_offsets [J + 1], gang_min [J]
-    const int32_t* dv;
-    const int32_t* rc;
-    const int32_t* rm;
-    const int32_t* off;
-    const int32_t* goff;
+    PodsArgs p;                      // tables, containers, pod_offsets, the outputs node, dev, tables and info, and the
+                                     // scratch best, set, count, ctl (p.ctl->in_domain unused)
+    const int32_t* goff;             // gang_offsets [J + 1], gang_min [J]
     const int32_t* gmin;
-    int N, D;
-    long long P, G, J;
-    int32_t* node;                   // outputs: node per pod [G], device per container [P], placed per gang [J],
-    int8_t* dev;                     // tables [N][D], info [3]
-    int32_t* placed;
-    int32_t* fc_out;
-    int32_t* fm_out;
-    int32_t* info;
-    unsigned long long* best;        // [G]: each pending pod's choice, inverted (0 = none yet)
-    int32_t* set[2];                 // [G] each: the pending pods of a round, in pod order
-    unsigned int* count[2];          // [G / 256] each, by round parity: deferred pods per compaction tile
+    long long J;
+    int32_t* placed;                 // output: placed pods per gang [J]
     unsigned int* in_domain;         // [J]: each gang's pods in the domain
     unsigned int* committed;         // [J]: each gang's committed pods
-    GangsCtl* ctl;
 };
 
+// Counts pod g, when ok, into in_domain[j] of its gang j, the last gang whose first pod is at or before g (a binary
+// search of gang_offsets [J + 1]).  Every lane of the warp calls it.
+__device__ __forceinline__ void count_into_gang(const int32_t* goff, long long J, long long g, bool ok,
+                                                unsigned int* in_domain) {
+    long long j = 0;
+    if (ok) {
+        long long lo = 0, hi = J - 1;
+        while (lo < hi) {
+            const long long mid = (lo + hi + 1) >> 1;
+            if (__ldg(goff + mid) <= g) lo = mid;
+            else hi = mid - 1;
+        }
+        j = lo;
+    }
+    // the pods of a warp are consecutive, so most share a gang: one atomic per gang and warp
+    const unsigned int peers = __match_any_sync(0xffffffffu, ok ? j : -1ll);
+    if (ok && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(in_domain + j, static_cast<unsigned int>(__popc(peers)));
+}
+
+// Gives the pods [g_lo, g_hi) back, grid-stride from `first`: a placed pod's containers' demand returns to free_*_out
+// by integer atomics (the tables hold other pods' commits too), and every pod and container becomes -1.
+template <class Args>
+__device__ __forceinline__ void give_back_pods(const Args& a, long long g_lo, long long g_hi, long long first,
+                                               long long stride) {
+    for (long long g = g_lo + first; g < g_hi; g += stride) {
+        const int32_t nd = __ldcg(a.node + g);
+        for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) {
+            if (nd >= 0) {
+                const size_t at = static_cast<size_t>(nd) * a.D + __ldcg(a.dev + c);
+                atomicAdd(a.fc_out + at, __ldg(a.rc + c));
+                atomicAdd(a.fm_out + at, __ldg(a.rm + c));
+            }
+            a.dev[c] = -1;
+        }
+        a.node[g] = -1;
+    }
+}
+
 __global__ void __launch_bounds__(kTabThreads, 2)
-place_gangs_kernel(const __grid_constant__ GangsArgs a) {
-    __shared__ unsigned long long sW[kTabWarps][kPodBlock];  // choose: each warp's (inverted) words for a block of pods
-    __shared__ int32_t sFc[kTabWarps][kMaxD], sFm[kTabWarps][kMaxD];      // the table as the round found it
-    __shared__ int32_t sAccC[kTabWarps][kMaxD], sAccM[kTabWarps][kMaxD];  // commit: demand committed per device
-    __shared__ int32_t sClosed[kTabWarps][kMaxD];                          // ... a pod did not commit: later pods cannot
-    __shared__ int32_t sPod[kPodStage];  // commit: the staged pods (their words are staged in sW)
-    __shared__ unsigned int sRed[2][kTabWarps];
+place_gangs_kernel(const __grid_constant__ GangsArgs ga) {
+    __shared__ PodsSmem s;
     __shared__ int sOk;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const PodsArgs& a = ga.p;
+    const int tid = threadIdx.x, lane = tid & 31;
     const unsigned int b = blockIdx.x, G = gridDim.x;
-    const int N = a.N, D = a.D, T = (N + kTabWarps - 1) / kTabWarps;
+    const int N = a.N, D = a.D;
     const long long stride = static_cast<long long>(G) * kTabThreads, first = static_cast<long long>(b) * kTabThreads + tid;
     unsigned int gen = 0;
     int round = 0;  // rounds run by every gang so far: info[0], and the parity of the deferred counts
@@ -1124,24 +1156,15 @@ place_gangs_kernel(const __grid_constant__ GangsArgs a) {
     {
         bool bad = false;
         for (long long g = first; g <= a.G; g += stride) {
-            const int32_t o = __ldg(a.off + g);
-            if (g == 0) bad |= o != 0;
-            if (g == a.G) bad |= o != a.P;
-            if (g < a.G) {
-                const long long step = static_cast<long long>(__ldg(a.off + g + 1)) - o;
-                bad |= step < 1 || step > kMaxPod;
-                a.node[g] = -2;
-            }
+            bad |= csr_bad(a.off, g, a.G, a.P, 1, kMaxPod);
+            if (g < a.G) a.node[g] = -2;
         }
-        for (long long j = first; j <= a.J; j += stride) {
-            const int32_t o = __ldg(a.goff + j);
-            if (j == 0) bad |= o != 0;
-            if (j == a.J) bad |= o != a.G;
-            if (j < a.J) {
-                const long long size = static_cast<long long>(__ldg(a.goff + j + 1)) - o;
-                const int32_t m = __ldg(a.gmin + j);
-                bad |= size < 1 || m < 1 || m > size;
-                a.placed[j] = 0;
+        for (long long j = first; j <= ga.J; j += stride) {
+            bad |= csr_bad(ga.goff, j, ga.J, a.G, 1, LLONG_MAX);
+            if (j < ga.J) {
+                const int32_t m = __ldg(ga.gmin + j);
+                bad |= m < 1 || m > static_cast<long long>(__ldg(ga.goff + j + 1)) - __ldg(ga.goff + j);
+                ga.placed[j] = 0;
             }
         }
         for (long long c = first; c < a.P; c += stride) a.dev[c] = -2;
@@ -1162,31 +1185,20 @@ place_gangs_kernel(const __grid_constant__ GangsArgs a) {
     for (long long g0 = static_cast<long long>(b) * kTabThreads; g0 < a.G; g0 += stride) {
         const long long g = g0 + tid;
         bool ok = g < a.G;
-        long long j = 0;
-        if (ok) {
+        if (ok)
             for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) {
                 const int32_t core = __ldg(a.rc + c), mem = __ldg(a.rm + c);
                 ok &= core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
             }
-            long long lo = 0, hi = a.J - 1;  // the last gang whose first pod is at or before g
-            while (lo < hi) {
-                const long long mid = (lo + hi + 1) >> 1;
-                if (__ldg(a.goff + mid) <= g) lo = mid;
-                else hi = mid - 1;
-            }
-            j = lo;
-        }
-        // the pods of a warp are consecutive, so most share a gang: one atomic per gang and warp
-        const unsigned int peers = __match_any_sync(0xffffffffu, ok ? j : -1ll);
-        if (ok && lane == __ffs(peers) - 1) atomicAdd(a.in_domain + j, static_cast<unsigned int>(__popc(peers)));
+        count_into_gang(ga.goff, ga.J, g, ok, ga.in_domain);
     }
     if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
 
-    for (long long gang = 0; gang < a.J; ++gang) {
-        const int32_t g_lo = __ldg(a.goff + gang), g_hi = __ldg(a.goff + gang + 1), need = __ldg(a.gmin + gang);
+    for (long long gang = 0; gang < ga.J; ++gang) {
+        const int32_t g_lo = __ldg(ga.goff + gang), g_hi = __ldg(ga.goff + gang + 1), need = __ldg(ga.gmin + gang);
         const int32_t* cur = nullptr;  // pending pods in pod order; round 1: the gang's range (position = pod - g_lo)
-        long long n = __ldcg(a.in_domain + gang);  // pending pods
-        long long m = g_hi - g_lo;                  // positions of the pending set
+        long long n = __ldcg(ga.in_domain + gang);  // pending pods
+        long long m = g_hi - g_lo;                   // positions of the pending set
         int which = 0;
         bool gang_done = n < need;  // also n == 0: never rounds, nothing committed
         if (gang_done)
@@ -1196,147 +1208,12 @@ place_gangs_kernel(const __grid_constant__ GangsArgs a) {
             }
         while (!gang_done) {
             ++round;
-
-            // ---- 1. choose
-            {
-                const long long blocks = (m + kPodBlock - 1) / kPodBlock, items = blocks * T;
-                const long long lo = items * b / G, hi = items * (b + 1) / G;
-                unsigned long long mine = 0;
-                long long held = -1;  // the block of pods `mine` belongs to
-                for (long long it = lo; it <= hi; ++it) {
-                    const long long blk = it < hi ? it / T : -1;
-                    if (held >= 0 && blk != held) {  // the CTA's last tile of a block: one atomic per pod
-                        const long long i = held * kPodBlock + tid;
-                        if (i < m && mine) atomicMax(a.best + (cur ? __ldcg(cur + i) : g_lo + i), mine);
-                        mine = 0;
-                    }
-                    if (it == hi) break;
-                    held = blk;
-                    const int tn = static_cast<int>(it - blk * T) * kTabWarps + warp;
-                    const size_t off = static_cast<size_t>(tn) * D;
-                    const int rows = stage_table_warp(a.fc_out + off, a.fm_out + off, tn < N ? __ldg(a.dv + tn) : 0, D,
-                                                      sFc[warp], sFm[warp]);
-                    for (int j = lane; j < kPodBlock; j += 32) {
-                        const long long i = blk * kPodBlock + j;
-                        unsigned long long w = 0;
-                        if (i < m && rows) {
-                            const long long g = cur ? __ldcg(cur + i) : g_lo + i;
-                            const int32_t c0 = __ldg(a.off + g);
-                            PodFit f;
-                            // ~(sum lc << 52 | sum lm << 31 | n): the unsigned order of the word is (sum lc, sum lm, n)
-                            if (pod_replay(sFc[warp], sFm[warp], rows, a.rc, a.rm, c0, __ldg(a.off + g + 1) - c0, f))
-                                w = ~((static_cast<unsigned long long>(f.slc) << 52) |
-                                      (static_cast<unsigned long long>(f.slm) << 31) | static_cast<unsigned long long>(tn));
-                        }
-                        sW[warp][j] = w;
-                    }
-                    __syncthreads();
-#pragma unroll
-                    for (int w = 0; w < kTabWarps; ++w) mine = max(mine, sW[w][tid]);
-                    __syncthreads();
-                }
-            }
+            pods_choose(a, cur, g_lo, m, s);
             if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
-
-            // ---- 2. commit
             unsigned int* const count = a.count[(round - 1) & 1];
             {
-                unsigned long long* const sStage = &sW[0][0];  // kPodStage words: the choose phase is over
-                long long staged = -1;                         // the first pending position staged in sStage / sPod
-                unsigned int committed = 0;                    // this warp's committed pods (lane 0's count)
-                for (int tile = static_cast<int>(b); tile < T; tile += static_cast<int>(G)) {
-                    const int tn = tile * kTabWarps + warp;
-                    const size_t off = static_cast<size_t>(tn) * D;
-                    // a table outside the domain offers no device, so no pod chose it: it keeps its copy
-                    const int rows = stage_table_warp(a.fc_out + off, a.fm_out + off, tn < N ? __ldg(a.dv + tn) : 0, D,
-                                                      sFc[warp], sFm[warp]);
-                    for (int j = lane; j < kMaxD; j += 32) {
-                        sAccC[warp][j] = 0;
-                        sAccM[warp][j] = 0;
-                        sClosed[warp][j] = 0;
-                    }
-                    __syncwarp();
-                    bool dirty = false;
-                    for (long long i0 = 0; i0 < m; i0 += kPodStage) {
-                        if (i0 != staged) {  // at most kPodStage pending pods are staged once per round for every tile
-                            __syncthreads();  // every warp is done with the pods staged before
-                            for (int k = tid; k < kPodStage; k += kTabThreads) {
-                                const long long i = i0 + k;
-                                unsigned long long w = ~0ull;  // names no table
-                                if (i < m) {
-                                    const int32_t g = cur ? __ldcg(cur + i) : static_cast<int32_t>(g_lo + i);
-                                    sPod[k] = g;
-                                    w = ~__ldcg(a.best + g);
-                                }
-                                sStage[k] = w;
-                            }
-                            __syncthreads();
-                            staged = i0;
-                        }
-                        if (!rows) continue;
-                        const int len = static_cast<int>(min(static_cast<long long>(kPodStage), m - i0));
-                        for (int j0 = 0; j0 < len; j0 += kPodBlock) {  // one compaction tile
-                            unsigned int deferred = 0;
-                            for (int j = j0 + lane; j < j0 + kPodBlock; j += 32) {
-                                const unsigned long long w = sStage[j];
-                                const bool matched = static_cast<int>(w & 0x7fffffffu) == tn;
-                                const unsigned int mb = __ballot_sync(0xffffffffu, matched);
-                                if (mb == 0u) continue;
-                                PodFit f;
-                                int32_t g = 0, c0 = 0, c1 = 0;
-                                if (matched) {  // the choose phase's replay, again: it fitted then, so it fits now
-                                    g = sPod[j];
-                                    c0 = __ldg(a.off + g);
-                                    c1 = __ldg(a.off + g + 1);
-                                    pod_replay(sFc[warp], sFm[warp], rows, a.rc, a.rm, c0, c1 - c0, f);
-                                }
-                                // one pod after another, in pod order (lane order)
-                                bool fits = false;
-                                for (unsigned int r = mb; r; r &= r - 1u) {
-                                    if (lane == __ffs(r) - 1) {
-                                        bool ok = true;
-#pragma unroll
-                                        for (int s = 0; s < kMaxPod; ++s)
-                                            if (s < f.nt) {  // committed + the pod's demand <= free  <=>  committed <= what the pod leaves
-                                                const int d = f.td[s];
-                                                ok &= !sClosed[warp][d] && sAccC[warp][d] <= f.tc[s] && sAccM[warp][d] <= f.tm[s];
-                                            }
-#pragma unroll
-                                        for (int s = 0; s < kMaxPod; ++s)
-                                            if (s < f.nt) {
-                                                const int d = f.td[s];
-                                                if (ok) {
-                                                    sAccC[warp][d] += sFc[warp][d] - f.tc[s];
-                                                    sAccM[warp][d] += sFm[warp][d] - f.tm[s];
-                                                } else {
-                                                    sClosed[warp][d] = 1;
-                                                }
-                                            }
-                                        fits = ok;
-                                    }
-                                    __syncwarp();
-                                }
-                                if (fits) {
-                                    a.node[g] = tn;
-                                    for (int32_t c = c0; c < c1; ++c)
-                                        a.dev[c] = static_cast<int8_t>((f.cdev >> (6 * (c - c0))) & 63u);
-                                }
-                                const unsigned int fb = __ballot_sync(0xffffffffu, fits);
-                                dirty |= fb != 0u;
-                                committed += __popc(fb);
-                                deferred += __popc(mb & ~fb);
-                            }
-                            if (lane == 0 && deferred) atomicAdd(count + (i0 + j0) / kPodBlock, deferred);
-                        }
-                    }
-                    __syncwarp();
-                    if (dirty)
-                        for (int j = lane; j < rows; j += 32) {
-                            a.fc_out[off + j] = sFc[warp][j] - sAccC[warp][j];
-                            a.fm_out[off + j] = sFm[warp][j] - sAccM[warp][j];
-                        }
-                }
-                if (lane == 0 && committed) atomicAdd(a.committed + gang, committed);
+                const unsigned int committed = pods_commit(a, count, cur, g_lo, m, s);
+                if (lane == 0 && committed) atomicAdd(ga.committed + gang, committed);
             }
             if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
 
@@ -1347,78 +1224,18 @@ place_gangs_kernel(const __grid_constant__ GangsArgs a) {
                 // the next round may be the next gang's first, over up to G positions
                 for (long long t = first; t < (a.G + kPodBlock - 1) / kPodBlock; t += stride) next_count[t] = 0u;
                 const long long lo = tiles * b / G, hi = tiles * (b + 1) / G;
-                unsigned int before = 0, total = 0;
-                for (long long t = tid; t < tiles; t += kTabThreads) {
-                    const unsigned int c = __ldcg(count + t);
-                    total += c;
-                    before += t < lo ? c : 0u;
-                }
-#pragma unroll
-                for (int o = 16; o; o >>= 1) {
-                    before += __shfl_xor_sync(0xffffffffu, before, o);
-                    total += __shfl_xor_sync(0xffffffffu, total, o);
-                }
-                if (lane == 0) {
-                    sRed[0][warp] = before;
-                    sRed[1][warp] = total;
-                }
-                __syncthreads();
-                before = 0;
-                total = 0;
-#pragma unroll
-                for (int w = 0; w < kTabWarps; ++w) {
-                    before += sRed[0][w];
-                    total += sRed[1][w];
-                }
-                __syncthreads();
-                const long long placed = __ldcg(a.committed + gang);
+                unsigned int before, total;
+                deferred_prefix(count, tiles, lo, before, total, s.Red);
+                const long long placed = __ldcg(ga.committed + gang);
                 gang_done = total == 0u || placed + total < need;
                 if (gang_done && placed < need) {  // roll back: every pod of the gang -1, its demand given back
-                    for (long long g = g_lo + first; g < g_hi; g += stride) {
-                        const int32_t nd = __ldcg(a.node + g);
-                        for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) {
-                            if (nd >= 0) {
-                                const size_t at = static_cast<size_t>(nd) * D + __ldcg(a.dev + c);
-                                atomicAdd(a.fc_out + at, __ldg(a.rc + c));
-                                atomicAdd(a.fm_out + at, __ldg(a.rm + c));
-                            }
-                            a.dev[c] = -1;
-                        }
-                        a.node[g] = -1;
-                    }
-                    if (gang + 1 < a.J && !grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+                    give_back_pods(a, g_lo, g_hi, first, stride);
+                    if (gang + 1 < ga.J && !grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
                 } else {
-                    if (gang_done && b == 0 && tid == 0) a.placed[gang] = static_cast<int32_t>(placed);
-                    int32_t* const next = a.set[which];
-                    for (long long t = lo; t < hi; ++t) {
-                        const long long i = t * kPodBlock + tid;
-                        bool defer = false;
-                        int32_t g = 0;
-                        if (i < m) {
-                            g = cur ? __ldcg(cur + i) : static_cast<int32_t>(g_lo + i);
-                            if (__ldcg(a.best + g) == 0ull) {
-                                a.node[g] = -1;
-                                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
-                            } else if (__ldcg(a.node + g) == -2) {
-                                defer = true;
-                                a.best[g] = 0ull;
-                            }
-                        }
-                        const unsigned int bal = __ballot_sync(0xffffffffu, defer);
-                        if (lane == 0) sRed[0][warp] = __popc(bal);
-                        __syncthreads();
-                        unsigned int at = before, in_tile = 0;
-#pragma unroll
-                        for (int w = 0; w < kTabWarps; ++w) {
-                            at += w < warp ? sRed[0][w] : 0u;
-                            in_tile += sRed[0][w];
-                        }
-                        if (defer) next[at + __popc(bal & ((1u << lane) - 1u))] = g;
-                        before += in_tile;
-                        __syncthreads();
-                    }
+                    if (gang_done && b == 0 && tid == 0) ga.placed[gang] = static_cast<int32_t>(placed);
+                    pods_compact(a, cur, g_lo, m, lo, hi, a.set[which], before, s);
                     if (!gang_done) {
-                        cur = next;
+                        cur = a.set[which];
                         m = n = total;
                         which ^= 1;
                         if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
@@ -1437,68 +1254,29 @@ finish:
     }
 }
 
-size_t gangs_scratch_bytes(int G, int J) {
-    const size_t blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
-    const size_t zeroed = 8 * static_cast<size_t>(G) + sizeof(GangsCtl) + 2 * 4 * blocks + 2 * 4 * static_cast<size_t>(J);
-    return ((zeroed + 15) & ~size_t(15)) + 2 * 4 * static_cast<size_t>(G);
-}
+size_t gangs_scratch_bytes(int G, int J) { return PodsScratch(G, J).total; }
 
 cudaError_t gangs_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
                          const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets, int G,
                          const int32_t* gang_offsets, const int32_t* gang_min, int J, int32_t* out_node, int8_t* out_dev,
                          int32_t* out_placed, int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch,
                          int device, cudaStream_t stream) {
-    // scratch: best uint64[G] | barrier words | deferred counts 2 x uint32[G / 256] | pods in the domain uint32[J] |
-    // committed pods uint32[J] | (16-aligned) two pending sets int32[G]; everything before the pending sets starts at 0
-    const size_t blocks = (static_cast<size_t>(G) + kPodBlock - 1) / kPodBlock;
-    char* s = static_cast<char*>(scratch);
-    GangsArgs a{};
+    const PodsScratch L(G, J);
+    GangsArgs ga{};
+    PodsArgs& a = ga.p;
     a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem; a.off = pod_offsets;
-    a.goff = gang_offsets; a.gmin = gang_min;
-    a.N = N; a.D = D; a.P = P; a.G = G; a.J = J;
-    a.node = out_node; a.dev = out_dev; a.placed = out_placed; a.fc_out = free_core_out; a.fm_out = free_mem_out;
-    a.info = info;
-    a.best = reinterpret_cast<unsigned long long*>(s);
-    a.ctl = reinterpret_cast<GangsCtl*>(s + 8 * static_cast<size_t>(G));
-    a.count[0] = reinterpret_cast<unsigned int*>(s + 8 * static_cast<size_t>(G) + sizeof(GangsCtl));
-    a.count[1] = a.count[0] + blocks;
-    a.in_domain = a.count[1] + blocks;
-    a.committed = a.in_domain + J;
-    const size_t zeroed = 8 * static_cast<size_t>(G) + sizeof(GangsCtl) + 2 * 4 * blocks + 2 * 4 * static_cast<size_t>(J);
-    a.set[0] = reinterpret_cast<int32_t*>(s + ((zeroed + 15) & ~size_t(15)));
-    a.set[1] = a.set[0] + G;
-    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    a.N = N; a.D = D; a.P = P; a.G = G;
+    a.node = out_node; a.dev = out_dev; a.fc_out = free_core_out; a.fm_out = free_mem_out; a.info = info;
+    ga.goff = gang_offsets; ga.gmin = gang_min; ga.J = J;
+    ga.placed = out_placed;
+    ga.in_domain = reinterpret_cast<unsigned int*>(static_cast<char*>(scratch) + L.in_domain);
+    ga.committed = reinterpret_cast<unsigned int*>(static_cast<char*>(scratch) + L.committed);
+    const cudaError_t err = pods_scratch(a, scratch, L, stream);
     if (err != cudaSuccess) return err;
-
-    // resident CTAs per SM on each device, asked once
-    static std::atomic<int> per_sm_cache[kPlaceDevices];
-    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
-    if (per_sm == 0) {
-        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, place_gangs_kernel, kTabThreads, 0);
-        if (err != cudaSuccess) return err;
-        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
-        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
-    }
-    int sms = 0;
-    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    if (err != cudaSuccess) return err;
-    // Grid: as pods_launch, from N and G alone (the gang sizes are device data): one resident wave, no more CTAs
-    // than a round over all G pods has choose work items; at least one, which finds G = 0's offsets bad.
+    // Grid: as pods_launch, from N and G alone (the gang sizes are device data): no more CTAs than a round over all G
+    // pods has choose work items; at least one, which finds G = 0's offsets bad.
     const long long tiles = (static_cast<long long>(N) + kTabWarps - 1) / kTabWarps;
-    const long long items = tiles * static_cast<long long>(blocks);
-    long long grid = static_cast<long long>(sms) * per_sm;
-    grid = std::max(1ll, std::min(grid, items));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(grid));
-    cfg.blockDim = dim3(kTabThreads);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, place_gangs_kernel, a);
+    return coop_launch<place_gangs_kernel>(ga, tiles * static_cast<long long>(L.blocks), device, stream);
 }
 
 // ---- egpu::preempt_pods (DESIGN.md §2.14, §4.9): whole pods with priority preemption, rounds to the fixed point ----
@@ -1509,19 +1287,21 @@ cudaError_t gangs_launch(const int32_t* free_core, const int32_t* free_mem, cons
 //   0. the grid checks pod_offsets, run_offsets and node_offsets before anything is read through them, marks every
 //      pod and container -2 and every running pod -1 (alive), and copies the tables to free_*_out (every round reads
 //      them there).  After a barrier: if an index is bad nothing is placed and info[2] = 1; otherwise pods outside
-//      the domain become -1, and each node is marked usable when its table is in §2.1's domain and its running data
-//      is consistent (an unusable node offers no candidate and is never written);
+//      the domain become -1, and each node is marked usable (pre_usable) when its table is in §2.1's domain and its
+//      running data is consistent (an unusable node offers no candidate and is never written);
 //   per round, over the pending pods (node = -2):
 //   1a. choose, empty victim set: work items are (pod, chunk of nodes), chunk-major so that one pod's chunks spread
 //       over CTAs.  Each warp replays the pod on its nodes of the chunk; the CTA reduces the warps' best keys and
-//       writes one record per item.  A pod that fits some node as it is is flagged;
+//       writes one record per item (pre_record).  A pod that fits some node as it is is flagged;
 //   1b. choose, with victims: the same items, for the pods no node took as it is: steps 2 and 3 of §2.14 per node
-//       where the pod outranks an alive running pod; the records are overwritten;
-//   2.  reduce: one thread per pending pod takes the smallest of its K records (§2.14's key is 142 bits, so the
-//       records are three 64-bit words compared in order, not an atomic); a pod with none becomes -1;
-//   3.  commit: the warp of node n walks the pending pods that chose n in pod order, §2.14's commit rule.  The replay
-//       and the chain are deterministic and nothing changed node n since the choose phases, so the warp recomputes a
-//       pod's devices, and a committing preemptor's victims, instead of storing them;
+//       where the pod outranks an alive running pod (pre_victims: C, then the reprieve walk pre_walk); the records
+//       are overwritten;
+//   2.  reduce (pre_reduce): one thread per pending pod takes the smallest of its K records (§2.14's key is 142 bits,
+//       so the records are three 64-bit words compared in order, not an atomic); a pod with none becomes -1;
+//   3.  commit: the warp of node n walks the pending pods that chose n in pod order, §2.14's commit rule (pre_fits
+//       for a pod that evicts nothing).  The replay and the chain are deterministic and nothing changed node n since
+//       the choose phases, so the warp recomputes a pod's devices, and a committing preemptor's victims, instead of
+//       storing them;
 //   then every CTA reads the round's deferred count: zero ends the launch.
 constexpr int kMaxRun = 128;     // running pods per node
 constexpr int kPreChunks = 32;   // node chunks per pending pod in the choose phases
@@ -1529,9 +1309,11 @@ constexpr int kPreChunks = 32;   // node chunks per pending pod in the choose ph
 struct PreemptCtl {
     RoundsCtl bar;                // grid-barrier words
     unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
-    unsigned int bad_index;       // pod_offsets, run_offsets or node_offsets failed the check (info[2])
-    unsigned int in_domain;       // some pod is in the domain
+    unsigned int bad_index;       // an index tensor (or run_gang_min) failed the check (info[2])
+    unsigned int in_domain;       // some pod is in the domain (preempt_pods)
     unsigned int deferred[2];     // pods deferred by a round's commit, by round parity
+    unsigned int budget[2];       // a round recorded a preemptor with a victim in a running job, by round parity
+                                  // (preempt_gangs)
 };
 
 struct PreemptArgs {
@@ -1634,28 +1416,16 @@ __device__ __forceinline__ void add_running(const PreemptArgs& a, WarpTab& t, lo
     }
 }
 
-// §2.14 steps 2 and 3 for the pod of priority p and containers [c0, c0 + len) on node n, whose table as the round
-// found it is t and whose running pods are [h0, h1) (at most kMaxRun: running pod h0 + lane + 32 i is slot i of the
-// lane).  The caller knows step 1 failed.  Returns false when n is not a candidate; otherwise t becomes the table plus
-// the demand of V minus the pod's (what committing leaves), in_v holds V by slot, cdev the pod's devices and k the
-// key.
-__device__ __forceinline__ bool pre_victims(const PreemptArgs& a, WarpTab& t, int rows, int32_t p, long long c0, int len,
-                                            long long h0, long long h1, int n, unsigned int& in_v, PreKey& k,
-                                            unsigned long long& cdev) {
+// §2.14 step 3 for the pod of containers [c0, c0 + len) on node n, whose table as the round found it is t and whose
+// running pods are [h0, h1) (at most kMaxRun: running pod h0 + lane + 32 i is slot i of the lane), from the victim
+// candidates C, which is not empty: cand holds the lane's slots of C (bit i: slot lane + 32 i) and q[i] slot i's
+// priority + 2^31 (its unsigned order is the priority's).  Returns false when n is not a candidate; otherwise t becomes
+// the table plus the demand of V minus the pod's (what committing leaves), in_v holds V by slot, cdev the pod's devices
+// and k the key.
+__device__ __forceinline__ bool pre_walk(const PreemptArgs& a, WarpTab& t, int rows, unsigned int cand,
+                                         const uint32_t (&q)[4], long long c0, int len, long long h0, int n,
+                                         unsigned int& in_v, PreKey& k, unsigned long long& cdev) {
     const int lane = threadIdx.x & 31;
-    unsigned int cand = 0;  // C: alive running pods of lower priority
-    uint32_t q[4];          // priority + 2^31: its unsigned order is the priority's
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const long long h = h0 + lane + 32 * i;
-        q[i] = 0;
-        if (h < h1) {
-            const int32_t r = __ldg(a.rprio + h);
-            q[i] = static_cast<uint32_t>(r) ^ 0x80000000u;
-            if (r < p && __ldcg(a.evicted + h) == -1) cand |= 1u << i;
-        }
-    }
-    if (!__any_sync(0xffffffffu, cand != 0u)) return false;
     WarpTab base = t;  // the table plus the demand of V
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -1714,6 +1484,43 @@ __device__ __forceinline__ bool pre_victims(const PreemptArgs& a, WarpTab& t, in
     return true;
 }
 
+// §2.14 steps 2 and 3 for the pod of priority p: C is the alive running pods of lower priority, walked by pre_walk.
+// The caller knows step 1 failed.
+__device__ __forceinline__ bool pre_victims(const PreemptArgs& a, WarpTab& t, int rows, int32_t p, long long c0, int len,
+                                            long long h0, long long h1, int n, unsigned int& in_v, PreKey& k,
+                                            unsigned long long& cdev) {
+    const int lane = threadIdx.x & 31;
+    unsigned int cand = 0;  // C: alive running pods of lower priority
+    uint32_t q[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const long long h = h0 + lane + 32 * i;
+        q[i] = 0;
+        if (h < h1) {
+            const int32_t r = __ldg(a.rprio + h);
+            q[i] = static_cast<uint32_t>(r) ^ 0x80000000u;
+            if (r < p && __ldcg(a.evicted + h) == -1) cand |= 1u << i;
+        }
+    }
+    if (!__any_sync(0xffffffffu, cand != 0u)) return false;
+    return pre_walk(a, t, rows, cand, q, c0, len, h0, n, in_v, k, cdev);
+}
+
+// pre_victims with C given: cand holds the lane's slots of C (bit i: slot lane + 32 i).
+__device__ __forceinline__ bool pre_victims_capped(const PreemptArgs& a, WarpTab& t, int rows, unsigned int cand,
+                                                   long long c0, int len, long long h0, long long h1, int n,
+                                                   unsigned int& in_v, PreKey& k, unsigned long long& cdev) {
+    const int lane = threadIdx.x & 31;
+    if (!__any_sync(0xffffffffu, cand != 0u)) return false;
+    uint32_t q[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const long long h = h0 + lane + 32 * i;
+        q[i] = h < h1 ? static_cast<uint32_t>(__ldg(a.rprio + h)) ^ 0x80000000u : 0u;
+    }
+    return pre_walk(a, t, rows, cand, q, c0, len, h0, n, in_v, k, cdev);
+}
+
 // Node n's table from free_*_out into the warp's registers (the values past `rows` are not read).
 __device__ __forceinline__ WarpTab load_tab(const PreemptArgs& a, int n, int rows) {
     const int lane = threadIdx.x & 31;
@@ -1726,6 +1533,110 @@ __device__ __forceinline__ WarpTab load_tab(const PreemptArgs& a, int n, int row
         t.m[i] = d < rows ? __ldcg(a.fm_out + off + d) : 0;
     }
     return t;
+}
+
+// ---- 0. (end) usable[n], one warp per node: the table is in §2.1's domain and the running data consistent (every
+// running container on a valid device and in the domain, and the free values plus the running demand within it).
+// sSumC / sSumM: kTabWarps rows of kMaxD words of shared memory.
+__device__ __forceinline__ void pre_usable(const PreemptArgs& a, int32_t (*sSumC)[kMaxD], int32_t (*sSumM)[kMaxD]) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int N = a.N, D = a.D;
+    const long long wstride = static_cast<long long>(gridDim.x) * kTabWarps;
+    for (long long n = static_cast<long long>(blockIdx.x) * kTabWarps + warp; n < N; n += wstride) {
+        const int dv = __ldg(a.dv + n);
+        bool ok = dv >= 1 && dv <= D;
+        const size_t off = static_cast<size_t>(n) * D;
+        for (int j = lane; j < kMaxD; j += 32) {
+            const int32_t c = ok && j < dv ? __ldg(a.fc + off + j) : 0, m = ok && j < dv ? __ldg(a.fm + off + j) : 0;
+            ok &= c >= 0 && c <= kCoreMax && m >= 0 && m <= kMemMax;
+            sSumC[warp][j] = c;
+            sSumM[warp][j] = m;
+        }
+        __syncwarp();
+        const int32_t q0 = __ldg(a.roff + __ldg(a.noff + n)), q1 = __ldg(a.roff + __ldg(a.noff + n + 1));
+        for (int32_t c = q0 + lane; ok && c < q1; c += 32) {
+            const int d = __ldg(a.qd + c);
+            const int32_t core = __ldg(a.qc + c), mem = __ldg(a.qm + c);
+            ok = d >= 0 && d < dv && core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
+            if (ok) {
+                atomicAdd(&sSumC[warp][d], core);
+                atomicAdd(&sSumM[warp][d], mem);
+            }
+        }
+        __syncwarp();
+        for (int j = lane; ok && j < dv; j += 32) ok = sSumC[warp][j] <= kCoreMax && sSumM[warp][j] <= kMemMax;
+        ok = __all_sync(0xffffffffu, ok);
+        if (lane == 0) a.usable[n] = ok ? 1u : 0u;
+        __syncwarp();
+    }
+}
+
+// ---- 1. (end of a choose item (g, k)) the smallest of the CTA's warps' keys is the item's record; in pass 0, a pod
+// that some node takes as it is is flagged.  Every thread of the CTA calls it with its warp's key.
+__device__ __forceinline__ void pre_record(const PreemptArgs& a, PreKey best, long long g, long long k, int pass,
+                                           PreKey* sKey) {
+    const int tid = threadIdx.x;
+    if ((tid & 31) == 0) sKey[tid >> 5] = best;
+    __syncthreads();
+    if (tid == 0) {
+        for (int w = 1; w < kTabWarps; ++w)
+            if (pre_less(sKey[w], best)) best = sKey[w];
+        unsigned long long* r = a.rec + 3 * (g * a.K + k);
+        r[0] = best.a;
+        r[1] = best.b;
+        r[2] = best.c;
+        if (pass == 0 && best.a == 0ull) a.has_empty[g] = 1u;
+    }
+    __syncthreads();
+}
+
+// ---- 2. reduce: each pending pod of [g_lo, g_hi) takes the smallest of its records
+__device__ __forceinline__ void pre_reduce(const PreemptArgs& a, long long g_lo, long long g_hi) {
+    const long long stride = static_cast<long long>(gridDim.x) * kTabThreads;
+    const PreKey none{~0ull, ~0ull, ~0ull};
+    for (long long g = g_lo + static_cast<long long>(blockIdx.x) * kTabThreads + threadIdx.x; g < g_hi; g += stride) {
+        if (__ldcg(a.node + g) != -2) continue;
+        PreKey best = none;
+        for (int k = 0; k < a.K; ++k) {
+            const unsigned long long* r = a.rec + 3 * (g * a.K + k);
+            const PreKey key{__ldcg(r), __ldcg(r + 1), __ldcg(r + 2)};
+            if (pre_less(key, best)) best = key;
+        }
+        a.has_empty[g] = 0u;
+        if (best.a == ~0ull) {  // fits no node when scored: -1 for good
+            a.choice[g] = ~0ull;
+            a.node[g] = -1;
+            for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
+        } else {
+            a.choice[g] = (best.a != 0ull ? 1ull << 32 : 0ull) | (best.c & 0x7fffffffull);
+        }
+    }
+}
+
+// ---- 3. (a pod that evicts nothing) §2.12 on node table t, in registers: w = t becomes what the pod leaves and cdev
+// holds its devices.  The pod commits when none of its devices is closed and the demand committed before (acc_*)
+// fits on top of its own; then its demand joins acc_*, otherwise its devices close.  Returns whether it commits.
+__device__ __forceinline__ bool pre_fits(const PreemptArgs& a, const WarpTab& t, WarpTab& w, int rows, long long c0,
+                                         int len, int32_t (&acc_c)[2], int32_t (&acc_m)[2], unsigned int& closed,
+                                         unsigned long long& cdev) {
+    uint32_t slc, slm;
+    unsigned int used;
+    warp_replay(w, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used);
+    bool ok = true;
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+        if ((used >> i) & 1u) ok &= !((closed >> i) & 1u) && acc_c[i] <= w.c[i] && acc_m[i] <= w.m[i];
+    const bool commit = __all_sync(0xffffffffu, ok);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        if (commit) {
+            acc_c[i] += t.c[i] - w.c[i];
+            acc_m[i] += t.m[i] - w.m[i];
+        } else {
+            closed |= used;
+        }
+    }
+    return commit;
 }
 
 __global__ void __launch_bounds__(kTabThreads, 2)
@@ -1747,34 +1658,14 @@ preempt_pods_kernel(const __grid_constant__ PreemptArgs a) {
     {
         bool bad = false;
         for (long long g = first; g <= a.G; g += stride) {
-            const int32_t o = __ldg(a.off + g);
-            if (g == 0) bad |= o != 0;
-            if (g == a.G) bad |= o != a.P;
-            if (g < a.G) {
-                const long long step = static_cast<long long>(__ldg(a.off + g + 1)) - o;
-                bad |= step < 1 || step > kMaxPod;
-                a.node[g] = -2;
-            }
+            bad |= csr_bad(a.off, g, a.G, a.P, 1, kMaxPod);
+            if (g < a.G) a.node[g] = -2;
         }
         for (long long h = first; h <= a.H; h += stride) {
-            const int32_t o = __ldg(a.roff + h);
-            if (h == 0) bad |= o != 0;
-            if (h == a.H) bad |= o != a.Q;
-            if (h < a.H) {
-                const long long step = static_cast<long long>(__ldg(a.roff + h + 1)) - o;
-                bad |= step < 1 || step > kMaxPod;
-                a.evicted[h] = -1;
-            }
+            bad |= csr_bad(a.roff, h, a.H, a.Q, 1, kMaxPod);
+            if (h < a.H) a.evicted[h] = -1;
         }
-        for (long long n = first; n <= N; n += stride) {
-            const int32_t o = __ldg(a.noff + n);
-            if (n == 0) bad |= o != 0;
-            if (n == N) bad |= o != a.H;
-            if (n < N) {
-                const long long step = static_cast<long long>(__ldg(a.noff + n + 1)) - o;
-                bad |= step < 0 || step > kMaxRun;
-            }
-        }
+        for (long long n = first; n <= N; n += stride) bad |= csr_bad(a.noff, n, N, a.H, 0, kMaxRun);
         for (long long c = first; c < a.P; c += stride) a.dev[c] = -2;
         for (long long j = first; j < static_cast<long long>(N) * D; j += stride) {
             a.fc_out[j] = a.fc[j];
@@ -1805,33 +1696,7 @@ preempt_pods_kernel(const __grid_constant__ PreemptArgs a) {
             in_domain |= ok;
         }
         if (__syncthreads_or(in_domain) && tid == 0) a.ctl->in_domain = 1u;
-        for (long long n = wfirst; n < N; n += wstride) {
-            const int dv = __ldg(a.dv + n);
-            bool ok = dv >= 1 && dv <= D;
-            const size_t off = static_cast<size_t>(n) * D;
-            for (int j = lane; j < kMaxD; j += 32) {
-                const int32_t c = ok && j < dv ? __ldg(a.fc + off + j) : 0, m = ok && j < dv ? __ldg(a.fm + off + j) : 0;
-                ok &= c >= 0 && c <= kCoreMax && m >= 0 && m <= kMemMax;
-                sSumC[warp][j] = c;
-                sSumM[warp][j] = m;
-            }
-            __syncwarp();
-            const int32_t q0 = __ldg(a.roff + __ldg(a.noff + n)), q1 = __ldg(a.roff + __ldg(a.noff + n + 1));
-            for (int32_t c = q0 + lane; ok && c < q1; c += 32) {
-                const int d = __ldg(a.qd + c);
-                const int32_t core = __ldg(a.qc + c), mem = __ldg(a.qm + c);
-                ok = d >= 0 && d < dv && core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
-                if (ok) {
-                    atomicAdd(&sSumC[warp][d], core);
-                    atomicAdd(&sSumM[warp][d], mem);
-                }
-            }
-            __syncwarp();
-            for (int j = lane; ok && j < dv; j += 32) ok = sSumC[warp][j] <= kCoreMax && sSumM[warp][j] <= kMemMax;
-            ok = __all_sync(0xffffffffu, ok);
-            if (lane == 0) a.usable[n] = ok ? 1u : 0u;
-            __syncwarp();
-        }
+        pre_usable(a, sSumC, sSumM);
     }
     if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
     done = *reinterpret_cast<volatile unsigned int*>(&a.ctl->in_domain) == 0u;
@@ -1869,40 +1734,12 @@ preempt_pods_kernel(const __grid_constant__ PreemptArgs a) {
                     }
                     if (pre_less(key, best)) best = key;
                 }
-                if (lane == 0) sKey[warp] = best;
-                __syncthreads();
-                if (tid == 0) {
-                    for (int w = 1; w < kTabWarps; ++w)
-                        if (pre_less(sKey[w], best)) best = sKey[w];
-                    unsigned long long* r = a.rec + 3 * (g * K + k);
-                    r[0] = best.a;
-                    r[1] = best.b;
-                    r[2] = best.c;
-                    if (pass == 0 && best.a == 0ull) a.has_empty[g] = 1u;
-                }
-                __syncthreads();
+                pre_record(a, best, g, k, pass, sKey);
             }
             if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
         }
 
-        // ---- 2. reduce: each pending pod's smallest record
-        for (long long g = first; g < a.G; g += stride) {
-            if (__ldcg(a.node + g) != -2) continue;
-            PreKey best = none;
-            for (int k = 0; k < K; ++k) {
-                const unsigned long long* r = a.rec + 3 * (g * K + k);
-                const PreKey key{__ldcg(r), __ldcg(r + 1), __ldcg(r + 2)};
-                if (pre_less(key, best)) best = key;
-            }
-            a.has_empty[g] = 0u;
-            if (best.a == ~0ull) {  // fits no node when scored: -1 for good
-                a.choice[g] = ~0ull;
-                a.node[g] = -1;
-                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
-            } else {
-                a.choice[g] = (best.a != 0ull ? 1ull << 32 : 0ull) | (best.c & 0x7fffffffull);
-            }
-        }
+        pre_reduce(a, 0, a.G);
         if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
 
         // ---- 3. commit: per node, the pods that chose it in pod order
@@ -1935,25 +1772,8 @@ preempt_pods_kernel(const __grid_constant__ PreemptArgs a) {
                     WarpTab w = t;
                     unsigned long long cdev;
                     bool commit = true;
-                    if (!evicts) {  // §2.12: no closed device, and the demand fits on top of what committed before
-                        uint32_t slc, slm;
-                        unsigned int used;
-                        warp_replay(w, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used);
-                        bool ok = true;
-#pragma unroll
-                        for (int i = 0; i < 2; ++i)
-                            if ((used >> i) & 1u)
-                                ok &= !((closed >> i) & 1u) && acc_c[i] <= w.c[i] && acc_m[i] <= w.m[i];
-                        commit = __all_sync(0xffffffffu, ok);
-#pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            if (commit) {
-                                acc_c[i] += t.c[i] - w.c[i];
-                                acc_m[i] += t.m[i] - w.m[i];
-                            } else {
-                                closed |= used;
-                            }
-                        }
+                    if (!evicts) {
+                        commit = pre_fits(a, t, w, rows, c0, len, acc_c, acc_m, closed, cdev);
                     } else {  // the first pod of the round on n: evict V, then take the pod's demand
                         unsigned int in_v;
                         PreKey key;
@@ -1998,11 +1818,45 @@ finish:
 
 static int preempt_chunks(int N) { return std::max(1, std::min(kPreChunks, (N + kTabWarps - 1) / kTabWarps)); }
 
-size_t preempt_scratch_bytes(int N, int G) {
-    const size_t zeroed = sizeof(PreemptCtl) + 4 * static_cast<size_t>(G);
-    return ((zeroed + 15) & ~size_t(15)) + 24 * static_cast<size_t>(G) * preempt_chunks(N) + 8 * static_cast<size_t>(G) +
-           4 * static_cast<size_t>(N);
+// preempt_pods' and preempt_gangs' scratch (preempt_pods: J = R = 0, and it leaves pre, vdev, vmask and cap alone),
+// byte offsets: barrier words | has_empty uint32[G] | pre uint32[G] | in_domain uint32[J] | committed uint32[J] |
+// alive int32[R] | used int32[R] | (16-aligned) records uint64[G][K][3] | choice uint64[G] | vdev uint64[G] | vmask
+// uint32[G][4] | cap uint32[N][4] | usable uint32[N]; everything before the records (`zeroed` bytes) starts at zero.
+struct PreemptScratch {
+    int K;
+    size_t has_empty, pre, in_domain, committed, alive, used, zeroed, rec, choice, vdev, vmask, cap, usable, total;
+    PreemptScratch(int N, int G, int J, int R) {
+        K = preempt_chunks(N);
+        has_empty = sizeof(PreemptCtl);
+        pre = has_empty + 4 * static_cast<size_t>(G);
+        in_domain = pre + 4 * static_cast<size_t>(G);
+        committed = in_domain + 4 * static_cast<size_t>(J);
+        alive = committed + 4 * static_cast<size_t>(J);
+        used = alive + 4 * static_cast<size_t>(R);
+        zeroed = used + 4 * static_cast<size_t>(R);
+        rec = (zeroed + 15) & ~size_t(15);
+        choice = rec + 24 * static_cast<size_t>(G) * K;
+        vdev = choice + 8 * static_cast<size_t>(G);
+        vmask = vdev + 8 * static_cast<size_t>(G);
+        cap = vmask + 16 * static_cast<size_t>(G);
+        usable = cap + 16 * static_cast<size_t>(N);
+        total = usable + 4 * static_cast<size_t>(N);
+    }
+};
+
+// Points a's scratch arrays into `scratch` as L lays them out and zeroes its head on `stream`.
+static cudaError_t preempt_scratch(PreemptArgs& a, void* scratch, const PreemptScratch& L, cudaStream_t stream) {
+    char* s = static_cast<char*>(scratch);
+    a.K = L.K;
+    a.ctl = reinterpret_cast<PreemptCtl*>(s);
+    a.has_empty = reinterpret_cast<unsigned int*>(s + L.has_empty);
+    a.rec = reinterpret_cast<unsigned long long*>(s + L.rec);
+    a.choice = reinterpret_cast<unsigned long long*>(s + L.choice);
+    a.usable = reinterpret_cast<unsigned int*>(s + L.usable);
+    return cudaMemsetAsync(scratch, 0, L.zeroed, stream);
 }
+
+size_t preempt_scratch_bytes(int N, int G) { return PreemptScratch(N, G, 0, 0).total; }
 
 cudaError_t preempt_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N, int D,
                            const int32_t* req_core, const int32_t* req_mem, int P, const int32_t* pod_offsets,
@@ -2011,53 +1865,18 @@ cudaError_t preempt_launch(const int32_t* free_core, const int32_t* free_mem, co
                            const int32_t* node_offsets, int32_t* out_node, int8_t* out_dev, int32_t* out_evicted,
                            int32_t* free_core_out, int32_t* free_mem_out, int32_t* info, void* scratch, int device,
                            cudaStream_t stream) {
-    // scratch: barrier words | has_empty uint32[G] | (16-aligned) records uint64[G][K][3] | choice uint64[G] |
-    // usable uint32[N]; everything before the records starts at zero
-    const int K = preempt_chunks(N);
-    char* s = static_cast<char*>(scratch);
+    const PreemptScratch L(N, G, 0, 0);
     PreemptArgs a{};
     a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem; a.off = pod_offsets;
     a.prio = pod_prio; a.qc = run_core; a.qm = run_mem; a.qd = run_dev; a.roff = run_offsets; a.rprio = run_prio;
     a.noff = node_offsets;
-    a.N = N; a.D = D; a.K = K; a.P = P; a.G = G; a.Q = Q; a.H = H;
+    a.N = N; a.D = D; a.P = P; a.G = G; a.Q = Q; a.H = H;
     a.node = out_node; a.dev = out_dev; a.evicted = out_evicted; a.fc_out = free_core_out; a.fm_out = free_mem_out;
     a.info = info;
-    a.ctl = reinterpret_cast<PreemptCtl*>(s);
-    a.has_empty = reinterpret_cast<unsigned int*>(s + sizeof(PreemptCtl));
-    const size_t zeroed = sizeof(PreemptCtl) + 4 * static_cast<size_t>(G);
-    a.rec = reinterpret_cast<unsigned long long*>(s + ((zeroed + 15) & ~size_t(15)));
-    a.choice = a.rec + 3 * static_cast<size_t>(G) * K;
-    a.usable = reinterpret_cast<unsigned int*>(a.choice + G);
-    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    const cudaError_t err = preempt_scratch(a, scratch, L, stream);
     if (err != cudaSuccess) return err;
-
-    // resident CTAs per SM on each device, asked once
-    static std::atomic<int> per_sm_cache[kPlaceDevices];
-    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
-    if (per_sm == 0) {
-        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, preempt_pods_kernel, kTabThreads, 0);
-        if (err != cudaSuccess) return err;
-        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
-        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
-    }
-    int sms = 0;
-    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    if (err != cudaSuccess) return err;
-    // Grid: one resident wave, no more CTAs than round 1 has choose items; at least one, which finds G = 0's offsets
-    // bad.
-    long long grid = static_cast<long long>(sms) * per_sm;
-    grid = std::max(1ll, std::min(grid, static_cast<long long>(K) * G));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(grid));
-    cfg.blockDim = dim3(kTabThreads);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, preempt_pods_kernel, a);
+    // Grid: no more CTAs than round 1 has choose items; at least one, which finds G = 0's offsets bad.
+    return coop_launch<preempt_pods_kernel>(a, static_cast<long long>(L.K) * G, device, stream);
 }
 
 // ---- egpu::preempt_gangs (DESIGN.md §2.15, §4.10): gangs with priority preemption, in gang order ----
@@ -2065,7 +1884,8 @@ cudaError_t preempt_launch(const int32_t* free_core, const int32_t* free_mem, co
 // One cooperative launch.  The outer loop over gangs is place_gangs_kernel's; a gang's rounds are preempt_pods_kernel's
 // phases over the gang's pending pods (node = -2 inside [gang_offsets[j], gang_offsets[j + 1])), with two changes:
 //   0. as preempt_pods, plus gang_offsets, gang_min, run_gang and run_gang_min checked before anything is read through
-//      them.  After the check's barrier, each gang's pods in the domain and each running job's alive pods are counted;
+//      them.  After the check's barrier, each gang's pods in the domain (count_into_gang) and each running job's alive
+//      pods are counted;
 //      a job's slack is max(0, alive - run_gang_min) wherever it is read, so evictions and their undoing only move
 //      the alive count;
 //   1a. before the choose items, one warp per usable node writes the capped C (§2.15 rule 1) as a 128-bit slot mask
@@ -2076,20 +1896,12 @@ cudaError_t preempt_launch(const int32_t* free_core, const int32_t* free_mem, co
 //       own victims finds the count at the job's slack), and after another barrier the passing ones are applied, one
 //       warp per pod.  Unflagged rounds (every round when no running pod is in a job) skip both barriers;
 //   end of a gang: placed + deferred < gang_min or nothing deferred ends it.  A gang given back is rolled back by
-//   integer atomics: its pods' demand returns to the tables, and every running pod it evicted is alive again, its
-//   demand taken from the tables and its job's count restored; one barrier follows before the next gang reads them.
-struct PreGangsCtl {
-    RoundsCtl bar;                // grid-barrier words
-    unsigned long long timeouts;  // grid_barrier's count of waits that gave up (info[1] says whether one did)
-    unsigned int bad_index;       // an index tensor or run_gang_min failed the check (info[2])
-    unsigned int deferred[2];     // pods deferred by a round's commit, by round parity
-    unsigned int budget[2];       // a round recorded a preemptor with a victim in a running job, by round parity
-    unsigned int pad_[3];
-};
-
+//   integer atomics: its pods' demand returns to the tables (give_back_pods), and every running pod it evicted is
+//   alive again, its demand taken from the tables and its job's count restored; one barrier follows before the next
+//   gang reads them.
 struct PreGangsArgs {
     PreemptArgs p;               // tables, containers, pod_offsets, running pods, the outputs node, dev, evicted,
-                                 // tables and info, and the scratch rec, choice, has_empty, usable (p.prio, p.ctl unused)
+                                 // tables and info, and the scratch ctl, rec, choice, has_empty, usable (p.prio unused)
     const int32_t* goff;         // gang_offsets [J + 1], gang_min [J], gang_prio [J], run_gang [H], run_gang_min [R]
     const int32_t* gmin;
     const int32_t* gprio;
@@ -2105,78 +1917,7 @@ struct PreGangsArgs {
     unsigned int* vmask;         // [G][4]: a waiting preemptor's victims by slot (bit lane of word i: slot lane + 32 i)
     unsigned long long* vdev;    // [G]: a waiting preemptor's devices
     unsigned int* cap;           // [N][4]: the round's capped C per node, by slot
-    PreGangsCtl* ctl;
 };
-
-// pre_victims with C given: cand holds the lane's slots of C (bit i: slot lane + 32 i).  The same walk, key and
-// result.
-__device__ __forceinline__ bool pre_victims_capped(const PreemptArgs& a, WarpTab& t, int rows, unsigned int cand,
-                                                   long long c0, int len, long long h0, long long h1, int n,
-                                                   unsigned int& in_v, PreKey& k, unsigned long long& cdev) {
-    const int lane = threadIdx.x & 31;
-    if (!__any_sync(0xffffffffu, cand != 0u)) return false;
-    uint32_t q[4];  // priority + 2^31: its unsigned order is the priority's
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const long long h = h0 + lane + 32 * i;
-        q[i] = h < h1 ? static_cast<uint32_t>(__ldg(a.rprio + h)) ^ 0x80000000u : 0u;
-    }
-    WarpTab base = t;  // the table plus the demand of V
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-        for (unsigned int m = __ballot_sync(0xffffffffu, (cand >> i) & 1u); m; m &= m - 1u)
-            add_running(a, base, h0 + (__ffs(m) - 1) + 32 * i, 1);
-    WarpTab w = base;
-    uint32_t slc, slm;
-    unsigned int used;
-    if (!warp_replay(w, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used)) return false;
-    in_v = cand;
-    unsigned int left = cand;
-    while (__any_sync(0xffffffffu, left != 0u)) {
-        uint32_t bq = 0;
-        int bi = 4;
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-            if (((left >> i) & 1u) && (bi == 4 || q[i] > bq)) {
-                bq = q[i];
-                bi = i;
-            }
-        const uint32_t top = __reduce_max_sync(0xffffffffu, bi < 4 ? bq : 0u);
-        const uint32_t at = __reduce_min_sync(0xffffffffu, bi < 4 && bq == top ? static_cast<uint32_t>(lane + 32 * bi) : ~0u);
-        const int slot = static_cast<int>(at >> 5), owner = static_cast<int>(at & 31u);
-        if (lane == owner) left &= ~(1u << slot);
-        WarpTab trial = base;
-        add_running(a, trial, h0 + at, -1);
-        WarpTab tw = trial;
-        uint32_t tlc, tlm;
-        unsigned long long tdev;
-        if (warp_replay(tw, rows, a.rc, a.rm, c0, len, tlc, tlm, tdev, used)) {
-            base = trial;
-            w = tw;
-            slc = tlc;
-            slm = tlm;
-            cdev = tdev;
-            if (lane == owner) in_v &= ~(1u << slot);
-        }
-    }
-    uint32_t top = 0;
-    unsigned long long sum = 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-        if ((in_v >> i) & 1u) {
-            top = max(top, q[i]);
-            sum += q[i];
-        }
-    top = __reduce_max_sync(0xffffffffu, top);
-    const unsigned int count = __reduce_add_sync(0xffffffffu, static_cast<unsigned int>(__popc(in_v)));
-#pragma unroll
-    for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    k.a = static_cast<unsigned long long>(top) + 1ull;
-    k.b = (sum << 8) | count;
-    k.c = (((static_cast<unsigned long long>(slc) << 21) | slm) << 31) | static_cast<unsigned long long>(n);
-    t = w;
-    return true;
-}
 
 __global__ void __launch_bounds__(kTabThreads, 2)
 preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
@@ -2198,56 +1939,36 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
     {
         bool bad = false;
         for (long long g = first; g <= a.G; g += stride) {
-            const int32_t o = __ldg(a.off + g);
-            if (g == 0) bad |= o != 0;
-            if (g == a.G) bad |= o != a.P;
-            if (g < a.G) {
-                const long long step = static_cast<long long>(__ldg(a.off + g + 1)) - o;
-                bad |= step < 1 || step > kMaxPod;
-                a.node[g] = -2;
-            }
+            bad |= csr_bad(a.off, g, a.G, a.P, 1, kMaxPod);
+            if (g < a.G) a.node[g] = -2;
         }
         for (long long j = first; j <= ga.J; j += stride) {
-            const int32_t o = __ldg(ga.goff + j);
-            if (j == 0) bad |= o != 0;
-            if (j == ga.J) bad |= o != a.G;
+            bad |= csr_bad(ga.goff, j, ga.J, a.G, 1, LLONG_MAX);
             if (j < ga.J) {
-                const long long size = static_cast<long long>(__ldg(ga.goff + j + 1)) - o;
                 const int32_t m = __ldg(ga.gmin + j);
-                bad |= size < 1 || m < 1 || m > size;
+                bad |= m < 1 || m > static_cast<long long>(__ldg(ga.goff + j + 1)) - __ldg(ga.goff + j);
                 ga.placed[j] = 0;
             }
         }
         for (long long h = first; h <= a.H; h += stride) {
-            const int32_t o = __ldg(a.roff + h);
-            if (h == 0) bad |= o != 0;
-            if (h == a.H) bad |= o != a.Q;
+            bad |= csr_bad(a.roff, h, a.H, a.Q, 1, kMaxPod);
             if (h < a.H) {
-                const long long step = static_cast<long long>(__ldg(a.roff + h + 1)) - o;
                 const int32_t r = __ldg(ga.rgang + h);
-                bad |= step < 1 || step > kMaxPod || r < -1 || r >= ga.R;
+                bad |= r < -1 || r >= ga.R;
                 a.evicted[h] = -1;
             }
         }
-        for (long long n = first; n <= N; n += stride) {
-            const int32_t o = __ldg(a.noff + n);
-            if (n == 0) bad |= o != 0;
-            if (n == N) bad |= o != a.H;
-            if (n < N) {
-                const long long step = static_cast<long long>(__ldg(a.noff + n + 1)) - o;
-                bad |= step < 0 || step > kMaxRun;
-            }
-        }
+        for (long long n = first; n <= N; n += stride) bad |= csr_bad(a.noff, n, N, a.H, 0, kMaxRun);
         for (long long r = first; r < ga.R; r += stride) bad |= __ldg(ga.rgmin + r) < 0;
         for (long long c = first; c < a.P; c += stride) a.dev[c] = -2;
         for (long long j = first; j < static_cast<long long>(N) * D; j += stride) {
             a.fc_out[j] = a.fc[j];
             a.fm_out[j] = a.fm[j];
         }
-        if (__syncthreads_or(bad) && tid == 0) atomicExch(&ga.ctl->bad_index, 1u);
+        if (__syncthreads_or(bad) && tid == 0) atomicExch(&a.ctl->bad_index, 1u);
     }
-    if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
-    if (*reinterpret_cast<volatile unsigned int*>(&ga.ctl->bad_index)) {  // nothing is placed or evicted
+    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
+    if (*reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_index)) {  // nothing is placed or evicted
         for (long long g = first; g < a.G; g += stride) a.node[g] = -1;
         for (long long c = first; c < a.P; c += stride) a.dev[c] = -1;
         done = true;
@@ -2257,7 +1978,6 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
         for (long long g0 = static_cast<long long>(b) * kTabThreads; g0 < a.G; g0 += stride) {
             const long long g = g0 + tid;
             bool ok = g < a.G;
-            long long j = 0;
             if (ok) {
                 const int32_t c0 = __ldg(a.off + g), c1 = __ldg(a.off + g + 1);
                 for (int32_t c = c0; c < c1; ++c) {
@@ -2268,50 +1988,16 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                     a.node[g] = -1;
                     for (int32_t c = c0; c < c1; ++c) a.dev[c] = -1;
                 }
-                long long lo = 0, hi = ga.J - 1;  // the last gang whose first pod is at or before g
-                while (lo < hi) {
-                    const long long mid = (lo + hi + 1) >> 1;
-                    if (__ldg(ga.goff + mid) <= g) lo = mid;
-                    else hi = mid - 1;
-                }
-                j = lo;
             }
-            const unsigned int peers = __match_any_sync(0xffffffffu, ok ? j : -1ll);
-            if (ok && lane == __ffs(peers) - 1) atomicAdd(ga.in_domain + j, static_cast<unsigned int>(__popc(peers)));
+            count_into_gang(ga.goff, ga.J, g, ok, ga.in_domain);
         }
         for (long long h = first; h < a.H; h += stride) {
             const int32_t r = __ldg(ga.rgang + h);
             if (r >= 0) atomicAdd(ga.alive + r, 1);
         }
-        for (long long n = wfirst; n < N; n += wstride) {
-            const int dv = __ldg(a.dv + n);
-            bool ok = dv >= 1 && dv <= D;
-            const size_t off = static_cast<size_t>(n) * D;
-            for (int j = lane; j < kMaxD; j += 32) {
-                const int32_t c = ok && j < dv ? __ldg(a.fc + off + j) : 0, m = ok && j < dv ? __ldg(a.fm + off + j) : 0;
-                ok &= c >= 0 && c <= kCoreMax && m >= 0 && m <= kMemMax;
-                sSumC[warp][j] = c;
-                sSumM[warp][j] = m;
-            }
-            __syncwarp();
-            const int32_t q0 = __ldg(a.roff + __ldg(a.noff + n)), q1 = __ldg(a.roff + __ldg(a.noff + n + 1));
-            for (int32_t c = q0 + lane; ok && c < q1; c += 32) {
-                const int d = __ldg(a.qd + c);
-                const int32_t core = __ldg(a.qc + c), mem = __ldg(a.qm + c);
-                ok = d >= 0 && d < dv && core >= 0 && core <= kCoreMax && mem >= 0 && mem <= kMemMax;
-                if (ok) {
-                    atomicAdd(&sSumC[warp][d], core);
-                    atomicAdd(&sSumM[warp][d], mem);
-                }
-            }
-            __syncwarp();
-            for (int j = lane; ok && j < dv; j += 32) ok = sSumC[warp][j] <= kCoreMax && sSumM[warp][j] <= kMemMax;
-            ok = __all_sync(0xffffffffu, ok);
-            if (lane == 0) a.usable[n] = ok ? 1u : 0u;
-            __syncwarp();
-        }
+        pre_usable(a, sSumC, sSumM);
     }
-    if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+    if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
 
     for (long long gang = 0; gang < ga.J; ++gang) {
         const int32_t g_lo = __ldg(ga.goff + gang), g_hi = __ldg(ga.goff + gang + 1), need = __ldg(ga.gmin + gang);
@@ -2371,8 +2057,8 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                         }
                     }
                 if (pass == 1 && b == 0 && tid == 0) {  // round - 2's counters, read before round - 1's barriers
-                    ga.ctl->deferred[round & 1] = 0u;
-                    ga.ctl->budget[round & 1] = 0u;
+                    a.ctl->deferred[round & 1] = 0u;
+                    a.ctl->budget[round & 1] = 0u;
                 }
                 const long long items = static_cast<long long>(K) * size;
                 for (long long it = items * b / G, hi = items * (b + 1) / G; it < hi; ++it) {
@@ -2403,41 +2089,13 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                         }
                         if (pre_less(key, best)) best = key;
                     }
-                    if (lane == 0) sKey[warp] = best;
-                    __syncthreads();
-                    if (tid == 0) {
-                        for (int w = 1; w < kTabWarps; ++w)
-                            if (pre_less(sKey[w], best)) best = sKey[w];
-                        unsigned long long* r = a.rec + 3 * (g * K + k);
-                        r[0] = best.a;
-                        r[1] = best.b;
-                        r[2] = best.c;
-                        if (pass == 0 && best.a == 0ull) a.has_empty[g] = 1u;
-                    }
-                    __syncthreads();
+                    pre_record(a, best, g, k, pass, sKey);
                 }
-                if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+                if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
             }
 
-            // ---- 2. reduce: each pending pod's smallest record
-            for (long long g = g_lo + first; g < g_hi; g += stride) {
-                if (__ldcg(a.node + g) != -2) continue;
-                PreKey best = none;
-                for (int k = 0; k < K; ++k) {
-                    const unsigned long long* r = a.rec + 3 * (g * K + k);
-                    const PreKey key{__ldcg(r), __ldcg(r + 1), __ldcg(r + 2)};
-                    if (pre_less(key, best)) best = key;
-                }
-                a.has_empty[g] = 0u;
-                if (best.a == ~0ull) {  // fits no node when scored: -1 for good
-                    a.choice[g] = ~0ull;
-                    a.node[g] = -1;
-                    for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) a.dev[c] = -1;
-                } else {
-                    a.choice[g] = (best.a != 0ull ? 1ull << 32 : 0ull) | (best.c & 0x7fffffffull);
-                }
-            }
-            if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+            pre_reduce(a, g_lo, g_hi);
+            if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
 
             // ---- 3. commit: per node, the gang's pods that chose it in pod order
             for (long long n = wfirst; n < N; n += wstride) {
@@ -2469,25 +2127,8 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                         WarpTab w = t;
                         unsigned long long cdev;
                         bool commit = true;
-                        if (!evicts) {  // §2.12: no closed device, and the demand fits on top of what committed before
-                            uint32_t slc, slm;
-                            unsigned int used;
-                            warp_replay(w, rows, a.rc, a.rm, c0, len, slc, slm, cdev, used);
-                            bool ok = true;
-#pragma unroll
-                            for (int i = 0; i < 2; ++i)
-                                if ((used >> i) & 1u)
-                                    ok &= !((closed >> i) & 1u) && acc_c[i] <= w.c[i] && acc_m[i] <= w.m[i];
-                            commit = __all_sync(0xffffffffu, ok);
-#pragma unroll
-                            for (int i = 0; i < 2; ++i) {
-                                if (commit) {
-                                    acc_c[i] += t.c[i] - w.c[i];
-                                    acc_m[i] += t.m[i] - w.m[i];
-                                } else {
-                                    closed |= used;
-                                }
-                            }
+                        if (!evicts) {
+                            commit = pre_fits(a, t, w, rows, c0, len, acc_c, acc_m, closed, cdev);
                             if (!commit) ++deferred;
                         } else {  // the first pod of the round on n: its victims from the same capped C
                             unsigned int cand = 0, in_v;
@@ -2509,7 +2150,7 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                                 if (lane == 0) {
                                     ga.vdev[g] = cdev;
                                     ga.pre[g] = 1u;
-                                    ga.ctl->budget[round & 1] = 1u;
+                                    a.ctl->budget[round & 1] = 1u;
                                 }
                                 continue;
                             }
@@ -2535,12 +2176,12 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                             a.fm_out[off + lane + 32 * i] = t.m[i] - acc_m[i];
                         }
                 }
-                if (lane == 0 && deferred) atomicAdd(&ga.ctl->deferred[round & 1], deferred);
+                if (lane == 0 && deferred) atomicAdd(&a.ctl->deferred[round & 1], deferred);
                 if (lane == 0 && committed) atomicAdd(ga.committed + gang, committed);
             }
-            if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+            if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
 
-            if (*reinterpret_cast<volatile unsigned int*>(&ga.ctl->budget[round & 1])) {
+            if (*reinterpret_cast<volatile unsigned int*>(&a.ctl->budget[round & 1])) {
                 // ---- 3b. the round budget: the recorded preemptors in pod order, their victims counted per job
                 if (b == 0 && warp == 0)
                     for (long long g0 = g_lo; g0 < g_hi; g0 += 32) {
@@ -2560,7 +2201,7 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                             if (!__any_sync(0xffffffffu, over) && lane == 0) ga.pre[g] = 2u;
                         }
                     }
-                if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+                if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
 
                 // ---- 3c. apply the preemptors that passed, one warp per pod; the others are deferred
                 unsigned int deferred = 0, committed = 0;
@@ -2615,13 +2256,13 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                     if (lane < len) a.dev[c0 + lane] = static_cast<int8_t>((cdev >> (6 * lane)) & 63u);
                     committed += lane == 0;
                 }
-                if (deferred) atomicAdd(&ga.ctl->deferred[round & 1], deferred);
+                if (deferred) atomicAdd(&a.ctl->deferred[round & 1], deferred);
                 if (committed) atomicAdd(ga.committed + gang, committed);
-                if (!grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+                if (!grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
             }
 
             // ---- 4. end the gang, or run another round
-            const unsigned int pending = *reinterpret_cast<volatile unsigned int*>(&ga.ctl->deferred[round & 1]);
+            const unsigned int pending = *reinterpret_cast<volatile unsigned int*>(&a.ctl->deferred[round & 1]);
             const long long placed = __ldcg(ga.committed + gang);
             gang_done = pending == 0u || placed + pending < need;
             if (!gang_done) continue;
@@ -2630,18 +2271,7 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                 break;  // nothing is pending: the next gang reads only what the barriers before published
             }
             // give the gang back: its pods' demand, and every running pod it evicted
-            for (long long g = g_lo + first; g < g_hi; g += stride) {
-                const int32_t nd = __ldcg(a.node + g);
-                for (int32_t c = __ldg(a.off + g), c1 = __ldg(a.off + g + 1); c < c1; ++c) {
-                    if (nd >= 0) {
-                        const size_t at = static_cast<size_t>(nd) * D + __ldcg(a.dev + c);
-                        atomicAdd(a.fc_out + at, __ldg(a.rc + c));
-                        atomicAdd(a.fm_out + at, __ldg(a.rm + c));
-                    }
-                    a.dev[c] = -1;
-                }
-                a.node[g] = -1;
-            }
+            give_back_pods(a, g_lo, g_hi, first, stride);
             for (long long n = wfirst; n < N; n += wstride)
                 for (long long h = __ldg(a.noff + n) + lane, h1 = __ldg(a.noff + n + 1); h < h1; h += 32) {
                     const int32_t e = __ldcg(a.evicted + h);
@@ -2655,26 +2285,20 @@ preempt_gangs_kernel(const __grid_constant__ PreGangsArgs ga) {
                     const int32_t r = __ldg(ga.rgang + h);
                     if (r >= 0) atomicAdd(ga.alive + r, 1);
                 }
-            if (gang + 1 < ga.J && !grid_barrier(&ga.ctl->bar, &ga.ctl->timeouts, gen, &sOk)) goto finish;
+            if (gang + 1 < ga.J && !grid_barrier(&a.ctl->bar, &a.ctl->timeouts, gen, &sOk)) goto finish;
         }
     }
     done = true;
 finish:
     if (b == 0 && tid == 0) {
-        const bool bad = *reinterpret_cast<volatile unsigned int*>(&ga.ctl->bad_index) != 0u;
+        const bool bad = *reinterpret_cast<volatile unsigned int*>(&a.ctl->bad_index) != 0u;
         a.info[0] = bad ? 0 : round;
         a.info[1] = done ? 0 : 1;
         a.info[2] = bad ? 1 : 0;
     }
 }
 
-size_t preempt_gangs_scratch_bytes(int N, int G, int J, int R) {
-    const size_t zeroed = sizeof(PreGangsCtl) + 4 * (2 * static_cast<size_t>(G) + 2 * static_cast<size_t>(J) +
-                                                     2 * static_cast<size_t>(R));
-    return ((zeroed + 15) & ~size_t(15)) + 24 * static_cast<size_t>(G) * preempt_chunks(N) +
-           16 * static_cast<size_t>(G) + 16 * static_cast<size_t>(G) + 16 * static_cast<size_t>(N) +
-           4 * static_cast<size_t>(N);
-}
+size_t preempt_gangs_scratch_bytes(int N, int G, int J, int R) { return PreemptScratch(N, G, J, R).total; }
 
 cudaError_t preempt_gangs_launch(const int32_t* free_core, const int32_t* free_mem, const int32_t* d_valid, int N,
                                  int D, const int32_t* req_core, const int32_t* req_mem, int P,
@@ -2685,66 +2309,31 @@ cudaError_t preempt_gangs_launch(const int32_t* free_core, const int32_t* free_m
                                  const int32_t* run_gang_min, int R, int32_t* out_node, int8_t* out_dev,
                                  int32_t* out_placed, int32_t* out_evicted, int32_t* free_core_out,
                                  int32_t* free_mem_out, int32_t* info, void* scratch, int device, cudaStream_t stream) {
-    // scratch: barrier words | has_empty uint32[G] | pre uint32[G] | in_domain uint32[J] | committed uint32[J] |
-    // alive int32[R] | used int32[R] | (16-aligned) records uint64[G][K][3] | choice uint64[G] | vdev uint64[G] |
-    // vmask uint32[G][4] | cap uint32[N][4] | usable uint32[N]; everything before the records starts at zero
-    const int K = preempt_chunks(N);
+    const PreemptScratch L(N, G, J, R);
     char* s = static_cast<char*>(scratch);
     PreGangsArgs ga{};
     PreemptArgs& a = ga.p;
     a.fc = free_core; a.fm = free_mem; a.dv = d_valid; a.rc = req_core; a.rm = req_mem; a.off = pod_offsets;
     a.qc = run_core; a.qm = run_mem; a.qd = run_dev; a.roff = run_offsets; a.rprio = run_prio; a.noff = node_offsets;
-    a.N = N; a.D = D; a.K = K; a.P = P; a.G = G; a.Q = Q; a.H = H;
+    a.N = N; a.D = D; a.P = P; a.G = G; a.Q = Q; a.H = H;
     a.node = out_node; a.dev = out_dev; a.evicted = out_evicted; a.fc_out = free_core_out; a.fm_out = free_mem_out;
     a.info = info;
     ga.goff = gang_offsets; ga.gmin = gang_min; ga.gprio = gang_prio; ga.rgang = run_gang; ga.rgmin = run_gang_min;
     ga.J = J; ga.R = R;
     ga.placed = out_placed;
-    ga.ctl = reinterpret_cast<PreGangsCtl*>(s);
-    a.has_empty = reinterpret_cast<unsigned int*>(s + sizeof(PreGangsCtl));
-    ga.pre = a.has_empty + G;
-    ga.in_domain = ga.pre + G;
-    ga.committed = ga.in_domain + J;
-    ga.alive = reinterpret_cast<int32_t*>(ga.committed + J);
-    ga.used = ga.alive + R;
-    const size_t zeroed = sizeof(PreGangsCtl) + 4 * (2 * static_cast<size_t>(G) + 2 * static_cast<size_t>(J) +
-                                                     2 * static_cast<size_t>(R));
-    a.rec = reinterpret_cast<unsigned long long*>(s + ((zeroed + 15) & ~size_t(15)));
-    a.choice = a.rec + 3 * static_cast<size_t>(G) * K;
-    ga.vdev = a.choice + G;
-    ga.vmask = reinterpret_cast<unsigned int*>(ga.vdev + G);
-    ga.cap = ga.vmask + 4 * static_cast<size_t>(G);
-    a.usable = ga.cap + 4 * static_cast<size_t>(N);
-    cudaError_t err = cudaMemsetAsync(scratch, 0, zeroed, stream);
+    ga.pre = reinterpret_cast<unsigned int*>(s + L.pre);
+    ga.in_domain = reinterpret_cast<unsigned int*>(s + L.in_domain);
+    ga.committed = reinterpret_cast<unsigned int*>(s + L.committed);
+    ga.alive = reinterpret_cast<int32_t*>(s + L.alive);
+    ga.used = reinterpret_cast<int32_t*>(s + L.used);
+    ga.vdev = reinterpret_cast<unsigned long long*>(s + L.vdev);
+    ga.vmask = reinterpret_cast<unsigned int*>(s + L.vmask);
+    ga.cap = reinterpret_cast<unsigned int*>(s + L.cap);
+    const cudaError_t err = preempt_scratch(a, scratch, L, stream);
     if (err != cudaSuccess) return err;
-
-    // resident CTAs per SM on each device, asked once
-    static std::atomic<int> per_sm_cache[kPlaceDevices];
-    int per_sm = device >= 0 && device < kPlaceDevices ? per_sm_cache[device].load(std::memory_order_relaxed) : 0;
-    if (per_sm == 0) {
-        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, preempt_gangs_kernel, kTabThreads, 0);
-        if (err != cudaSuccess) return err;
-        if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
-        if (device >= 0 && device < kPlaceDevices) per_sm_cache[device].store(per_sm, std::memory_order_relaxed);
-    }
-    int sms = 0;
-    err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    if (err != cudaSuccess) return err;
-    // Grid: as preempt_launch, from N and G alone (the gang sizes are device data): one resident wave, no more CTAs
-    // than a round over all G pods has choose items; at least one, which finds G = 0's offsets bad.
-    long long grid = static_cast<long long>(sms) * per_sm;
-    grid = std::max(1ll, std::min(grid, static_cast<long long>(K) * G));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(grid));
-    cfg.blockDim = dim3(kTabThreads);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, preempt_gangs_kernel, ga);
+    // Grid: as preempt_launch, from N and G alone (the gang sizes are device data): no more CTAs than a round over
+    // all G pods has choose items; at least one, which finds G = 0's offsets bad.
+    return coop_launch<preempt_gangs_kernel>(ga, static_cast<long long>(L.K) * G, device, stream);
 }
 
 }  // namespace egpu
