@@ -69,9 +69,14 @@ def _round(fc, fm, valid, rc, rm, off, pending, node, dev):
     return committed, sorted(deferred)
 
 
-def place(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_offsets, gang_min):
+def place(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_offsets, gang_min, trace=None):
     """Returns (node int32[G], dev int8[P], placed int32[J], free_core_out int32[N, D], free_mem_out int32[N, D],
-    info [3])."""
+    info [3]).
+
+    trace: a list, or None.  Each round appends (j, positions, deferred) to it: gang j, the pods of the round's
+    pending set in the order the kernel lays it out (a gang's round 1: the gang's whole range, pods outside the
+    domain included; later rounds: the pods the round before deferred), and the indices into `positions` of the pods
+    this round defers."""
     fc = np.array(free_core, dtype=np.int64, copy=True)
     fm = np.array(free_mem, dtype=np.int64, copy=True)
     rc = np.asarray(req_core, dtype=np.int64)
@@ -98,10 +103,14 @@ def place(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, gang_off
         t_node = np.full(G, -1, np.int32)
         t_dev = np.full(P, -1, np.int8)
         k = 0
+        positions = pods
         while pending and k + len(pending) >= gmin[j]:
             rounds += 1
             committed, pending = _round(t_fc, t_fm, valid, rc, rm, off, pending, t_node, t_dev)
             k += committed
+            if trace is not None:
+                trace.append((j, positions, np.searchsorted(positions, pending)))
+            positions = np.array(pending, np.int64)
         if k >= gmin[j]:  # then nothing is pending: the rounds ran to the fixed point
             fc, fm = t_fc, t_fm
             node[pods] = t_node[pods]

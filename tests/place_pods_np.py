@@ -59,8 +59,12 @@ def replay_all(fc, fm, valid, cores, mems):
     return fits, devs, slc, slm
 
 
-def place(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets):
-    """Returns (node int32[G], dev int8[P], free_core_out int32[N, D], free_mem_out int32[N, D], info [3])."""
+def place(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets, trace=None):
+    """Returns (node int32[G], dev int8[P], free_core_out int32[N, D], free_mem_out int32[N, D], info [3]).
+
+    trace: a list, or None.  Each round appends (0, positions, deferred) to it: the pods of the round's pending set
+    in the order the kernel lays it out (round 1: every pod, those outside the domain included; later rounds: the
+    pods the round before deferred), and the indices into `positions` of the pods this round defers."""
     fc = np.array(free_core, dtype=np.int64, copy=True)
     fm = np.array(free_mem, dtype=np.int64, copy=True)
     rc = np.asarray(req_core, dtype=np.int64)
@@ -114,5 +118,8 @@ def place(free_core, free_mem, d_valid, req_core, req_mem, pod_offsets):
                     deferred.append(g)
             fc[n] -= acc_c
             fm[n] -= acc_m
+        positions = np.arange(G) if rounds == 1 else pending
         pending = np.array(sorted(deferred), np.int64)
+        if trace is not None:
+            trace.append((0, positions, np.searchsorted(positions, pending)))
     return node, dev, fc.astype(np.int32), fm.astype(np.int32), [rounds, 0, 0]

@@ -6,7 +6,9 @@ kept when at least gang_min of its pods are placed and given back otherwise, in 
      sizes and gang_min, contended seeds;
   3. bit-identical to the loop of §2.13 written in torch around egpu::place_pods (torch.where keeps or drops each
      gang) at N = 5 000 x D = 8 and N = 512 x D = 64, with at most its round count; J = 1 is place_pods when every
-     pod is placed;
+     pod is placed.  Both sides run the same choose, commit and compact phases, so this checks the gang loop (the
+     rounds of each gang, keeping and giving back), not the phases: tests/test_gpu_pods_scale.py checks those against
+     the restatement past every block, stage, tile and grid threshold;
   4. the invariants (conservation of kept demand per device, rolled-back gangs all -1, placed in {0} or
      [gang_min, size], no -2, no grid wait that gave up);
   5. ragged tiles, empty calls, every pod out of the domain;
@@ -62,9 +64,10 @@ def gangs(g, G, lo=1, hi=8, all_or_nothing=0.5):
     return np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32), gmin.astype(np.int32)
 
 
-def check(a, out, rounds=None):
-    """Exactly the numpy restatement's placement, placed counts, tables and info."""
-    exp = ref.place(*a)
+def check(a, out, rounds=None, exp=None):
+    """Exactly the numpy restatement's placement, placed counts, tables and info (`exp`: its outputs, when already
+    computed)."""
+    exp = ref.place(*a) if exp is None else exp
     assert out[0].dtype == np.int32 and out[1].dtype == np.int8 and out[2].dtype == np.int32
     for x, y in zip(out[:5], exp[:5]):
         np.testing.assert_array_equal(x, y)

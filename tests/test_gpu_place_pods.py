@@ -59,10 +59,10 @@ def pods(g, P, hi=8):
     return np.concatenate([[0], np.cumsum(sizes, dtype=np.int64)]).astype(np.int32)
 
 
-def check(fc, fm, dv, rc, rm, off, out, rounds=None):
-    """Exactly the numpy restatement's placement, tables and info."""
+def check(fc, fm, dv, rc, rm, off, out, rounds=None, exp=None):
+    """Exactly the numpy restatement's placement, tables and info (`exp`: its outputs, when already computed)."""
     node, dev, fco, fmo, info = out
-    e_node, e_dev, e_fc, e_fm, e_info = ref.place(fc, fm, dv, rc, rm, off)
+    e_node, e_dev, e_fc, e_fm, e_info = ref.place(fc, fm, dv, rc, rm, off) if exp is None else exp
     assert node.dtype == np.int32 and dev.dtype == np.int8
     np.testing.assert_array_equal(node, e_node)
     np.testing.assert_array_equal(dev, e_dev)
